@@ -268,7 +268,12 @@ bool build_host_bvh(const double* Vd, uint64_t nV, const uint32_t* F, uint64_t n
                 for (int d = 0; d < 3; d++) { f.v0[d] = (float)(L.v0[d] - out.center[d]); f.e0[d] = (float)L.e0[d]; f.e1[d] = (float)L.e1[d]; e2[d] = L.e1[d] - L.e0[d]; }
                 n3[0] = L.e0[1] * L.e1[2] - L.e0[2] * L.e1[1]; n3[1] = L.e0[2] * L.e1[0] - L.e0[0] * L.e1[2]; n3[2] = L.e0[0] * L.e1[1] - L.e0[1] * L.e1[0];
                 f.d00 = (float)L.a00; f.d01 = (float)L.a01; f.d11 = (float)L.a11; f.d22 = (float)(e2[0] * e2[0] + e2[1] * e2[1] + e2[2] * e2[2]);
-                for (int d = 0; d < 3; d++) f.n[d] = (float)n3[d];
+                // UNIT normal: the filter's (w.n)^2 then scales like a squared distance and stays a normal fp32 number wherever the filter runs
+                // (e0 x e1 scales like length^2, so with it (w.n)^2 overflows fp32 for meshes of size ~1e6 and goes subnormal at ~1e-7).  Zero
+                // area (or a non-finite mesh): n = 0, i.e. no plane bound.  The max-component scaling keeps n.n clear of fp64 under/overflow.
+                const double s = std::max(std::fabs(n3[0]), std::max(std::fabs(n3[1]), std::fabs(n3[2])));
+                const double len = (s > 0 && std::isfinite(s)) ? s * std::sqrt((n3[0] / s) * (n3[0] / s) + (n3[1] / s) * (n3[1] / s) + (n3[2] / s) * (n3[2] / s)) : 0.0;
+                for (int d = 0; d < 3; d++) f.n[d] = (len > 0) ? (float)(n3[d] / len) : 0.f;
             }
         });
     }

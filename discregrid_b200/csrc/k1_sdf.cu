@@ -218,8 +218,20 @@ __device__ __forceinline__ double sphere_dist(double px, double py, double pz, d
 //   Mq = max(mesh half extent, |p - ctr|_inf).  With D = |p - c| <= 2 sqrt(3) Mq and r <= 2 sqrt(3) Mq the fp32 value of
 //   sqrt(dx^2+dy^2+dz^2) - r differs from the real one by < 2^-24 (sqrt(3) 2 Mq + 8 D + r) < 35 * 2^-24 Mq (sqrt.approx: 2 ulp);
 //   the reference's own fp64 rounding adds < 1e-15 Mq.  E = 64 * 2^-24 * Mq.
+//   Range.  The relative bound above assumes normal fp32 numbers.  Below them the errors are absolute: a square under 2^-126 is subnormal
+//   (off by up to 2^-149, its root by up to 2^-74.5), and sqrt.approx.ftz reads it as 0, so a distance below 2^-63 comes out as 0.
+//   The spare (64 - 35) 2^-24 Mq of E covers both once Mq >= 2^-40 (a factor 14 over 2^-63).  Above, squares of lengths 1e18+ overflow.
+//   So the budget holds for 2^-40 <= Mq < 1e18; outside that range E = +inf (filter_slack): every fp32 test is undecided and every
+//   decision is made in fp64, exactly as the reference makes it (the packet walk hands such a lane to the per-lane walk).
 // The fp64 chains (two IEEE square roots per node, ~10 cycles per dependent instruction) were the critical path of the kernel.
 // ---------------------------------------------------------------------------------------------------------------
+// E for a query with Mq = max(half extent, |q - ctr|_inf) in fp32: 64 * 2^-24 * Mq rounded up where the budget holds, else +inf.  (A NaN
+// query does not reach Mq -- fmaxf drops NaN -- and is caught by the callers.)
+__device__ __forceinline__ float filter_slack(float Mq)
+{
+    return (Mq >= 9.094947017729282379e-13f /* 2^-40 */ && Mq < 1.0e18f) ? __fmul_ru(Mq, 3.814697265625e-06f) : __int_as_float(0x7f800000);
+}
+
 struct MeshDev {
     const SpherePair* spheres;
     const float4* nodes_f;                 // [T][K1_NODEF_STRIDE]: sphere pair (2 float4) + box pair (3 float4)
@@ -241,7 +253,7 @@ __device__ __forceinline__ void prefetch_l1(const void* p) { asm volatile("prefe
 __device__ __forceinline__ float sqrt_approx(float x)
 {
 #ifdef DG_EMU
-    return std::sqrt(x);
+    return dg_emu_ftz(std::sqrt(dg_emu_ftz(x)));     // the flush of .ftz (the 2-ulp error of .approx is not modelled: the budget covers it)
 #else
     float r;
     asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
@@ -258,6 +270,11 @@ __device__ __forceinline__ float sqrt_approx(float x)
 //   * the projection is declared "outside" only if one edge function is negative beyond a tolerance that covers the fp32 rounding
 //     of the products and the 2^-24-relative perturbation of every coordinate (so: classified outside => truly outside).
 //   bound = outside ? min(edge distances) : min(plane distance, edge distances), minus 4E for the fp32 evaluation itself.
+// Range: the bound is valid wherever E is finite (2^-40 <= Mq < 1e18, filter_slack).  The shadow's normal is a unit vector, so (w.n)^2 is a
+// squared distance (< 1e38), never inf or NaN: with plane2 = inf, min(inf, mseg) = mseg would NOT be a lower bound when the projection falls
+// inside.  |e|^2 < 1.2e37 stays below the 2^126 where __fdividef returns 0.  Products of the outside test that overflow make tol = inf (never
+// "outside"); products that go subnormal lose their relative error bound, and the 2^-146 floor of tol covers them (meshes of size ~1e-11
+// need it).  A zero normal (zero area) gives plane2 = 0: no plane bound.
 // The caller rejects the leaf only if bound > best_hi + 2E (same slack accounting as the box skip).  On bunny/dragon this rejects
 // 83-90 % of the leaf tests; the rest (accepted ones, ties, near misses) take the exact fp64 test.  Prototype with 0 invalid
 // rejections in 3 M leaf tests: see DESIGN.md.
@@ -287,14 +304,15 @@ __device__ __forceinline__ float leaf_lower_bound(const LeafF* __restrict__ rec,
     t = (d22 > 0.f) ? __fdividef(u2, d22) : 0.f; t = fminf(fmaxf(t, 0.f), 1.f);
     rx = ux - t * e2x; ry = uy - t * e2y; rz = uz - t * e2z;
     mseg = fminf(mseg, dot3f(rx, ry, rz, rx, ry, rz));
-    // plane
+    // plane (n is a unit normal, or 0: no plane bound)
     const float nn = dot3f(d.y, d.z, d.w, d.y, d.z, d.w), wn = dot3f(wx, wy, wz, d.y, d.z, d.w);
     const float plane2 = (nn > 0.f) ? __fdividef(wn * wn, nn) : 0.f;
     // is the projection certainly outside the triangle?
     const float p1 = d11 * w0, p2 = d01 * w1, p3 = d00 * w1, p4 = d01 * w0, p5 = d00 * d11, p6 = d01 * d01;
     const float numv = p1 - p2, numu = p3 - p4, den = p5 - p6;
     const float S = d00 + d11, W = sqrt_approx(dot3f(wx, wy, wz, wx, wy, wz));
-    const float tol = 32.f * (1.2e-7f * (fabsf(p1) + fabsf(p2) + fabsf(p3) + fabsf(p4) + p5 + p6) + 0.25f * E * S * (W + sqrt_approx(S)));
+    const float tol = 32.f * (1.2e-7f * (fabsf(p1) + fabsf(p2) + fabsf(p3) + fabsf(p4) + p5 + p6) + 0.25f * E * S * (W + sqrt_approx(S)))
+                    + 1.1210387714598537e-44f;                                   // 2^-146: 16 half-ulps of the subnormal products
     const bool outside = (numv < -tol) || (numu < -tol) || (den - numu - numv < -tol);
     const float lb2 = outside ? mseg : fminf(plane2, mseg);
     return sqrt_approx(fmaxf(lb2, 0.f)) - 4.f * E;      // NaN (degenerate input) compares false in the caller: no rejection
@@ -326,8 +344,8 @@ __device__ __forceinline__ QueryResult nearest_triangle(const MeshDev& M, bool a
     // query point relative to the mesh centre, in fp32, and the interval half-width for this query
     const float qx = (float)(px - M.cx), qy = (float)(py - M.cy), qz = (float)(pz - M.cz);
     const float Mq = fmaxf(fmaxf(M.half_extent, fabsf(qx)), fmaxf(fabsf(qy), fabsf(qz)));
-    // beyond ~1e18 the fp32 squares overflow: switch the filter off for such a query (E = inf leaves every test undecided)
-    const float E = (Mq < 1.0e18f) ? __fmul_ru(Mq, 3.814697265625e-06f) : __int_as_float(0x7f800000);     // 64 * 2^-24 * Mq
+    // outside the budget's range (below 2^-40 or beyond ~1e18) the filter is off for this query: E = inf leaves every test undecided
+    const float E = filter_slack(Mq);
     const float E2 = E + E;
     // BOX SKIP (K1_BOX_SKIP).  A subtree may be skipped when visiting it provably changes nothing: no triangle in it can be
     // accepted, i.e. every d2 the reference would compute there is >= best_sq.  With L = (fp32 distance to the subtree's
@@ -598,11 +616,12 @@ __device__ __forceinline__ QueryResult nearest_triangle_packet(const MeshDev& M,
     res.dist = DBL_MAX; res.s = 0; res.t = 0; res.pos = -1; res.entity = 0;
     const float qx = (float)(px - M.cx), qy = (float)(py - M.cy), qz = (float)(pz - M.cz);
     const float Mq = fmaxf(fmaxf(M.half_extent, fabsf(qx)), fmaxf(fabsf(qy), fabsf(qz)));
-    const float E = __fmul_ru(Mq, 3.814697265625e-06f), E2 = E + E;        // as in nearest_triangle
+    const float E = filter_slack(Mq), E2 = E + E;      // as in nearest_triangle
     const float tiny_best = 1.0e-6f * Mq;
     bool need_fb = false;
     bool act = alive;                                   // lane still takes part in the shared walk
-    if (alive && (!(Mq < 1.0e18f) || !(qx == qx) || !(qy == qy) || !(qz == qz) || n_tri < 2)) { need_fb = true; act = false; }
+    // no certified pruning outside the budget's range (E = inf) or for NaN input: the per-lane walk decides everything in fp64
+    if (alive && (!(E < INF) || !(qx == qx) || !(qy == qy) || !(qz == qz) || n_tri < 2)) { need_fb = true; act = false; }
     float skip_lin = INF, skip_sq = INF, best_lo = INF;
     double dropped = DINF;                              // smallest evaluated value that is NOT in the list
     int cnt = 0;                                        // list: cv[0] <= cv[1] <= ... (stride apart), all within 1e-6 of the minimum when inserted
@@ -1034,7 +1053,7 @@ sdf_sample_nodes_wave_kernel(MeshDev M, const PseudoNormals* __restrict__ normal
                 if (wave_brick_node(g, w, cur_unit, cur_off + lane, px, py, pz, oi)) {
                     const float qx = (float)(px - M.cx), qy = (float)(py - M.cy), qz = (float)(pz - M.cz);
                     const float Mq = fmaxf(fmaxf(M.half_extent, fabsf(qx)), fmaxf(fabsf(qy), fabsf(qz)));
-                    const float E = (Mq < 1.0e18f) ? __fmul_ru(Mq, 3.814697265625e-06f) : F_INF;     // 64 * 2^-24 * Mq
+                    const float E = filter_slack(Mq);                                                 // 64 * 2^-24 * Mq, or inf
                     W.px[slot] = px; W.py[slot] = py; W.pz[slot] = pz; W.out[slot] = oi;
                     W.Q[slot] = make_float4(qx, qy, qz, E);
                     W.best[slot] = DBL_MAX; W.s[slot] = 0.0; W.t[slot] = 0.0;

@@ -4,9 +4,14 @@
 // The emulation TU defines DG_EMU, includes this header and then the .cu file itself.  A kernel "launch" runs the blocks one after the
 // other; the 32 lanes of a warp are fibers on one OS thread, resumed round-robin, and a warp collective (__ballot_sync,
 // __reduce_add_sync) parks a lane until all live lanes of its warp have arrived -- i.e. the code sees exactly the values it would see
-// on the device.  fp64 arithmetic is the host's IEEE arithmetic (the TU is built with -ffp-contract=off, like -fmad=false); the fp32
-// directed-rounding intrinsics are emulated exactly where that is cheap (products) and to within a double rounding elsewhere -- they
-// only feed the traversal FILTER, whose decisions must be valid, not bit-identical to the device's.
+// on the device.  fp64 arithmetic is the host's IEEE arithmetic (the TU is built with -ffp-contract=off, like -fmad=false).
+// fp32 arithmetic only feeds the traversal FILTERS, whose decisions must be valid, not bit-identical to the device's -- but a filter whose
+// error budget does not cover the device's arithmetic changes results, so what the device does differently from IEEE fp32 is modelled where
+// that is cheap: plain fp32 operations are IEEE with subnormals on both sides (no -ftz); sqrt.approx.ftz.f32 flushes subnormal inputs and
+// results to zero (dg_emu_ftz; k1_sdf.cu's sqrt_approx); __fdividef returns 0 for 2^126 < |b| (NaN for an infinite numerator, since
+// it multiplies by an approximate reciprocal that is 0 there).  The directed-rounding intrinsics are exact for products and within a
+// double rounding elsewhere.  NOT modelled, and therefore carried by the error budgets in k1_sdf.cu rather than checked here: the 2-ulp
+// error of sqrt.approx and the 2-ulp error of __fdividef on normal operands, and __fdividef on subnormal denominators.
 // Not emulated: block-level barriers and shared-memory exchange between warps (K1 has none), inline PTX (guarded in the sources).
 #pragma once
 #include <cuda_runtime.h>          // vector types, cudaError_t ... (declarations only; nothing of the runtime is called)
@@ -175,7 +180,10 @@ inline float __fadd_ru(float a, float b) { return dg_emu_round_up((double)a + (d
 inline float __fmaf_rd(float a, float b, float c) { return dg_emu_round_dn(std::fma((double)a, (double)b, (double)c)); }
 inline double __dmul_rn(double a, double b) { return a * b; }
 inline double __fma_rn(double a, double b, double c) { return std::fma(a, b, c); }
-inline float __fdividef(float a, float b) { return a / b; }
+// a * approximate reciprocal of b: for 2^126 < |b| (and b = inf) the reciprocal is 0, so the result is 0 -- or NaN when a is infinite
+inline float __fdividef(float a, float b) { return (std::fabs(b) > 0x1p126f) ? a * std::copysign(0.f, b) : a / b; }
+// flush-to-zero of the .ftz instructions: a subnormal reads / is written as a zero of the same sign
+inline float dg_emu_ftz(float x) { return (std::fabs(x) < 0x1p-126f) ? std::copysign(0.f, x) : x; }
 using std::max;
 using std::min;
 #ifdef __launch_bounds__

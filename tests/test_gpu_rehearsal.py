@@ -12,7 +12,7 @@ import pytest
 from conftest import ROOT, ref_resource
 
 EMU = os.path.join(ROOT, "build", "bin", "libdgemu.so")
-FILES = ["tests/test_gpu_k1_sdf.py", "tests/test_gpu_k2_interp.py", "tests/test_gpu_k3_density.py", "tests/test_gpu_reference_tools.py",
+FILES = ["tests/test_gpu_k1_sdf.py", "tests/test_gpu_k1_scales.py", "tests/test_gpu_k2_interp.py", "tests/test_gpu_k3_density.py", "tests/test_gpu_reference_tools.py",
          "tests/test_gpu_cpp_facade.py", "tests/test_gpu_multi_capi.py", "tests/test_gpu_reduce_field.py"]
 # left to the real GPU: device tensors through torch, the full-size configuration, the 69k-855k-triangle meshes (minutes when emulated)
 SKIP = "not large_grid and not host_pipeline and not device_form and not full_size and not slab_parts and not interleaved_parts and not reference_meshes_vs_oracle"

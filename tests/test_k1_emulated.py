@@ -1,15 +1,22 @@
 """The product's K1 device code and launchers (discregrid_b200/csrc/k1_sdf.cu), compiled for the CPU by tests/emu (lanes of a warp as
 fibers, warp votes resolved exactly) and compared with the oracle / the reference's golden vectors bit for bit -- the kernel logic is
-therefore exercised by the CPU suite too (the real GPU runs are tests/test_gpu_k1_sdf.py).  What is emulated is the logic, not the
-device's fp32 filter arithmetic, which by construction cannot change a result."""
+therefore exercised by the CPU suite too (the real GPU runs are tests/test_gpu_k1_sdf.py and tests/test_gpu_k1_scales.py).
+The fp32 filters (sphere interval, box skip, leaf_lower_bound) may only drop or order work where the fp64 answer is certain, so their
+arithmetic CAN change a result whenever their error budget fails to cover it.  tests/emu/cuda_emu.h models what is cheap to model of the
+device's fp32 arithmetic (the flush to zero of sqrt.approx.ftz, __fdividef's huge-denominator rule); the 2-ulp errors of sqrt.approx and
+__fdividef are not modelled and are left to the budget -- which is why the scale sweep runs on the device too."""
 import ctypes as C
 import os
+import sys
 
 import numpy as np
 import pytest
 
 from conftest import GOLDEN, ROOT, bits_equal, grid_for
 from test_oracle_golden import read_cdf, read_obj
+
+sys.path.insert(0, os.path.join(ROOT, "tools"))
+import k1_fuzz  # noqa: E402  (tools/k1_fuzz.py: mesh generators, backends and checks shared with the fuzzer and the GPU tests)
 
 # default knobs, the knob variants (K1_VOTE_REDUX + K1_BRICK_AUTO), the wavefront kernel, the per-lane kernel and the packet walk (K1_PACKET); DG_K1_EMU_LIB adds any other build of tests/emu/k1_emu.cpp
 LIBS = [os.path.join(ROOT, "build", "bin", n) for n in ("libk1emu.so", "libk1emu_knobs.so", "libk1emu_wave.so", "libk1emu_perlane.so", "libk1emu_packet.so")] + \
@@ -131,34 +138,16 @@ def test_emulated_distance_queries_match_reference_header(emu):
     emu.lib.emu_mesh_destroy(h)
 
 
-def _rand_mesh(rng, n_tri, scale=1.0, offset=0.0, degenerate=False):
-    V = rng.standard_normal((n_tri + 2, 3)) * scale + offset
-    F = np.array([[i, i + 1, i + 2] for i in range(n_tri)], np.uint32)        # a strip: neighbours share edges and vertices (ties)
-    if degenerate and n_tri >= 3:
-        V[3] = V[2]                                                            # zero-length edge -> zero-area triangles
-        F[-1] = [0, 0, 1]                                                      # a triangle with a repeated vertex
-    return np.ascontiguousarray(V), F
-
-
-@pytest.mark.parametrize("n_tri,scale,offset,degenerate", [(1, 1.0, 0.0, False), (2, 1.0, 0.0, False), (3, 1.0, 0.0, False), (7, 1e-9, 0.0, False),
-                                                           (40, 1.0, 1e9, False), (33, 1e6, -3e7, False), (9, 1.0, 0.0, True), (64, 1.0, 0.0, True)])
+@pytest.mark.parametrize("n_tri,scale,offset,degenerate", k1_fuzz.AWKWARD)
 def test_emulated_queries_on_awkward_meshes_vs_reference_header(emu, orc, n_tri, scale, offset, degenerate):
     """corner cases against the reference's own TriangleMeshDistance.h where it is compiled (oracle/_ref), else against the oracle port
     pinned to it: one- and two-triangle meshes (the root is a leaf / has leaf children), tiny and huge coordinates (the fp32 filter's error
     bound scales with them), far-away and non-finite queries (filter switched off / NaN comparisons), degenerate triangles (0/0 in the
     reference's formulas): same distance bits -- NaN for NaN --, same nearest entity and triangle"""
     from oracle_api import RefMesh, have_ref
-    rng = np.random.default_rng(1000 + n_tri)
-    V, F = _rand_mesh(rng, n_tri, scale, offset, degenerate)
-    x = np.concatenate([rng.standard_normal((300, 3)) * scale * 2 + offset,                    # around the mesh
-                        V[:min(len(V), 20)],                                                  # exactly on vertices
-                        0.5 * (V[F[:, 0]] + V[F[:, 1]])[:20],                                  # on edges
-                        rng.standard_normal((40, 3)) * scale * 1e6 + offset,                   # far
-                        np.array([[1e19, -1e19, 3e18], [0.0, 0.0, 0.0], [-0.0, 0.0, -0.0]])])
-    x = np.ascontiguousarray(x)
-    # queries for which the reference accepts no triangle (NaN, infinite, or so large that the squared distance overflows) make it index
-    # triangles[-1] (undefined behaviour: it crashes for some meshes): not sent to the reference; the kernel must answer DBL_MAX / -1
-    lost = np.ascontiguousarray(np.array([[1e300, 0, 0], [np.nan, 0, 0], [np.inf, 1, 2], [0, -np.inf, 0]]))
+    # `lost`: queries for which the reference accepts no triangle (NaN, infinite, or so large that the squared distance overflows) make it
+    # index triangles[-1] (undefined behaviour: it crashes for some meshes): not sent to the reference; the kernel must answer DBL_MAX / -1
+    V, F, x, lost = k1_fuzz.awkward_case(n_tri, scale, offset, degenerate)
     ref = RefMesh(V, F) if have_ref() else orc.mesh(V, F)
     h = emu.mesh(V, F)
     for signed in (1, 0):
@@ -177,6 +166,37 @@ def test_emulated_queries_on_awkward_meshes_vs_reference_header(emu, orc, n_tri,
         same_p = (near.view(np.uint64) == want_near.view(np.uint64)) | (np.isnan(near) & np.isnan(want_near))
         assert same_p[found].all()
     emu.lib.emu_mesh_destroy(h)
+
+
+@pytest.mark.parametrize("mode", ["points", "grid"])
+@pytest.mark.parametrize("so", LIBS, ids=[os.path.basename(p) for p in LIBS])
+def test_scale_sweep_vs_reference_header(so, mode):
+    """the fp32 filters across mesh scales (tools/k1_fuzz.py, `scales`): random soups, strips and coplanar grids at 10^k for k = -24 .. 17,
+    each centred and with an offset 10^3 - 10^6 times its size, plus soups whose half extent is just below / above the 1e18 limit of the
+    filters; arbitrary points (signed + unsigned: distance bits, nearest point, entity, triangle id) and the node loop on a (9, 7, 6)
+    lattice over each mesh (sign * distance bits) == the reference's own header (where compiled, else the oracle port pinned to it).
+    Large meshes once broke leaf_lower_bound (its plane term overflowed fp32 and the true nearest triangle was rejected), tiny ones the
+    budget of every filter (fp32 squares going subnormal, sqrt.approx.ftz flushing them)"""
+    if not os.path.exists(so):
+        pytest.skip(f"{so} not built (make cpp)")
+    msgs = []
+    meshes, checked, bad = k1_fuzz.run_scales(k1_fuzz.EmuK1(so), seed=0, modes=(mode,), log=msgs.append)
+    assert meshes == 2 * 3 * len(k1_fuzz.SCALE_EXPONENTS) + 2 and checked > 100000
+    assert bad == 0, f"{bad} mismatches: " + "\n".join(msgs[:8])
+
+
+@pytest.mark.parametrize("name", ["libk1emu.so", "libk1emu_packet.so"])
+def test_small_meshes_leaf_bound_vs_reference_header(name):
+    """the packet walk's leaf_lower_bound on meshes of size 1e-12 .. 1e-7, where its filter is on but the degree-4 products of its
+    inside / outside test go subnormal and lose their relative error bound (the absolute floor of its tolerance covers them): sweep seeds
+    that each produced a wrong node without that floor"""
+    so = os.path.join(ROOT, "build", "bin", name)
+    if not os.path.exists(so):
+        pytest.skip(f"{so} not built (make cpp)")
+    be, msgs, bad = k1_fuzz.EmuK1(so), [], 0
+    for seed in (13, 18, 26, 29, 30, 31):
+        bad += k1_fuzz.run_scales(be, seed=seed, modes=("grid",), exponents=tuple(range(-12, -6)), log=msgs.append)[2]
+    assert bad == 0, f"{bad} mismatches: " + "\n".join(msgs[:8])
 
 
 def test_tie_rich_fuzz_against_reference_header():
