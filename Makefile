@@ -24,7 +24,7 @@ CPPBIN   := build/bin
 CPPFLAGS := -std=c++11 -O2 -ffp-contract=off -I$(EIGEN3_INCLUDE_DIR) -Icpp/include -Iinclude
 CPPLINK  := -Ldiscregrid_b200/lib -ldiscregrid_b200 -Wl,-rpath,'$$ORIGIN/../../discregrid_b200/lib'
 CPPHDRS  := $(wildcard cpp/include/Discregrid/* cpp/include/Discregrid/*/*) include/discregrid_b200.h
-cpp: $(CPPBIN)/GenerateSDF $(CPPBIN)/GenerateDensityMap $(CPPBIN)/DiscreteFieldToBitmap $(CPPBIN)/facade_check $(CPPBIN)/bvh_host_check $(CPPBIN)/reduce_facade_check $(CPPBIN)/sort_replay_check $(CPPBIN)/fast_div_check $(CPPBIN)/libk1emu.so $(CPPBIN)/libk1emu_knobs.so $(CPPBIN)/libk1emu_wave.so $(CPPBIN)/libk1emu_perlane.so $(CPPBIN)/libk1emu_packet.so $(CPPBIN)/libk23emu.so $(CPPBIN)/libk23emu_knobs.so $(CPPBIN)/libdgemu.so
+cpp: $(CPPBIN)/GenerateSDF $(CPPBIN)/GenerateDensityMap $(CPPBIN)/DiscreteFieldToBitmap $(CPPBIN)/facade_check $(CPPBIN)/bvh_host_check $(CPPBIN)/reduce_facade_check $(CPPBIN)/sort_replay_check $(CPPBIN)/fast_div_check $(CPPBIN)/libk1emu.so $(CPPBIN)/libk1emu_knobs.so $(CPPBIN)/libk1emu_wave.so $(CPPBIN)/libk1emu_perlane.so $(CPPBIN)/libk1emu_packet.so $(CPPBIN)/libk1emu_band.so $(CPPBIN)/libk1emu_band_perlane.so $(CPPBIN)/libk23emu.so $(CPPBIN)/libk23emu_knobs.so $(CPPBIN)/libdgemu.so
 $(CPPBIN)/DiscreteFieldToBitmap: cpp/cmd/discrete_field_to_bitmap.cpp $(CPPHDRS) $(LIB)
 	@mkdir -p $(CPPBIN)
 	$(HOSTCXX) $(CPPFLAGS) $< -o $@ $(CPPLINK)
@@ -52,6 +52,14 @@ $(CPPBIN)/libk1emu_packet.so: $(K1EMU_DEP)
 $(CPPBIN)/libk1emu_perlane.so: $(K1EMU_DEP)
 	@mkdir -p $(CPPBIN)
 	$(HOSTCXX) -std=c++17 -O2 -ffp-contract=off -fPIC -shared -DK1_WAVE=0 -DK1_PACKET=0 -I$(CUDA_INC) -Itests/emu -I$(SRC) $(K1EMU_SRC) -o $@ -lpthread
+# the narrow-band launcher (classifier + band node loop) on top of the same TU: packet walk (default) and per-lane walk
+K1BAND_SRC := tests/emu/k1_band_emu.cpp $(SRC)/bvh_build.cpp $(SRC)/host_threads.cpp $(SRC)/sort_replay.cpp
+$(CPPBIN)/libk1emu_band.so: $(K1EMU_DEP) tests/emu/k1_band_emu.cpp
+	@mkdir -p $(CPPBIN)
+	$(HOSTCXX) -std=c++17 -O2 -ffp-contract=off -fPIC -shared -I$(CUDA_INC) -Itests/emu -I$(SRC) $(K1BAND_SRC) -o $@ -lpthread
+$(CPPBIN)/libk1emu_band_perlane.so: $(K1EMU_DEP) tests/emu/k1_band_emu.cpp
+	@mkdir -p $(CPPBIN)
+	$(HOSTCXX) -std=c++17 -O2 -ffp-contract=off -fPIC -shared -DK1_PACKET=0 -I$(CUDA_INC) -Itests/emu -I$(SRC) $(K1BAND_SRC) -o $@ -lpthread
 K23EMU_SRC := tests/emu/k2_emu.cpp tests/emu/k3_emu.cpp
 K23EMU_DEP := $(K23EMU_SRC) tests/emu/cuda_emu.h $(SRC)/k2_interp.cu $(SRC)/k3_density.cu $(HDRS)
 $(CPPBIN)/libk23emu.so: $(K23EMU_DEP)

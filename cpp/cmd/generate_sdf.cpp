@@ -1,6 +1,9 @@
 // GenerateSDF -- same command line and output as the reference tool (cmd/generate_sdf/main.cpp:28-130), sampling on the GPU.
-//   GenerateSDF [-r "nx ny nz"] [-d "minx miny minz maxx maxy maxz"] [-i] [-o out.cdf] [--gpus N] input.obj
+//   GenerateSDF [-r "nx ny nz"] [-d "minx miny minz maxx maxy maxz"] [-i] [-o out.cdf] [--gpus N] [--band W [--no-reduction]] input.obj
 // --gpus N (new, SURVEY 5 "same flags + --gpus N"): the node loop is dealt to N GPUs of this node (dg_add_function_sdf_multi); same file.
+// --band W (new): a narrow-band field -- addFunction(func, verbose, pred) with pred(x) = |distance(x)| <= W (world units), DBL_MAX
+//   elsewhere, then reduceField with an always-true predicate (drops the DBL_MAX nodes and the cells without a kept node), as
+//   GenerateDensityMap does (cmd/generate_density_map/main.cpp:119-147).  --no-reduction keeps the dense field.  One GPU only.
 // The one functional change against the reference source: the functor handed to addFunction is the recognisable
 // MeshSignedDistanceFunction instead of an anonymous lambda (main.cpp:94-102).
 #include <Discregrid/All>
@@ -17,12 +20,16 @@ int main(int argc, char* argv[])
     std::string domain_str, output_file, filename;
     bool invert = false;
     int n_gpus = 1;
+    bool use_band = false, no_reduction = false;
+    double band = 0.0;
     for (int a = 1; a < argc; a++) {
         const std::string s = argv[a];
         auto next = [&]() -> std::string { if (a + 1 >= argc) { std::cerr << "missing value for " << s << std::endl; std::exit(1); } return argv[++a]; };
         if (s == "-h" || s == "--help") {
             std::cout << "Generates a signed distance field from a closed two-manifold triangle mesh.\n"
                          "  -r, --resolution \"nx ny nz\"   -d, --domain \"minx miny minz maxx maxy maxz\"   -i, --invert   -o, --output file.cdf   --gpus N\n"
+                         "  --band W   keep only nodes within distance W of the surface (others DBL_MAX), then reduce the field\n"
+                         "  --no-reduction   with --band: keep the dense field (no reduceField)\n"
                          "Example: GenerateSDF -r \"50 50 50\" dragon.obj" << std::endl;
             return 0;
         } else if (s == "-r" || s == "--resolution") { std::istringstream is(next()); is >> resolution[0] >> resolution[1] >> resolution[2]; }
@@ -30,10 +37,14 @@ int main(int argc, char* argv[])
         else if (s == "-i" || s == "--invert") invert = true;
         else if (s == "-o" || s == "--output") output_file = next();
         else if (s == "--gpus") n_gpus = std::atoi(next().c_str());
+        else if (s == "--band") { use_band = true; band = std::strtod(next().c_str(), nullptr); }
+        else if (s == "--no-reduction") no_reduction = true;
         else filename = s;
     }
     if (filename.empty()) { std::cout << "ERROR: No input mesh given." << std::endl; return 1; }
     if (!std::ifstream(filename).good()) { std::cerr << "ERROR: Input file does not exist!" << std::endl; return 1; }
+    if (use_band && n_gpus > 1) { std::cerr << "ERROR: --band runs on one GPU; it cannot be combined with --gpus " << n_gpus << std::endl; return 1; }
+    if (use_band && !(band >= 0.0)) { std::cerr << "ERROR: --band needs a width >= 0" << std::endl; return 1; }
     try {
         std::cout << "Load mesh...";
         Discregrid::TriangleMesh mesh(filename);
@@ -56,7 +67,14 @@ int main(int argc, char* argv[])
         Discregrid::CubicLagrangeDiscreteGrid sdf(domain, resolution);
         Discregrid::DiscreteGrid::ContinuousFunction func = Discregrid::MeshSignedDistanceFunction(md, invert);
         std::cout << "Generate discretization..." << std::endl;
-        sdf.addFunction(func, true);
+        if (use_band) {
+            sdf.addFunction(func, true, Discregrid::MeshDistanceBandPredicate(md, band));
+            if (!no_reduction) {
+                std::cout << "Reduce discretization...";
+                sdf.reduceField(0, [](Vector3d const&, double) { return true; });
+                std::cout << "DONE" << std::endl;
+            }
+        } else sdf.addFunction(func, true);
         std::cout << "DONE" << std::endl;
         std::cout << "Serialize discretization...";
         if (output_file.empty()) {

@@ -1,7 +1,9 @@
 // Discregrid::CubicLagrangeDiscreteGrid -- the reference's public surface and members
 // (discregrid/include/Discregrid/cubic_lagrange_discrete_grid.hpp:8-72) with the hot path on the H100:
 //
-//   addFunction(MeshSignedDistanceFunction)  -> dg_sample_sdf   (K1)   replaces the OpenMP node loop :806-831
+//   addFunction(MeshSignedDistanceFunction)  -> dg_add_function_sdf (K1)   replaces the OpenMP node loop :806-831
+//   addFunction(MeshSignedDistanceFunction, verbose, MeshDistanceBandPredicate)
+//                                            -> dg_add_function_sdf_band (K1, narrow band: DBL_MAX where |distance| > band, :811-817)
 //   addFunction(DensityMapFunction)          -> dg_density_map  (K3)   (GenerateDensityMap's functor + predicate)
 //   interpolate(field, x, grad*)             -> dg_interpolate_batch (K2), also batched: interpolate(field, n, x, phi, grad)
 //   connectivity table of addFunction        -> dg_build_cells  (GPU)  replaces the serial loop :833-886
@@ -108,7 +110,14 @@ public:
         std::uint64_t n_nodes = 0;
         check(dg_grid_num_nodes(d.resolution, &n_nodes));
         if (auto const* sdf = func.target<MeshSignedDistanceFunction>()) {
-            if (pred) throw std::invalid_argument("addFunction: a sample predicate is only supported with DensityMapFunction");
+            auto const* band = pred ? pred.target<MeshDistanceBandPredicate>() : nullptr;
+            if (pred && !band)
+                throw std::invalid_argument("addFunction: a sample predicate is only supported with DensityMapFunction, or as MeshDistanceBandPredicate "
+                                            "with MeshSignedDistanceFunction");
+            if (band && band->md != sdf->md)
+                throw std::invalid_argument("addFunction: the MeshDistanceBandPredicate must use the same TriangleMeshDistance as the MeshSignedDistanceFunction");
+            if (band && sdf->md->group())
+                throw std::invalid_argument("addFunction: narrow-band sampling runs on one GPU; it is not available after TriangleMeshDistance::useGpus(n > 1)");
             // the whole of :780-899 in one library call: node loop on the GPU; connectivity (:833-886) and cell map (:888-891) written by
             // the library's host threads into these arrays while the GPU works
             FieldVector<double> coeffs(n_nodes);
@@ -117,6 +126,9 @@ public:
             if (sdf->md->group())             // TriangleMeshDistance::useGpus(n): the same call spread over n GPUs
                 check(dg_add_function_sdf_multi(sdf->md->group(), &d, sdf->sign, coeffs.data(), reinterpret_cast<std::uint32_t*>(cells.data()), cell_map.data(),
                                                 m_last_add_function_ms));
+            else if (band)
+                check(dg_add_function_sdf_band(sdf->md->handle(), &d, sdf->sign, band->band, coeffs.data(), reinterpret_cast<std::uint32_t*>(cells.data()),
+                                               cell_map.data(), m_last_add_function_ms));
             else
                 check(dg_add_function_sdf(sdf->md->handle(), &d, sdf->sign, coeffs.data(), reinterpret_cast<std::uint32_t*>(cells.data()), cell_map.data(),
                                           m_last_add_function_ms));

@@ -118,4 +118,13 @@ struct MeshSignedDistanceFunction {
     double operator()(Eigen::Vector3d const& xi) const { const double d = md->signed_distance(xi).distance; return sign == 1.0 ? d : sign * d; }
 };
 
+// new: the narrow-band sample predicate x -> |md.signed_distance(x).distance| <= band as a recognisable type.  A valid SamplePredicate on its
+// own; handed to addFunction next to a MeshSignedDistanceFunction over the same md, the band is sampled on the GPU (DBL_MAX outside it).
+struct MeshDistanceBandPredicate {
+    const TriangleMeshDistance* md;
+    double band;
+    MeshDistanceBandPredicate(const TriangleMeshDistance& m, double w) : md(&m), band(w) {}
+    bool operator()(Eigen::Vector3d const& xi) const { return std::abs(md->signed_distance(xi).distance) <= band; }
+};
+
 }  // namespace Discregrid

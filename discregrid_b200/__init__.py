@@ -7,10 +7,10 @@ discregrid_b200/lib/libdiscregrid_b200.so and fails if it has not been built; th
 from . import _capi
 from ._capi import DiscregridError, DBL_MAX, LIB_PATH
 from .mesh import TriangleMesh, bumpy_torus, uv_sphere, box
-from .distance import TriangleMeshDistance, MeshSignedDistance, NearestEntity, Result
+from .distance import TriangleMeshDistance, MeshSignedDistance, MeshDistanceBand, NearestEntity, Result
 from .grid import CubicLagrangeDiscreteGrid, DensityMapFunction, grid_desc, generate_sdf_domain
 
-__all__ = ["TriangleMesh", "TriangleMeshDistance", "MeshSignedDistance", "NearestEntity", "Result",
+__all__ = ["TriangleMesh", "TriangleMeshDistance", "MeshSignedDistance", "MeshDistanceBand", "NearestEntity", "Result",
            "CubicLagrangeDiscreteGrid", "DensityMapFunction", "grid_desc", "generate_sdf_domain", "DiscregridError",
            "DBL_MAX", "LIB_PATH", "bumpy_torus", "uv_sphere", "box"]
 

@@ -74,6 +74,8 @@ SIGNATURES = {
     "dg_add_function_sdf_multi": (C.c_int, [_vp, _gp, C.c_double, _dp, _u32p, _u32p, _dp]),
     "dg_sample_sdf_multi_device": (C.c_int, [_vp, _gp, C.c_double, C.POINTER(_vp)]),
     "dg_sample_sdf_device": (C.c_int, [_vp, _gp, C.c_double, C.c_uint64, C.c_uint64, _vp, _vp]),
+    "dg_sample_sdf_band_device": (C.c_int, [_vp, _gp, C.c_double, C.c_double, C.c_uint64, C.c_uint64, _vp, _vp]),
+    "dg_add_function_sdf_band": (C.c_int, [_vp, _gp, C.c_double, C.c_double, _dp, _u32p, _u32p, _dp]),
     "dg_slab_ranges": (C.c_int, [_gp, C.c_uint32, C.c_uint32, _u64p]),
     "dg_sample_sdf_slab_device": (C.c_int, [_vp, _gp, C.c_double, C.c_uint32, C.c_uint32, _vp, _vp]),
     "dg_interleaved_slot_elems": (C.c_int, [_gp, C.c_uint32, _u64p]),

@@ -468,6 +468,40 @@ int dg_sample_sdf_device(const dg_mesh* m, const dg_grid_desc* grid, double sign
     return DG_OK;
 }
 
+static int check_band(double band, const char* who)
+{
+    if (!(band >= 0.0)) return fail(DG_ERR_INVALID, "%s: band must be >= 0 (got %g)", who, band);     // negative or NaN
+    return DG_OK;
+}
+
+// addFunction(func, verbose, pred) with pred(x) = |md.signed_distance(x).distance| <= band (cubic_lagrange_discrete_grid.cpp:806-817): the
+// classifier passes and the band form of the node loop, in stream order; the scratch is allocated and released on the same stream.
+int dg_sample_sdf_band_device(const dg_mesh* m, const dg_grid_desc* grid, double sign, double band, uint64_t l_begin, uint64_t l_end, double* d_out,
+                              void* stream)
+{
+    if (!m) return fail(DG_ERR_INVALID, "dg_sample_sdf_band: mesh is NULL (not constructed)");
+    GridDev g;
+    if (int rc = check_range(grid, l_begin, l_end, g, "dg_sample_sdf_band")) return rc;
+    if (int rc = check_band(band, "dg_sample_sdf_band")) return rc;
+    if (l_end > l_begin && !d_out) return fail(DG_ERR_INVALID, "dg_sample_sdf_band: output is NULL");
+    if (int rc = check_handle_device(m->device, "dg_sample_sdf_band")) return rc;
+    if (l_end == l_begin) return DG_OK;
+    const cudaStream_t st = (cudaStream_t)stream;
+    const size_t bytes = k1_band_scratch_bytes(g, l_begin, l_end - l_begin);
+    void* scratch = nullptr;
+#ifdef DG_EMU
+    DG_CUDA(cudaMalloc(&scratch, bytes));
+    const cudaError_t e = k1_launch_sample_nodes_band(m->dev, g, sign, band, l_begin, l_end - l_begin, d_out, scratch, st);
+    cudaFree(scratch);
+#else
+    DG_CUDA(cudaMallocAsync(&scratch, bytes, st));
+    const cudaError_t e = k1_launch_sample_nodes_band(m->dev, g, sign, band, l_begin, l_end - l_begin, d_out, scratch, st);
+    cudaFreeAsync(scratch, st);
+#endif
+    DG_LAUNCH(e);
+    return DG_OK;
+}
+
 // Host-buffer path of K1.  Resources that are expensive to create per call (device scratch, two pinned staging buffers,
 // streams, events) live in a per-process pool.  The range is cut into a few kernel launches dealt to two streams (a K1
 // launch ends with a tail of long-running warps; the next launch fills the machine meanwhile); a third stream DMAs
@@ -481,8 +515,9 @@ struct HostPathPool {
     cudaStream_t s_k[2] = {nullptr, nullptr}, s_c = nullptr;
     cudaEvent_t dma_ev[2] = {nullptr, nullptr};
     std::vector<cudaEvent_t> chunk_ev;
+    void* band_scratch[2] = {nullptr, nullptr}; size_t band_cap = 0;   // scratch of the narrow-band classifier, one per kernel stream
     static constexpr size_t kPiece = 4u << 20;          // doubles per staging buffer (32 MiB)
-    cudaError_t prepare(size_t n, size_t n_chunks)
+    cudaError_t prepare(size_t n, size_t n_chunks, size_t band_bytes = 0)
     {
         int dev = 0;
         cudaError_t e = cudaGetDevice(&dev);
@@ -502,6 +537,12 @@ struct HostPathPool {
             if (e != cudaSuccess) return e;
             d_cap = n;
         }
+        if (band_bytes > band_cap) {
+            for (int i = 0; i < 2; i++) { if (band_scratch[i]) cudaFree(band_scratch[i]); band_scratch[i] = nullptr; }
+            band_cap = 0;
+            for (int i = 0; i < 2; i++) { e = cudaMalloc(&band_scratch[i], band_bytes); if (e != cudaSuccess) return e; }
+            band_cap = band_bytes;
+        }
         while (chunk_ev.size() < n_chunks) {
             cudaEvent_t ev;
             e = cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
@@ -514,6 +555,8 @@ struct HostPathPool {
     {
         if (d_out) cudaFree(d_out);
         d_out = nullptr; d_cap = 0;
+        for (int i = 0; i < 2; i++) { if (band_scratch[i]) cudaFree(band_scratch[i]); band_scratch[i] = nullptr; }
+        band_cap = 0;
         for (int i = 0; i < 2; i++) { if (stage[i]) cudaFreeHost(stage[i]); stage[i] = nullptr; if (s_k[i]) cudaStreamDestroy(s_k[i]); s_k[i] = nullptr;
                                       if (dma_ev[i]) cudaEventDestroy(dma_ev[i]); dma_ev[i] = nullptr; }
         if (s_c) cudaStreamDestroy(s_c);
@@ -527,10 +570,12 @@ HostPathPool g_pool;
 
 // the pipeline of the host-buffer path; the caller holds g_pool.mu.  copier: the table workers of dg_add_function_sdf, which share the copies
 // from the pinned piece into the caller's memory with this thread (fresh pageable memory: page faults and remote NUMA nodes make a single
-// thread's copy the bottleneck on a loaded host); NULL: this thread copies alone
+// thread's copy the bottleneck on a loaded host); NULL: this thread copies alone.  band: NULL = the plain node loop (exactly the kernels it
+// always launched); else every chunk is the narrow-band form (classifier + band node loop, k1_launch_sample_nodes_band)
 namespace { struct HostTablesJob; }
 static void tables_job_copy(HostTablesJob* job, void* dst, const void* src, size_t bytes);
-static int sample_sdf_host_locked(const dg_mesh* m, const GridDev& g, double sign, uint64_t l_begin, uint64_t n, double* out_host, HostTablesJob* copier = nullptr)
+static int sample_sdf_host_locked(const dg_mesh* m, const GridDev& g, double sign, uint64_t l_begin, uint64_t n, double* out_host, HostTablesJob* copier = nullptr,
+                                  const double* band = nullptr)
 {
     // kernel chunks: a handful, each a multiple of the staging piece so that pieces never straddle chunks
     const uint64_t piece = HostPathPool::kPiece;
@@ -538,10 +583,17 @@ static int sample_sdf_host_locked(const dg_mesh* m, const GridDev& g, double sig
     const uint64_t pieces_per_chunk = n_pieces <= 4 ? 1 : (n_pieces + 7) / 8;
     const uint64_t chunk = pieces_per_chunk * piece;
     const uint64_t n_chunks = (n + chunk - 1) / chunk;
-    DG_CUDA(g_pool.prepare(n, n_chunks));
+    size_t band_bytes = 0;
+    if (band)
+        for (uint64_t c = 0; c < n_chunks; c++) {
+            const uint64_t b = c * chunk, cnt = (b + chunk <= n) ? chunk : n - b;
+            band_bytes = std::max(band_bytes, k1_band_scratch_bytes(g, l_begin + b, cnt));
+        }
+    DG_CUDA(g_pool.prepare(n, n_chunks, band_bytes));
     for (uint64_t c = 0; c < n_chunks; c++) {
         const uint64_t b = c * chunk, cnt = (b + chunk <= n) ? chunk : n - b;
-        DG_LAUNCH(k1_launch_sample_nodes(m->dev, g, sign, l_begin + b, cnt, g_pool.d_out + b, g_pool.s_k[c & 1]));
+        if (band) DG_LAUNCH(k1_launch_sample_nodes_band(m->dev, g, sign, *band, l_begin + b, cnt, g_pool.d_out + b, g_pool.band_scratch[c & 1], g_pool.s_k[c & 1]));
+        else DG_LAUNCH(k1_launch_sample_nodes(m->dev, g, sign, l_begin + b, cnt, g_pool.d_out + b, g_pool.s_k[c & 1]));
         DG_CUDA(cudaEventRecord(g_pool.chunk_ev[c], g_pool.s_k[c & 1]));
     }
     for (uint64_t i = 0; i <= n_pieces; i++) {
@@ -744,9 +796,10 @@ int dg_sample_sdf(const dg_mesh* m, const dg_grid_desc* grid, double sign, uint6
 // map (:888-891) straight into the caller's memory and pre-fault the coefficient array, so that the call ends one D2H piece after
 // the last kernel chunk.
 static int dg_add_function_sdf_impl(const dg_mesh* m, const dg_grid_desc* grid, double sign, double* nodes_host, uint32_t* cells_host, uint32_t* cell_map_host,
-                        double* timings_ms)
+                        double* timings_ms, const double* band = nullptr)
 {
     if (!m) return fail(DG_ERR_INVALID, "dg_add_function_sdf: mesh is NULL (not constructed)");
+    if (band) { if (int rc = check_band(*band, "dg_add_function_sdf_band")) return rc; }
     GridDev g;
     uint64_t n_nodes = 0;
     if (grid && dg_grid_num_nodes(grid->resolution, &n_nodes)) return DG_ERR_INVALID;
@@ -760,7 +813,7 @@ static int dg_add_function_sdf_impl(const dg_mesh* m, const dg_grid_desc* grid, 
     int rc;
     {
         std::lock_guard<std::mutex> lock(g_pool.mu);
-        rc = sample_sdf_host_locked(m, g, sign, 0, n_nodes, nodes_host, &job);
+        rc = sample_sdf_host_locked(m, g, sign, 0, n_nodes, nodes_host, &job, band);
     }
     const double ms_nodes = ms_since(t0);
     job.finish();
@@ -1572,6 +1625,14 @@ int dg_add_function_sdf(const dg_mesh* m, const dg_grid_desc* grid, double sign,
                         double* timings_ms)
 {
     return guarded("dg_add_function_sdf", [&]() { return dg_add_function_sdf_impl(m, grid, sign, nodes_host, cells_host, cell_map_host, timings_ms); });
+}
+
+// addFunction(func, verbose, pred) with pred(x) = |md.signed_distance(x).distance| <= band (cubic_lagrange_discrete_grid.cpp:780-899, node
+// loop :806-817): the same pipeline as dg_add_function_sdf, every kernel chunk in its narrow-band form
+int dg_add_function_sdf_band(const dg_mesh* m, const dg_grid_desc* grid, double sign, double band, double* nodes_host, uint32_t* cells_host,
+                             uint32_t* cell_map_host, double* timings_ms)
+{
+    return guarded("dg_add_function_sdf_band", [&]() { return dg_add_function_sdf_impl(m, grid, sign, nodes_host, cells_host, cell_map_host, timings_ms, &band); });
 }
 
 int dg_add_function_sdf_multi(dg_mesh_group* grp, const dg_grid_desc* grid, double sign, double* nodes_host, uint32_t* cells_host,

@@ -824,13 +824,12 @@ extern __shared__ __align__(16) unsigned char k1_smem[];
 // owns a 4 x 4 x 2 brick (fast x mid x slow) of one of them and a 128-thread block four bricks side by side along the
 // fast axis, so the 32 queries of a warp are spatial neighbours: they visit nearly the same tree nodes (L1 hits) and
 // take similar numbers of steps.  Whole slow-planes are covered; nodes outside [l_begin, l_end) are masked.
-__global__ void __launch_bounds__(K1_THREADS, K1_PACKET ? K1_PKT_MIN_BLOCKS : K1_MIN_BLOCKS)
-sdf_sample_nodes_kernel(MeshDev mesh, const PseudoNormals* __restrict__ normals, int stack_depth, GridDev g, K1Work w, double sign,
-                        double* __restrict__ out)
+// BAND = true is the narrow-band form (sdf_sample_nodes_band_kernel): same walk, same replay, same fallback; only the block id comes from the
+// classifier's list and the epilogue keeps the value where |distance| <= band and writes DBL_MAX elsewhere.
+template <bool BAND>
+__device__ __forceinline__ void sample_nodes_body(MeshDev mesh, const PseudoNormals* __restrict__ normals, int stack_depth, GridDev g,
+                                                  K1Work w, double sign, double* __restrict__ out, unsigned this_block, double band)
 {
-    // blocks run in launch order: neighbouring bricks running at the same time share tree nodes in L1, which orders that end a launch with
-    // short walks (plane groups from the outside in, heaviest distance class first) give up.
-    const unsigned this_block = blockIdx.x;
     DG_EMU_TRACE_BLOCK(this_block);
     float* stack_d = reinterpret_cast<float*>(k1_smem);
     unsigned* stack_rng = reinterpret_cast<unsigned*>(k1_smem + (size_t)stack_depth * K1_THREADS * sizeof(float));
@@ -888,7 +887,29 @@ sdf_sample_nodes_kernel(MeshDev mesh, const PseudoNormals* __restrict__ normals,
     double dist, qx, qy, qz; int tri;
     finish_query(mesh.leaves, normals, r, px, py, pz, true, dist, qx, qy, qz, tri);
     const unsigned out_idx = w.compact ? S.out_base + ((ts * SEG_BS(S) + lane_s) * S.Dm + m) * S.Df + f : l - w.l_begin;
-    out[out_idx] = (sign == 1.0) ? dist : sign * dist;           // cmd/generate_sdf/main.cpp:97 (-1.0 * d) / :101
+    if (BAND)   // addFunction's predicate (cubic_lagrange_discrete_grid.cpp:811-817): |md.signed_distance(x).distance| <= band, else DBL_MAX
+        out[out_idx] = (fabs(dist) <= band) ? ((sign == 1.0) ? dist : sign * dist) : DBL_MAX;
+    else
+        out[out_idx] = (sign == 1.0) ? dist : sign * dist;       // cmd/generate_sdf/main.cpp:97 (-1.0 * d) / :101
+}
+
+__global__ void __launch_bounds__(K1_THREADS, K1_PACKET ? K1_PKT_MIN_BLOCKS : K1_MIN_BLOCKS)
+sdf_sample_nodes_kernel(MeshDev mesh, const PseudoNormals* __restrict__ normals, int stack_depth, GridDev g, K1Work w, double sign,
+                        double* __restrict__ out)
+{
+    // blocks run in launch order: neighbouring bricks running at the same time share tree nodes in L1, which orders that end a launch with
+    // short walks (plane groups from the outside in, heaviest distance class first) give up.
+    sample_nodes_body<false>(mesh, normals, stack_depth, g, w, sign, out, blockIdx.x, 0.0);
+}
+
+// narrow band: block i of the launch is block list[i] of the node-loop geometry (the classifier's order-preserving list of the blocks that
+// may hold a node within the band); the launch is sized for every block and the blocks past *n_list return at once
+__global__ void __launch_bounds__(K1_THREADS, K1_PACKET ? K1_PKT_MIN_BLOCKS : K1_MIN_BLOCKS)
+sdf_sample_nodes_band_kernel(MeshDev mesh, const PseudoNormals* __restrict__ normals, int stack_depth, GridDev g, K1Work w, double sign,
+                             double band, const unsigned* __restrict__ list, const unsigned* __restrict__ n_list, double* __restrict__ out)
+{
+    if (blockIdx.x >= *n_list) return;
+    sample_nodes_body<true>(mesh, normals, stack_depth, g, w, sign, out, list[blockIdx.x], band);
 }
 
 #if K1_WAVE
@@ -944,8 +965,10 @@ __device__ __forceinline__ void dg_syncwarp() { __syncwarp(); }
 #endif
 
 __device__ __forceinline__ int wave_meta(int depth, int sp, int phase, int ent) { return depth | (sp << 8) | (phase << 16) | (ent << 20); }
+#endif  // K1_WAVE
 
-// grid node of lane `ln` of brick unit `unit` (= 2 * block + warp of the per-lane kernel's launch geometry): position, output index
+// grid node of lane `ln` of brick unit `unit` (= 2 * block + warp of the per-lane kernel's launch geometry): position, output index.
+// Used by the wavefront kernel and by the narrow-band classifier.
 __device__ __forceinline__ bool wave_brick_node(const GridDev& g, const K1Work& w, unsigned unit, unsigned ln, double& px, double& py, double& pz, unsigned& out_idx)
 {
     const unsigned this_block = unit / (unsigned)(K1_THREADS / 32), warp = unit % (unsigned)(K1_THREADS / 32);
@@ -986,6 +1009,7 @@ __device__ __forceinline__ bool wave_brick_node(const GridDev& g, const K1Work& 
     return alive;
 }
 
+#if K1_WAVE
 __global__ void __launch_bounds__(K1_THREADS, K1_WAVE_MIN_BLOCKS)
 sdf_sample_nodes_wave_kernel(MeshDev M, const PseudoNormals* __restrict__ normals, int stack_depth, GridDev g, K1Work w, unsigned n_units, double sign,
                              double* __restrict__ out, unsigned* __restrict__ unit_counter)
@@ -1226,6 +1250,149 @@ sdf_sample_nodes_wave_kernel(MeshDev M, const PseudoNormals* __restrict__ normal
 }
 #endif  // K1_WAVE
 
+// =====================================================================================================================================
+// NARROW-BAND CLASSIFIER.  addFunction(func, pred) with pred(x) = |md.signed_distance(x).distance| <= band (cubic_lagrange_discrete_grid.cpp:
+// 806-817) stores DBL_MAX wherever pred is false.  Before the node loop runs, every block of its launch geometry (K1_THREADS / 32 bricks of
+// 32 nodes) is classified: a block may be DROPPED only when every one of its nodes has a reference distance > band; its nodes then get
+// DBL_MAX here and it is never sampled.  The kept blocks form an order-preserving list (launch order matters, see the node-loop kernel) that
+// sdf_sample_nodes_band_kernel walks.  Dropping is certified; keeping is free to be conservative (it costs time, never bits).
+//   Bound.  Per brick: the fp64 box of its in-range node positions, taken relative to the mesh centre and rounded OUTWARD to fp32.  The tree's
+//   fp32 child boxes are rounded outward too (bvh_build.h), so the box-to-box gap, evaluated with round-down operations, is a lower bound L of
+//   the true distance from every node of the brick to every triangle of the subtree (up to the fp64 rounding of p - centre, < 2^-52 Mq).  A
+//   subtree is pruned when L > thr = band + 2E (E = filter_slack(Mq), Mq = max(half extent, |box|_inf)); the brick is kept as soon as a leaf
+//   survives.  If no leaf survives, every triangle T has true distance d_T > band + 2E to every node.  The reference's d2 for T is >= d_T^2 -
+//   240 eps64 R^2 with R <= 7 Mq (the box-skip budget above), i.e. its distance is >= d_T - 1.3e-12 Mq^2 / d_T > d_T - 1.4e-6 Mq since
+//   d_T > 2E >= 7.6e-6 Mq: so every distance the reference can compute, hence the one it returns, is > band and pred(x) is false.
+//   Range: E must be finite (2^-40 <= Mq < 1e18, filter_slack); otherwise the brick is kept.  A mesh with non-finite vertices has half
+//   extent +inf (bvh_build.cpp): every brick is kept.  NaN positions or band = +inf keep the brick too (no comparison can prune).
+// Passes (all warp-synchronous -- ballot / popc / redux -- so tests/emu runs them): classify (one thread per brick) -> count per chunk of
+// K1_BAND_CHUNK blocks -> compact (one warp per chunk; its offset = sum of the earlier chunks' counts) -> the band form of the node loop.
+// =====================================================================================================================================
+constexpr unsigned K1_BRICKS = K1_THREADS / 32;                  // bricks per block of the node-loop kernel
+static_assert(K1_BRICKS >= 1 && K1_BRICKS <= 32 && (K1_BRICKS & (K1_BRICKS - 1)) == 0, "a block's bricks must share a warp of the classifier");
+constexpr unsigned K1_BAND_CHUNK = 1024;                         // blocks per warp in the count / compaction passes
+constexpr unsigned K1_BAND_THREADS = 128;
+
+// squared gap between two fp32 boxes, rounded down
+__device__ __forceinline__ float box_gap2_rd(float alx, float aly, float alz, float ahx, float ahy, float ahz, const float* lo, const float* hi)
+{
+    const float gx = fmaxf(fmaxf(__fmaf_rd(alx, 1.f, -hi[0]), __fmaf_rd(lo[0], 1.f, -ahx)), 0.f);
+    const float gy = fmaxf(fmaxf(__fmaf_rd(aly, 1.f, -hi[1]), __fmaf_rd(lo[1], 1.f, -ahy)), 0.f);
+    const float gz = fmaxf(fmaxf(__fmaf_rd(alz, 1.f, -hi[2]), __fmaf_rd(lo[2], 1.f, -ahz)), 0.f);
+    return __fmaf_rd(gz, gz, __fmaf_rd(gy, gy, __fmul_rd(gx, gx)));
+}
+
+// may some triangle lie within sqrt(thr2) of the box [lo, hi] (fp32, relative to the mesh centre)?  Depth-first over the implicit tree; true
+// at the first leaf whose box is not certainly farther.  NaN gaps compare false: not pruned.
+__device__ bool band_box_near_mesh(const MeshDev M, const float* lo, const float* hi, float thr2)
+{
+    if (M.n_tri < 2) return true;
+    int stk_b[32], stk_e[32];                                    // one deferred sibling per level; node ids hold 25 bits (pack_range)
+    int b = 0, e = M.n_tri, sp = 0;
+    for (;;) {
+        const int m = (b + e) >> 1;
+        const float4* f4 = M.nodes_f + (size_t)m * K1_NODEF_STRIDE;
+        const float4 b0 = __ldg(f4 + 2), b1 = __ldg(f4 + 3), b2 = __ldg(f4 + 4);   // l_lo.xyz l_hi.x | l_hi.yz r_lo.xy | r_lo.z r_hi.xyz
+        const bool wl = !(box_gap2_rd(b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, lo, hi) > thr2);
+        const bool wr = !(box_gap2_rd(b1.z, b1.w, b2.x, b2.y, b2.z, b2.w, lo, hi) > thr2);
+        if ((wl && m - b == 1) || (wr && e - m == 1)) return true;
+        if (wl && wr) { stk_b[sp] = m; stk_e[sp] = e; sp++; e = m; }
+        else if (wl) e = m;
+        else if (wr) b = m;
+        else {
+            if (sp == 0) return false;
+            sp--; b = stk_b[sp]; e = stk_e[sp];
+        }
+    }
+}
+
+// one thread per brick (unit = K1_BRICKS * block + warp, as wave_brick_node numbers them); keep[block] = any of its bricks may be in the band;
+// the in-range nodes of a dropped block get DBL_MAX
+__global__ void __launch_bounds__(K1_BAND_THREADS)
+band_classify_kernel(MeshDev M, GridDev g, K1Work w, unsigned n_blocks, double band, double* __restrict__ out, unsigned char* __restrict__ keep)
+{
+    const unsigned FULL = 0xffffffffu;
+    const float INF = __int_as_float(0x7f800000);
+    const unsigned unit = blockIdx.x * K1_BAND_THREADS + threadIdx.x, lane = threadIdx.x & 31u;
+    const bool live = unit < n_blocks * K1_BRICKS;
+    double lo[3] = {DBL_MAX, DBL_MAX, DBL_MAX}, hi[3] = {-DBL_MAX, -DBL_MAX, -DBL_MAX};
+    bool any = false, finite = true;
+    if (live) {
+        for (unsigned ln = 0; ln < 32u; ln++) {
+            double p[3]; unsigned oi;
+            if (!wave_brick_node(g, w, unit, ln, p[0], p[1], p[2], oi)) continue;
+            any = true;
+            for (int k = 0; k < 3; k++) {
+                if (!(fabs(p[k]) <= DBL_MAX)) finite = false;
+                lo[k] = fmin(lo[k], p[k]); hi[k] = fmax(hi[k], p[k]);
+            }
+        }
+    }
+    bool near = false;
+    if (any) {
+        if (!finite) near = true;
+        else {
+            const double ctr[3] = {M.cx, M.cy, M.cz};
+            float flo[3], fhi[3];
+            float Mq = M.half_extent;
+            for (int k = 0; k < 3; k++) {
+                flo[k] = __double2float_rd(lo[k] - ctr[k]); fhi[k] = __double2float_ru(hi[k] - ctr[k]);
+                Mq = fmaxf(Mq, fmaxf(fabsf(flo[k]), fabsf(fhi[k])));
+            }
+            const float E = filter_slack(Mq);                       // +inf outside the budget's range (and for a non-finite mesh)
+            const float thr = __fadd_ru(__double2float_ru(band), __fadd_ru(E, E));
+            const float thr2 = __fmul_ru(thr, thr);
+            near = !(thr2 < INF) || band_box_near_mesh(M, flo, fhi, thr2);
+        }
+    }
+    // the K1_BRICKS bricks of a block are adjacent lanes of one warp
+    const unsigned votes = __ballot_sync(FULL, near);
+    const unsigned group = (K1_BRICKS == 32u ? FULL : ((1u << K1_BRICKS) - 1u)) << (lane & ~(K1_BRICKS - 1u));
+    const bool block_kept = (votes & group) != 0u;
+    if (live && (lane & (K1_BRICKS - 1u)) == 0u) keep[unit / K1_BRICKS] = block_kept ? 1 : 0;
+    if (any && !block_kept) {
+        for (unsigned ln = 0; ln < 32u; ln++) {
+            double px, py, pz; unsigned oi;
+            if (wave_brick_node(g, w, unit, ln, px, py, pz, oi)) out[oi] = DBL_MAX;
+        }
+    }
+}
+
+// kept blocks per chunk of K1_BAND_CHUNK blocks (one warp per chunk)
+__global__ void __launch_bounds__(K1_BAND_THREADS) band_count_kernel(const unsigned char* __restrict__ keep, unsigned n_blocks, unsigned* __restrict__ chunk_count)
+{
+    const unsigned chunk = (blockIdx.x * K1_BAND_THREADS + threadIdx.x) >> 5, lane = threadIdx.x & 31u;
+    const unsigned long long base = (unsigned long long)chunk * K1_BAND_CHUNK;
+    if (base >= n_blocks) return;                                // whole warps
+    unsigned cnt = 0;
+    for (unsigned k = 0; k < K1_BAND_CHUNK; k += 32) {
+        const unsigned long long i = base + k + lane;
+        cnt += (unsigned)__popc(__ballot_sync(0xffffffffu, i < n_blocks && keep[i] != 0));
+    }
+    if (lane == 0) chunk_count[chunk] = cnt;
+}
+
+// list of the kept blocks in launch order (one warp per chunk); the warp of the last chunk writes the list length
+__global__ void __launch_bounds__(K1_BAND_THREADS) band_compact_kernel(const unsigned char* __restrict__ keep, unsigned n_blocks,
+                                                                       const unsigned* __restrict__ chunk_count, unsigned* __restrict__ list,
+                                                                       unsigned* __restrict__ n_list)
+{
+    const unsigned chunk = (blockIdx.x * K1_BAND_THREADS + threadIdx.x) >> 5, lane = threadIdx.x & 31u;
+    const unsigned long long base = (unsigned long long)chunk * K1_BAND_CHUNK;
+    if (base >= n_blocks) return;
+    unsigned run = 0;
+    for (unsigned c = 0; c < chunk; c += 32) run += __reduce_add_sync(0xffffffffu, (c + lane < chunk) ? chunk_count[c + lane] : 0u);
+    const unsigned lt = (1u << lane) - 1u;
+    for (unsigned k = 0; k < K1_BAND_CHUNK; k += 32) {
+        const unsigned long long i = base + k + lane;
+        const bool kept = i < n_blocks && keep[i] != 0;
+        const unsigned msk = __ballot_sync(0xffffffffu, kept);
+        if (kept) list[run + (unsigned)__popc(msk & lt)] = (unsigned)i;
+        run += (unsigned)__popc(msk);
+    }
+    if (lane == 0 && base + K1_BAND_CHUNK >= n_blocks) *n_list = run;
+}
+
 // batched TriangleMeshDistance::{signed,unsigned}_distance on arbitrary points (a warp = 32 consecutive points)
 __global__ void __launch_bounds__(K1_THREADS, K1_MIN_BLOCKS)
 mesh_distance_kernel(MeshDev mesh, const PseudoNormals* __restrict__ normals, int stack_depth,
@@ -1321,6 +1488,8 @@ cudaError_t k1_configure(int stack_depth)
     const size_t bytes = k1_smem_bytes(stack_depth);
     e = cudaFuncSetAttribute(sdf_sample_nodes_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
     if (e != cudaSuccess) return e;
+    e = cudaFuncSetAttribute(sdf_sample_nodes_band_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    if (e != cudaSuccess) return e;
     e = cudaFuncSetAttribute(mesh_distance_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
     if (e == cudaSuccess && dev >= 0 && dev < 64) configured[dev] = stack_depth;
     return e;
@@ -1408,17 +1577,14 @@ static void choose_brick(const GridDev& g, int kind, unsigned& lf, unsigned& lm)
 #endif
 
 // Splits [l_begin, l_begin+count) into the (at most four) node arrays it touches and tiles whole slow-planes of each.
-cudaError_t k1_launch_sample_nodes(const DeviceBvh& m, const GridDev& g, double sign, uint64_t l_begin, uint64_t count,
-                                   double* d_out, cudaStream_t stream)
+static unsigned node_range_work(const GridDev& g, uint64_t l_begin, uint64_t count, K1Work& w)
 {
-    if (count == 0) return cudaSuccess;
     const uint64_t l_end = l_begin + count;
     const unsigned nx = g.n[0], ny = g.n[1], nz = g.n[2];
     // {base, Ds, Dm, Df} of the four row-major node arrays (cubic_lagrange_discrete_grid.cpp:618-662)
     const uint64_t base[5] = {0, g.nv, (uint64_t)g.nv + 2ull * g.ne_x, (uint64_t)g.nv + 2ull * (g.ne_x + (uint64_t)g.ne_y),
                               (uint64_t)g.nv + 2ull * ((uint64_t)g.ne_x + g.ne_y + g.ne_z)};
     const unsigned dims[4][3] = {{nz + 1, ny + 1, nx + 1}, {nz + 1, ny + 1, 2 * nx}, {nx + 1, nz + 1, 2 * ny}, {ny + 1, nx + 1, 2 * nz}};
-    K1Work w;
     w.nseg = 0; w.l_begin = (unsigned)l_begin; w.l_end = (unsigned)l_end; w.compact = 0;
     unsigned blocks = 0;
     for (int k = 0; k < 4; k++) {
@@ -1440,7 +1606,59 @@ cudaError_t k1_launch_sample_nodes(const DeviceBvh& m, const GridDev& g, double 
         blocks += S.tiles_f * S.tiles_m * tiles_s;
     }
     for (int k = w.nseg; k < 4; k++) { w.seg[k] = w.seg[0]; w.seg[k].block_begin = 0xffffffffu; }
+    return blocks;
+}
+
+cudaError_t k1_launch_sample_nodes(const DeviceBvh& m, const GridDev& g, double sign, uint64_t l_begin, uint64_t count,
+                                   double* d_out, cudaStream_t stream)
+{
+    if (count == 0) return cudaSuccess;
+    K1Work w;
+    const unsigned blocks = node_range_work(g, l_begin, count, w);
     DG_LAUNCH_SAMPLING(m, g, w, blocks, sign, d_out, stream);
+}
+
+// scratch of the band form: keep flag per block (bytes), count per chunk, the list, its length
+static void band_scratch_layout(unsigned blocks, size_t off[4], size_t& total)
+{
+    const unsigned chunks = (blocks + K1_BAND_CHUNK - 1) / K1_BAND_CHUNK;
+    off[0] = 0;
+    off[1] = ((size_t)blocks + 255) / 256 * 256;
+    off[2] = off[1] + ((size_t)chunks * sizeof(unsigned) + 255) / 256 * 256;
+    off[3] = off[2] + ((size_t)blocks * sizeof(unsigned) + 255) / 256 * 256;
+    total = off[3] + 256;
+}
+
+size_t k1_band_scratch_bytes(const GridDev& g, uint64_t l_begin, uint64_t count)
+{
+    if (count == 0) return 0;
+    K1Work w;
+    size_t off[4], total;
+    band_scratch_layout(node_range_work(g, l_begin, count, w), off, total);
+    return total;
+}
+
+cudaError_t k1_launch_sample_nodes_band(const DeviceBvh& m, const GridDev& g, double sign, double band, uint64_t l_begin, uint64_t count,
+                                        double* d_out, void* d_scratch, cudaStream_t stream)
+{
+    if (count == 0) return cudaSuccess;
+    K1Work w;
+    const unsigned blocks = node_range_work(g, l_begin, count, w);
+    size_t off[4], total;
+    band_scratch_layout(blocks, off, total);
+    unsigned char* keep = static_cast<unsigned char*>(d_scratch) + off[0];
+    unsigned* chunk_count = reinterpret_cast<unsigned*>(static_cast<unsigned char*>(d_scratch) + off[1]);
+    unsigned* list = reinterpret_cast<unsigned*>(static_cast<unsigned char*>(d_scratch) + off[2]);
+    unsigned* n_list = reinterpret_cast<unsigned*>(static_cast<unsigned char*>(d_scratch) + off[3]);
+    const unsigned long long units = (unsigned long long)blocks * K1_BRICKS, chunks = (blocks + K1_BAND_CHUNK - 1) / K1_BAND_CHUNK;
+    DG_KERNEL_LAUNCH(band_classify_kernel, (unsigned)((units + K1_BAND_THREADS - 1) / K1_BAND_THREADS), K1_BAND_THREADS, 0, stream,
+                     mesh_dev(m), g, w, blocks, band, d_out, keep);
+    const unsigned warps_blocks = (unsigned)((chunks * 32ull + K1_BAND_THREADS - 1) / K1_BAND_THREADS);
+    DG_KERNEL_LAUNCH(band_count_kernel, warps_blocks, K1_BAND_THREADS, 0, stream, keep, blocks, chunk_count);
+    DG_KERNEL_LAUNCH(band_compact_kernel, warps_blocks, K1_BAND_THREADS, 0, stream, keep, blocks, chunk_count, list, n_list);
+    DG_KERNEL_LAUNCH(sdf_sample_nodes_band_kernel, blocks, K1_THREADS, k1_smem_bytes(m.stack_depth), stream, mesh_dev(m), m.normals, m.stack_depth,
+                     g, w, sign, band, list, n_list, d_out);
+    return DG_AFTER_LAUNCH();
 }
 
 cudaError_t k1_launch_sample_slab(const DeviceBvh& m, const GridDev& g, double sign, const unsigned plane_begin[4], const unsigned plane_end[4],

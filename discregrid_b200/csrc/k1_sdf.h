@@ -155,6 +155,13 @@ struct DeviceBvh {                 // device mirrors of HostBvh, uploaded once b
 cudaError_t k1_configure(int stack_depth);
 cudaError_t k1_launch_sample_nodes(const DeviceBvh& m, const GridDev& g, double sign, uint64_t l_begin, uint64_t count,
                                    double* d_out, cudaStream_t stream);
+// narrow-band form of k1_launch_sample_nodes (addFunction with pred(x) = |distance| <= band): the node-range [l_begin, l_begin + count) is
+// written exactly as by k1_launch_sample_nodes where |distance| <= band and DBL_MAX elsewhere; nodes outside the range are never written.
+// A classifier drops the blocks that provably hold no node within the band before the node loop runs (k1_sdf.cu, NARROW-BAND CLASSIFIER).
+// d_scratch: k1_band_scratch_bytes(g, l_begin, count) bytes of device memory, used in stream order (one buffer per concurrent stream).
+size_t k1_band_scratch_bytes(const GridDev& g, uint64_t l_begin, uint64_t count);
+cudaError_t k1_launch_sample_nodes_band(const DeviceBvh& m, const GridDev& g, double sign, double band, uint64_t l_begin, uint64_t count,
+                                        double* d_out, void* d_scratch, cudaStream_t stream);
 // slab form: planes [plane_begin[a], plane_end[a]) of node array a (a = 0..3), written at d_full[l]
 cudaError_t k1_launch_sample_slab(const DeviceBvh& m, const GridDev& g, double sign, const unsigned plane_begin[4], const unsigned plane_end[4],
                                   double* d_full, cudaStream_t stream);

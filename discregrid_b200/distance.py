@@ -119,3 +119,19 @@ class MeshSignedDistance:
     def __call__(self, points):
         d = self.md.signed_distance(points).distance
         return d if self.sign == 1.0 else self.sign * d
+
+
+class MeshDistanceBand:
+    """The narrow-band sample predicate x -> |md.signed_distance(x).distance| <= band (fp64, the reference's own distance): what a
+    reference user passes as addFunction's `pred` to keep a signed distance field only near the surface.  Callable on points like the
+    reference's predicate (returns bool per point).  CubicLagrangeDiscreteGrid.addFunction(MeshSignedDistance(md), pred=MeshDistanceBand(md, w))
+    recognises it and samples the band on the GPU: nodes outside hold DBL_MAX, blocks of nodes provably outside are never queried."""
+
+    def __init__(self, md, band):
+        band = float(band)
+        if not band >= 0.0:
+            raise ValueError(f"band must be >= 0 (got {band})")
+        self.md, self.band = md, band
+
+    def __call__(self, points):
+        return np.abs(self.md.signed_distance(points).distance) <= self.band

@@ -5,7 +5,9 @@ m_nodes, m_cells, m_cell_map -- discrete_grid.hpp:93-98, cubic_lagrange_discrete
 that save()/load() stay byte-compatible with the reference's .cdf/.cdm files
 (cubic_lagrange_discrete_grid.cpp:678-778), and routes the hot path to the GPU:
 
-  addFunction(MeshSignedDistance)        -> dg_sample_sdf        (K1, csrc/k1_sdf.cu)
+  addFunction(MeshSignedDistance)        -> dg_add_function_sdf  (K1, csrc/k1_sdf.cu)
+  addFunction(MeshSignedDistance, pred=MeshDistanceBand)
+                                         -> dg_add_function_sdf_band (K1 narrow band: DBL_MAX outside |distance| <= band)
   addFunction(DensityMapFunction, pred)  -> dg_density_map       (K3, csrc/k3_density.cu)
   interpolate(field_id, x[, gradient])   -> dg_interpolate_batch (K2, csrc/k2_interp.cu), batched over x
 
@@ -19,7 +21,7 @@ import struct
 import numpy as np
 
 from . import _capi as capi
-from .distance import MeshSignedDistance
+from .distance import MeshDistanceBand, MeshSignedDistance
 
 
 class DensityMapFunction:
@@ -123,15 +125,20 @@ class CubicLagrangeDiscreteGrid:
     # ------------------------------------------------------------------ addFunction (cubic_lagrange_discrete_grid.cpp:780-899)
     def addFunction(self, func, verbose=False, pred=None):
         if isinstance(func, MeshSignedDistance):
-            if pred is not None:
-                raise TypeError("a sample predicate is only supported with DensityMapFunction")
+            if pred is not None and not isinstance(pred, MeshDistanceBand):
+                raise TypeError("a sample predicate is only supported with DensityMapFunction, or as MeshDistanceBand with MeshSignedDistance")
+            if pred is not None and pred.md is not func.md:
+                raise TypeError("MeshDistanceBand must use the same TriangleMeshDistance as the MeshSignedDistance it restricts")
             # the whole addFunction in one call: node loop on the GPU, connectivity + cell map written by the library's host threads meanwhile
             coeffs = np.empty(self.nNodes())
             cells = np.empty((self.m_n_cells, 32), np.uint32)
             cmap = np.empty(self.m_n_cells, np.uint32)
             self.last_add_function_ms = np.zeros(6)
-            capi.check(capi.lib.dg_add_function_sdf(func.md.handle, C.byref(self._desc), func.sign, capi.ptr(coeffs, capi.F64P),
-                                                    capi.ptr(cells, capi.U32P), capi.ptr(cmap, capi.U32P), capi.ptr(self.last_add_function_ms, capi.F64P)))
+            out = (capi.ptr(coeffs, capi.F64P), capi.ptr(cells, capi.U32P), capi.ptr(cmap, capi.U32P), capi.ptr(self.last_add_function_ms, capi.F64P))
+            if pred is None:
+                capi.check(capi.lib.dg_add_function_sdf(func.md.handle, C.byref(self._desc), func.sign, *out))
+            else:
+                capi.check(capi.lib.dg_add_function_sdf_band(func.md.handle, C.byref(self._desc), func.sign, pred.band, *out))
             self.m_nodes.append(coeffs); self.m_cells.append(cells); self.m_cell_map.append(cmap)
             self.m_n_fields += 1
             return self.m_n_fields - 1

@@ -153,6 +153,21 @@ DG_API int dg_sample_sdf_device(const dg_mesh* mesh, const dg_grid_desc* grid, d
  * This is what the C++ facade's addFunction(MeshSignedDistanceFunction) calls and what bench.py times as `e2e`. */
 DG_API int dg_add_function_sdf(const dg_mesh* mesh, const dg_grid_desc* grid, double sign, double* nodes_host, uint32_t* cells_host,
                         uint32_t* cell_map_host, double* timings_ms);
+/* ---- K1, narrow band: addFunction(func, verbose, pred) with the band predicate ----------------------------------------------------
+ * replaces the node loop cubic_lagrange_discrete_grid.cpp:806-817 with func as above and
+ *     pred(x) = std::abs(md.signed_distance(x).distance) <= band      (fp64, the reference's own distance)
+ * i.e. out = sign * distance where pred holds and DBL_MAX (:817) elsewhere -- the pattern GenerateDensityMap uses
+ * (cmd/generate_density_map/main.cpp:119-147) and what reduceField (:1065-1174) then sparsifies.  In-band nodes hold exactly the bits
+ * dg_sample_sdf writes.  A classifier first drops the blocks of nodes that provably lie farther than `band` from every triangle (their
+ * nodes get DBL_MAX without a tree query); only the rest is sampled.  band must be >= 0 (negative or NaN: DG_ERR_INVALID); +inf keeps
+ * every node.
+ *   dg_sample_sdf_band_device: nodes [l_begin, l_end) into d_out, asynchronous on `stream` like dg_sample_sdf_device (its scratch is
+ *       allocated and freed in stream order); nodes outside the range are never written.
+ *   dg_add_function_sdf_band: the whole addFunction into host arrays, as dg_add_function_sdf (same pipeline, same timings_ms). */
+DG_API int dg_sample_sdf_band_device(const dg_mesh* mesh, const dg_grid_desc* grid, double sign, double band, uint64_t l_begin, uint64_t l_end,
+                              double* d_out, void* stream);
+DG_API int dg_add_function_sdf_band(const dg_mesh* mesh, const dg_grid_desc* grid, double sign, double band, double* nodes_host,
+                             uint32_t* cells_host, uint32_t* cell_map_host, double* timings_ms);
 /* ---- multi-GPU from ONE process (SURVEY 8b: `dg_sample_sdf(..., n_gpus, ...)`; 8e) -------------------------------------------
  * A dg_mesh_group replicates the device records of `mesh` on n_gpus - 1 further GPUs (peer copies from the mesh's device; the host
  * build is not repeated).  devices: NULL = the mesh's device first, then the lowest other ids; else n_gpus ids with devices[0] == the

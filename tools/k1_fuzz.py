@@ -4,7 +4,7 @@ not compiled, the oracle port pinned to it) on meshes built to provoke exact tie
 triangles, cubes / octahedra with queries on symmetry planes, duplicated triangles, slivers, lattice-aligned queries, random soups at scales
 1e-24 .. 1e17 -- signed and unsigned, distance bits, nearest point, entity and triangle id.
 
-usage: tools/k1_fuzz.py [rounds=200] [seed=0] [lib=build/bin/libk1emu.so] [points|grid|scales]
+usage: tools/k1_fuzz.py [rounds=200] [seed=0] [lib=build/bin/libk1emu.so] [points|grid|scales] [band]
   lib    a build of tests/emu/k1_emu.cpp (the K1 translation unit compiled for the CPU), or `dg`: the product library through its C-ABI
          (dg_mesh_create, dg_mesh_distance, dg_node_positions, dg_sample_sdf), i.e. the CUDA kernels -- needs a GPU
   points mesh_distance on arbitrary points (the per-lane walk)
@@ -13,6 +13,9 @@ usage: tools/k1_fuzz.py [rounds=200] [seed=0] [lib=build/bin/libk1emu.so] [point
          reference evaluated at the node positions
   scales the scale sweep (`rounds` is ignored): soups, strips and coplanar grids at scales 10^k, k = -24 .. 17, with and without an offset
          large against the mesh, and meshes whose half extent lies just below / just above the 1e18 limit of the fp32 filters; both forms
+  band   grid / scales only: the node loop in its narrow-band form (addFunction with pred(x) = |distance| <= band; classifier + band kernel,
+         k1_launch_sample_nodes_band) with band = `band` times the largest cell size; compared with the reference's distance where it is
+         <= band and DBL_MAX elsewhere.  Needs a build of tests/emu/k1_band_emu.cpp or `dg`
 The functions are shared with tests/test_k1_emulated.py and tests/test_gpu_k1_scales.py."""
 import ctypes as C
 import os
@@ -48,6 +51,8 @@ class EmuK1:
         lib.emu_mesh_distance.argtypes = [C.c_void_p, dp, C.c_uint64, C.c_int, dp, dp, i32p, i32p]
         lib.emu_sample_sdf.argtypes = [C.c_void_p, dp, u32p, C.c_double, C.c_uint64, C.c_uint64, dp]
         lib.emu_node_positions.argtypes = [dp, u32p, C.c_uint64, C.c_uint64, dp]
+        if hasattr(lib, "emu_sample_sdf_band"):
+            lib.emu_sample_sdf_band.argtypes = [C.c_void_p, dp, u32p, C.c_double, C.c_double, C.c_uint64, C.c_uint64, dp]
 
     def mesh(self, V, F):
         h = self.lib.emu_mesh_create(_p(V, dp), len(V), _p(F, u32p), len(F))
@@ -72,11 +77,17 @@ class EmuK1:
         assert self.lib.emu_node_positions(_p(gd, dp), _p(r, u32p), 0, n, _p(xs, dp)) == 0
         return xs
 
-    def sample(self, h, g, sign, n):
+    def sample(self, h, g, sign, n, band=None):
         gd, r = g
         out = np.full(n, np.nan)
-        assert self.lib.emu_sample_sdf(h, _p(gd, dp), _p(r, u32p), sign, 0, n, _p(out, dp)) == 0
+        if band is None:
+            assert self.lib.emu_sample_sdf(h, _p(gd, dp), _p(r, u32p), sign, 0, n, _p(out, dp)) == 0
+        else:
+            assert self.lib.emu_sample_sdf_band(h, _p(gd, dp), _p(r, u32p), sign, band, 0, n, _p(out, dp)) == 0
         return out
+
+    def cell_size(self, g):
+        return g[0][6:9]
 
 
 class DgK1:
@@ -113,10 +124,16 @@ class DgK1:
         self.capi.check(self.lib.dg_node_positions(C.byref(g), 0, n, _p(xs, dp)))
         return xs
 
-    def sample(self, h, g, sign, n):
+    def sample(self, h, g, sign, n, band=None):
         out = np.full(n, np.nan)
-        self.capi.check(self.lib.dg_sample_sdf(h, C.byref(g), sign, 0, n, _p(out, dp)))
+        if band is None:
+            self.capi.check(self.lib.dg_sample_sdf(h, C.byref(g), sign, 0, n, _p(out, dp)))
+        else:
+            self.capi.check(self.lib.dg_add_function_sdf_band(h, C.byref(g), sign, band, _p(out, dp), None, None, None))
         return out
+
+    def cell_size(self, g):
+        return np.array(g.cell_size[:])
 
 
 def backend(lib):
@@ -146,14 +163,21 @@ def check_points(be, h, ref, x, label=""):
     return 2 * len(x), bad, first
 
 
-def check_grid(be, h, ref, mn, mx, res, sign, label=""):
-    """the node loop over the lattice (mn, mx, res) == sign * the reference's signed distance at the node positions, bit for bit"""
+def band_expect(wd, sign, band):
+    """addFunction(func, pred) with pred(x) = |d| <= band: sign * d where it holds, DBL_MAX elsewhere (NaN fails the predicate)"""
+    return np.where(np.abs(wd) <= band, wd if sign == 1.0 else sign * wd, np.finfo(np.float64).max)
+
+
+def check_grid(be, h, ref, mn, mx, res, sign, label="", band_cells=None):
+    """the node loop over the lattice (mn, mx, res) == sign * the reference's signed distance at the node positions, bit for bit; with
+    band_cells, the narrow-band form with band = band_cells * the largest cell size"""
     g = be.grid(mn, mx, res)
     nn = num_nodes(res)
     xs = be.node_positions(g, nn)
     wd = ref.distance(xs, signed=True)[0]
-    want = wd if sign == 1.0 else sign * wd
-    got = be.sample(h, g, sign, nn)
+    band = None if band_cells is None else band_cells * float(np.max(be.cell_size(g)))
+    want = (wd if sign == 1.0 else sign * wd) if band is None else band_expect(wd, sign, band)
+    got = be.sample(h, g, sign, nn, band) if band is not None else be.sample(h, g, sign, nn)
     ok = _same(got, want)
     if ok.all():
         return nn, 0, None
@@ -256,8 +280,8 @@ def scale_cases(seed=0, exponents=SCALE_EXPONENTS):
         yield f"soup@half_extent{h:.4g}", np.ascontiguousarray(V), np.arange(3 * n, dtype=np.uint32).reshape(n, 3)
 
 
-def run_scales(be, seed=0, modes=("points", "grid"), exponents=SCALE_EXPONENTS, log=print):
-    """the scale sweep through backend `be` -> (meshes, queries + nodes checked, mismatches)"""
+def run_scales(be, seed=0, modes=("points", "grid"), exponents=SCALE_EXPONENTS, log=print, band_cells=None):
+    """the scale sweep through backend `be` -> (meshes, queries + nodes checked, mismatches); band_cells: the grid form in its narrow-band form"""
     rng = np.random.default_rng(seed + 1)
     meshes = total = bad = 0
     for i, (label, V, F) in enumerate(scale_cases(seed, exponents)):
@@ -271,7 +295,7 @@ def run_scales(be, seed=0, modes=("points", "grid"), exponents=SCALE_EXPONENTS, 
         if "grid" in modes:
             lo, hi = V.min(0), V.max(0)
             ext = np.maximum(hi - lo, 0.25 * (hi - lo).max())
-            n, b, msg = check_grid(be, h, ref, lo - 0.3 * ext, hi + 0.3 * ext, (9, 7, 6), -1.0 if i % 2 else 1.0, label)
+            n, b, msg = check_grid(be, h, ref, lo - 0.3 * ext, hi + 0.3 * ext, (9, 7, 6), -1.0 if i % 2 else 1.0, label, band_cells)
             total += n; bad += b
             if msg: log(msg)
         be.destroy(h)
@@ -312,9 +336,10 @@ def main(argv):
     seed = int(argv[2]) if len(argv) > 2 else 0
     lib = argv[3] if len(argv) > 3 else os.path.join(ROOT, "build", "bin", "libk1emu.so")
     mode = argv[4] if len(argv) > 4 else "points"
+    band_cells = float(argv[5]) if len(argv) > 5 else None
     be = backend(lib)
     if mode == "scales":
-        meshes, total, bad = run_scales(be, seed)
+        meshes, total, bad = run_scales(be, seed, band_cells=band_cells)
         print(f"{meshes} meshes, {total} queries, {bad} mismatches")
         return 1 if bad else 0
     rng = np.random.default_rng(seed)
@@ -329,7 +354,7 @@ def main(argv):
         label = f"case {k} (kind {k % 7}, {len(F)} tris)"
         if mode == "grid":
             mn, mx, res = case_lattice(k, V)
-            n, b, msg = check_grid(be, h, ref, mn, mx, res, 1.0 if k % 2 else -1.0, label)
+            n, b, msg = check_grid(be, h, ref, mn, mx, res, 1.0 if k % 2 else -1.0, label, band_cells)
         else:
             n, b, msg = check_points(be, h, ref, x, label)
         total += n; bad += b
