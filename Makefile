@@ -24,7 +24,7 @@ CPPBIN   := build/bin
 CPPFLAGS := -std=c++11 -O2 -ffp-contract=off -I$(EIGEN3_INCLUDE_DIR) -Icpp/include -Iinclude
 CPPLINK  := -Ldiscregrid_b200/lib -ldiscregrid_b200 -Wl,-rpath,'$$ORIGIN/../../discregrid_b200/lib'
 CPPHDRS  := $(wildcard cpp/include/Discregrid/* cpp/include/Discregrid/*/*) include/discregrid_b200.h
-cpp: $(CPPBIN)/GenerateSDF $(CPPBIN)/GenerateDensityMap $(CPPBIN)/DiscreteFieldToBitmap $(CPPBIN)/facade_check $(CPPBIN)/bvh_host_check $(CPPBIN)/reduce_facade_check $(CPPBIN)/sort_replay_check $(CPPBIN)/fast_div_check $(CPPBIN)/libk1emu.so $(CPPBIN)/libk1emu_knobs.so $(CPPBIN)/libk1emu_wave.so $(CPPBIN)/libk1emu_perlane.so $(CPPBIN)/libk1emu_packet.so $(CPPBIN)/libk1emu_band.so $(CPPBIN)/libk1emu_band_perlane.so $(CPPBIN)/libk23emu.so $(CPPBIN)/libk23emu_knobs.so $(CPPBIN)/libdgemu.so
+cpp: $(CPPBIN)/GenerateSDF $(CPPBIN)/GenerateDensityMap $(CPPBIN)/DiscreteFieldToBitmap $(CPPBIN)/facade_check $(CPPBIN)/bvh_host_check $(CPPBIN)/reduce_facade_check $(CPPBIN)/sort_replay_check $(CPPBIN)/fast_div_check $(CPPBIN)/libk1emu.so $(CPPBIN)/libk1emu_knobs.so $(CPPBIN)/libk1emu_wave.so $(CPPBIN)/libk1emu_perlane.so $(CPPBIN)/libk1emu_packet.so $(CPPBIN)/libk1emu_band.so $(CPPBIN)/libk1emu_band_perlane.so $(CPPBIN)/libk23emu.so $(CPPBIN)/libk23emu_knobs.so $(CPPBIN)/libdgemu.so $(CPPBIN)/libk4emu.so
 $(CPPBIN)/DiscreteFieldToBitmap: cpp/cmd/discrete_field_to_bitmap.cpp $(CPPHDRS) $(LIB)
 	@mkdir -p $(CPPBIN)
 	$(HOSTCXX) $(CPPFLAGS) $< -o $@ $(CPPLINK)
@@ -75,6 +75,11 @@ DGEMU_SRC := tests/emu/dgapi_emu.cpp tests/emu/k1_emu.cpp tests/emu/k2_emu.cpp t
 $(CPPBIN)/libdgemu.so: $(DGEMU_SRC) tests/emu/cuda_emu.h $(wildcard $(SRC)/*.cu) $(HDRS)
 	@mkdir -p $(CPPBIN)
 	$(HOSTCXX) -std=c++17 -O2 -ffp-contract=off -fPIC -shared -Wl,-Bsymbolic -Wno-subobject-linkage -I$(CUDA_INC) -Itests/emu -I$(SRC) -Iinclude $(DGEMU_SRC) -o $@ -lpthread
+# test library: the device swap walk of k4_reduce.cu (emulated) next to the serial host walk of reduce_field.cpp it replaces
+K4EMU_SRC := tests/emu/k4_walk_emu.cpp tests/emu/cudart_stub.cpp $(SRC)/reduce_field.cpp $(SRC)/host_threads.cpp $(SRC)/sort_replay.cpp
+$(CPPBIN)/libk4emu.so: $(K4EMU_SRC) tests/emu/cuda_emu.h $(SRC)/k4_reduce.cu $(HDRS)
+	@mkdir -p $(CPPBIN)
+	$(HOSTCXX) -std=c++17 -O2 -ffp-contract=off -fPIC -shared -Wl,-Bsymbolic -I$(CUDA_INC) -Itests/emu -I$(SRC) $(K4EMU_SRC) -o $@ -lpthread
 # test binary: the reciprocal-based exact division of fast_div.h against '/' (brute force)
 $(CPPBIN)/fast_div_check: tests/cpp/fast_div_check.cpp $(SRC)/fast_div.h $(SRC)/dg_device.cuh
 	@mkdir -p $(CPPBIN)

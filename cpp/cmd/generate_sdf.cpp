@@ -3,7 +3,8 @@
 // --gpus N (new, SURVEY 5 "same flags + --gpus N"): the node loop is dealt to N GPUs of this node (dg_add_function_sdf_multi); same file.
 // --band W (new): a narrow-band field -- addFunction(func, verbose, pred) with pred(x) = |distance(x)| <= W (world units), DBL_MAX
 //   elsewhere, then reduceField with an always-true predicate (drops the DBL_MAX nodes and the cells without a kept node), as
-//   GenerateDensityMap does (cmd/generate_density_map/main.cpp:119-147).  --no-reduction keeps the dense field.  One GPU only.
+//   GenerateDensityMap does (cmd/generate_density_map/main.cpp:119-147) -- both in one call (addReducedBandField), so that only the reduced
+//   field reaches the host.  --no-reduction keeps the dense field (addFunction with the band predicate).  One GPU only.
 // The one functional change against the reference source: the functor handed to addFunction is the recognisable
 // MeshSignedDistanceFunction instead of an anonymous lambda (main.cpp:94-102).
 #include <Discregrid/All>
@@ -67,13 +68,12 @@ int main(int argc, char* argv[])
         Discregrid::CubicLagrangeDiscreteGrid sdf(domain, resolution);
         Discregrid::DiscreteGrid::ContinuousFunction func = Discregrid::MeshSignedDistanceFunction(md, invert);
         std::cout << "Generate discretization..." << std::endl;
-        if (use_band) {
-            sdf.addFunction(func, true, Discregrid::MeshDistanceBandPredicate(md, band));
-            if (!no_reduction) {
-                std::cout << "Reduce discretization...";
-                sdf.reduceField(0, [](Vector3d const&, double) { return true; });
-                std::cout << "DONE" << std::endl;
-            }
+        if (use_band && no_reduction) sdf.addFunction(func, true, Discregrid::MeshDistanceBandPredicate(md, band));
+        else if (use_band) {
+            // addFunction(func, pred) + reduceField(always true) in one call: only the reduced field reaches the host
+            std::cout << "Reduce discretization...";
+            sdf.addReducedBandField(Discregrid::MeshSignedDistanceFunction(md, invert), Discregrid::MeshDistanceBandPredicate(md, band), true);
+            std::cout << "DONE" << std::endl;
         } else sdf.addFunction(func, true);
         std::cout << "DONE" << std::endl;
         std::cout << "Serialize discretization...";

@@ -4,6 +4,8 @@
 //   addFunction(MeshSignedDistanceFunction)  -> dg_add_function_sdf (K1)   replaces the OpenMP node loop :806-831
 //   addFunction(MeshSignedDistanceFunction, verbose, MeshDistanceBandPredicate)
 //                                            -> dg_add_function_sdf_band (K1, narrow band: DBL_MAX where |distance| > band, :811-817)
+//   addReducedBandField(MeshSignedDistanceFunction, MeshDistanceBandPredicate)
+//                                            -> dg_reduced_band_create (the same band + reduceField(always true), on the GPU)
 //   addFunction(DensityMapFunction)          -> dg_density_map  (K3)   (GenerateDensityMap's functor + predicate)
 //   interpolate(field, x, grad*)             -> dg_interpolate_batch (K2), also batched: interpolate(field, n, x, phi, grad)
 //   connectivity table of addFunction        -> dg_build_cells  (GPU)  replaces the serial loop :833-886
@@ -158,6 +160,29 @@ public:
         if (verbose) std::cout << "Construction: " << n_nodes << " nodes sampled on the GPU" << std::endl;
         return addSampledFunction(std::move(coeffs));
     }
+    // new: addFunction(func, verbose, pred) followed by reduceField(id, always true) in one library call (dg_reduced_band_create).  The field
+    // holds exactly what those two calls leave; the dense field never reaches the host, only the survivors and the cell map do.
+    unsigned int addReducedBandField(MeshSignedDistanceFunction const& func, MeshDistanceBandPredicate const& pred, bool verbose = false)
+    {
+        if (pred.md != func.md)
+            throw std::invalid_argument("addReducedBandField: the MeshDistanceBandPredicate must use the same TriangleMeshDistance as the MeshSignedDistanceFunction");
+        if (func.md->group())
+            throw std::invalid_argument("addReducedBandField: narrow-band sampling runs on one GPU; it is not available after TriangleMeshDistance::useGpus(n > 1)");
+        const dg_grid_desc d = desc();
+        dg_reduced_band* r = nullptr;
+        check(dg_reduced_band_create(func.md->handle(), &d, func.sign, pred.band, 0u, &r, m_last_reduced_band_ms));
+        struct Release { dg_reduced_band* r; ~Release() { dg_reduced_band_destroy(r); } } release{r};
+        std::uint64_t n_nodes = 0, n_cells = 0;
+        check(dg_reduced_band_sizes(r, &n_nodes, &n_cells));
+        FieldVector<double> coeffs(n_nodes);
+        FieldVector<std::array<unsigned int, 32>> cells(n_cells);
+        FieldVector<unsigned int> cell_map(m_n_cells);
+        check(dg_reduced_band_copy(r, coeffs.data(), reinterpret_cast<std::uint32_t*>(cells.data()), cell_map.data()));
+        if (verbose) std::cout << "Construction: " << n_nodes << " nodes kept, " << n_cells << " cells, on the GPU in " << m_last_reduced_band_ms[6] << " ms" << std::endl;
+        invalidate();
+        m_nodes.push_back(std::move(coeffs)); m_cells.push_back(std::move(cells)); m_cell_map.push_back(std::move(cell_map));
+        return static_cast<unsigned int>(m_n_fields++);
+    }
     // appends a field from node values + the closed-form connectivity (:833-886, built on the GPU) + identity cell map (:888-891)
     unsigned int addSampledFunction(FieldVector<double> coeffs)
     {
@@ -247,6 +272,8 @@ public:
     FieldVector<unsigned int> const& cellMap(unsigned int f) const { return m_cell_map[f]; }
     // ms since entry of the last addFunction(MeshSignedDistanceFunction): total, node pipeline, index tables, pre-fault; workers
     const double* lastAddFunctionTimings() const { return m_last_add_function_ms; }
+    // ms of the last addReducedBandField: sampling, cells, nodes, sort, write-back; tie path (1.0 / 0.0); total
+    const double* lastReducedBandTimings() const { return m_last_reduced_band_ms; }
     std::size_t nFields() const { return m_n_fields; }
     dg_grid_desc desc() const
     {
@@ -272,6 +299,7 @@ private:
     std::vector<FieldVector<std::array<unsigned int, 32>>> m_cells;
     std::vector<FieldVector<unsigned int>> m_cell_map;
     double m_last_add_function_ms[6] = {0, 0, 0, 0, 0, 0};
+    double m_last_reduced_band_ms[7] = {0, 0, 0, 0, 0, 0, 0};
     mutable std::map<unsigned int, dg_field*> m_dev;
 
     static void check(int rc) { if (rc != DG_OK) throw std::runtime_error(std::string("discregrid_b200: ") + dg_last_error()); }

@@ -94,6 +94,10 @@ SIGNATURES = {
     "dg_density_map": (C.c_int, [_vp, C.c_double, C.c_double, C.c_int, C.c_uint64, C.c_uint64, _dp]),
     "dg_reduce_field": (C.c_int, [_gp, _dp, C.c_uint64, C.POINTER(C.c_uint8), _u32p, C.c_uint64, _u32p, C.c_uint32, _u64p, _u64p, _dp]),
     "dg_density_map_device": (C.c_int, [_vp, C.c_double, C.c_double, C.c_int, C.c_uint64, C.c_uint64, _vp, _vp]),
+    "dg_reduced_band_create": (C.c_int, [_vp, _gp, C.c_double, C.c_double, C.c_uint32, C.POINTER(_vp), _dp]),
+    "dg_reduced_band_sizes": (C.c_int, [_vp, _u64p, _u64p]),
+    "dg_reduced_band_copy": (C.c_int, [_vp, _dp, _u32p, _u32p]),
+    "dg_reduced_band_destroy": (C.c_int, [_vp]),
 }
 for _name, (_res, _args) in SIGNATURES.items():
     _f = getattr(lib, _name)          # AttributeError here = the library does not export a declared symbol

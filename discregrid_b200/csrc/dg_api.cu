@@ -1599,6 +1599,135 @@ static int dg_reduce_field_impl(const dg_grid_desc* grid, double* nodes, uint64_
     return DG_OK;
 }
 
+// ------------------------------------------------------------------------------------------------ reduced narrow band
+// addFunction(func, verbose, band predicate) + reduceField(id, always true) on one GPU: every array the size of the grid (dense coefficients,
+// cell flags, node marks, the swap-walk positions, new ids) lives on the device only.  The host holds one count per 1024 flags for the two
+// scans and the survivors' Z-curve keys for the tie-order-preserving sort; the results stay on the device until dg_reduced_band_copy.
+struct dg_reduced_band {
+    DevBuf<double> d_nodes;
+    DevBuf<unsigned> d_cells, d_cell_map;
+    uint64_t n_nodes = 0, n_cells = 0, n_grid_cells = 0;
+    int device = 0;
+};
+
+static int reduced_band_create_impl(const dg_mesh* m, const dg_grid_desc* grid, double sign, double band, uint32_t flags, dg_reduced_band** out,
+                                    double* timings_ms)
+{
+    static const char* who = "dg_reduced_band_create";
+    if (!out) return fail(DG_ERR_INVALID, "%s: out is NULL", who);
+    *out = nullptr;
+    if (!m) return fail(DG_ERR_INVALID, "%s: mesh is NULL (not constructed)", who);
+    GridDev g; const char* why = "";
+    if (!grid_to_dev(grid, g, &why)) return fail(DG_ERR_INVALID, "%s: %s", who, why);
+    if (int rc = check_band(band, who)) return rc;
+    if (flags & ~DG_REDUCE_REFERENCE_SORT) return fail(DG_ERR_INVALID, "%s: unknown flags 0x%x (only DG_REDUCE_REFERENCE_SORT)", who, flags);
+    const uint64_t n = (uint64_t)g.nv + 2ull * ((uint64_t)g.ne_x + g.ne_y + g.ne_z);
+    const uint64_t n_cells = (uint64_t)g.n[0] * g.n[1] * g.n[2];       // grid_to_dev has refused grids of 2^31 nodes or more
+    if (int rc = require_device()) return rc;
+    if (int rc = check_handle_device(m->device, who)) return rc;
+    const auto t_start = std::chrono::steady_clock::now();
+    auto t0 = t_start;
+    auto lap = [&]() { const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count(); t0 = std::chrono::steady_clock::now(); return ms; };
+    const cudaStream_t st = nullptr;
+    double ms[5] = {0, 0, 0, 0, 0};
+    std::unique_ptr<dg_reduced_band> h(new dg_reduced_band());
+    DG_CUDA(cudaGetDevice(&h->device));
+    h->n_grid_cells = n_cells;
+    // ---- 1. the dense band coefficients (addFunction(func, pred), :806-817), on the device only
+    DevBuf<double> d_dense;
+    DG_CUDA(d_dense.alloc(n));
+    if (int rc = dg_sample_sdf_band_device(m, grid, sign, band, 0, n, d_dense.p, st)) return rc;
+    DG_CUDA(cudaStreamSynchronize(st));
+    ms[0] = lap();
+    // ---- 2. kept cells (:1081-1098): flags from the closed-form rows, cell map + the kept rows
+    const uint64_t tile = k4_tile();
+    uint64_t kept_cells = 0;
+    {
+        DevBuf<unsigned char> d_cell_keep;
+        DevBuf<unsigned> d_tile;
+        DG_CUDA(d_cell_keep.alloc(n_cells)); DG_CUDA(d_tile.alloc((n_cells + tile - 1) / tile)); DG_CUDA(h->d_cell_map.alloc(n_cells));
+        DG_LAUNCH(k4_launch_band_cell_keep(g, d_dense.p, n_cells, d_cell_keep.p, st));
+        DG_LAUNCH(k4_scan_flags(d_cell_keep.p, n_cells, d_tile.p, kept_cells, st));
+        DG_CUDA(h->d_cells.alloc(32 * kept_cells));
+        DG_LAUNCH(k4_launch_band_cell_compact(g, n_cells, d_cell_keep.p, d_tile.p, h->d_cells.p, h->d_cell_map.p, st));
+        DG_CUDA(cudaStreamSynchronize(st));
+    }
+    h->n_cells = kept_cells;
+    ms[1] = lap();
+    // ---- 3. surviving nodes = nodes of kept cells (:1117-1134), compacted by the reference's swap walk (:1135-1156) on the device
+    DevBuf<unsigned> d_walk;
+    uint64_t m_nodes = 0;
+    {
+        DevBuf<unsigned char> d_used;
+        DevBuf<unsigned> d_tile, d_flag;
+        DG_CUDA(d_used.alloc(n)); DG_CUDA(d_tile.alloc((n + tile - 1) / tile)); DG_CUDA(d_flag.alloc(1)); DG_CUDA(d_walk.alloc(n));
+        DG_CUDA(cudaMemsetAsync(d_used.p, 0, n, st));
+        DG_LAUNCH(k4_launch_mark_used(h->d_cells.p, 32 * kept_cells, d_used.p, st));
+        unsigned rounds = 0;
+        DG_LAUNCH(k4_swap_walk(d_used.p, n, d_tile.p, d_flag.p, d_walk.p, m_nodes, rounds, st));
+        DG_CUDA(cudaStreamSynchronize(st));
+    }
+    h->n_nodes = m_nodes;
+    ms[2] = lap();
+    // ---- 4. Z-curve keys in swap-walk position order on the device; their order on the host (std::sort's order among equal keys)
+    int tie_path = 0;
+    std::vector<uint32_t> order;
+    {
+        DevBuf<unsigned long long> d_key;
+        DG_CUDA(d_key.alloc(m_nodes));
+        DG_LAUNCH(k4_launch_morton_keys(g, d_walk.p, m_nodes, d_key.p, st));
+        std::vector<KeyPos> kp(m_nodes);
+        {
+            std::vector<unsigned long long> key(m_nodes);
+            if (m_nodes) DG_CUDA(cudaMemcpyAsync(key.data(), d_key.p, m_nodes * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+            DG_CUDA(cudaStreamSynchronize(st));
+            parallel_for(m_nodes, [&](uint64_t b0, uint64_t e0) { for (uint64_t i = b0; i < e0; i++) { kp[i].key = key[i]; kp[i].pos = (uint32_t)i; } });
+        }
+        reduce_order_survivors(kp, (flags & DG_REDUCE_REFERENCE_SORT) != 0, order, tie_path);
+    }
+    ms[3] = lap();
+    // ---- 5. new ids, renumbered rows, gathered coefficients (:1158-1173) into the handle's buffers
+    {
+        DevBuf<unsigned> d_order, d_new_id;
+        DG_CUDA(d_order.alloc(m_nodes)); DG_CUDA(d_new_id.alloc(n)); DG_CUDA(h->d_nodes.alloc(m_nodes));
+        if (m_nodes) DG_CUDA(cudaMemcpyAsync(d_order.p, order.data(), m_nodes * sizeof(unsigned), cudaMemcpyHostToDevice, st));
+        DG_LAUNCH(k4_launch_renumber(d_walk.p, d_order.p, m_nodes, d_dense.p, d_new_id.p, h->d_nodes.p, h->d_cells.p, 32 * kept_cells, st));
+        DG_CUDA(cudaStreamSynchronize(st));
+    }
+    ms[4] = lap();
+    if (timings_ms) {
+        for (int k = 0; k < 5; k++) timings_ms[k] = ms[k];
+        timings_ms[5] = (double)tie_path;
+        timings_ms[6] = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_start).count();
+    }
+    *out = h.release();
+    return DG_OK;
+}
+
+int dg_reduced_band_sizes(const dg_reduced_band* h, uint64_t* n_nodes, uint64_t* n_cells)
+{
+    if (!h || !n_nodes || !n_cells) return fail(DG_ERR_INVALID, "dg_reduced_band_sizes: NULL argument");
+    *n_nodes = h->n_nodes; *n_cells = h->n_cells;
+    return DG_OK;
+}
+
+int dg_reduced_band_copy(const dg_reduced_band* h, double* nodes, uint32_t* cells, uint32_t* cell_map)
+{
+    if (!h) return fail(DG_ERR_INVALID, "dg_reduced_band_copy: handle is NULL");
+    if ((!nodes && h->n_nodes) || (!cells && h->n_cells) || !cell_map) return fail(DG_ERR_INVALID, "dg_reduced_band_copy: NULL output");
+    if (int rc = check_handle_device(h->device, "dg_reduced_band_copy")) return rc;
+    if (h->n_nodes) DG_CUDA(cudaMemcpy(nodes, h->d_nodes.p, h->n_nodes * sizeof(double), cudaMemcpyDeviceToHost));
+    if (h->n_cells) DG_CUDA(cudaMemcpy(cells, h->d_cells.p, 32 * h->n_cells * sizeof(unsigned), cudaMemcpyDeviceToHost));
+    if (h->n_grid_cells) DG_CUDA(cudaMemcpy(cell_map, h->d_cell_map.p, h->n_grid_cells * sizeof(unsigned), cudaMemcpyDeviceToHost));
+    return DG_OK;
+}
+
+int dg_reduced_band_destroy(dg_reduced_band* h)
+{
+    delete h;
+    return DG_OK;
+}
+
 int dg_obj_read(const char* path, double** vertices, uint64_t* n_vertices, uint32_t** triangles, uint64_t* n_triangles)
 {
     if (!path || !vertices || !n_vertices || !triangles || !n_triangles) return fail(DG_ERR_INVALID, "dg_obj_read: NULL argument");
@@ -1650,6 +1779,11 @@ int dg_reduce_field(const dg_grid_desc* grid, double* nodes, uint64_t n_nodes, c
                     uint32_t* cell_map, uint32_t flags, uint64_t* n_nodes_out, uint64_t* n_cells_out, double* timings_ms)
 {
     return guarded("dg_reduce_field", [&]() { return dg_reduce_field_impl(grid, nodes, n_nodes, keep_node, cells, n_cells_in, cell_map, flags, n_nodes_out, n_cells_out, timings_ms); });
+}
+
+int dg_reduced_band_create(const dg_mesh* m, const dg_grid_desc* grid, double sign, double band, uint32_t flags, dg_reduced_band** out, double* timings_ms)
+{
+    return guarded("dg_reduced_band_create", [&]() { return reduced_band_create_impl(m, grid, sign, band, flags, out, timings_ms); });
 }
 
 }  // extern "C"

@@ -8,12 +8,15 @@
 //                  coefficients (:1158-1173)
 //   host (reduce_field.cpp): the reference's back-to-front swap compaction replayed on a permutation array (:1135-1156, O(n), inherently
 //                  serial) and the sort of the survivors by key, whose order among EQUAL keys is libstdc++'s introsort's (reduce_field.h).
+// The reduced narrow band (dg_reduced_band_create) runs the same passes on the device only: cell flags and rows from the closed form instead
+// of a cell table, and the swap walk itself as pointer jumping (swap_walk_*); the sort of the survivors stays on the host.
 // All kernels are warp-synchronous (ballot / popc), so tests/emu runs them unchanged.  Integer work, bit-exact by construction; the one
 // floating-point step (the key's cast of inv * x) uses the reference's operations in the reference's order (no FMA: -fmad=false).
 #include "k4_reduce.h"
 #include "dg_launch.h"
 
 #include <climits>
+#include <vector>
 
 namespace dgb {
 namespace {
@@ -131,6 +134,105 @@ __global__ void renumber_cells_kernel(unsigned* __restrict__ cells_out, unsigned
     if (i < n_entries) cells_out[i] = new_id[cells_out[i]];
 }
 
+// ---- the reduced narrow band (dg_reduced_band_create): the same passes on the dense band coefficients, with the rows of the cells taken
+// from the closed form (cell_node_id) instead of a 32-index table of the whole grid.  A node is kept iff its coefficient is not DBL_MAX
+// (:1073, bit for bit; the predicate is "always true").
+constexpr unsigned long long DBL_MAX_BITS = 0x7fefffffffffffffull;
+
+__device__ __forceinline__ void cell_ijk(const GridDev& g, unsigned long long c, unsigned& i, unsigned& j, unsigned& k)
+{
+    const unsigned long long s = (unsigned long long)g.n[0] * g.n[1];
+    k = (unsigned)(c / s);
+    const unsigned t = (unsigned)(c - (unsigned long long)k * s);
+    j = t / g.n[0]; i = t - j * g.n[0];
+}
+
+// keep flag per cell: one warp per cell, lane j reads the coefficient of the cell's closed-form node j
+__global__ void band_cell_keep_kernel(GridDev g, const double* __restrict__ nodes, unsigned long long n_cells, unsigned char* __restrict__ cell_keep)
+{
+    const unsigned long long c = ((unsigned long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const unsigned lane = threadIdx.x & 31u;
+    const bool live = c < n_cells;                    // whole warps: uniform
+    bool kept = false;
+    if (live) {
+        unsigned i, j, k;
+        cell_ijk(g, c, i, j, k);
+        kept = (unsigned long long)__double_as_longlong(__ldg(nodes + cell_node_id(g, i, j, k, lane))) != DBL_MAX_BITS;
+    }
+    const unsigned any = __ballot_sync(0xffffffffu, kept);
+    if (live && lane == 0) cell_keep[c] = any ? 1 : 0;
+}
+
+// cell_map and the closed-form rows of the kept cells, order kept: cell_compact_kernel with the rows computed instead of copied
+__global__ void band_cell_compact_kernel(GridDev g, unsigned long long n_cells, const unsigned char* __restrict__ cell_keep,
+                                         const unsigned* __restrict__ tile_offset, unsigned* __restrict__ cells_out, unsigned* __restrict__ cell_map)
+{
+    const unsigned long long tile = ((unsigned long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const unsigned lane = threadIdx.x & 31u;
+    const unsigned long long base = tile * TILE;
+    if (base >= n_cells) return;
+    unsigned run = tile_offset[tile];
+    const unsigned lt = (1u << lane) - 1u;
+    for (unsigned k = 0; k < TILE; k += 32) {
+        const unsigned long long c = base + k + lane;
+        const bool kept = c < n_cells && cell_keep[c] != 0;
+        const unsigned m = __ballot_sync(0xffffffffu, kept);
+        if (c < n_cells) cell_map[c] = kept ? run + (unsigned)__popc(m & lt) : 0xffffffffu;
+        unsigned rest = m, r = run;
+        while (rest) {
+            const unsigned src_lane = (unsigned)__ffs((int)rest) - 1u;
+            rest &= rest - 1u;
+            unsigned ci, cj, ck;
+            cell_ijk(g, base + k + src_lane, ci, cj, ck);
+            cells_out[(unsigned long long)r * 32ull + lane] = cell_node_id(g, ci, cj, ck, lane);
+            r++;
+        }
+        run += (unsigned)__popc(m);
+    }
+}
+
+// The reference's back-to-front swap walk (:1135-1156) in parallel.  With m used positions, a used position p < m keeps its node; a dead
+// position p < m ends up holding the first USED position of q0 = m + dead(p), q_{i+1} = m + dead(q_i), where dead(q) = number of dead
+// positions before q (the k-th dead position from the front is swapped with position m + k).  walk[q] = q for a used q, m + dead(q) for a
+// dead one; tile_offset = exclusive scan of the used counts per tile, so dead(q) = q - used positions before q.
+__global__ void swap_walk_start_kernel(const unsigned char* __restrict__ used, unsigned long long n, unsigned long long m,
+                                       const unsigned* __restrict__ tile_offset, unsigned* __restrict__ walk)
+{
+    const unsigned long long tile = ((unsigned long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const unsigned lane = threadIdx.x & 31u;
+    const unsigned long long base = tile * TILE;
+    if (base >= n) return;
+    unsigned long long run = tile_offset[tile];
+    const unsigned lt = (1u << lane) - 1u;
+    for (unsigned k = 0; k < TILE; k += 32) {
+        const unsigned long long q = base + k + lane;
+        const bool u = q < n && used[q] != 0;
+        const unsigned mask = __ballot_sync(0xffffffffu, u);
+        if (q < n) walk[q] = u ? (unsigned)q : (unsigned)(m + (q - (run + (unsigned)__popc(mask & lt))));
+        run += (unsigned)__popc(mask);
+    }
+}
+
+// one round of pointer jumping over [m, n): walk[q] <- walk[walk[q]].  In place: a value read while another thread rewrites it is either
+// the old or the new pointer, both further along the same chain, so a round advances every pointer at least as far as a double-buffered one.
+__global__ void swap_walk_jump_kernel(unsigned* walk, unsigned long long m, unsigned long long n, unsigned* __restrict__ changed)
+{
+    const unsigned long long q = m + (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+    bool moved = false;
+    if (q < n) {
+        const unsigned a = walk[q], b = walk[a];
+        if (b != a) { walk[q] = b; moved = true; }
+    }
+    if (__ballot_sync(0xffffffffu, moved) && (threadIdx.x & 31u) == 0) atomicAdd(changed, 1u);
+}
+
+// positions [0, m): walk[p] = p (used) or a position >= m whose pointer now names the used position at the end of its chain
+__global__ void swap_walk_finish_kernel(unsigned* walk, unsigned long long m)
+{
+    const unsigned long long p = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (p < m) walk[p] = walk[walk[p]];
+}
+
 inline unsigned blocks_for(unsigned long long threads, unsigned block) { return (unsigned)((threads + block - 1) / block); }
 
 }  // namespace
@@ -183,6 +285,71 @@ cudaError_t k4_launch_renumber(const unsigned* d_perm, const unsigned* d_order, 
 {
     if (m) { DG_KERNEL_LAUNCH(renumber_nodes_kernel, blocks_for(m, 256), 256, 0, stream, d_perm, d_order, (unsigned long long)m, d_nodes, d_new_id, d_nodes_out); }
     if (n_entries) { DG_KERNEL_LAUNCH(renumber_cells_kernel, blocks_for(n_entries, 256), 256, 0, stream, d_cells_out, (unsigned long long)n_entries, d_new_id); }
+    return DG_AFTER_LAUNCH();
+}
+
+cudaError_t k4_launch_band_cell_keep(const GridDev& g, const double* d_nodes, uint64_t n_cells, unsigned char* d_cell_keep, cudaStream_t stream)
+{
+    if (n_cells == 0) return cudaSuccess;
+    DG_KERNEL_LAUNCH(band_cell_keep_kernel, blocks_for(n_cells * 32ull, 128), 128, 0, stream, g, d_nodes, (unsigned long long)n_cells, d_cell_keep);
+    return DG_AFTER_LAUNCH();
+}
+
+cudaError_t k4_launch_band_cell_compact(const GridDev& g, uint64_t n_cells, const unsigned char* d_cell_keep, const unsigned* d_tile_offset,
+                                        unsigned* d_cells_out, unsigned* d_cell_map, cudaStream_t stream)
+{
+    if (n_cells == 0) return cudaSuccess;
+    const uint64_t tiles = (n_cells + TILE - 1) / TILE;
+    DG_KERNEL_LAUNCH(band_cell_compact_kernel, blocks_for(tiles * 32ull, 128), 128, 0, stream, g, (unsigned long long)n_cells, d_cell_keep, d_tile_offset,
+                     d_cells_out, d_cell_map);
+    return DG_AFTER_LAUNCH();
+}
+
+// exclusive scan of per-tile counts on the host (one entry per TILE flags) through d_tile, in place; returns the total
+static cudaError_t scan_tile_counts(unsigned* d_tile, uint64_t n_tiles, uint64_t& total, cudaStream_t stream)
+{
+    std::vector<unsigned> cnt(n_tiles);
+    total = 0;
+    if (n_tiles == 0) return cudaSuccess;
+    cudaError_t e = cudaMemcpyAsync(cnt.data(), d_tile, n_tiles * sizeof(unsigned), cudaMemcpyDeviceToHost, stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
+    if (e != cudaSuccess) return e;
+    for (uint64_t t = 0; t < n_tiles; t++) { const unsigned c = cnt[t]; cnt[t] = (unsigned)total; total += c; }
+    e = cudaMemcpyAsync(d_tile, cnt.data(), n_tiles * sizeof(unsigned), cudaMemcpyHostToDevice, stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(stream);         // cnt goes out of scope
+    return e;
+}
+
+cudaError_t k4_scan_flags(const unsigned char* d_flag, uint64_t n, unsigned* d_tile, uint64_t& total, cudaStream_t stream)
+{
+    cudaError_t e = k4_launch_tile_count(d_flag, n, d_tile, stream);
+    if (e != cudaSuccess) return e;
+    return scan_tile_counts(d_tile, (n + TILE - 1) / TILE, total, stream);
+}
+
+cudaError_t k4_swap_walk(const unsigned char* d_used, uint64_t n, unsigned* d_tile, unsigned* d_flag, unsigned* d_walk, uint64_t& m, unsigned& rounds,
+                         cudaStream_t stream)
+{
+    rounds = 0;
+    cudaError_t e = k4_scan_flags(d_used, n, d_tile, m, stream);
+    if (e != cudaSuccess || m == 0) return e;
+    const uint64_t tiles = (n + TILE - 1) / TILE;
+    DG_KERNEL_LAUNCH(swap_walk_start_kernel, blocks_for(tiles * 32ull, 128), 128, 0, stream, d_used, (unsigned long long)n, (unsigned long long)m, d_tile, d_walk);
+    if ((e = DG_AFTER_LAUNCH()) != cudaSuccess) return e;
+    // a chain visits distinct positions of [m, n), so ceil(log2(n - m)) rounds reach its end; stop as soon as a round moves nothing
+    unsigned max_rounds = 0;
+    while ((1ull << max_rounds) < n - m) max_rounds++;
+    for (unsigned r = 0; r < max_rounds; r++) {
+        unsigned changed = 0;
+        if ((e = cudaMemsetAsync(d_flag, 0, sizeof(unsigned), stream)) != cudaSuccess) return e;
+        DG_KERNEL_LAUNCH(swap_walk_jump_kernel, blocks_for(n - m, 256), 256, 0, stream, d_walk, (unsigned long long)m, (unsigned long long)n, d_flag);
+        if ((e = DG_AFTER_LAUNCH()) != cudaSuccess) return e;
+        if ((e = cudaMemcpyAsync(&changed, d_flag, sizeof(unsigned), cudaMemcpyDeviceToHost, stream)) != cudaSuccess) return e;
+        if ((e = cudaStreamSynchronize(stream)) != cudaSuccess) return e;
+        rounds++;
+        if (!changed) break;
+    }
+    if (m) { DG_KERNEL_LAUNCH(swap_walk_finish_kernel, blocks_for(m, 256), 256, 0, stream, d_walk, (unsigned long long)m); }
     return DG_AFTER_LAUNCH();
 }
 

@@ -17,4 +17,15 @@ cudaError_t k4_launch_morton_keys(const GridDev& g, const unsigned* d_perm, uint
 cudaError_t k4_launch_renumber(const unsigned* d_perm, const unsigned* d_order, uint64_t m, const double* d_nodes, unsigned* d_new_id, double* d_nodes_out,
                                unsigned* d_cells_out, uint64_t n_entries, cudaStream_t stream);
 
+// reduced narrow band: cell flags and compaction with the closed-form rows (cell_node_id) of the dense band coefficients d_nodes
+cudaError_t k4_launch_band_cell_keep(const GridDev& g, const double* d_nodes, uint64_t n_cells, unsigned char* d_cell_keep, cudaStream_t stream);
+cudaError_t k4_launch_band_cell_compact(const GridDev& g, uint64_t n_cells, const unsigned char* d_cell_keep, const unsigned* d_tile_offset,
+                                        unsigned* d_cells_out, unsigned* d_cell_map, cudaStream_t stream);
+// d_tile (ceil(n / k4_tile()) entries) <- exclusive scan of the set flags per tile; total = number of set flags.  Synchronises `stream`.
+cudaError_t k4_scan_flags(const unsigned char* d_flag, uint64_t n, unsigned* d_tile, uint64_t& total, cudaStream_t stream);
+// The reference's swap-walk compaction (:1135-1156, reduce_swap_walk) on the device: m = number of used positions, d_walk[0..m) = the
+// node at each position afterwards.  d_walk: n entries, d_tile: ceil(n / k4_tile()), d_flag: 1.  rounds = pointer-jumping rounds run.
+cudaError_t k4_swap_walk(const unsigned char* d_used, uint64_t n, unsigned* d_tile, unsigned* d_flag, unsigned* d_walk, uint64_t& m, unsigned& rounds,
+                         cudaStream_t stream);
+
 }  // namespace dgb

@@ -8,6 +8,8 @@ that save()/load() stay byte-compatible with the reference's .cdf/.cdm files
   addFunction(MeshSignedDistance)        -> dg_add_function_sdf  (K1, csrc/k1_sdf.cu)
   addFunction(MeshSignedDistance, pred=MeshDistanceBand)
                                          -> dg_add_function_sdf_band (K1 narrow band: DBL_MAX outside |distance| <= band)
+  addReducedBandField(MeshSignedDistance, MeshDistanceBand)
+                                         -> dg_reduced_band_create (the same band, then reduceField(always true), all on the GPU)
   addFunction(DensityMapFunction, pred)  -> dg_density_map       (K3, csrc/k3_density.cu)
   interpolate(field_id, x[, gradient])   -> dg_interpolate_batch (K2, csrc/k2_interp.cu), batched over x
 
@@ -150,6 +152,33 @@ class CubicLagrangeDiscreteGrid:
             raise TypeError("addFunction runs on the GPU and only accepts MeshSignedDistance or DensityMapFunction; "
                             "for any other function evaluate it at nodePositions() and call addSampledFunction(values)")
         return self.addSampledFunction(coeffs)
+
+    def addReducedBandField(self, func, pred, verbose=False):
+        """addFunction(func, verbose, pred) followed by reduceField(id, always true), in one GPU call (dg_reduced_band_create): the field
+        holds exactly what those two calls leave, but only the survivors and the cell map ever reach the host.  func: MeshSignedDistance,
+        pred: MeshDistanceBand over the same TriangleMeshDistance.  Returns the field id."""
+        if not isinstance(func, MeshSignedDistance) or not isinstance(pred, MeshDistanceBand):
+            raise TypeError("addReducedBandField takes a MeshSignedDistance and a MeshDistanceBand")
+        if pred.md is not func.md:
+            raise TypeError("MeshDistanceBand must use the same TriangleMeshDistance as the MeshSignedDistance it restricts")
+        h = C.c_void_p()
+        self.last_reduced_band_ms = np.zeros(7)
+        capi.check(capi.lib.dg_reduced_band_create(func.md.handle, C.byref(self._desc), func.sign, pred.band, 0, C.byref(h),
+                                                   capi.ptr(self.last_reduced_band_ms, capi.F64P)))
+        try:
+            n_nodes, n_cells = C.c_uint64(), C.c_uint64()
+            capi.check(capi.lib.dg_reduced_band_sizes(h, C.byref(n_nodes), C.byref(n_cells)))
+            coeffs = np.empty(n_nodes.value)
+            cells = np.empty((n_cells.value, 32), np.uint32)
+            cmap = np.empty(self.m_n_cells, np.uint32)
+            capi.check(capi.lib.dg_reduced_band_copy(h, capi.ptr(coeffs, capi.F64P), capi.ptr(cells, capi.U32P), capi.ptr(cmap, capi.U32P)))
+        finally:
+            capi.lib.dg_reduced_band_destroy(h)
+        if verbose:
+            print(f"Construction: {len(coeffs)} of {self.nNodes()} nodes kept in {self.last_reduced_band_ms[6]:.1f} ms on the GPU")
+        self.m_nodes.append(coeffs); self.m_cells.append(cells); self.m_cell_map.append(cmap)
+        self.m_n_fields += 1
+        return self.m_n_fields - 1
 
     def addSampledFunction(self, coeffs):
         """Appends a field from node values (what addFunction's loop :806-831 produces), then builds the cell

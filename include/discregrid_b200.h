@@ -265,6 +265,29 @@ DG_API int dg_reduce_field(const dg_grid_desc* grid, double* nodes, uint64_t n_n
                     uint64_t n_cells_in, uint32_t* cell_map, uint32_t flags, uint64_t* n_nodes_out, uint64_t* n_cells_out,
                     double* timings_ms);
 
+/* ---- reduced narrow band: addFunction(band) + reduceField(always true) in one call -----------------------------------------------
+ * replaces
+ *     id = addFunction(func, verbose, pred);  reduceField(id, [](Vector3d const&, double) { return true; });
+ * with func and pred as for dg_add_function_sdf_band: the result is exactly what the reference holds afterwards -- the same nodes in the
+ * same Z-curve order (including the order among equal keys), the same renumbered cells and the same cell map -- bit for bit what
+ * dg_add_function_sdf_band followed by dg_reduce_field gives.  Everything the size of the grid stays on the current device (dense band
+ * coefficients, cell flags, node marks, the swap-walk positions); the host holds one count per 1024 flags and the survivors' keys.  The
+ * results stay on the device in the handle (created on, and only usable from, the current device) until dg_reduced_band_copy copies
+ * them into the caller's arrays, sized with dg_reduced_band_sizes.
+ *   band: >= 0 (negative or NaN: DG_ERR_INVALID); +inf keeps every node.  Grids of 2^31 nodes or more are refused before anything is
+ *       allocated (as dg_reduce_field).  One GPU.
+ *   flags: 0 or DG_REDUCE_REFERENCE_SORT (as for dg_reduce_field).
+ *   timings_ms: NULL or 7 doubles = ms of band sampling, kept cells, node compaction, sort, write-back; 1.0 if surviving nodes shared
+ *       Morton keys (dg_reduce_field's tie path); total ms.  Every stage ends with a device synchronise.
+ *   dg_reduced_band_copy: nodes[n_nodes], cells[n_cells x 32], cell_map[nx*ny*nz] (0xffffffff = removed cell); nodes / cells may be NULL
+ *       only when their count is 0. */
+typedef struct dg_reduced_band dg_reduced_band;
+DG_API int dg_reduced_band_create(const dg_mesh* mesh, const dg_grid_desc* grid, double sign, double band, uint32_t flags,
+                           dg_reduced_band** out, double* timings_ms);
+DG_API int dg_reduced_band_sizes(const dg_reduced_band* result, uint64_t* n_nodes, uint64_t* n_cells);
+DG_API int dg_reduced_band_copy(const dg_reduced_band* result, double* nodes, uint32_t* cells, uint32_t* cell_map);
+DG_API int dg_reduced_band_destroy(dg_reduced_band* result);
+
 #ifdef __cplusplus
 }
 #endif
