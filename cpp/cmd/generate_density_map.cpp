@@ -1,6 +1,7 @@
 // GenerateDensityMap -- same command line and output as the reference tool (cmd/generate_density_map/main.cpp:29-171):
 //   GenerateDensityMap [-r rho0] [-s h] [-o out.cdm] [--no-reduction] field.cdf
-// density_func / gamma / predicate / 16^3 Gauss quadrature run in the K3 kernel (dg_density_map); reduceField is host code.
+// density_func / gamma / predicate / 16^3 Gauss quadrature run in the K3 kernel; with reduction, K3 and both reduceField calls run in one
+// library call (addReducedDensityMap -> dg_reduced_density_map_create), without --no-reduction's dense fields on the host.
 #include <Discregrid/All>
 #include <cstdlib>
 #include <iostream>
@@ -30,14 +31,16 @@ int main(int argc, char* argv[])
         std::cout << "Load SDF...";
         Discregrid::CubicLagrangeDiscreteGrid sdf(filename);
         std::cout << "DONE" << std::endl;
-        const double cell_diag = sdf.cellSize().norm();
         std::cout << "Generate density map..." << std::endl;
-        Discregrid::DiscreteGrid::ContinuousFunction func = Discregrid::DensityMapFunction{&sdf, 0u, h, rho0, no_reduction};
-        sdf.addFunction(func, true);
-        if (!no_reduction) {
-            std::cout << "Reduce discrete fields...";
-            sdf.reduceField(0u, [&](const Vector3d&, double v) { return -6.0 * h < v + cell_diag && v - cell_diag < 2.0 * h; });
-            sdf.reduceField(1u, [&](const Vector3d&, double v) { return 0.0 <= v && v <= 3.0 * rho0; });
+        const Discregrid::DensityMapFunction density{&sdf, 0u, h, rho0, no_reduction};
+        if (no_reduction) {
+            Discregrid::DiscreteGrid::ContinuousFunction func = density;
+            sdf.addFunction(func, true);
+        } else {
+            // addFunction(func, true) + reduceField(0u, -6h < v + cell_diag && v - cell_diag < 2h) + reduceField(1u, 0 <= v && v <= 3 rho0),
+            // with cell_diag = sdf.cellSize().norm(), in one library call: the dense density field stays on the GPU
+            std::cout << "Reduce discrete fields..." << std::endl;
+            sdf.addReducedDensityMap(density, true);
             std::cout << "DONE" << std::endl;
         }
         std::cout << "Serialize discretization...";

@@ -7,6 +7,7 @@
 //   addReducedBandField(MeshSignedDistanceFunction, MeshDistanceBandPredicate)
 //                                            -> dg_reduced_band_create (the same band + reduceField(always true), on the GPU)
 //   addFunction(DensityMapFunction)          -> dg_density_map  (K3)   (GenerateDensityMap's functor + predicate)
+//   addReducedDensityMap(DensityMapFunction) -> dg_reduced_density_map_create (K3 + both of GenerateDensityMap's reduceField calls, on the GPU)
 //   interpolate(field, x, grad*)             -> dg_interpolate_batch (K2), also batched: interpolate(field, n, x, phi, grad)
 //   connectivity table of addFunction        -> dg_build_cells  (GPU)  replaces the serial loop :833-886
 //
@@ -183,6 +184,41 @@ public:
         m_nodes.push_back(std::move(coeffs)); m_cells.push_back(std::move(cells)); m_cell_map.push_back(std::move(cell_map));
         return static_cast<unsigned int>(m_n_fields++);
     }
+    // new: GenerateDensityMap with reduction in one library call (dg_reduced_density_map_create).  Leaves exactly what
+    //   id = addFunction(f, verbose);  reduceField(f.sdf_field_id, p0);  reduceField(id, p1);
+    // leave, with the tool's predicates p0(x, v) = -6h < v + cell_diag && v - cell_diag < 2h and p1(x, v) = 0 <= v && v <= 3 rho0
+    // (main.cpp:139-140): the SDF field is replaced by its reduction, the reduced density field is appended and its id returned.  The dense
+    // density field never reaches the host; only the survivors and the cell maps do.
+    unsigned int addReducedDensityMap(DensityMapFunction const& f, bool verbose = false)
+    {
+        if (f.grid != this) throw std::invalid_argument("addReducedDensityMap: the DensityMapFunction must sample this grid's own SDF field");
+        if (f.no_reduction) throw std::invalid_argument("addReducedDensityMap: the DensityMapFunction has no_reduction set (use addFunction)");
+        const unsigned int id = f.sdf_field_id;
+        if (id >= m_n_fields) throw std::invalid_argument("addReducedDensityMap: no SDF field with that id");
+        if (m_cell_map[id].size() != m_n_cells) throw std::invalid_argument("addReducedDensityMap: the SDF field's cell map must cover every grid cell");
+        const dg_grid_desc d = desc();
+        dg_reduced_band* r[2] = {nullptr, nullptr};
+        check(dg_reduced_density_map_create(&d, m_nodes[id].data(), m_nodes[id].size(), reinterpret_cast<const std::uint32_t*>(m_cells[id].data()),
+                                            m_cells[id].size(), m_cell_map[id].data(), f.smoothing_length, f.rest_density, 0u, &r[0], &r[1],
+                                            m_last_reduced_density_ms));
+        struct Release { dg_reduced_band** r; ~Release() { dg_reduced_band_destroy(r[0]); dg_reduced_band_destroy(r[1]); } } release{r};
+        FieldVector<double> coeffs[2];
+        FieldVector<std::array<unsigned int, 32>> cells[2];
+        FieldVector<unsigned int> cell_map[2];
+        for (int k = 0; k < 2; k++) {         // both copied before anything changes, so a failure leaves the grid as it was
+            std::uint64_t n_nodes = 0, n_cells = 0;
+            check(dg_reduced_band_sizes(r[k], &n_nodes, &n_cells));
+            coeffs[k].resize(n_nodes); cells[k].resize(n_cells); cell_map[k].resize(m_n_cells);
+            check(dg_reduced_band_copy(r[k], coeffs[k].data(), reinterpret_cast<std::uint32_t*>(cells[k].data()), cell_map[k].data()));
+        }
+        if (verbose)
+            std::cout << "Construction: density map sampled and both fields reduced on the GPU in " << m_last_reduced_density_ms[12] << " ms ("
+                      << coeffs[0].size() << " SDF nodes and " << coeffs[1].size() << " density nodes kept)" << std::endl;
+        invalidate();
+        m_nodes[id] = std::move(coeffs[0]); m_cells[id] = std::move(cells[0]); m_cell_map[id] = std::move(cell_map[0]);
+        m_nodes.push_back(std::move(coeffs[1])); m_cells.push_back(std::move(cells[1])); m_cell_map.push_back(std::move(cell_map[1]));
+        return static_cast<unsigned int>(m_n_fields++);
+    }
     // appends a field from node values + the closed-form connectivity (:833-886, built on the GPU) + identity cell map (:888-891)
     unsigned int addSampledFunction(FieldVector<double> coeffs)
     {
@@ -274,6 +310,8 @@ public:
     const double* lastAddFunctionTimings() const { return m_last_add_function_ms; }
     // ms of the last addReducedBandField: sampling, cells, nodes, sort, write-back; tie path (1.0 / 0.0); total
     const double* lastReducedBandTimings() const { return m_last_reduced_band_ms; }
+    // ms of the last addReducedDensityMap: upload + pack, density; cells, nodes, sort, write-back of field 0 then of field 1; tie paths; total
+    const double* lastReducedDensityTimings() const { return m_last_reduced_density_ms; }
     std::size_t nFields() const { return m_n_fields; }
     dg_grid_desc desc() const
     {
@@ -300,6 +338,7 @@ private:
     std::vector<FieldVector<unsigned int>> m_cell_map;
     double m_last_add_function_ms[6] = {0, 0, 0, 0, 0, 0};
     double m_last_reduced_band_ms[7] = {0, 0, 0, 0, 0, 0, 0};
+    double m_last_reduced_density_ms[13] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
     mutable std::map<unsigned int, dg_field*> m_dev;
 
     static void check(int rc) { if (rc != DG_OK) throw std::runtime_error(std::string("discregrid_b200: ") + dg_last_error()); }

@@ -98,6 +98,8 @@ SIGNATURES = {
     "dg_reduced_band_sizes": (C.c_int, [_vp, _u64p, _u64p]),
     "dg_reduced_band_copy": (C.c_int, [_vp, _dp, _u32p, _u32p]),
     "dg_reduced_band_destroy": (C.c_int, [_vp]),
+    "dg_reduced_density_map_create": (C.c_int, [_gp, _dp, C.c_uint64, _u32p, C.c_uint64, _u32p, C.c_double, C.c_double, C.c_uint32,
+                                                 C.POINTER(_vp), C.POINTER(_vp), _dp]),
 }
 for _name, (_res, _args) in SIGNATURES.items():
     _f = getattr(lib, _name)          # AttributeError here = the library does not export a declared symbol

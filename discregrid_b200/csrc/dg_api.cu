@@ -1599,10 +1599,11 @@ static int dg_reduce_field_impl(const dg_grid_desc* grid, double* nodes, uint64_
     return DG_OK;
 }
 
-// ------------------------------------------------------------------------------------------------ reduced narrow band
-// addFunction(func, verbose, band predicate) + reduceField(id, always true) on one GPU: every array the size of the grid (dense coefficients,
-// cell flags, node marks, the swap-walk positions, new ids) lives on the device only.  The host holds one count per 1024 flags for the two
-// scans and the survivors' Z-curve keys for the tie-order-preserving sort; the results stay on the device until dg_reduced_band_copy.
+// ------------------------------------------------------------------------------------------------ reduced fields on the device
+// reduceField(id, pred) for a dense field that is already on the device and a predicate of the node value alone (K4ValuePred): every array
+// the size of the grid (coefficients, cell flags, node marks, the swap-walk positions, new ids) lives on the device only.  The host holds one
+// count per 1024 flags for the scans and the survivors' Z-curve keys for the tie-order-preserving sort; the results stay on the device in a
+// dg_reduced_band (a reduced field kept on its device) until dg_reduced_band_copy.
 struct dg_reduced_band {
     DevBuf<double> d_nodes;
     DevBuf<unsigned> d_cells, d_cell_map;
@@ -1610,6 +1611,118 @@ struct dg_reduced_band {
     int device = 0;
 };
 
+namespace {
+// ms since the last lap
+struct StageClock {
+    std::chrono::steady_clock::time_point t0 = std::chrono::steady_clock::now();
+    double lap()
+    {
+        const auto t = std::chrono::steady_clock::now();
+        const double ms = std::chrono::duration<double, std::milli>(t - t0).count();
+        t0 = t;
+        return ms;
+    }
+};
+
+// the rows of the field being reduced: an uploaded table of n_cells rows, or (d_cells == nullptr) the closed form of every grid cell
+struct DenseRows {
+    const unsigned* d_cells;
+    uint64_t n_cells;
+};
+}  // namespace
+
+// kept cells (:1081-1098), first half: d_cell_keep[c] = some node of row c is kept by pred.  Uploaded rows are checked on the way: a row
+// that names a node >= n is refused, as dg_reduce_field refuses it.  Synchronises `st`.
+static int device_cell_flags(const GridDev& g, const double* d_dense, uint64_t n, const DenseRows& rows, const K4ValuePred& pred,
+                             DevBuf<unsigned char>& d_cell_keep, const char* who, cudaStream_t st)
+{
+    DG_CUDA(d_cell_keep.alloc(rows.n_cells));
+    if (!rows.d_cells) {
+        DG_LAUNCH(k4_launch_closed_cell_keep(g, d_dense, rows.n_cells, pred, d_cell_keep.p, st));
+        DG_CUDA(cudaStreamSynchronize(st));
+        return DG_OK;
+    }
+    DevBuf<unsigned char> d_keep;
+    DevBuf<unsigned> d_bad;
+    DG_CUDA(d_keep.alloc(n)); DG_CUDA(d_bad.alloc(1));
+    DG_CUDA(cudaMemsetAsync(d_bad.p, 0, sizeof(unsigned), st));
+    DG_LAUNCH(k4_launch_node_keep(d_dense, n, pred, d_keep.p, st));
+    DG_LAUNCH(k4_launch_cell_keep(rows.d_cells, rows.n_cells, d_keep.p, (unsigned)n, d_cell_keep.p, d_bad.p, st));
+    unsigned bad = 0;
+    DG_CUDA(cudaMemcpyAsync(&bad, d_bad.p, sizeof bad, cudaMemcpyDeviceToHost, st));
+    DG_CUDA(cudaStreamSynchronize(st));
+    if (bad) return fail(DG_ERR_INVALID, "%s: a cell refers to a node id >= n_nodes", who);
+    return DG_OK;
+}
+
+// the rest of reduceField (:1076-1173) into `out`: cell map + kept rows, surviving nodes by the swap walk, their Z-curve order, renumbered
+// rows and gathered coefficients.  ms[0..4) += kept cells, node compaction, sort, write-back; each stage ends with a synchronise.
+static int device_reduce(const GridDev& g, const double* d_dense, uint64_t n, const DenseRows& rows, const unsigned char* d_cell_keep,
+                         uint64_t n_grid_cells, bool reference_sort, dg_reduced_band& out, double ms[4], int& tie_path, StageClock& clock,
+                         cudaStream_t st)
+{
+    const uint64_t tile = k4_tile();
+    // ---- kept cells, second half: cell map + the kept rows, order kept; cells the field has no row for map to themselves (:1076-1078)
+    uint64_t kept_cells = 0;
+    {
+        DevBuf<unsigned> d_tile;
+        DG_CUDA(d_tile.alloc((rows.n_cells + tile - 1) / tile)); DG_CUDA(out.d_cell_map.alloc(n_grid_cells));
+        DG_LAUNCH(k4_scan_flags(d_cell_keep, rows.n_cells, d_tile.p, kept_cells, st));
+        DG_CUDA(out.d_cells.alloc(32 * kept_cells));
+        if (rows.d_cells)
+            DG_LAUNCH(k4_launch_cell_compact(rows.d_cells, rows.n_cells, d_cell_keep, d_tile.p, out.d_cells.p, out.d_cell_map.p, st));
+        else
+            DG_LAUNCH(k4_launch_closed_cell_compact(g, rows.n_cells, d_cell_keep, d_tile.p, out.d_cells.p, out.d_cell_map.p, st));
+        DG_LAUNCH(k4_launch_iota(out.d_cell_map.p, rows.n_cells, n_grid_cells, st));
+        DG_CUDA(cudaStreamSynchronize(st));
+    }
+    out.n_cells = kept_cells;
+    out.n_grid_cells = n_grid_cells;
+    ms[0] += clock.lap();
+    // ---- surviving nodes = nodes of kept cells (:1117-1134), compacted by the reference's swap walk (:1135-1156) on the device
+    DevBuf<unsigned> d_walk;
+    uint64_t m_nodes = 0;
+    {
+        DevBuf<unsigned char> d_used;
+        DevBuf<unsigned> d_tile, d_flag;
+        DG_CUDA(d_used.alloc(n)); DG_CUDA(d_tile.alloc((n + tile - 1) / tile)); DG_CUDA(d_flag.alloc(1)); DG_CUDA(d_walk.alloc(n));
+        DG_CUDA(cudaMemsetAsync(d_used.p, 0, n, st));
+        DG_LAUNCH(k4_launch_mark_used(out.d_cells.p, 32 * kept_cells, d_used.p, st));
+        unsigned rounds = 0;
+        DG_LAUNCH(k4_swap_walk(d_used.p, n, d_tile.p, d_flag.p, d_walk.p, m_nodes, rounds, st));
+        DG_CUDA(cudaStreamSynchronize(st));
+    }
+    out.n_nodes = m_nodes;
+    ms[1] += clock.lap();
+    // ---- Z-curve keys in swap-walk position order on the device; their order on the host (std::sort's order among equal keys)
+    std::vector<uint32_t> order;
+    {
+        DevBuf<unsigned long long> d_key;
+        DG_CUDA(d_key.alloc(m_nodes));
+        DG_LAUNCH(k4_launch_morton_keys(g, d_walk.p, m_nodes, d_key.p, st));
+        std::vector<KeyPos> kp(m_nodes);
+        {
+            std::vector<unsigned long long> key(m_nodes);
+            if (m_nodes) DG_CUDA(cudaMemcpyAsync(key.data(), d_key.p, m_nodes * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+            DG_CUDA(cudaStreamSynchronize(st));
+            parallel_for(m_nodes, [&](uint64_t b0, uint64_t e0) { for (uint64_t i = b0; i < e0; i++) { kp[i].key = key[i]; kp[i].pos = (uint32_t)i; } });
+        }
+        reduce_order_survivors(kp, reference_sort, order, tie_path);
+    }
+    ms[2] += clock.lap();
+    // ---- new ids, renumbered rows, gathered coefficients (:1158-1173) into the handle's buffers
+    {
+        DevBuf<unsigned> d_order, d_new_id;
+        DG_CUDA(d_order.alloc(m_nodes)); DG_CUDA(d_new_id.alloc(n)); DG_CUDA(out.d_nodes.alloc(m_nodes));
+        if (m_nodes) DG_CUDA(cudaMemcpyAsync(d_order.p, order.data(), m_nodes * sizeof(unsigned), cudaMemcpyHostToDevice, st));
+        DG_LAUNCH(k4_launch_renumber(d_walk.p, d_order.p, m_nodes, d_dense, d_new_id.p, out.d_nodes.p, out.d_cells.p, 32 * kept_cells, st));
+        DG_CUDA(cudaStreamSynchronize(st));
+    }
+    ms[3] += clock.lap();
+    return DG_OK;
+}
+
+// addFunction(func, verbose, band predicate) + reduceField(id, always true) on one GPU
 static int reduced_band_create_impl(const dg_mesh* m, const dg_grid_desc* grid, double sign, double band, uint32_t flags, dg_reduced_band** out,
                                     double* timings_ms)
 {
@@ -1625,82 +1738,123 @@ static int reduced_band_create_impl(const dg_mesh* m, const dg_grid_desc* grid, 
     const uint64_t n_cells = (uint64_t)g.n[0] * g.n[1] * g.n[2];       // grid_to_dev has refused grids of 2^31 nodes or more
     if (int rc = require_device()) return rc;
     if (int rc = check_handle_device(m->device, who)) return rc;
-    const auto t_start = std::chrono::steady_clock::now();
-    auto t0 = t_start;
-    auto lap = [&]() { const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count(); t0 = std::chrono::steady_clock::now(); return ms; };
+    StageClock clock;
+    const auto t_start = clock.t0;
     const cudaStream_t st = nullptr;
     double ms[5] = {0, 0, 0, 0, 0};
     std::unique_ptr<dg_reduced_band> h(new dg_reduced_band());
     DG_CUDA(cudaGetDevice(&h->device));
-    h->n_grid_cells = n_cells;
     // ---- 1. the dense band coefficients (addFunction(func, pred), :806-817), on the device only
     DevBuf<double> d_dense;
     DG_CUDA(d_dense.alloc(n));
     if (int rc = dg_sample_sdf_band_device(m, grid, sign, band, 0, n, d_dense.p, st)) return rc;
     DG_CUDA(cudaStreamSynchronize(st));
-    ms[0] = lap();
-    // ---- 2. kept cells (:1081-1098): flags from the closed-form rows, cell map + the kept rows
-    const uint64_t tile = k4_tile();
-    uint64_t kept_cells = 0;
+    ms[0] = clock.lap();
+    // ---- 2.-5. reduceField(id, always true): a node is kept iff its coefficient is not DBL_MAX; rows from the closed form
+    const DenseRows rows{nullptr, n_cells};
+    int tie_path = 0;
     {
         DevBuf<unsigned char> d_cell_keep;
-        DevBuf<unsigned> d_tile;
-        DG_CUDA(d_cell_keep.alloc(n_cells)); DG_CUDA(d_tile.alloc((n_cells + tile - 1) / tile)); DG_CUDA(h->d_cell_map.alloc(n_cells));
-        DG_LAUNCH(k4_launch_band_cell_keep(g, d_dense.p, n_cells, d_cell_keep.p, st));
-        DG_LAUNCH(k4_scan_flags(d_cell_keep.p, n_cells, d_tile.p, kept_cells, st));
-        DG_CUDA(h->d_cells.alloc(32 * kept_cells));
-        DG_LAUNCH(k4_launch_band_cell_compact(g, n_cells, d_cell_keep.p, d_tile.p, h->d_cells.p, h->d_cell_map.p, st));
-        DG_CUDA(cudaStreamSynchronize(st));
+        if (int rc = device_cell_flags(g, d_dense.p, n, rows, K4ValuePred{K4_KEEP_ANY, 0.0, 0.0, 0.0}, d_cell_keep, who, st)) return rc;
+        if (int rc = device_reduce(g, d_dense.p, n, rows, d_cell_keep.p, n_cells, (flags & DG_REDUCE_REFERENCE_SORT) != 0, *h, ms + 1, tie_path, clock, st))
+            return rc;
     }
-    h->n_cells = kept_cells;
-    ms[1] = lap();
-    // ---- 3. surviving nodes = nodes of kept cells (:1117-1134), compacted by the reference's swap walk (:1135-1156) on the device
-    DevBuf<unsigned> d_walk;
-    uint64_t m_nodes = 0;
-    {
-        DevBuf<unsigned char> d_used;
-        DevBuf<unsigned> d_tile, d_flag;
-        DG_CUDA(d_used.alloc(n)); DG_CUDA(d_tile.alloc((n + tile - 1) / tile)); DG_CUDA(d_flag.alloc(1)); DG_CUDA(d_walk.alloc(n));
-        DG_CUDA(cudaMemsetAsync(d_used.p, 0, n, st));
-        DG_LAUNCH(k4_launch_mark_used(h->d_cells.p, 32 * kept_cells, d_used.p, st));
-        unsigned rounds = 0;
-        DG_LAUNCH(k4_swap_walk(d_used.p, n, d_tile.p, d_flag.p, d_walk.p, m_nodes, rounds, st));
-        DG_CUDA(cudaStreamSynchronize(st));
-    }
-    h->n_nodes = m_nodes;
-    ms[2] = lap();
-    // ---- 4. Z-curve keys in swap-walk position order on the device; their order on the host (std::sort's order among equal keys)
-    int tie_path = 0;
-    std::vector<uint32_t> order;
-    {
-        DevBuf<unsigned long long> d_key;
-        DG_CUDA(d_key.alloc(m_nodes));
-        DG_LAUNCH(k4_launch_morton_keys(g, d_walk.p, m_nodes, d_key.p, st));
-        std::vector<KeyPos> kp(m_nodes);
-        {
-            std::vector<unsigned long long> key(m_nodes);
-            if (m_nodes) DG_CUDA(cudaMemcpyAsync(key.data(), d_key.p, m_nodes * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-            DG_CUDA(cudaStreamSynchronize(st));
-            parallel_for(m_nodes, [&](uint64_t b0, uint64_t e0) { for (uint64_t i = b0; i < e0; i++) { kp[i].key = key[i]; kp[i].pos = (uint32_t)i; } });
-        }
-        reduce_order_survivors(kp, (flags & DG_REDUCE_REFERENCE_SORT) != 0, order, tie_path);
-    }
-    ms[3] = lap();
-    // ---- 5. new ids, renumbered rows, gathered coefficients (:1158-1173) into the handle's buffers
-    {
-        DevBuf<unsigned> d_order, d_new_id;
-        DG_CUDA(d_order.alloc(m_nodes)); DG_CUDA(d_new_id.alloc(n)); DG_CUDA(h->d_nodes.alloc(m_nodes));
-        if (m_nodes) DG_CUDA(cudaMemcpyAsync(d_order.p, order.data(), m_nodes * sizeof(unsigned), cudaMemcpyHostToDevice, st));
-        DG_LAUNCH(k4_launch_renumber(d_walk.p, d_order.p, m_nodes, d_dense.p, d_new_id.p, h->d_nodes.p, h->d_cells.p, 32 * kept_cells, st));
-        DG_CUDA(cudaStreamSynchronize(st));
-    }
-    ms[4] = lap();
     if (timings_ms) {
         for (int k = 0; k < 5; k++) timings_ms[k] = ms[k];
         timings_ms[5] = (double)tie_path;
         timings_ms[6] = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_start).count();
     }
     *out = h.release();
+    return DG_OK;
+}
+
+// GenerateDensityMap with reduction (cmd/generate_density_map/main.cpp:117-147) on one GPU: K3 on the uploaded SDF field, then reduceField
+// of the SDF field over its own rows and of the density field over the closed-form rows, each with the tool's predicate.
+static int reduced_density_map_create_impl(const dg_grid_desc* grid, const double* sdf_nodes, uint64_t n_nodes, const uint32_t* sdf_cells,
+                                           uint64_t n_cells, const uint32_t* sdf_cell_map, double h, double rho0, uint32_t flags,
+                                           dg_reduced_band** sdf_out, dg_reduced_band** density_out, double* timings_ms)
+{
+    static const char* who = "dg_reduced_density_map_create";
+    if (!sdf_out || !density_out) return fail(DG_ERR_INVALID, "%s: out is NULL", who);
+    *sdf_out = nullptr; *density_out = nullptr;
+    GridDev g; const char* why = "";
+    if (!grid_to_dev(grid, g, &why)) return fail(DG_ERR_INVALID, "%s: %s", who, why);     // refuses grids of 2^31 nodes or more
+    const uint64_t n = (uint64_t)g.nv + 2ull * ((uint64_t)g.ne_x + g.ne_y + g.ne_z);
+    const uint64_t n_grid_cells = (uint64_t)g.n[0] * g.n[1] * g.n[2];
+    if (!sdf_nodes || !sdf_cell_map || (n_cells && !sdf_cells)) return fail(DG_ERR_INVALID, "%s: NULL argument", who);
+    if (n_nodes != n)                     // node ids must be the grid's own numbering: their positions feed the Z-curve key (:1113)
+        return fail(DG_ERR_INVALID, "%s: the SDF field has %llu nodes, the grid %llu (already reduced?)", who, (unsigned long long)n_nodes,
+                    (unsigned long long)n);
+    if (n_cells > n_grid_cells) return fail(DG_ERR_INVALID, "%s: more cells than the grid has", who);
+    if (!(h > 0.0)) return fail(DG_ERR_INVALID, "%s: smoothing length must be > 0", who);
+    if (flags & ~DG_REDUCE_REFERENCE_SORT) return fail(DG_ERR_INVALID, "%s: unknown flags 0x%x (only DG_REDUCE_REFERENCE_SORT)", who, flags);
+    if (int rc = require_device()) return rc;
+    if (int rc = ensure_selftest()) return rc;
+    // the tool's predicates (main.cpp:139-140) with their bounds computed as its lambdas compute them
+    const double cell_diag = k3_cell_diag(g);
+    const K4ValuePred sdf_pred{K4_KEEP_SDF, -6.0 * h, 2.0 * h, cell_diag};
+    const K4ValuePred density_pred{K4_KEEP_RANGE, 0.0, 3.0 * rho0, 0.0};
+    const bool reference_sort = (flags & DG_REDUCE_REFERENCE_SORT) != 0;
+    StageClock clock;
+    const auto t_start = clock.t0;
+    const cudaStream_t st = nullptr;
+    double ms[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};       // upload + pack, density, field 0: 4 stages, field 1: 4 stages
+    int tie[2] = {0, 0};
+    std::unique_ptr<dg_reduced_band> r0(new dg_reduced_band()), r1(new dg_reduced_band());
+    DG_CUDA(cudaGetDevice(&r0->device));
+    r1->device = r0->device;
+    // ---- 1. upload the SDF field; flag the kept cells of its reduction (this checks the rows) and check the cell map before K2 packs
+    //         through them (dg_field_create's checks); pack the SDF field for K3
+    DevBuf<double> d_sdf, d_density;
+    DevBuf<unsigned> d_cells;
+    DevBuf<unsigned char> d_cell_keep0;
+    std::unique_ptr<dg_field> f(new dg_field());
+    f->desc = *grid; f->dev.g = g; f->n_nodes = n; f->n_cells_kept = n_cells;
+    DG_CUDA(d_sdf.alloc(n)); DG_CUDA(d_cells.alloc(32 * n_cells)); DG_CUDA(f->d_cell_map.alloc(n_grid_cells));
+    DG_CUDA(cudaMemcpyAsync(d_sdf.p, sdf_nodes, n * sizeof(double), cudaMemcpyHostToDevice, st));
+    if (n_cells) DG_CUDA(cudaMemcpyAsync(d_cells.p, sdf_cells, 32 * n_cells * sizeof(unsigned), cudaMemcpyHostToDevice, st));
+    DG_CUDA(cudaMemcpyAsync(f->d_cell_map.p, sdf_cell_map, n_grid_cells * sizeof(unsigned), cudaMemcpyHostToDevice, st));
+    DG_CUDA(cudaStreamSynchronize(st));
+    ms[0] = clock.lap();
+    if (int rc = device_cell_flags(g, d_sdf.p, n, DenseRows{d_cells.p, n_cells}, sdf_pred, d_cell_keep0, who, st)) return rc;
+    ms[2] = clock.lap();                                   // counted as field 0's kept cells
+    {
+        DevBuf<unsigned> d_bad;
+        unsigned bad = 0;
+        DG_CUDA(d_bad.alloc(1));
+        DG_CUDA(cudaMemsetAsync(d_bad.p, 0, sizeof(unsigned), st));
+        DG_LAUNCH(k4_launch_cell_map_check(f->d_cell_map.p, n_grid_cells, n_cells, d_bad.p, st));
+        DG_CUDA(cudaMemcpyAsync(&bad, d_bad.p, sizeof bad, cudaMemcpyDeviceToHost, st));
+        DG_CUDA(cudaStreamSynchronize(st));
+        if (bad) return fail(DG_ERR_INVALID, "%s: a cell_map entry is >= n_cells", who);
+    }
+    if (int rc = field_finish(f.get(), d_sdf.p, d_cells.p, st)) return rc;
+    DG_CUDA(cudaStreamSynchronize(st));
+    ms[0] += clock.lap();
+    // ---- 2. addFunction(density_func, verbose, pred) (main.cpp:96-133): K3 over every node, predicate on
+    DG_CUDA(d_density.alloc(n));
+    DG_LAUNCH(k3_launch_density(f->dev, h, rho0, 0, 0, n, d_density.p, st));
+    DG_CUDA(cudaStreamSynchronize(st));
+    ms[1] = clock.lap();
+    // ---- 3. the packed SDF field is not needed any more: free it before reducing anything
+    f.reset();
+    // ---- 4. reduceField(0, -6h < v + cell_diag && v - cell_diag < 2h) over the SDF field's own rows
+    if (int rc = device_reduce(g, d_sdf.p, n, DenseRows{d_cells.p, n_cells}, d_cell_keep0.p, n_grid_cells, reference_sort, *r0, ms + 2, tie[0], clock, st))
+        return rc;
+    d_cell_keep0.release(); d_cells.release(); d_sdf.release();
+    // ---- 5. reduceField(1, 0 <= v && v <= 3 rho0) over the closed-form rows of the density field (addSampledFunction's cells, identity map)
+    {
+        const DenseRows rows1{nullptr, n_grid_cells};
+        DevBuf<unsigned char> d_cell_keep1;
+        if (int rc = device_cell_flags(g, d_density.p, n, rows1, density_pred, d_cell_keep1, who, st)) return rc;
+        if (int rc = device_reduce(g, d_density.p, n, rows1, d_cell_keep1.p, n_grid_cells, reference_sort, *r1, ms + 6, tie[1], clock, st)) return rc;
+    }
+    if (timings_ms) {
+        for (int k = 0; k < 10; k++) timings_ms[k] = ms[k];
+        timings_ms[10] = (double)tie[0]; timings_ms[11] = (double)tie[1];
+        timings_ms[12] = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_start).count();
+    }
+    *sdf_out = r0.release(); *density_out = r1.release();
     return DG_OK;
 }
 
@@ -1784,6 +1938,15 @@ int dg_reduce_field(const dg_grid_desc* grid, double* nodes, uint64_t n_nodes, c
 int dg_reduced_band_create(const dg_mesh* m, const dg_grid_desc* grid, double sign, double band, uint32_t flags, dg_reduced_band** out, double* timings_ms)
 {
     return guarded("dg_reduced_band_create", [&]() { return reduced_band_create_impl(m, grid, sign, band, flags, out, timings_ms); });
+}
+
+int dg_reduced_density_map_create(const dg_grid_desc* grid, const double* sdf_nodes, uint64_t n_nodes, const uint32_t* sdf_cells, uint64_t n_cells,
+                                  const uint32_t* sdf_cell_map, double h, double rho0, uint32_t flags, dg_reduced_band** sdf_out,
+                                  dg_reduced_band** density_out, double* timings_ms)
+{
+    return guarded("dg_reduced_density_map_create", [&]() {
+        return reduced_density_map_create_impl(grid, sdf_nodes, n_nodes, sdf_cells, n_cells, sdf_cell_map, h, rho0, flags, sdf_out, density_out, timings_ms);
+    });
 }
 
 }  // extern "C"

@@ -173,6 +173,13 @@ density_map_kernel(FieldDev f, QuadParams qp, const double* __restrict__ Wtab, i
 
 // Host tables.  This TU is compiled without FP contraction on the host side as well (x86-64 baseline has no FMA;
 // -ffp-contract=off is passed explicitly), so these match the reference's CPU arithmetic bit for bit.
+
+// cell_diag = cellSize().norm(); Eigen >= 3.3 reduces a Vector3d as (a0 + a1) + a2 (main.cpp:117)
+double k3_cell_diag(const GridDev& g)
+{
+    return std::sqrt((g.cell[0] * g.cell[0] + g.cell[1] * g.cell[1]) + g.cell[2] * g.cell[2]);
+}
+
 cudaError_t k3_launch_density(const FieldDev& f, double h, double rho0, int no_reduction, uint64_t l_begin, uint64_t count,
                               double* d_out, cudaStream_t stream)
 {
@@ -187,8 +194,7 @@ cudaError_t k3_launch_density(const FieldDev& f, double h, double rho0, int no_r
     qp.inv_h = 1.0 / h;
 #endif
     qp.c0prod = c0 * c0 * c0;                                        // Eigen prod(): (c0*c0)*c0
-    // cell_diag = cellSize().norm(); Eigen >= 3.3 reduces a Vector3d as (a0 + a1) + a2 (main.cpp:117)
-    qp.cell_diag = std::sqrt((f.g.cell[0] * f.g.cell[0] + f.g.cell[1] * f.g.cell[1]) + f.g.cell[2] * f.g.cell[2]);
+    qp.cell_diag = k3_cell_diag(f.g);
     // W at the 4096 points (sph_kernel.hpp:10-42): k = 8/(pi h^3)
     const double pi = static_cast<double>(M_PI);
     const double h3 = h * h * h;

@@ -5,6 +5,8 @@
 #include "k2_interp.h"
 
 namespace dgb {
+// GenerateDensityMap's cell_diag = cellSize().norm() (main.cpp:117): the value K3's predicate uses, and the SDF field's reduceField with it
+double k3_cell_diag(const GridDev& g);
 cudaError_t k3_launch_density(const FieldDev& f, double h, double rho0, int no_reduction, uint64_t l_begin, uint64_t count,
                               double* d_out, cudaStream_t stream);
 }

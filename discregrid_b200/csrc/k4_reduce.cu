@@ -8,13 +8,15 @@
 //                  coefficients (:1158-1173)
 //   host (reduce_field.cpp): the reference's back-to-front swap compaction replayed on a permutation array (:1135-1156, O(n), inherently
 //                  serial) and the sort of the survivors by key, whose order among EQUAL keys is libstdc++'s introsort's (reduce_field.h).
-// The reduced narrow band (dg_reduced_band_create) runs the same passes on the device only: cell flags and rows from the closed form instead
-// of a cell table, and the swap walk itself as pointer jumping (swap_walk_*); the sort of the survivors stays on the host.
+// The reduced narrow band (dg_reduced_band_create) and the reduced density map (dg_reduced_density_map_create) run the same passes on the
+// device only: keep flags from a value predicate, cell flags and rows from an uploaded table or from the closed form instead of a cell
+// table, and the swap walk itself as pointer jumping (swap_walk_*); the sort of the survivors stays on the host.
 // All kernels are warp-synchronous (ballot / popc), so tests/emu runs them unchanged.  Integer work, bit-exact by construction; the one
 // floating-point step (the key's cast of inv * x) uses the reference's operations in the reference's order (no FMA: -fmad=false).
 #include "k4_reduce.h"
 #include "dg_launch.h"
 
+#include <cfloat>
 #include <climits>
 #include <vector>
 
@@ -134,10 +136,27 @@ __global__ void renumber_cells_kernel(unsigned* __restrict__ cells_out, unsigned
     if (i < n_entries) cells_out[i] = new_id[cells_out[i]];
 }
 
-// ---- the reduced narrow band (dg_reduced_band_create): the same passes on the dense band coefficients, with the rows of the cells taken
-// from the closed form (cell_node_id) instead of a 32-index table of the whole grid.  A node is kept iff its coefficient is not DBL_MAX
-// (:1073, bit for bit; the predicate is "always true").
-constexpr unsigned long long DBL_MAX_BITS = 0x7fefffffffffffffull;
+// ---- reduction on the device only (dg_reduced_band_create, dg_reduced_density_map_create): the same passes on a dense field whose keep
+// flags come from a value predicate (K4ValuePred), with the rows of the cells either uploaded or taken from the closed form (cell_node_id)
+// instead of a 32-index table of the whole grid.
+
+// pred(x, v) && v != DBL_MAX (:1069-1074) for the predicates that depend on v alone, in the expression order of the reference's tool:
+// v + c and v - c are rounded first, then compared with the bounds as given (no rearranged bounds)
+template <int KIND>
+__device__ __forceinline__ bool value_kept(const K4ValuePred& p, double v)
+{
+    if (KIND == K4_KEEP_SDF) return (p.a < v + p.c && v - p.c < p.b) && v != DBL_MAX;
+    if (KIND == K4_KEEP_RANGE) return (p.a <= v && v <= p.b) && v != DBL_MAX;
+    return v != DBL_MAX;
+}
+
+// keep flag per node of a dense field (for rows read through cell_keep_kernel)
+template <int KIND>
+__global__ void node_keep_kernel(const double* __restrict__ nodes, unsigned long long n, K4ValuePred p, unsigned char* __restrict__ keep)
+{
+    const unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) keep[i] = value_kept<KIND>(p, __ldg(nodes + i)) ? 1 : 0;
+}
 
 __device__ __forceinline__ void cell_ijk(const GridDev& g, unsigned long long c, unsigned& i, unsigned& j, unsigned& k)
 {
@@ -147,8 +166,10 @@ __device__ __forceinline__ void cell_ijk(const GridDev& g, unsigned long long c,
     j = t / g.n[0]; i = t - j * g.n[0];
 }
 
-// keep flag per cell: one warp per cell, lane j reads the coefficient of the cell's closed-form node j
-__global__ void band_cell_keep_kernel(GridDev g, const double* __restrict__ nodes, unsigned long long n_cells, unsigned char* __restrict__ cell_keep)
+// keep flag per cell: one warp per cell, lane j applies the predicate to the coefficient of the cell's closed-form node j
+template <int KIND>
+__global__ void closed_cell_keep_kernel(GridDev g, const double* __restrict__ nodes, unsigned long long n_cells, K4ValuePred p,
+                                        unsigned char* __restrict__ cell_keep)
 {
     const unsigned long long c = ((unsigned long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const unsigned lane = threadIdx.x & 31u;
@@ -157,15 +178,31 @@ __global__ void band_cell_keep_kernel(GridDev g, const double* __restrict__ node
     if (live) {
         unsigned i, j, k;
         cell_ijk(g, c, i, j, k);
-        kept = (unsigned long long)__double_as_longlong(__ldg(nodes + cell_node_id(g, i, j, k, lane))) != DBL_MAX_BITS;
+        kept = value_kept<KIND>(p, __ldg(nodes + cell_node_id(g, i, j, k, lane)));
     }
     const unsigned any = __ballot_sync(0xffffffffu, kept);
     if (live && lane == 0) cell_keep[c] = any ? 1 : 0;
 }
 
+// bad[0] += 1 per warp that sees a cell map entry that is neither 0xffffffff nor a row id < n_rows
+__global__ void cell_map_check_kernel(const unsigned* __restrict__ cell_map, unsigned long long n, unsigned long long n_rows, unsigned* __restrict__ bad)
+{
+    const unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+    bool b = false;
+    if (i < n) { const unsigned v = cell_map[i]; b = v != 0xffffffffu && v >= n_rows; }
+    if (__ballot_sync(0xffffffffu, b) && (threadIdx.x & 31u) == 0) atomicAdd(bad, 1u);
+}
+
+// cell_map[i] = i on [begin, end): the reference's resize + iota (:1076-1078) for cells a field never had rows for
+__global__ void iota_kernel(unsigned* __restrict__ out, unsigned long long begin, unsigned long long end)
+{
+    const unsigned long long i = begin + (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < end) out[i] = (unsigned)i;
+}
+
 // cell_map and the closed-form rows of the kept cells, order kept: cell_compact_kernel with the rows computed instead of copied
-__global__ void band_cell_compact_kernel(GridDev g, unsigned long long n_cells, const unsigned char* __restrict__ cell_keep,
-                                         const unsigned* __restrict__ tile_offset, unsigned* __restrict__ cells_out, unsigned* __restrict__ cell_map)
+__global__ void closed_cell_compact_kernel(GridDev g, unsigned long long n_cells, const unsigned char* __restrict__ cell_keep,
+                                           const unsigned* __restrict__ tile_offset, unsigned* __restrict__ cells_out, unsigned* __restrict__ cell_map)
 {
     const unsigned long long tile = ((unsigned long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const unsigned lane = threadIdx.x & 31u;
@@ -288,20 +325,55 @@ cudaError_t k4_launch_renumber(const unsigned* d_perm, const unsigned* d_order, 
     return DG_AFTER_LAUNCH();
 }
 
-cudaError_t k4_launch_band_cell_keep(const GridDev& g, const double* d_nodes, uint64_t n_cells, unsigned char* d_cell_keep, cudaStream_t stream)
+cudaError_t k4_launch_node_keep(const double* d_nodes, uint64_t n, const K4ValuePred& p, unsigned char* d_keep, cudaStream_t stream)
 {
-    if (n_cells == 0) return cudaSuccess;
-    DG_KERNEL_LAUNCH(band_cell_keep_kernel, blocks_for(n_cells * 32ull, 128), 128, 0, stream, g, d_nodes, (unsigned long long)n_cells, d_cell_keep);
+    if (n == 0) return cudaSuccess;
+    const unsigned blocks = blocks_for(n, 256);
+    switch (p.kind) {
+    case K4_KEEP_ANY: DG_KERNEL_LAUNCH(node_keep_kernel<K4_KEEP_ANY>, blocks, 256, 0, stream, d_nodes, (unsigned long long)n, p, d_keep); break;
+    case K4_KEEP_SDF: DG_KERNEL_LAUNCH(node_keep_kernel<K4_KEEP_SDF>, blocks, 256, 0, stream, d_nodes, (unsigned long long)n, p, d_keep); break;
+    case K4_KEEP_RANGE: DG_KERNEL_LAUNCH(node_keep_kernel<K4_KEEP_RANGE>, blocks, 256, 0, stream, d_nodes, (unsigned long long)n, p, d_keep); break;
+    default: return cudaErrorInvalidValue;
+    }
     return DG_AFTER_LAUNCH();
 }
 
-cudaError_t k4_launch_band_cell_compact(const GridDev& g, uint64_t n_cells, const unsigned char* d_cell_keep, const unsigned* d_tile_offset,
-                                        unsigned* d_cells_out, unsigned* d_cell_map, cudaStream_t stream)
+cudaError_t k4_launch_closed_cell_keep(const GridDev& g, const double* d_nodes, uint64_t n_cells, const K4ValuePred& p, unsigned char* d_cell_keep,
+                                       cudaStream_t stream)
+{
+    if (n_cells == 0) return cudaSuccess;
+    const unsigned blocks = blocks_for(n_cells * 32ull, 128);
+    const unsigned long long nc = n_cells;
+    switch (p.kind) {
+    case K4_KEEP_ANY: DG_KERNEL_LAUNCH(closed_cell_keep_kernel<K4_KEEP_ANY>, blocks, 128, 0, stream, g, d_nodes, nc, p, d_cell_keep); break;
+    case K4_KEEP_SDF: DG_KERNEL_LAUNCH(closed_cell_keep_kernel<K4_KEEP_SDF>, blocks, 128, 0, stream, g, d_nodes, nc, p, d_cell_keep); break;
+    case K4_KEEP_RANGE: DG_KERNEL_LAUNCH(closed_cell_keep_kernel<K4_KEEP_RANGE>, blocks, 128, 0, stream, g, d_nodes, nc, p, d_cell_keep); break;
+    default: return cudaErrorInvalidValue;
+    }
+    return DG_AFTER_LAUNCH();
+}
+
+cudaError_t k4_launch_closed_cell_compact(const GridDev& g, uint64_t n_cells, const unsigned char* d_cell_keep, const unsigned* d_tile_offset,
+                                          unsigned* d_cells_out, unsigned* d_cell_map, cudaStream_t stream)
 {
     if (n_cells == 0) return cudaSuccess;
     const uint64_t tiles = (n_cells + TILE - 1) / TILE;
-    DG_KERNEL_LAUNCH(band_cell_compact_kernel, blocks_for(tiles * 32ull, 128), 128, 0, stream, g, (unsigned long long)n_cells, d_cell_keep, d_tile_offset,
+    DG_KERNEL_LAUNCH(closed_cell_compact_kernel, blocks_for(tiles * 32ull, 128), 128, 0, stream, g, (unsigned long long)n_cells, d_cell_keep, d_tile_offset,
                      d_cells_out, d_cell_map);
+    return DG_AFTER_LAUNCH();
+}
+
+cudaError_t k4_launch_cell_map_check(const unsigned* d_cell_map, uint64_t n, uint64_t n_rows, unsigned* d_bad, cudaStream_t stream)
+{
+    if (n == 0) return cudaSuccess;
+    DG_KERNEL_LAUNCH(cell_map_check_kernel, blocks_for(n, 256), 256, 0, stream, d_cell_map, (unsigned long long)n, (unsigned long long)n_rows, d_bad);
+    return DG_AFTER_LAUNCH();
+}
+
+cudaError_t k4_launch_iota(unsigned* d_out, uint64_t begin, uint64_t end, cudaStream_t stream)
+{
+    if (end <= begin) return cudaSuccess;
+    DG_KERNEL_LAUNCH(iota_kernel, blocks_for(end - begin, 256), 256, 0, stream, d_out, (unsigned long long)begin, (unsigned long long)end);
     return DG_AFTER_LAUNCH();
 }
 

@@ -11,6 +11,8 @@ that save()/load() stay byte-compatible with the reference's .cdf/.cdm files
   addReducedBandField(MeshSignedDistance, MeshDistanceBand)
                                          -> dg_reduced_band_create (the same band, then reduceField(always true), all on the GPU)
   addFunction(DensityMapFunction, pred)  -> dg_density_map       (K3, csrc/k3_density.cu)
+  addReducedDensityMap(DensityMapFunction)
+                                         -> dg_reduced_density_map_create (K3, then both of GenerateDensityMap's reduceField calls, on the GPU)
   interpolate(field_id, x[, gradient])   -> dg_interpolate_batch (K2, csrc/k2_interp.cu), batched over x
 
 The reference's addFunction takes an opaque std::function; only the two functor types the reference's own tools
@@ -177,6 +179,43 @@ class CubicLagrangeDiscreteGrid:
         if verbose:
             print(f"Construction: {len(coeffs)} of {self.nNodes()} nodes kept in {self.last_reduced_band_ms[6]:.1f} ms on the GPU")
         self.m_nodes.append(coeffs); self.m_cells.append(cells); self.m_cell_map.append(cmap)
+        self.m_n_fields += 1
+        return self.m_n_fields - 1
+
+    def addReducedDensityMap(self, func):
+        """GenerateDensityMap with reduction in one GPU call (dg_reduced_density_map_create): leaves exactly what
+        addFunction(func) followed by reduceField(func.field_id, p0) and reduceField(new_id, p1) leave, with the tool's predicates
+        p0(x, v) = -6h < v + cell_diag & v - cell_diag < 2h and p1(x, v) = 0 <= v <= 3 rho0 (main.cpp:139-140).  The SDF field is replaced by
+        its reduction and the reduced density field is appended; the dense density field never reaches the host.  Returns the new field id."""
+        if not isinstance(func, DensityMapFunction):
+            raise TypeError("addReducedDensityMap takes a DensityMapFunction")
+        if func.no_reduction:
+            raise TypeError("addReducedDensityMap: the DensityMapFunction has no_reduction set (use addFunction)")
+        fid = func.field_id
+        nodes = np.ascontiguousarray(self.m_nodes[fid], np.float64)
+        cells = np.ascontiguousarray(self.m_cells[fid], np.uint32)
+        cmap = np.ascontiguousarray(self.m_cell_map[fid], np.uint32)
+        if len(cmap) != self.m_n_cells:
+            raise ValueError("addReducedDensityMap: the SDF field's cell map must cover every grid cell")
+        r = (C.c_void_p(), C.c_void_p())
+        self.last_reduced_density_ms = np.zeros(13)
+        capi.check(capi.lib.dg_reduced_density_map_create(C.byref(self._desc), capi.ptr(nodes, capi.F64P), len(nodes), capi.ptr(cells, capi.U32P),
+                                                          len(cells), capi.ptr(cmap, capi.U32P), func.h, func.rho0, 0, C.byref(r[0]), C.byref(r[1]),
+                                                          capi.ptr(self.last_reduced_density_ms, capi.F64P)))
+        out = []
+        try:
+            for h in r:
+                n_nodes, n_cells = C.c_uint64(), C.c_uint64()
+                capi.check(capi.lib.dg_reduced_band_sizes(h, C.byref(n_nodes), C.byref(n_cells)))
+                f = (np.empty(n_nodes.value), np.empty((n_cells.value, 32), np.uint32), np.empty(self.m_n_cells, np.uint32))
+                capi.check(capi.lib.dg_reduced_band_copy(h, capi.ptr(f[0], capi.F64P), capi.ptr(f[1], capi.U32P), capi.ptr(f[2], capi.U32P)))
+                out.append(f)
+        finally:
+            for h in r:
+                capi.lib.dg_reduced_band_destroy(h)
+        self._invalidate()
+        self.m_nodes[fid], self.m_cells[fid], self.m_cell_map[fid] = out[0]
+        self.m_nodes.append(out[1][0]); self.m_cells.append(out[1][1]); self.m_cell_map.append(out[1][2])
         self.m_n_fields += 1
         return self.m_n_fields - 1
 

@@ -280,13 +280,37 @@ DG_API int dg_reduce_field(const dg_grid_desc* grid, double* nodes, uint64_t n_n
  *   timings_ms: NULL or 7 doubles = ms of band sampling, kept cells, node compaction, sort, write-back; 1.0 if surviving nodes shared
  *       Morton keys (dg_reduce_field's tie path); total ms.  Every stage ends with a device synchronise.
  *   dg_reduced_band_copy: nodes[n_nodes], cells[n_cells x 32], cell_map[nx*ny*nz] (0xffffffff = removed cell); nodes / cells may be NULL
- *       only when their count is 0. */
+ *       only when their count is 0.
+ * dg_reduced_band: a reduced field kept on its device (also returned by dg_reduced_density_map_create). */
 typedef struct dg_reduced_band dg_reduced_band;
 DG_API int dg_reduced_band_create(const dg_mesh* mesh, const dg_grid_desc* grid, double sign, double band, uint32_t flags,
                            dg_reduced_band** out, double* timings_ms);
 DG_API int dg_reduced_band_sizes(const dg_reduced_band* result, uint64_t* n_nodes, uint64_t* n_cells);
 DG_API int dg_reduced_band_copy(const dg_reduced_band* result, double* nodes, uint32_t* cells, uint32_t* cell_map);
 DG_API int dg_reduced_band_destroy(dg_reduced_band* result);
+
+/* ---- reduced density map: GenerateDensityMap with reduction in one call -----------------------------------------------------------
+ * GenerateDensityMap with reduction (cmd/generate_density_map/main.cpp:117-147) in one call:
+ *   id = addFunction(density_func, verbose, pred);  reduceField(0, p0);  reduceField(id, p1);
+ * on the SDF field (sdf_nodes, sdf_cells, sdf_cell_map) of `grid`, with
+ *   p0(x, v) = -6h < v + cell_diag && v - cell_diag < 2h,   p1(x, v) = 0 <= v && v <= 3 rho0,   cell_diag = cellSize().norm().
+ * The two handles hold exactly what those calls leave, bit for bit what dg_density_map (no_reduction = 0), dg_build_cells + identity map
+ * and dg_reduce_field on each field give: *sdf_out the reduced SDF field, *density_out the reduced density field, each with its nodes in
+ * the reference's Z-curve order (including the order among equal keys), renumbered cells and cell map.  Read them with
+ * dg_reduced_band_sizes / _copy, free them with dg_reduced_band_destroy.  Every array the size of the grid stays on the current device;
+ * the packed SDF field that K3 reads is freed before the reductions start.  One GPU.
+ *   sdf_nodes: n_nodes = the grid's node count (a field that is already reduced: DG_ERR_INVALID, as dg_reduce_field).
+ *   sdf_cells: n_cells <= nx*ny*nz rows of 32 node ids (an id >= n_nodes: DG_ERR_INVALID); sdf_cell_map: nx*ny*nz entries, each
+ *       0xffffffff or < n_cells.  When n_cells < nx*ny*nz the reduced SDF cell map holds i at every i >= n_cells, as reduceField leaves it.
+ *   h: > 0 (NaN refused, as dg_density_map).  flags: 0 or DG_REDUCE_REFERENCE_SORT.  Grids of 2^31 nodes or more are refused before
+ *       anything is allocated.
+ *   timings_ms: NULL or 13 doubles = ms of upload + pack; density sampling; for field 0 then field 1: kept cells, node compaction, sort,
+ *       write-back; the tie flags of field 0 and field 1 (1.0 when survivors shared Morton keys); total ms.  Every stage ends with a device
+ *       synchronise; field 0's cell flags, computed before packing because they check the rows, count as its kept cells. */
+DG_API int dg_reduced_density_map_create(const dg_grid_desc* grid, const double* sdf_nodes, uint64_t n_nodes,
+                                         const uint32_t* sdf_cells, uint64_t n_cells, const uint32_t* sdf_cell_map,
+                                         double h, double rho0, uint32_t flags,
+                                         dg_reduced_band** sdf_out, dg_reduced_band** density_out, double* timings_ms);
 
 #ifdef __cplusplus
 }
