@@ -8,6 +8,11 @@
 //                                            -> dg_reduced_band_create (the same band + reduceField(always true), on the GPU)
 //   addFunction(DensityMapFunction)          -> dg_density_map  (K3)   (GenerateDensityMap's functor + predicate)
 //   addReducedDensityMap(DensityMapFunction) -> dg_reduced_density_map_create (K3 + both of GenerateDensityMap's reduceField calls, on the GPU)
+//   addFunction(DeviceFunction, verbose, DeviceSamplePredicate)
+//                                            -> dg_add_function_device (the caller's own GPU code on batches of node positions)
+//   reduceField(field, DeviceNodePredicate)  -> dg_reduce_field_device (the caller's predicate on the GPU, reduceField's passes there)
+//   addReducedFunction(DeviceFunction, DeviceSamplePredicate*, DeviceNodePredicate*)
+//                                            -> dg_reduced_function_create (both calls in one, the dense field kept on the GPU)
 //   interpolate(field, x, grad*)             -> dg_interpolate_batch (K2), also batched: interpolate(field, n, x, phi, grad)
 //   connectivity table of addFunction        -> dg_build_cells  (GPU)  replaces the serial loop :833-886
 //
@@ -16,13 +21,16 @@
 // Device copies of fields are caches owned by this object, dropped by addFunction / load / reduceField.
 //
 // addFunction takes the reference's opaque std::function.  Functors of the two types the reference's own tools build are
-// recognised with std::function::target<>() and run on the GPU.  Any other callable cannot run on a GPU: it throws
+// recognised with std::function::target<>() and run on the GPU, and so are DeviceFunction / DeviceSamplePredicate /
+// DeviceNodePredicate, which carry the caller's own GPU code in batched form.  Any other callable cannot run on a GPU: it throws
 // std::invalid_argument unless DISCREGRID_B200_ALLOW_HOST_CALLBACK is defined, in which case YOUR callback is invoked
 // once per node on the host (node positions still come from the GPU); that path is never part of any reported number.
 #pragma once
 #include <algorithm>
 #include <cstdint>
 #include <cstring>
+#include <exception>
+#include <functional>
 #include <iostream>
 #include <limits>
 #include <map>
@@ -65,6 +73,57 @@ struct DensityMapFunction {
     bool no_reduction;
     double operator()(Eigen::Vector3d const&) const { throw std::logic_error("DensityMapFunction is evaluated by addFunction on the GPU"); }
 };
+
+// The caller's own GPU code as recognisable types (include/discregrid_b200.h, dg_device_function & co.): f is called once per chunk of node
+// ids, in ascending order, on the calling thread, with device pointers (positions d_x: n x 3; masks: n bytes, nonzero = keep) and the
+// cudaStream_t the library works on (as void*); it enqueues its work there or finishes it before returning, and returns 0 (nonzero aborts
+// the call; an exception it throws is rethrown by the grid method).  The reference-signature call operators only exist so that the types
+// convert to ContinuousFunction / SamplePredicate / Predicate; they throw.
+struct DeviceFunction {
+    std::function<int(const double* d_x, const std::uint8_t* d_sample_keep, std::uint64_t n, double* d_values, void* stream)> f;
+    double operator()(Eigen::Vector3d const&) const { throw std::logic_error("DeviceFunction is evaluated in batches on the GPU by addFunction"); }
+};
+struct DeviceSamplePredicate {
+    std::function<int(const double* d_x, std::uint64_t n, std::uint8_t* d_keep, void* stream)> f;
+    bool operator()(Eigen::Vector3d const&) const { throw std::logic_error("DeviceSamplePredicate is evaluated in batches on the GPU by addFunction"); }
+};
+struct DeviceNodePredicate {
+    std::function<int(const double* d_x, const double* d_values, std::uint64_t n, std::uint8_t* d_keep, void* stream)> f;
+    bool operator()(Eigen::Vector3d const&, double) const { throw std::logic_error("DeviceNodePredicate is evaluated in batches on the GPU by reduceField"); }
+};
+
+namespace detail {
+// C trampolines for the device callbacks: an exception thrown by a callback is kept and the call aborted (nonzero)
+struct DeviceCallbackContext {
+    DeviceFunction const* func = nullptr;
+    DeviceSamplePredicate const* sample = nullptr;
+    DeviceNodePredicate const* node = nullptr;
+    std::exception_ptr error;
+    template <class F> int run(F&& f)
+    {
+        try { return f(); } catch (...) { error = std::current_exception(); return -1; }
+    }
+    static int func_cb(void* u, const double* x, const std::uint8_t* keep, std::uint64_t n, double* v, void* s)
+    {
+        auto* c = static_cast<DeviceCallbackContext*>(u);
+        return c->run([&] { return c->func->f(x, keep, n, v, s); });
+    }
+    static int sample_cb(void* u, const double* x, std::uint64_t n, std::uint8_t* keep, void* s)
+    {
+        auto* c = static_cast<DeviceCallbackContext*>(u);
+        return c->run([&] { return c->sample->f(x, n, keep, s); });
+    }
+    static int node_cb(void* u, const double* x, const double* v, std::uint64_t n, std::uint8_t* keep, void* s)
+    {
+        auto* c = static_cast<DeviceCallbackContext*>(u);
+        return c->run([&] { return c->node->f(x, v, n, keep, s); });
+    }
+    dg_device_function func_ptr() const { return func ? &func_cb : nullptr; }
+    dg_device_sample_predicate sample_ptr() const { return sample ? &sample_cb : nullptr; }
+    dg_device_node_predicate node_ptr() const { return node ? &node_cb : nullptr; }
+    void rethrow() const { if (error) std::rethrow_exception(error); }
+};
+}  // namespace detail
 
 class CubicLagrangeDiscreteGrid : public DiscreteGrid {
 public:
@@ -112,6 +171,27 @@ public:
         const dg_grid_desc d = desc();
         std::uint64_t n_nodes = 0;
         check(dg_grid_num_nodes(d.resolution, &n_nodes));
+        auto const* dev_func = func.target<DeviceFunction>();
+        auto const* dev_pred = pred ? pred.target<DeviceSamplePredicate>() : nullptr;
+        if (dev_func || dev_pred) {
+            if (!dev_func || (pred && !dev_pred))
+                throw std::invalid_argument("addFunction: a DeviceFunction takes a DeviceSamplePredicate (or none), and a DeviceSamplePredicate only goes "
+                                            "with a DeviceFunction");
+            // the whole of :780-899 in one library call: the caller's code on the GPU, connectivity + cell map by the library's host threads
+            FieldVector<double> coeffs(n_nodes);
+            FieldVector<std::array<unsigned int, 32>> cells(m_n_cells);
+            FieldVector<unsigned int> cell_map(m_n_cells);
+            detail::DeviceCallbackContext ctx;
+            ctx.func = dev_func; ctx.sample = dev_pred;
+            const int rc = dg_add_function_device(&d, ctx.func_ptr(), &ctx, ctx.sample_ptr(), &ctx, 0, coeffs.data(),
+                                                  reinterpret_cast<std::uint32_t*>(cells.data()), cell_map.data(), m_last_add_function_ms);
+            ctx.rethrow();
+            check(rc);
+            if (verbose) std::cout << "Construction: " << n_nodes << " nodes sampled on the GPU in " << m_last_add_function_ms[0] << " ms" << std::endl;
+            invalidate();
+            m_nodes.push_back(std::move(coeffs)); m_cells.push_back(std::move(cells)); m_cell_map.push_back(std::move(cell_map));
+            return static_cast<unsigned int>(m_n_fields++);
+        }
         if (auto const* sdf = func.target<MeshSignedDistanceFunction>()) {
             auto const* band = pred ? pred.target<MeshDistanceBandPredicate>() : nullptr;
             if (pred && !band)
@@ -180,6 +260,26 @@ public:
         FieldVector<unsigned int> cell_map(m_n_cells);
         check(dg_reduced_band_copy(r, coeffs.data(), reinterpret_cast<std::uint32_t*>(cells.data()), cell_map.data()));
         if (verbose) std::cout << "Construction: " << n_nodes << " nodes kept, " << n_cells << " cells, on the GPU in " << m_last_reduced_band_ms[6] << " ms" << std::endl;
+        invalidate();
+        m_nodes.push_back(std::move(coeffs)); m_cells.push_back(std::move(cells)); m_cell_map.push_back(std::move(cell_map));
+        return static_cast<unsigned int>(m_n_fields++);
+    }
+    // new: addFunction(func, verbose, sample) followed by reduceField(id, reduce) in one library call (dg_reduced_function_create); sample /
+    // reduce may be nullptr (every node sampled / always true).  The field holds exactly what those two calls leave; the dense field stays
+    // on the GPU, only the survivors and the cell map reach the host.  Returns the new field id.
+    unsigned int addReducedFunction(DeviceFunction const& func, DeviceSamplePredicate const* sample = nullptr, DeviceNodePredicate const* reduce = nullptr,
+                                    bool verbose = false)
+    {
+        const dg_grid_desc d = desc();
+        detail::DeviceCallbackContext ctx;
+        ctx.func = &func; ctx.sample = sample; ctx.node = reduce;
+        dg_reduced_band* r = nullptr;
+        const int rc = dg_reduced_function_create(&d, ctx.func_ptr(), &ctx, ctx.sample_ptr(), &ctx, ctx.node_ptr(), &ctx, 0, 0u, &r, m_last_reduced_function_ms);
+        ctx.rethrow();
+        check(rc);
+        FieldVector<double> coeffs; FieldVector<std::array<unsigned int, 32>> cells; FieldVector<unsigned int> cell_map;
+        take_reduced(r, coeffs, cells, cell_map);
+        if (verbose) std::cout << "Construction: " << coeffs.size() << " nodes kept, " << cells.size() << " cells, in " << m_last_reduced_function_ms[6] << " ms" << std::endl;
         invalidate();
         m_nodes.push_back(std::move(coeffs)); m_cells.push_back(std::move(cells)); m_cell_map.push_back(std::move(cell_map));
         return static_cast<unsigned int>(m_n_fields++);
@@ -312,6 +412,9 @@ public:
     const double* lastReducedBandTimings() const { return m_last_reduced_band_ms; }
     // ms of the last addReducedDensityMap: upload + pack, density; cells, nodes, sort, write-back of field 0 then of field 1; tie paths; total
     const double* lastReducedDensityTimings() const { return m_last_reduced_density_ms; }
+    // ms of the last addReducedFunction / reduceField(DeviceNodePredicate): positions + callbacks (reduceField: with the upload), cells, nodes,
+    // sort, write-back; tie path (1.0 / 0.0); total; inside the callbacks
+    const double* lastReducedFunctionTimings() const { return m_last_reduced_function_ms; }
     std::size_t nFields() const { return m_n_fields; }
     dg_grid_desc desc() const
     {
@@ -339,7 +442,18 @@ private:
     double m_last_add_function_ms[6] = {0, 0, 0, 0, 0, 0};
     double m_last_reduced_band_ms[7] = {0, 0, 0, 0, 0, 0, 0};
     double m_last_reduced_density_ms[13] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+    double m_last_reduced_function_ms[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     mutable std::map<unsigned int, dg_field*> m_dev;
+
+    // the arrays of a dg_reduced_band handle, which is destroyed
+    void take_reduced(dg_reduced_band* r, FieldVector<double>& coeffs, FieldVector<std::array<unsigned int, 32>>& cells, FieldVector<unsigned int>& cell_map) const
+    {
+        struct Release { dg_reduced_band* r; ~Release() { dg_reduced_band_destroy(r); } } release{r};
+        std::uint64_t n_nodes = 0, n_cells = 0;
+        check(dg_reduced_band_sizes(r, &n_nodes, &n_cells));
+        coeffs.resize(n_nodes); cells.resize(n_cells); cell_map.resize(m_n_cells);
+        check(dg_reduced_band_copy(r, coeffs.data(), reinterpret_cast<std::uint32_t*>(cells.data()), cell_map.data()));
+    }
 
     static void check(int rc) { if (rc != DG_OK) throw std::runtime_error(std::string("discregrid_b200: ") + dg_last_error()); }
     void invalidate() { for (auto& kv : m_dev) dg_field_destroy(kv.second); m_dev.clear(); }
@@ -354,6 +468,22 @@ private:
 
 inline void CubicLagrangeDiscreteGrid::reduceField(unsigned int field_id, Predicate pred)
 {
+    if (auto const* dev = pred.target<DeviceNodePredicate>()) {
+        // the predicate on the GPU and every pass there (dg_reduce_field_device); the field is replaced only once the result is in
+        const dg_grid_desc d = desc();
+        detail::DeviceCallbackContext ctx;
+        ctx.node = dev;
+        dg_reduced_band* r = nullptr;
+        const int rc = dg_reduce_field_device(&d, m_nodes[field_id].data(), m_nodes[field_id].size(), reinterpret_cast<const std::uint32_t*>(m_cells[field_id].data()),
+                                              m_cells[field_id].size(), ctx.node_ptr(), &ctx, 0, 0u, &r, m_last_reduced_function_ms);
+        ctx.rethrow();
+        check(rc);
+        FieldVector<double> coeffs; FieldVector<std::array<unsigned int, 32>> cells; FieldVector<unsigned int> cell_map;
+        take_reduced(r, coeffs, cells, cell_map);
+        invalidate();
+        m_nodes[field_id] = std::move(coeffs); m_cells[field_id] = std::move(cells); m_cell_map[field_id] = std::move(cell_map);
+        return;
+    }
     invalidate();
     auto& coeffs = m_nodes[field_id];
     auto& cells = m_cells[field_id];

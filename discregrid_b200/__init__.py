@@ -8,10 +8,12 @@ from . import _capi
 from ._capi import DiscregridError, DBL_MAX, LIB_PATH
 from .mesh import TriangleMesh, bumpy_torus, uv_sphere, box
 from .distance import TriangleMeshDistance, MeshSignedDistance, MeshDistanceBand, NearestEntity, Result
-from .grid import CubicLagrangeDiscreteGrid, DensityMapFunction, grid_desc, generate_sdf_domain
+from .grid import (CubicLagrangeDiscreteGrid, DensityMapFunction, DeviceFunction, DeviceNodePredicate, DeviceSamplePredicate, grid_desc,
+                   generate_sdf_domain)
 
 __all__ = ["TriangleMesh", "TriangleMeshDistance", "MeshSignedDistance", "MeshDistanceBand", "NearestEntity", "Result",
-           "CubicLagrangeDiscreteGrid", "DensityMapFunction", "grid_desc", "generate_sdf_domain", "DiscregridError",
+           "CubicLagrangeDiscreteGrid", "DensityMapFunction", "DeviceFunction", "DeviceSamplePredicate", "DeviceNodePredicate", "grid_desc",
+           "generate_sdf_domain", "DiscregridError",
            "DBL_MAX", "LIB_PATH", "bumpy_torus", "uv_sphere", "box"]
 
 

@@ -11,7 +11,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # DISCREGRID_B200_LIB: tuning builds of the same library (tools/build_variants.py); never a different implementation
 LIB_PATH = os.environ.get("DISCREGRID_B200_LIB") or os.path.join(_HERE, "lib", "libdiscregrid_b200.so")
 
-DG_OK, DG_ERR_INVALID, DG_ERR_NO_DEVICE, DG_ERR_CUDA, DG_ERR_NOMEM, DG_ERR_SELFTEST, DG_ERR_IO = 0, -1, -2, -3, -4, -5, -6
+DG_OK, DG_ERR_INVALID, DG_ERR_NO_DEVICE, DG_ERR_CUDA, DG_ERR_NOMEM, DG_ERR_SELFTEST, DG_ERR_IO, DG_ERR_CALLBACK = 0, -1, -2, -3, -4, -5, -6, -7
 DBL_MAX = 1.7976931348623157e308
 UINT32_MAX = 0xFFFFFFFF
 
@@ -40,9 +40,17 @@ if hasattr(lib, "emu_mesh_create") and os.environ.get("DG_ALLOW_EMULATED_LIBRARY
     raise ImportError(f"{LIB_PATH} is the CPU-emulated TEST build of the library (tests/emu); discregrid_b200 only runs on the CUDA build "
                       "(set DG_ALLOW_EMULATED_LIBRARY=1 only from the test rehearsal)")
 
+# True for the CPU-emulated test build: "device" pointers are host memory there
+EMULATED = hasattr(lib, "emu_mesh_create")
+
 _dp, _u32p, _i32p, _u64p, _vp = (C.POINTER(C.c_double), C.POINTER(C.c_uint32), C.POINTER(C.c_int32),
                                  C.POINTER(C.c_uint64), C.c_void_p)
 _gp = C.POINTER(GridDesc)
+
+# the device callbacks (dg_device_function, dg_device_sample_predicate, dg_device_node_predicate); every pointer as an integer address
+DEVICE_FUNCTION = C.CFUNCTYPE(C.c_int, _vp, _vp, _vp, C.c_uint64, _vp, _vp)
+DEVICE_SAMPLE_PREDICATE = C.CFUNCTYPE(C.c_int, _vp, _vp, C.c_uint64, _vp, _vp)
+DEVICE_NODE_PREDICATE = C.CFUNCTYPE(C.c_int, _vp, _vp, _vp, C.c_uint64, _vp, _vp)
 
 # name -> (restype, argtypes); every symbol of include/discregrid_b200.h
 SIGNATURES = {
@@ -100,6 +108,11 @@ SIGNATURES = {
     "dg_reduced_band_destroy": (C.c_int, [_vp]),
     "dg_reduced_density_map_create": (C.c_int, [_gp, _dp, C.c_uint64, _u32p, C.c_uint64, _u32p, C.c_double, C.c_double, C.c_uint32,
                                                  C.POINTER(_vp), C.POINTER(_vp), _dp]),
+    "dg_add_function_device": (C.c_int, [_gp, DEVICE_FUNCTION, _vp, DEVICE_SAMPLE_PREDICATE, _vp, C.c_uint64, _dp, _u32p, _u32p, _dp]),
+    "dg_reduced_function_create": (C.c_int, [_gp, DEVICE_FUNCTION, _vp, DEVICE_SAMPLE_PREDICATE, _vp, DEVICE_NODE_PREDICATE, _vp, C.c_uint64,
+                                              C.c_uint32, C.POINTER(_vp), _dp]),
+    "dg_reduce_field_device": (C.c_int, [_gp, _dp, C.c_uint64, _u32p, C.c_uint64, DEVICE_NODE_PREDICATE, _vp, C.c_uint64, C.c_uint32,
+                                          C.POINTER(_vp), _dp]),
 }
 for _name, (_res, _args) in SIGNATURES.items():
     _f = getattr(lib, _name)          # AttributeError here = the library does not export a declared symbol

@@ -574,6 +574,30 @@ HostPathPool g_pool;
 // always launched); else every chunk is the narrow-band form (classifier + band node loop, k1_launch_sample_nodes_band)
 namespace { struct HostTablesJob; }
 static void tables_job_copy(HostTablesJob* job, void* dst, const void* src, size_t bytes);
+// the D2H half of the pipeline: d_src[0, n) -> out_host, one staging piece at a time; piece i first waits for g_pool.chunk_ev[off / chunk], so
+// a piece must not straddle two chunks that complete on different streams.  The caller holds g_pool.mu.
+static int drain_to_host_locked(const double* d_src, uint64_t n, uint64_t chunk, double* out_host, HostTablesJob* copier)
+{
+    const uint64_t piece = HostPathPool::kPiece;
+    const uint64_t n_pieces = (n + piece - 1) / piece;
+    for (uint64_t i = 0; i <= n_pieces; i++) {
+        if (i < n_pieces) {
+            const uint64_t off = i * piece, cnt = (off + piece <= n) ? piece : n - off;
+            DG_CUDA(cudaStreamWaitEvent(g_pool.s_c, g_pool.chunk_ev[off / chunk], 0));
+            DG_CUDA(cudaMemcpyAsync(g_pool.stage[i & 1], d_src + off, cnt * sizeof(double), cudaMemcpyDeviceToHost, g_pool.s_c));
+            DG_CUDA(cudaEventRecord(g_pool.dma_ev[i & 1], g_pool.s_c));
+        }
+        if (i >= 1) {
+            const uint64_t off = (i - 1) * piece, cnt = (off + piece <= n) ? piece : n - off;
+            DG_CUDA(cudaEventSynchronize(g_pool.dma_ev[(i - 1) & 1]));
+            const double* src = g_pool.stage[(i - 1) & 1];
+            if (copier) tables_job_copy(copier, out_host + off, src, cnt * sizeof(double));
+            else std::memcpy(out_host + off, src, cnt * sizeof(double));
+        }
+    }
+    return DG_OK;
+}
+
 static int sample_sdf_host_locked(const dg_mesh* m, const GridDev& g, double sign, uint64_t l_begin, uint64_t n, double* out_host, HostTablesJob* copier = nullptr,
                                   const double* band = nullptr)
 {
@@ -596,22 +620,7 @@ static int sample_sdf_host_locked(const dg_mesh* m, const GridDev& g, double sig
         else DG_LAUNCH(k1_launch_sample_nodes(m->dev, g, sign, l_begin + b, cnt, g_pool.d_out + b, g_pool.s_k[c & 1]));
         DG_CUDA(cudaEventRecord(g_pool.chunk_ev[c], g_pool.s_k[c & 1]));
     }
-    for (uint64_t i = 0; i <= n_pieces; i++) {
-        if (i < n_pieces) {
-            const uint64_t off = i * piece, cnt = (off + piece <= n) ? piece : n - off;
-            DG_CUDA(cudaStreamWaitEvent(g_pool.s_c, g_pool.chunk_ev[off / chunk], 0));
-            DG_CUDA(cudaMemcpyAsync(g_pool.stage[i & 1], g_pool.d_out + off, cnt * sizeof(double), cudaMemcpyDeviceToHost, g_pool.s_c));
-            DG_CUDA(cudaEventRecord(g_pool.dma_ev[i & 1], g_pool.s_c));
-        }
-        if (i >= 1) {
-            const uint64_t off = (i - 1) * piece, cnt = (off + piece <= n) ? piece : n - off;
-            DG_CUDA(cudaEventSynchronize(g_pool.dma_ev[(i - 1) & 1]));
-            const double* src = g_pool.stage[(i - 1) & 1];
-            if (copier) tables_job_copy(copier, out_host + off, src, cnt * sizeof(double));
-            else std::memcpy(out_host + off, src, cnt * sizeof(double));
-        }
-    }
-    return DG_OK;
+    return drain_to_host_locked(g_pool.d_out, n, chunk, out_host, copier);
 }
 
 // Makes the pages of [p, p + bytes) present and writable WITHOUT changing their content (safe against a concurrent writer).
@@ -1631,23 +1640,29 @@ struct DenseRows {
 };
 }  // namespace
 
-// kept cells (:1081-1098), first half: d_cell_keep[c] = some node of row c is kept by pred.  Uploaded rows are checked on the way: a row
-// that names a node >= n is refused, as dg_reduce_field refuses it.  Synchronises `st`.
+// kept cells (:1081-1098), first half: d_cell_keep[c] = some node of row c is kept by pred, or -- d_mask != nullptr -- has a nonzero byte in
+// d_mask (a node predicate already combined with v != DBL_MAX).  Uploaded rows are checked on the way: a row that names a node >= n is
+// refused, as dg_reduce_field refuses it.  Synchronises `st`.
 static int device_cell_flags(const GridDev& g, const double* d_dense, uint64_t n, const DenseRows& rows, const K4ValuePred& pred,
-                             DevBuf<unsigned char>& d_cell_keep, const char* who, cudaStream_t st)
+                             DevBuf<unsigned char>& d_cell_keep, const char* who, cudaStream_t st, const unsigned char* d_mask = nullptr)
 {
     DG_CUDA(d_cell_keep.alloc(rows.n_cells));
     if (!rows.d_cells) {
-        DG_LAUNCH(k4_launch_closed_cell_keep(g, d_dense, rows.n_cells, pred, d_cell_keep.p, st));
+        if (d_mask) DG_LAUNCH(k4_launch_closed_cell_keep_mask(g, d_mask, rows.n_cells, d_cell_keep.p, st));
+        else DG_LAUNCH(k4_launch_closed_cell_keep(g, d_dense, rows.n_cells, pred, d_cell_keep.p, st));
         DG_CUDA(cudaStreamSynchronize(st));
         return DG_OK;
     }
     DevBuf<unsigned char> d_keep;
     DevBuf<unsigned> d_bad;
-    DG_CUDA(d_keep.alloc(n)); DG_CUDA(d_bad.alloc(1));
+    DG_CUDA(d_bad.alloc(1));
     DG_CUDA(cudaMemsetAsync(d_bad.p, 0, sizeof(unsigned), st));
-    DG_LAUNCH(k4_launch_node_keep(d_dense, n, pred, d_keep.p, st));
-    DG_LAUNCH(k4_launch_cell_keep(rows.d_cells, rows.n_cells, d_keep.p, (unsigned)n, d_cell_keep.p, d_bad.p, st));
+    if (!d_mask) {
+        DG_CUDA(d_keep.alloc(n));
+        DG_LAUNCH(k4_launch_node_keep(d_dense, n, pred, d_keep.p, st));
+        d_mask = d_keep.p;
+    }
+    DG_LAUNCH(k4_launch_cell_keep(rows.d_cells, rows.n_cells, d_mask, (unsigned)n, d_cell_keep.p, d_bad.p, st));
     unsigned bad = 0;
     DG_CUDA(cudaMemcpyAsync(&bad, d_bad.p, sizeof bad, cudaMemcpyDeviceToHost, st));
     DG_CUDA(cudaStreamSynchronize(st));
@@ -1858,6 +1873,231 @@ static int reduced_density_map_create_impl(const dg_grid_desc* grid, const doubl
     return DG_OK;
 }
 
+// ------------------------------------------------------------------------------------------------ user functions on the GPU (device callbacks)
+// addFunction(func, verbose, pred) and reduceField(id, pred) for the caller's own GPU code: the library produces the node positions of each
+// chunk of ids on the device and calls the callbacks for it on the calling thread (ctypes callbacks need that), on the library's call stream.
+namespace {
+struct DeviceCallbacks {
+    dg_device_function func = nullptr; void* fu = nullptr;
+    dg_device_sample_predicate sample = nullptr; void* su = nullptr;
+    dg_device_node_predicate node = nullptr; void* nu = nullptr;
+};
+
+// The stream the device-callback calls work on: one per device, created at first use and kept.  It is a BLOCKING stream, so its work starts
+// after the work the caller queued before the call on the legacy default stream (torch's default stream, and CUDA code that names no
+// stream): a callback that reads data produced just before the call sees it.  Kept rather than created per call, so that what the caller's
+// allocator caches for the callbacks' temporaries (torch tags freed blocks with the stream they were used on) serves every later call.
+std::mutex g_call_stream_mu;
+std::vector<cudaStream_t> g_call_streams;
+
+int call_stream(cudaStream_t& s)
+{
+    int dev = 0, n_dev = 0;
+    DG_CUDA(cudaGetDevice(&dev));
+    DG_CUDA(cudaGetDeviceCount(&n_dev));
+    std::lock_guard<std::mutex> lock(g_call_stream_mu);
+    if (g_call_streams.size() < (size_t)n_dev) g_call_streams.resize((size_t)n_dev, nullptr);
+    if (!g_call_streams[dev]) DG_CUDA(cudaStreamCreateWithFlags(&g_call_streams[dev], cudaStreamDefault));
+    s = g_call_streams[dev];
+    return DG_OK;
+}
+
+// the call's work on the call stream has finished when the call returns, on every path (its buffers are freed after it)
+struct CallStreamSync {
+    cudaStream_t s = nullptr;
+    ~CallStreamSync() { if (s) cudaStreamSynchronize(s); }
+};
+}  // namespace
+
+static uint64_t callback_chunk(uint64_t chunk_nodes, uint64_t n) { return std::max<uint64_t>(1, std::min<uint64_t>(chunk_nodes ? chunk_nodes : (1ull << 24), n)); }
+
+// Runs the callbacks over nodes [0, n) chunk by chunk, in ascending order: positions (k1_launch_node_positions: the bits of dg_node_positions),
+// then cb.sample -> a chunk mask, cb.func -> d_values + b and DBL_MAX where the mask is 0 (:806-817), then cb.node -> d_keep + b, ANDed with
+// v != DBL_MAX (:1073).  cb.func == NULL: d_values already holds the field.  ms_callbacks += host time inside the callbacks.  Synchronises `st`.
+static int run_device_callbacks(const GridDev& g, uint64_t n, uint64_t chunk_nodes, const DeviceCallbacks& cb, double* d_values, unsigned char* d_keep,
+                                double& ms_callbacks, const char* who, cudaStream_t st)
+{
+    const uint64_t chunk = callback_chunk(chunk_nodes, n);
+    DevBuf<double> d_x;
+    DevBuf<unsigned char> d_smask;
+    DG_CUDA(d_x.alloc(3 * chunk));
+    if (cb.sample) DG_CUDA(d_smask.alloc(chunk));
+    auto call = [&](const char* name, uint64_t b, uint64_t e, auto&& f) -> int {
+        const auto t0 = std::chrono::steady_clock::now();
+        const int rc = f();
+        ms_callbacks += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+        if (rc == 0) return DG_OK;
+        cudaStreamSynchronize(st);                  // whatever the callbacks enqueued has finished before the buffers are freed
+        cudaGetLastError();
+        return fail(DG_ERR_CALLBACK, "%s: the %s callback returned %d for the chunk of nodes [%llu, %llu)", who, name, rc, (unsigned long long)b,
+                    (unsigned long long)e);
+    };
+    for (uint64_t b = 0; b < n; b += chunk) {
+        const uint64_t cnt = std::min(chunk, n - b), e = b + cnt;
+        DG_LAUNCH(k1_launch_node_positions(g, b, cnt, d_x.p, st));
+        if (cb.sample) {
+            if (int rc = call("sample predicate", b, e, [&] { return cb.sample(cb.su, d_x.p, cnt, d_smask.p, st); })) return rc;
+        }
+        if (cb.func) {
+            if (int rc = call("function", b, e, [&] { return cb.func(cb.fu, d_x.p, cb.sample ? d_smask.p : nullptr, cnt, d_values + b, st); })) return rc;
+            if (cb.sample) DG_LAUNCH(k4_launch_sample_mask_apply(d_values + b, d_smask.p, cnt, st));
+        }
+        if (cb.node) {
+            if (int rc = call("node predicate", b, e, [&] { return cb.node(cb.nu, d_x.p, d_values + b, cnt, d_keep + b, st); })) return rc;
+            DG_LAUNCH(k4_launch_node_mask_combine(d_keep + b, d_values + b, cnt, st));
+        }
+    }
+    DG_CUDA(cudaStreamSynchronize(st));
+    return DG_OK;
+}
+
+// checks shared by the three entry points: the grid (grid_to_dev refuses grids of 2^31 nodes or more), then a device
+static int device_callback_setup(const dg_grid_desc* grid, GridDev& g, uint64_t& n, const char* who)
+{
+    const char* why = "";
+    if (!grid_to_dev(grid, g, &why)) return fail(DG_ERR_INVALID, "%s: %s", who, why);
+    n = (uint64_t)g.nv + 2ull * ((uint64_t)g.ne_x + g.ne_y + g.ne_z);
+    if (int rc = require_device()) return rc;
+    return ensure_selftest();
+}
+
+static int add_function_device_impl(const dg_grid_desc* grid, dg_device_function func, void* fu, dg_device_sample_predicate pred, void* pu,
+                                    uint64_t chunk_nodes, double* nodes_host, uint32_t* cells_host, uint32_t* cell_map_host, double* timings_ms)
+{
+    static const char* who = "dg_add_function_device";
+    if (!func) return fail(DG_ERR_INVALID, "%s: the function callback is NULL", who);
+    if (!nodes_host) return fail(DG_ERR_INVALID, "%s: nodes output is NULL", who);
+    GridDev g; uint64_t n = 0;
+    if (int rc = device_callback_setup(grid, g, n, who)) return rc;
+    const auto t0 = std::chrono::steady_clock::now();
+    auto ms_since = [&](std::chrono::steady_clock::time_point t) { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t).count(); };
+    // host threads pre-fault nodes_host and write the connectivity + cell map (dg_add_function_sdf's HostTablesJob) while the callbacks run
+    HostTablesJob job;
+    job.start(g, n, nodes_host, cells_host, cell_map_host);
+    double ms_callbacks = 0.0;
+    int rc = DG_OK;
+    {
+        CallStreamSync st;
+        DevBuf<double> d_values;
+        if (int e = call_stream(st.s)) return e;
+        DG_CUDA(d_values.alloc(n));
+        DeviceCallbacks cb;
+        cb.func = func; cb.fu = fu; cb.sample = pred; cb.su = pu;
+        rc = run_device_callbacks(g, n, chunk_nodes, cb, d_values.p, nullptr, ms_callbacks, who, st.s);
+        if (rc == DG_OK) {
+            // the values -> nodes_host through dg_add_function_sdf's pinned double buffer, the table workers sharing the copies
+            std::lock_guard<std::mutex> lock(g_pool.mu);
+            DG_CUDA(g_pool.prepare(0, 1));
+            DG_CUDA(cudaEventRecord(g_pool.chunk_ev[0], st.s));
+            rc = drain_to_host_locked(d_values.p, n, n, nodes_host, &job);
+        }
+    }
+    const double ms_nodes = ms_since(t0);
+    job.finish();
+    if (rc == DG_OK && timings_ms) {
+        timings_ms[0] = ms_since(t0); timings_ms[1] = ms_nodes; timings_ms[2] = timings_ms[0]; timings_ms[3] = job.ms_prefault;
+        timings_ms[4] = (double)job.n_workers; timings_ms[5] = ms_callbacks;
+    }
+    return rc;
+}
+
+// the reduction shared by both reduced forms: rows from `rows`, keep flags from d_mask (NULL: v != DBL_MAX alone), the device_reduce stages
+static int reduce_device_field(const GridDev& g, const double* d_values, uint64_t n, const DenseRows& rows, const unsigned char* d_mask,
+                               uint32_t flags, dg_reduced_band& out, double ms[5], int& tie_path, StageClock& clock, const char* who, cudaStream_t st)
+{
+    const uint64_t n_grid_cells = (uint64_t)g.n[0] * g.n[1] * g.n[2];
+    DevBuf<unsigned char> d_cell_keep;
+    if (int rc = device_cell_flags(g, d_values, n, rows, K4ValuePred{K4_KEEP_ANY, 0.0, 0.0, 0.0}, d_cell_keep, who, st, d_mask)) return rc;
+    return device_reduce(g, d_values, n, rows, d_cell_keep.p, n_grid_cells, (flags & DG_REDUCE_REFERENCE_SORT) != 0, out, ms + 1, tie_path, clock, st);
+}
+
+static void reduced_timings(double* timings_ms, const double ms[5], int tie_path, std::chrono::steady_clock::time_point t_start, double ms_callbacks)
+{
+    if (!timings_ms) return;
+    for (int k = 0; k < 5; k++) timings_ms[k] = ms[k];
+    timings_ms[5] = (double)tie_path;
+    timings_ms[6] = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_start).count();
+    timings_ms[7] = ms_callbacks;
+}
+
+static int reduced_function_create_impl(const dg_grid_desc* grid, dg_device_function func, void* fu, dg_device_sample_predicate sample_pred, void* su,
+                                        dg_device_node_predicate reduce_pred, void* ru, uint64_t chunk_nodes, uint32_t flags, dg_reduced_band** out,
+                                        double* timings_ms)
+{
+    static const char* who = "dg_reduced_function_create";
+    if (!out) return fail(DG_ERR_INVALID, "%s: out is NULL", who);
+    *out = nullptr;
+    if (!func) return fail(DG_ERR_INVALID, "%s: the function callback is NULL", who);
+    if (flags & ~DG_REDUCE_REFERENCE_SORT) return fail(DG_ERR_INVALID, "%s: unknown flags 0x%x (only DG_REDUCE_REFERENCE_SORT)", who, flags);
+    GridDev g; uint64_t n = 0;
+    if (int rc = device_callback_setup(grid, g, n, who)) return rc;
+    StageClock clock;
+    const auto t_start = clock.t0;
+    double ms[5] = {0, 0, 0, 0, 0}, ms_callbacks = 0.0;
+    int tie_path = 0;
+    std::unique_ptr<dg_reduced_band> h(new dg_reduced_band());
+    DG_CUDA(cudaGetDevice(&h->device));
+    CallStreamSync st;
+    if (int rc = call_stream(st.s)) return rc;
+    // ---- 1. addFunction(func, verbose, sample_pred) into a dense array on the device; the reduce predicate's mask per chunk meanwhile
+    DevBuf<double> d_values;
+    DevBuf<unsigned char> d_keep;
+    DG_CUDA(d_values.alloc(n));
+    if (reduce_pred) DG_CUDA(d_keep.alloc(n));
+    DeviceCallbacks cb;
+    cb.func = func; cb.fu = fu; cb.sample = sample_pred; cb.su = su; cb.node = reduce_pred; cb.nu = ru;
+    if (int rc = run_device_callbacks(g, n, chunk_nodes, cb, d_values.p, d_keep.p, ms_callbacks, who, st.s)) return rc;
+    ms[0] = clock.lap();
+    // ---- 2.-5. reduceField(id, reduce_pred) over the closed-form rows of the new field (addFunction's cells, identity map)
+    if (int rc = reduce_device_field(g, d_values.p, n, DenseRows{nullptr, (uint64_t)g.n[0] * g.n[1] * g.n[2]}, d_keep.p, flags, *h, ms, tie_path, clock, who,
+                                     st.s))
+        return rc;
+    reduced_timings(timings_ms, ms, tie_path, t_start, ms_callbacks);
+    *out = h.release();
+    return DG_OK;
+}
+
+static int reduce_field_device_impl(const dg_grid_desc* grid, const double* nodes, uint64_t n_nodes, const uint32_t* cells, uint64_t n_cells,
+                                    dg_device_node_predicate pred, void* pu, uint64_t chunk_nodes, uint32_t flags, dg_reduced_band** out,
+                                    double* timings_ms)
+{
+    static const char* who = "dg_reduce_field_device";
+    if (!out) return fail(DG_ERR_INVALID, "%s: out is NULL", who);
+    *out = nullptr;
+    if (!pred) return fail(DG_ERR_INVALID, "%s: the node predicate callback is NULL", who);
+    if (!nodes || (n_cells && !cells)) return fail(DG_ERR_INVALID, "%s: NULL argument", who);
+    if (flags & ~DG_REDUCE_REFERENCE_SORT) return fail(DG_ERR_INVALID, "%s: unknown flags 0x%x (only DG_REDUCE_REFERENCE_SORT)", who, flags);
+    GridDev g; uint64_t n = 0;
+    if (int rc = device_callback_setup(grid, g, n, who)) return rc;
+    if (n_nodes != n)                     // node ids must be the grid's own numbering: their positions feed the Z-curve key (:1113)
+        return fail(DG_ERR_INVALID, "%s: the field has %llu nodes, the grid %llu (already reduced?)", who, (unsigned long long)n_nodes, (unsigned long long)n);
+    if (n_cells > (uint64_t)g.n[0] * g.n[1] * g.n[2]) return fail(DG_ERR_INVALID, "%s: more cells than the grid has", who);
+    StageClock clock;
+    const auto t_start = clock.t0;
+    double ms[5] = {0, 0, 0, 0, 0}, ms_callbacks = 0.0;
+    int tie_path = 0;
+    std::unique_ptr<dg_reduced_band> h(new dg_reduced_band());
+    DG_CUDA(cudaGetDevice(&h->device));
+    CallStreamSync st;
+    if (int rc = call_stream(st.s)) return rc;
+    // ---- 1. upload the field and its rows; the predicate's mask per chunk, ANDed with v != DBL_MAX (the rows are checked by the cell flags)
+    DevBuf<double> d_values;
+    DevBuf<unsigned> d_cells;
+    DevBuf<unsigned char> d_keep;
+    DG_CUDA(d_values.alloc(n)); DG_CUDA(d_cells.alloc(32 * n_cells)); DG_CUDA(d_keep.alloc(n));
+    DG_CUDA(cudaMemcpyAsync(d_values.p, nodes, n * sizeof(double), cudaMemcpyHostToDevice, st.s));
+    if (n_cells) DG_CUDA(cudaMemcpyAsync(d_cells.p, cells, 32 * n_cells * sizeof(unsigned), cudaMemcpyHostToDevice, st.s));
+    DeviceCallbacks cb;
+    cb.node = pred; cb.nu = pu;
+    if (int rc = run_device_callbacks(g, n, chunk_nodes, cb, d_values.p, d_keep.p, ms_callbacks, who, st.s)) return rc;
+    ms[0] = clock.lap();
+    // ---- 2.-5. reduceField over the uploaded rows
+    if (int rc = reduce_device_field(g, d_values.p, n, DenseRows{d_cells.p, n_cells}, d_keep.p, flags, *h, ms, tie_path, clock, who, st.s)) return rc;
+    reduced_timings(timings_ms, ms, tie_path, t_start, ms_callbacks);
+    *out = h.release();
+    return DG_OK;
+}
+
 int dg_reduced_band_sizes(const dg_reduced_band* h, uint64_t* n_nodes, uint64_t* n_cells)
 {
     if (!h || !n_nodes || !n_cells) return fail(DG_ERR_INVALID, "dg_reduced_band_sizes: NULL argument");
@@ -1946,6 +2186,31 @@ int dg_reduced_density_map_create(const dg_grid_desc* grid, const double* sdf_no
 {
     return guarded("dg_reduced_density_map_create", [&]() {
         return reduced_density_map_create_impl(grid, sdf_nodes, n_nodes, sdf_cells, n_cells, sdf_cell_map, h, rho0, flags, sdf_out, density_out, timings_ms);
+    });
+}
+
+int dg_add_function_device(const dg_grid_desc* grid, dg_device_function func, void* fu, dg_device_sample_predicate pred, void* pu, uint64_t chunk_nodes,
+                           double* nodes_host, uint32_t* cells_host, uint32_t* cell_map_host, double* timings_ms)
+{
+    return guarded("dg_add_function_device", [&]() {
+        return add_function_device_impl(grid, func, fu, pred, pu, chunk_nodes, nodes_host, cells_host, cell_map_host, timings_ms);
+    });
+}
+
+int dg_reduced_function_create(const dg_grid_desc* grid, dg_device_function func, void* fu, dg_device_sample_predicate sample_pred, void* su,
+                               dg_device_node_predicate reduce_pred, void* ru, uint64_t chunk_nodes, uint32_t flags, dg_reduced_band** out,
+                               double* timings_ms)
+{
+    return guarded("dg_reduced_function_create", [&]() {
+        return reduced_function_create_impl(grid, func, fu, sample_pred, su, reduce_pred, ru, chunk_nodes, flags, out, timings_ms);
+    });
+}
+
+int dg_reduce_field_device(const dg_grid_desc* grid, const double* nodes, uint64_t n_nodes, const uint32_t* cells, uint64_t n_cells,
+                           dg_device_node_predicate pred, void* pu, uint64_t chunk_nodes, uint32_t flags, dg_reduced_band** out, double* timings_ms)
+{
+    return guarded("dg_reduce_field_device", [&]() {
+        return reduce_field_device_impl(grid, nodes, n_nodes, cells, n_cells, pred, pu, chunk_nodes, flags, out, timings_ms);
     });
 }
 

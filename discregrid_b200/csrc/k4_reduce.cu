@@ -8,9 +8,10 @@
 //                  coefficients (:1158-1173)
 //   host (reduce_field.cpp): the reference's back-to-front swap compaction replayed on a permutation array (:1135-1156, O(n), inherently
 //                  serial) and the sort of the survivors by key, whose order among EQUAL keys is libstdc++'s introsort's (reduce_field.h).
-// The reduced narrow band (dg_reduced_band_create) and the reduced density map (dg_reduced_density_map_create) run the same passes on the
-// device only: keep flags from a value predicate, cell flags and rows from an uploaded table or from the closed form instead of a cell
-// table, and the swap walk itself as pointer jumping (swap_walk_*); the sort of the survivors stays on the host.
+// The reduced narrow band (dg_reduced_band_create), the reduced density map (dg_reduced_density_map_create) and the reductions of fields
+// sampled by device callbacks (dg_reduced_function_create, dg_reduce_field_device) run the same passes on the device only: keep flags from
+// a value predicate or a node mask, cell flags and rows from an uploaded table or from the closed form instead of a cell table, and the swap
+// walk itself as pointer jumping (swap_walk_*); the sort of the survivors stays on the host.
 // All kernels are warp-synchronous (ballot / popc), so tests/emu runs them unchanged.  Integer work, bit-exact by construction; the one
 // floating-point step (the key's cast of inv * x) uses the reference's operations in the reference's order (no FMA: -fmad=false).
 #include "k4_reduce.h"
@@ -158,6 +159,20 @@ __global__ void node_keep_kernel(const double* __restrict__ nodes, unsigned long
     if (i < n) keep[i] = value_kept<KIND>(p, __ldg(nodes + i)) ? 1 : 0;
 }
 
+// addFunction(func, verbose, pred) stores DBL_MAX where the sample predicate rejects (:817): v = keep ? v : DBL_MAX
+__global__ void sample_mask_apply_kernel(double* __restrict__ values, const unsigned char* __restrict__ keep, unsigned long long n)
+{
+    const unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n && keep[i] == 0) values[i] = DBL_MAX;
+}
+
+// reduceField keeps node l iff pred(x_l, c_l) && c_l != DBL_MAX (:1069-1074): keep = keep && v != DBL_MAX, as 0 / 1
+__global__ void node_mask_combine_kernel(unsigned char* __restrict__ keep, const double* __restrict__ values, unsigned long long n)
+{
+    const unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) keep[i] = (keep[i] != 0 && __ldg(values + i) != DBL_MAX) ? 1 : 0;
+}
+
 __device__ __forceinline__ void cell_ijk(const GridDev& g, unsigned long long c, unsigned& i, unsigned& j, unsigned& k)
 {
     const unsigned long long s = (unsigned long long)g.n[0] * g.n[1];
@@ -166,10 +181,22 @@ __device__ __forceinline__ void cell_ijk(const GridDev& g, unsigned long long c,
     j = t / g.n[0]; i = t - j * g.n[0];
 }
 
-// keep flag per cell: one warp per cell, lane j applies the predicate to the coefficient of the cell's closed-form node j
+// where a node's keep decision comes from: a value predicate of its coefficient, or a node mask computed beforehand (a device predicate
+// combined with v != DBL_MAX by node_mask_combine_kernel)
 template <int KIND>
-__global__ void closed_cell_keep_kernel(GridDev g, const double* __restrict__ nodes, unsigned long long n_cells, K4ValuePred p,
-                                        unsigned char* __restrict__ cell_keep)
+struct ValueKeep {
+    const double* __restrict__ nodes;
+    K4ValuePred p;
+    __device__ __forceinline__ bool operator()(unsigned l) const { return value_kept<KIND>(p, __ldg(nodes + l)); }
+};
+struct MaskKeep {
+    const unsigned char* __restrict__ keep;
+    __device__ __forceinline__ bool operator()(unsigned l) const { return __ldg(keep + l) != 0; }
+};
+
+// keep flag per cell: one warp per cell, lane j asks `keep` about the cell's closed-form node j
+template <class Keep>
+__global__ void closed_cell_keep_kernel(GridDev g, Keep keep, unsigned long long n_cells, unsigned char* __restrict__ cell_keep)
 {
     const unsigned long long c = ((unsigned long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const unsigned lane = threadIdx.x & 31u;
@@ -178,7 +205,7 @@ __global__ void closed_cell_keep_kernel(GridDev g, const double* __restrict__ no
     if (live) {
         unsigned i, j, k;
         cell_ijk(g, c, i, j, k);
-        kept = value_kept<KIND>(p, __ldg(nodes + cell_node_id(g, i, j, k, lane)));
+        kept = keep(cell_node_id(g, i, j, k, lane));
     }
     const unsigned any = __ballot_sync(0xffffffffu, kept);
     if (live && lane == 0) cell_keep[c] = any ? 1 : 0;
@@ -345,11 +372,33 @@ cudaError_t k4_launch_closed_cell_keep(const GridDev& g, const double* d_nodes, 
     const unsigned blocks = blocks_for(n_cells * 32ull, 128);
     const unsigned long long nc = n_cells;
     switch (p.kind) {
-    case K4_KEEP_ANY: DG_KERNEL_LAUNCH(closed_cell_keep_kernel<K4_KEEP_ANY>, blocks, 128, 0, stream, g, d_nodes, nc, p, d_cell_keep); break;
-    case K4_KEEP_SDF: DG_KERNEL_LAUNCH(closed_cell_keep_kernel<K4_KEEP_SDF>, blocks, 128, 0, stream, g, d_nodes, nc, p, d_cell_keep); break;
-    case K4_KEEP_RANGE: DG_KERNEL_LAUNCH(closed_cell_keep_kernel<K4_KEEP_RANGE>, blocks, 128, 0, stream, g, d_nodes, nc, p, d_cell_keep); break;
+    case K4_KEEP_ANY: DG_KERNEL_LAUNCH(closed_cell_keep_kernel<ValueKeep<K4_KEEP_ANY>>, blocks, 128, 0, stream, g, ValueKeep<K4_KEEP_ANY>{d_nodes, p}, nc, d_cell_keep); break;
+    case K4_KEEP_SDF: DG_KERNEL_LAUNCH(closed_cell_keep_kernel<ValueKeep<K4_KEEP_SDF>>, blocks, 128, 0, stream, g, ValueKeep<K4_KEEP_SDF>{d_nodes, p}, nc, d_cell_keep); break;
+    case K4_KEEP_RANGE: DG_KERNEL_LAUNCH(closed_cell_keep_kernel<ValueKeep<K4_KEEP_RANGE>>, blocks, 128, 0, stream, g, ValueKeep<K4_KEEP_RANGE>{d_nodes, p}, nc, d_cell_keep); break;
     default: return cudaErrorInvalidValue;
     }
+    return DG_AFTER_LAUNCH();
+}
+
+cudaError_t k4_launch_closed_cell_keep_mask(const GridDev& g, const unsigned char* d_keep_node, uint64_t n_cells, unsigned char* d_cell_keep, cudaStream_t stream)
+{
+    if (n_cells == 0) return cudaSuccess;
+    DG_KERNEL_LAUNCH(closed_cell_keep_kernel<MaskKeep>, blocks_for(n_cells * 32ull, 128), 128, 0, stream, g, MaskKeep{d_keep_node}, (unsigned long long)n_cells,
+                     d_cell_keep);
+    return DG_AFTER_LAUNCH();
+}
+
+cudaError_t k4_launch_sample_mask_apply(double* d_values, const unsigned char* d_keep, uint64_t n, cudaStream_t stream)
+{
+    if (n == 0) return cudaSuccess;
+    DG_KERNEL_LAUNCH(sample_mask_apply_kernel, blocks_for(n, 256), 256, 0, stream, d_values, d_keep, (unsigned long long)n);
+    return DG_AFTER_LAUNCH();
+}
+
+cudaError_t k4_launch_node_mask_combine(unsigned char* d_keep, const double* d_values, uint64_t n, cudaStream_t stream)
+{
+    if (n == 0) return cudaSuccess;
+    DG_KERNEL_LAUNCH(node_mask_combine_kernel, blocks_for(n, 256), 256, 0, stream, d_keep, d_values, (unsigned long long)n);
     return DG_AFTER_LAUNCH();
 }
 

@@ -31,6 +31,12 @@ cudaError_t k4_launch_node_keep(const double* d_nodes, uint64_t n, const K4Value
 // cell flags and compaction with the closed-form rows (cell_node_id) of the dense coefficients d_nodes
 cudaError_t k4_launch_closed_cell_keep(const GridDev& g, const double* d_nodes, uint64_t n_cells, const K4ValuePred& p, unsigned char* d_cell_keep,
                                        cudaStream_t stream);
+// the same cell flags from a node mask (0 = not kept) instead of a value predicate
+cudaError_t k4_launch_closed_cell_keep_mask(const GridDev& g, const unsigned char* d_keep_node, uint64_t n_cells, unsigned char* d_cell_keep, cudaStream_t stream);
+// node masks of device callbacks: d_values[i] = DBL_MAX where d_keep[i] == 0 (a sample predicate, :817); d_keep[i] = d_keep[i] != 0 &&
+// d_values[i] != DBL_MAX, as 0 / 1 (a reduce predicate, :1073)
+cudaError_t k4_launch_sample_mask_apply(double* d_values, const unsigned char* d_keep, uint64_t n, cudaStream_t stream);
+cudaError_t k4_launch_node_mask_combine(unsigned char* d_keep, const double* d_values, uint64_t n, cudaStream_t stream);
 cudaError_t k4_launch_closed_cell_compact(const GridDev& g, uint64_t n_cells, const unsigned char* d_cell_keep, const unsigned* d_tile_offset,
                                           unsigned* d_cells_out, unsigned* d_cell_map, cudaStream_t stream);
 // d_bad[0] becomes non-zero when an entry of d_cell_map[0..n) is neither 0xffffffff nor < n_rows

@@ -13,13 +13,21 @@ that save()/load() stay byte-compatible with the reference's .cdf/.cdm files
   addFunction(DensityMapFunction, pred)  -> dg_density_map       (K3, csrc/k3_density.cu)
   addReducedDensityMap(DensityMapFunction)
                                          -> dg_reduced_density_map_create (K3, then both of GenerateDensityMap's reduceField calls, on the GPU)
+  addFunction(DeviceFunction, pred=DeviceSamplePredicate)
+                                         -> dg_add_function_device (your torch code on batches of node positions made on the GPU)
+  reduceField(field_id, DeviceNodePredicate)
+                                         -> dg_reduce_field_device (your predicate on the GPU, then reduceField's passes there)
+  addReducedFunction(DeviceFunction, DeviceSamplePredicate, DeviceNodePredicate)
+                                         -> dg_reduced_function_create (addFunction + reduceField, the dense field kept on the GPU)
   interpolate(field_id, x[, gradient])   -> dg_interpolate_batch (K2, csrc/k2_interp.cu), batched over x
 
-The reference's addFunction takes an opaque std::function; only the two functor types the reference's own tools
-build are recognised.  Any other callable raises TypeError -- sample it yourself at nodePositions() and hand the
-values to addSampledFunction(); there is no hidden host loop.
+The reference's addFunction takes an opaque std::function.  The two functor types the reference's own tools build are recognised
+and run on the library's kernels; a function of your own runs as your own GPU code when wrapped in DeviceFunction (and its
+predicates in DeviceSamplePredicate / DeviceNodePredicate).  Any other callable raises TypeError; there is no hidden host loop.
 """
+import contextlib
 import ctypes as C
+import math
 import struct
 
 import numpy as np
@@ -34,6 +42,143 @@ class DensityMapFunction:
 
     def __init__(self, sdf_field_id=0, smoothing_length=0.1, rest_density=1000.0, no_reduction=False):
         self.field_id, self.h, self.rho0, self.no_reduction = sdf_field_id, float(smoothing_length), float(rest_density), bool(no_reduction)
+
+
+class DeviceFunction:
+    """A function evaluated by your own GPU code, batch by batch: fn(x, keep) -> values.
+    x: float64 tensor (n, 3), the positions indexToNodePosition(l) of a chunk of node ids, made on the GPU.  keep: uint8 tensor (n,) of the
+    sample predicate's decisions for the same nodes (nonzero = sampled), or None without a predicate; nodes with keep == 0 may be skipped,
+    they get DBL_MAX anyway.  values: float64 tensor (n,) on the same device.  Both tensors view the library's buffers (no copy) and are only
+    valid during the call.  fn runs on the library's stream (torch.cuda.ExternalStream), which first waits for the torch stream that was current
+    when the grid method was called, so fn sees every tensor computed before the call; plain torch operations inside fn are ordered with the
+    library's own work."""
+
+    def __init__(self, fn):
+        if not callable(fn):
+            raise TypeError("DeviceFunction wraps a callable fn(x, keep) -> float64 tensor")
+        self.fn = fn
+
+
+class DeviceSamplePredicate:
+    """addFunction's sample predicate on the GPU: fn(x) -> bool tensor (n,); DBL_MAX is stored where it is False (:817)."""
+
+    def __init__(self, fn):
+        if not callable(fn):
+            raise TypeError("DeviceSamplePredicate wraps a callable fn(x) -> bool tensor")
+        self.fn = fn
+
+
+class DeviceNodePredicate:
+    """reduceField's predicate on the GPU: fn(x, values) -> bool tensor (n,); a node is kept where it is True and its value is not
+    DBL_MAX (:1069-1074).  values: float64 tensor (n,), the field's coefficients of the chunk."""
+
+    def __init__(self, fn):
+        if not callable(fn):
+            raise TypeError("DeviceNodePredicate wraps a callable fn(x, values) -> bool tensor")
+        self.fn = fn
+
+
+class _DeviceCallbacks:
+    """The ctypes trampolines of one library call.  The first exception raised inside a callback is kept (the callback returns 1, the
+    library stops with DG_ERR_CALLBACK) and re-raised by check()."""
+
+    def __init__(self, func=None, sample=None, node=None):
+        import torch
+        self.torch = torch
+        self.error = None
+        # the caller's stream at the call: the library's stream waits for it before the first callback runs (work queued on it, e.g. the
+        # weights of a model just trained, must be finished before fn reads it)
+        self.caller_stream = None if capi.EMULATED else torch.cuda.current_stream()
+        self.func = capi.DEVICE_FUNCTION(self._func(func.fn)) if func is not None else capi.DEVICE_FUNCTION()
+        self.sample = capi.DEVICE_SAMPLE_PREDICATE(self._sample(sample.fn)) if sample is not None else capi.DEVICE_SAMPLE_PREDICATE()
+        self.node = capi.DEVICE_NODE_PREDICATE(self._node(node.fn)) if node is not None else capi.DEVICE_NODE_PREDICATE()
+
+    def check(self, rc):
+        if self.error is not None:
+            raise self.error
+        capi.check(rc)
+
+    def _view(self, addr, shape, typestr, dtype):
+        """a tensor over library memory: CUDA memory through __cuda_array_interface__, host memory under the emulated test build"""
+        count = math.prod(shape)
+        if capi.EMULATED:
+            buf = (C.c_char * (count * dtype.itemsize)).from_address(addr)
+            return self.torch.frombuffer(buf, dtype=dtype).view(shape)
+
+        class _Cai:
+            __cuda_array_interface__ = {"shape": shape, "typestr": typestr, "data": (addr, False), "version": 3, "strides": None}
+        return self.torch.as_tensor(_Cai(), device="cuda")
+
+    def _stream(self, stream):
+        if capi.EMULATED:
+            return contextlib.nullcontext()
+        ext = self.torch.cuda.ExternalStream(stream)
+        if self.caller_stream is not None:
+            ext.wait_stream(self.caller_stream)                # once per call: later callbacks follow on the same stream
+            self.caller_stream = None
+        return self.torch.cuda.stream(ext)
+
+    def _run(self, body, stream):
+        try:
+            with self._stream(stream):
+                body()
+            return 0
+        except BaseException as e:          # noqa: BLE001 -- kept and re-raised after the library call returns
+            if self.error is None:
+                self.error = e
+            return 1
+
+    def _result(self, r, n, dtype, like, what):
+        t = self.torch
+        if not isinstance(r, t.Tensor) or r.dtype != dtype or tuple(r.shape) != (n,) or r.device != like.device:
+            raise TypeError(f"{what} must return a {dtype} tensor of shape ({n},) on {like.device}, got "
+                            f"{type(r).__name__ if not isinstance(r, t.Tensor) else (r.dtype, tuple(r.shape), r.device)}")
+        return r
+
+    def _func(self, fn):
+        t = self.torch
+
+        def cb(_user, x, keep, n, values, stream):
+            def body():
+                xs = self._view(x, (n, 3), "<f8", t.float64)
+                ks = self._view(keep, (n,), "|u1", t.uint8) if keep else None
+                out = self._view(values, (n,), "<f8", t.float64)
+                out.copy_(self._result(fn(xs, ks), n, t.float64, out, "DeviceFunction"))
+            return self._run(body, stream)
+        return cb
+
+    def _sample(self, fn):
+        t = self.torch
+
+        def cb(_user, x, n, keep, stream):
+            def body():
+                out = self._view(keep, (n,), "|u1", t.uint8)
+                out.copy_(self._result(fn(self._view(x, (n, 3), "<f8", t.float64)), n, t.bool, out, "DeviceSamplePredicate"))
+            return self._run(body, stream)
+        return cb
+
+    def _node(self, fn):
+        t = self.torch
+
+        def cb(_user, x, values, n, keep, stream):
+            def body():
+                out = self._view(keep, (n,), "|u1", t.uint8)
+                r = fn(self._view(x, (n, 3), "<f8", t.float64), self._view(values, (n,), "<f8", t.float64))
+                out.copy_(self._result(r, n, t.bool, out, "DeviceNodePredicate"))
+            return self._run(body, stream)
+        return cb
+
+
+def _copy_reduced(h, n_grid_cells):
+    """the (nodes, cells, cell map) of a dg_reduced_band handle, which is destroyed"""
+    try:
+        n_nodes, n_cells = C.c_uint64(), C.c_uint64()
+        capi.check(capi.lib.dg_reduced_band_sizes(h, C.byref(n_nodes), C.byref(n_cells)))
+        f = (np.empty(n_nodes.value), np.empty((n_cells.value, 32), np.uint32), np.empty(n_grid_cells, np.uint32))
+        capi.check(capi.lib.dg_reduced_band_copy(h, capi.ptr(f[0], capi.F64P), capi.ptr(f[1], capi.U32P), capi.ptr(f[2], capi.U32P)))
+        return f
+    finally:
+        capi.lib.dg_reduced_band_destroy(h)
 
 
 def grid_desc(domain_min, domain_max, resolution, cell_size=None, inv_cell_size=None):
@@ -128,6 +273,23 @@ class CubicLagrangeDiscreteGrid:
 
     # ------------------------------------------------------------------ addFunction (cubic_lagrange_discrete_grid.cpp:780-899)
     def addFunction(self, func, verbose=False, pred=None):
+        if isinstance(func, DeviceFunction) or isinstance(pred, DeviceSamplePredicate):
+            if not isinstance(func, DeviceFunction) or (pred is not None and not isinstance(pred, DeviceSamplePredicate)):
+                raise TypeError("a DeviceFunction takes a DeviceSamplePredicate (or none), and a DeviceSamplePredicate only goes with a DeviceFunction")
+            # the whole addFunction in one call: your function on the GPU, connectivity + cell map written by the library's host threads meanwhile
+            coeffs = np.empty(self.nNodes())
+            cells = np.empty((self.m_n_cells, 32), np.uint32)
+            cmap = np.empty(self.m_n_cells, np.uint32)
+            self.last_add_function_ms = np.zeros(6)
+            cb = _DeviceCallbacks(func=func, sample=pred)
+            cb.check(capi.lib.dg_add_function_device(C.byref(self._desc), cb.func, None, cb.sample, None, 0, capi.ptr(coeffs, capi.F64P),
+                                                     capi.ptr(cells, capi.U32P), capi.ptr(cmap, capi.U32P), capi.ptr(self.last_add_function_ms, capi.F64P)))
+            if verbose:
+                print(f"Construction: {len(coeffs)} nodes sampled on the GPU in {self.last_add_function_ms[0]:.1f} ms")
+            self._invalidate()
+            self.m_nodes.append(coeffs); self.m_cells.append(cells); self.m_cell_map.append(cmap)
+            self.m_n_fields += 1
+            return self.m_n_fields - 1
         if isinstance(func, MeshSignedDistance):
             if pred is not None and not isinstance(pred, MeshDistanceBand):
                 raise TypeError("a sample predicate is only supported with DensityMapFunction, or as MeshDistanceBand with MeshSignedDistance")
@@ -151,8 +313,8 @@ class CubicLagrangeDiscreteGrid:
             capi.check(capi.lib.dg_density_map(self._device_field(func.field_id), func.h, func.rho0, int(func.no_reduction), 0,
                                                len(coeffs), capi.ptr(coeffs, capi.F64P)))
         else:
-            raise TypeError("addFunction runs on the GPU and only accepts MeshSignedDistance or DensityMapFunction; "
-                            "for any other function evaluate it at nodePositions() and call addSampledFunction(values)")
+            raise TypeError("addFunction runs on the GPU and only accepts MeshSignedDistance, DensityMapFunction or DeviceFunction; "
+                            "wrap a function of your own that runs on the GPU (e.g. torch operations) in DeviceFunction")
         return self.addSampledFunction(coeffs)
 
     def addReducedBandField(self, func, pred, verbose=False):
@@ -178,6 +340,27 @@ class CubicLagrangeDiscreteGrid:
             capi.lib.dg_reduced_band_destroy(h)
         if verbose:
             print(f"Construction: {len(coeffs)} of {self.nNodes()} nodes kept in {self.last_reduced_band_ms[6]:.1f} ms on the GPU")
+        self.m_nodes.append(coeffs); self.m_cells.append(cells); self.m_cell_map.append(cmap)
+        self.m_n_fields += 1
+        return self.m_n_fields - 1
+
+    def addReducedFunction(self, func, sample_pred=None, reduce_pred=None, verbose=False):
+        """addFunction(func, verbose, sample_pred) followed by reduceField(id, reduce_pred), in one call (dg_reduced_function_create): the
+        field holds exactly what those two calls leave, but the dense values stay on the GPU; only the survivors and the cell map reach the
+        host.  func: DeviceFunction; sample_pred: DeviceSamplePredicate or None; reduce_pred: DeviceNodePredicate or None (always true).
+        Returns the field id."""
+        if not isinstance(func, DeviceFunction) or not isinstance(sample_pred, (DeviceSamplePredicate, type(None))) \
+                or not isinstance(reduce_pred, (DeviceNodePredicate, type(None))):
+            raise TypeError("addReducedFunction takes a DeviceFunction, a DeviceSamplePredicate or None and a DeviceNodePredicate or None")
+        h = C.c_void_p()
+        self.last_reduced_function_ms = np.zeros(8)
+        cb = _DeviceCallbacks(func=func, sample=sample_pred, node=reduce_pred)
+        cb.check(capi.lib.dg_reduced_function_create(C.byref(self._desc), cb.func, None, cb.sample, None, cb.node, None, 0, 0, C.byref(h),
+                                                     capi.ptr(self.last_reduced_function_ms, capi.F64P)))
+        coeffs, cells, cmap = _copy_reduced(h, self.m_n_cells)
+        if verbose:
+            print(f"Construction: {len(coeffs)} of {self.nNodes()} nodes kept in {self.last_reduced_function_ms[6]:.1f} ms")
+        self._invalidate()
         self.m_nodes.append(coeffs); self.m_cells.append(cells); self.m_cell_map.append(cmap)
         self.m_n_fields += 1
         return self.m_n_fields - 1
@@ -236,7 +419,19 @@ class CubicLagrangeDiscreteGrid:
     # ------------------------------------------------------------------ reduceField (cubic_lagrange_discrete_grid.cpp:1065-1174)
     def reduceField(self, field_id, pred):
         """Sparsifies a field.  pred(x[n,3], values[n]) -> bool[n] is the reference's Predicate, vectorised; nodes, cells and the
-        cell map end up exactly as the reference leaves them (dg_reduce_field)."""
+        cell map end up exactly as the reference leaves them (dg_reduce_field).  A DeviceNodePredicate runs on the GPU instead, on
+        positions made there, and so does the whole reduction (dg_reduce_field_device)."""
+        if isinstance(pred, DeviceNodePredicate):
+            nodes = np.ascontiguousarray(self.m_nodes[field_id], np.float64)
+            cells = np.ascontiguousarray(self.m_cells[field_id], np.uint32)
+            h = C.c_void_p()
+            cb = _DeviceCallbacks(node=pred)
+            cb.check(capi.lib.dg_reduce_field_device(C.byref(self._desc), capi.ptr(nodes, capi.F64P), len(nodes), capi.ptr(cells, capi.U32P),
+                                                     len(cells), cb.node, None, 0, 0, C.byref(h), None))
+            out = _copy_reduced(h, self.m_n_cells)
+            self._invalidate()
+            self.m_nodes[field_id], self.m_cells[field_id], self.m_cell_map[field_id] = out
+            return
         nodes = np.ascontiguousarray(self.m_nodes[field_id], np.float64).copy()
         keep = np.asarray(pred(self.nodePositions(0, len(nodes)), nodes), bool) & (nodes != np.finfo(np.float64).max)   # :1073
         keep = np.ascontiguousarray(keep, np.uint8)

@@ -49,7 +49,8 @@ typedef enum dg_status {
     DG_ERR_CUDA = -3,        /* a CUDA runtime call failed; dg_last_error() has the cudaError string */
     DG_ERR_NOMEM = -4,       /* host or device allocation failed */
     DG_ERR_SELFTEST = -5,    /* device self-test failed (e.g. library built with FMA contraction on) */
-    DG_ERR_IO = -6           /* a file could not be opened or read */
+    DG_ERR_IO = -6,          /* a file could not be opened or read */
+    DG_ERR_CALLBACK = -7     /* a caller-supplied callback returned nonzero; dg_last_error() names the callback and the chunk */
 } dg_status;
 
 /* TriangleMeshDistance.h:75 -- same numbering */
@@ -311,6 +312,59 @@ DG_API int dg_reduced_density_map_create(const dg_grid_desc* grid, const double*
                                          const uint32_t* sdf_cells, uint64_t n_cells, const uint32_t* sdf_cell_map,
                                          double h, double rho0, uint32_t flags,
                                          dg_reduced_band** sdf_out, dg_reduced_band** density_out, double* timings_ms);
+
+/* ---- user functions on the GPU: addFunction(func, verbose, pred) and reduceField(id, pred) with batched device callbacks ----------------
+ * The reference's addFunction and reduceField take any callable.  These entry points take the caller's OWN GPU code instead, as batched
+ * callbacks: the library generates the node positions x = indexToNodePosition(l) (cubic_lagrange_discrete_grid.cpp:604-665, the bits of
+ * dg_node_positions) for contiguous id ranges [b, e) ("chunks") on the device and calls the callbacks once per chunk, in ascending order, ON
+ * THE CALLING THREAD, with n = e - b and device pointers of the current device:
+ *   d_x            n x 3 doubles, the positions of nodes b .. e-1 (valid until the callback's work on `stream` has run)
+ *   d_sample_keep  n bytes written by the sample predicate of the same chunk, or NULL without one; a function may skip the nodes whose byte
+ *                  is 0 -- the library writes DBL_MAX there anyway (:817)
+ *   d_values       function: n doubles to write (node b first); node predicate: the chunk's values, DBL_MAX where the sample predicate rejected
+ *   d_keep         n bytes to write: nonzero = keep.  A node predicate's mask is ANDed with v != DBL_MAX (:1073) on the device.
+ *   stream         the cudaStream_t the library works on: enqueue the work there, or finish it before returning.  It is one stream per
+ *                  device, kept for the life of the process (calls from several threads share it), and it is a blocking stream: its work
+ *                  -- the first positions and every callback's work on it -- starts after everything queued on the legacy default stream
+ *                  (NULL; torch's default stream) before the call.  Work the caller queued on OTHER streams is not waited for: order it first
+ *                  (e.g. cudaStreamSynchronize, or a cudaStreamWaitEvent on `stream` in the first callback).  When the call returns, all
+ *                  its work on `stream` has finished.
+ * A callback returns 0, or nonzero to abort the call: the call then returns DG_ERR_CALLBACK (dg_last_error() names the callback and the chunk),
+ * produces no handle and leaves the output arrays' contents unspecified.  Callbacks may call the library's _device entry points (e.g.
+ * dg_mesh_distance_device on d_x); they must not call the entry point that is calling them.
+ * chunk_nodes: ids per chunk, 0 = 2^24 (positions of one chunk: 384 MiB).  The values do not depend on it.  One GPU (the current device);
+ * grids of 2^31 nodes or more are refused before anything is allocated. */
+typedef int (*dg_device_function)(void* user, const double* d_x, const uint8_t* d_sample_keep, uint64_t n, double* d_values, void* stream);
+typedef int (*dg_device_sample_predicate)(void* user, const double* d_x, uint64_t n, uint8_t* d_keep, void* stream);
+typedef int (*dg_device_node_predicate)(void* user, const double* d_x, const double* d_values, uint64_t n, uint8_t* d_keep, void* stream);
+/* addFunction(func, verbose, pred) (:780-899) into the caller's three arrays, as dg_add_function_sdf fills them: nodes_host[n_nodes] = func(x)
+ * where pred(x) holds (pred NULL: everywhere) and DBL_MAX elsewhere (:806-817); cells_host[n_cells x 32] and cell_map_host[n_cells] (each
+ * nullable) are written by host threads while the callbacks run.  func must not be NULL.
+ * timings_ms: NULL or 6 doubles = total, node pipeline done, index tables done, coefficient array pre-faulted (all ms since entry), worker
+ * threads used, ms spent inside the callbacks (host time from call to return; work they only enqueue counts in the node pipeline). */
+DG_API int dg_add_function_device(const dg_grid_desc* grid, dg_device_function func, void* fu, dg_device_sample_predicate pred, void* pu,
+                                  uint64_t chunk_nodes, double* nodes_host, uint32_t* cells_host, uint32_t* cell_map_host, double* timings_ms);
+/* id = addFunction(func, verbose, sample_pred); reduceField(id, reduce_pred); in one call: the dense values stay on the device, the rows come
+ * from the closed form, and the handle holds exactly what those two calls leave (nodes in the reference's Z-curve order, including the order
+ * among equal keys; renumbered cells; cell map) -- bit for bit dg_add_function_device followed by dg_reduce_field with
+ * keep = reduce_pred && v != DBL_MAX.  Read it with dg_reduced_band_sizes / _copy, free it with dg_reduced_band_destroy.
+ *   func: required.  sample_pred: NULL = every node sampled.  reduce_pred: NULL = always true.  flags: 0 or DG_REDUCE_REFERENCE_SORT.
+ *   Per chunk the callbacks run in the order sample_pred, func, reduce_pred.
+ *   timings_ms: NULL or 8 doubles = ms of positions + callbacks (synchronised), kept cells, node compaction, sort, write-back; 1.0 if surviving
+ *       nodes shared Morton keys; total ms; ms spent inside the callbacks (part of [0]). */
+DG_API int dg_reduced_function_create(const dg_grid_desc* grid, dg_device_function func, void* fu, dg_device_sample_predicate sample_pred, void* su,
+                                      dg_device_node_predicate reduce_pred, void* ru, uint64_t chunk_nodes, uint32_t flags, dg_reduced_band** out,
+                                      double* timings_ms);
+/* reduceField(id, pred) (:1065-1174) of a dense field held on the host (nodes[n_nodes], its rows cells[n_cells x 32]), e.g. one just loaded:
+ * the field and its rows are uploaded, the rows checked on the device (an id >= n_nodes: DG_ERR_INVALID), pred evaluated per chunk, and the
+ * handle holds exactly what dg_reduce_field leaves with keep = pred && v != DBL_MAX (the cell map holds i at every i >= n_cells, as
+ * reduceField leaves it).  pred: required.  n_nodes must be the grid's node count (a field that is already reduced: DG_ERR_INVALID, as
+ * dg_reduce_field); n_cells <= nx*ny*nz.  flags: 0 or DG_REDUCE_REFERENCE_SORT.
+ *   timings_ms: NULL or 8 doubles = ms of upload + positions + callbacks, then as dg_reduced_function_create (the rows are checked in the
+ *       kept-cells stage). */
+DG_API int dg_reduce_field_device(const dg_grid_desc* grid, const double* nodes, uint64_t n_nodes, const uint32_t* cells, uint64_t n_cells,
+                                  dg_device_node_predicate pred, void* pu, uint64_t chunk_nodes, uint32_t flags, dg_reduced_band** out,
+                                  double* timings_ms);
 
 #ifdef __cplusplus
 }
