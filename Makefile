@@ -24,7 +24,7 @@ CPPBIN   := build/bin
 CPPFLAGS := -std=c++11 -O2 -ffp-contract=off -I$(EIGEN3_INCLUDE_DIR) -Icpp/include -Iinclude
 CPPLINK  := -Ldiscregrid_b200/lib -ldiscregrid_b200 -Wl,-rpath,'$$ORIGIN/../../discregrid_b200/lib'
 CPPHDRS  := $(wildcard cpp/include/Discregrid/* cpp/include/Discregrid/*/*) include/discregrid_b200.h
-cpp: $(CPPBIN)/GenerateSDF $(CPPBIN)/GenerateDensityMap $(CPPBIN)/DiscreteFieldToBitmap $(CPPBIN)/facade_check $(CPPBIN)/bvh_host_check $(CPPBIN)/reduce_facade_check $(CPPBIN)/sort_replay_check $(CPPBIN)/fast_div_check $(CPPBIN)/libk1emu.so $(CPPBIN)/libk1emu_knobs.so $(CPPBIN)/libk1emu_wave.so $(CPPBIN)/libk1emu_perlane.so $(CPPBIN)/libk1emu_packet.so $(CPPBIN)/libk1emu_band.so $(CPPBIN)/libk1emu_band_perlane.so $(CPPBIN)/libk23emu.so $(CPPBIN)/libk23emu_knobs.so $(CPPBIN)/libdgemu.so $(CPPBIN)/libk4emu.so $(CPPBIN)/device_function_check
+cpp: $(CPPBIN)/GenerateSDF $(CPPBIN)/GenerateDensityMap $(CPPBIN)/DiscreteFieldToBitmap $(CPPBIN)/facade_check $(CPPBIN)/bvh_host_check $(CPPBIN)/reduce_facade_check $(CPPBIN)/sort_replay_check $(CPPBIN)/fast_div_check $(CPPBIN)/libk1emu.so $(CPPBIN)/libk1emu_knobs.so $(CPPBIN)/libk1emu_wave.so $(CPPBIN)/libk1emu_perlane.so $(CPPBIN)/libk1emu_packet.so $(CPPBIN)/libk1emu_band.so $(CPPBIN)/libk1emu_band_perlane.so $(CPPBIN)/libk23emu.so $(CPPBIN)/libk23emu_knobs.so $(CPPBIN)/libdgemu.so $(CPPBIN)/libk4emu.so $(CPPBIN)/device_function_check $(CPPBIN)/device_query_check
 $(CPPBIN)/DiscreteFieldToBitmap: cpp/cmd/discrete_field_to_bitmap.cpp $(CPPHDRS) $(LIB)
 	@mkdir -p $(CPPBIN)
 	$(HOSTCXX) $(CPPFLAGS) $< -o $@ $(CPPLINK)
@@ -97,6 +97,10 @@ CUDA_LIB ?= /usr/local/cuda/lib64
 $(CPPBIN)/device_function_check: tests/cpp/device_function_check.cpp $(CPPHDRS) $(LIB)
 	@mkdir -p $(CPPBIN)
 	$(HOSTCXX) $(CPPFLAGS) -I$(CUDA_INC) $< -o $@ $(CPPLINK) -L$(CUDA_LIB) -lcudart_static -ldl -lrt -lpthread
+# test binary: the facade's reduced calls feed interpolate from the kept handle; it defines its own dg_field_create, which refuses
+$(CPPBIN)/device_query_check: tests/cpp/device_query_check.cpp $(CPPHDRS) $(LIB)
+	@mkdir -p $(CPPBIN)
+	$(HOSTCXX) $(CPPFLAGS) $< -o $@ $(CPPLINK)
 oracle/liboracle.so:
 	$(MAKE) -C oracle oracle
 $(CPPBIN)/GenerateSDF: cpp/cmd/generate_sdf.cpp $(CPPHDRS) $(LIB)

@@ -18,7 +18,9 @@
 //
 // m_nodes / m_cells / m_cell_map hold exactly what the reference would have produced, so save()/load() stay
 // byte-compatible (.cdf/.cdm, :678-778) and reduceField() (host bookkeeping, restated from :1065-1174) keeps working.
-// Device copies of fields are caches owned by this object, dropped by addFunction / load / reduceField.
+// Device copies of fields are caches owned by this object, dropped by addFunction / load / reduceField.  The reduced calls keep the
+// library's handle on their result until the field's first deviceField(), which builds the device copy from it without the host
+// (dg_field_create_reduced); until then the handle's arrays stay in GPU memory.
 //
 // addFunction takes the reference's opaque std::function.  Functors of the two types the reference's own tools build are
 // recognised with std::function::target<>() and run on the GPU, and so are DeviceFunction / DeviceSamplePredicate /
@@ -252,16 +254,13 @@ public:
         const dg_grid_desc d = desc();
         dg_reduced_band* r = nullptr;
         check(dg_reduced_band_create(func.md->handle(), &d, func.sign, pred.band, 0u, &r, m_last_reduced_band_ms));
-        struct Release { dg_reduced_band* r; ~Release() { dg_reduced_band_destroy(r); } } release{r};
-        std::uint64_t n_nodes = 0, n_cells = 0;
-        check(dg_reduced_band_sizes(r, &n_nodes, &n_cells));
-        FieldVector<double> coeffs(n_nodes);
-        FieldVector<std::array<unsigned int, 32>> cells(n_cells);
-        FieldVector<unsigned int> cell_map(m_n_cells);
-        check(dg_reduced_band_copy(r, coeffs.data(), reinterpret_cast<std::uint32_t*>(cells.data()), cell_map.data()));
-        if (verbose) std::cout << "Construction: " << n_nodes << " nodes kept, " << n_cells << " cells, on the GPU in " << m_last_reduced_band_ms[6] << " ms" << std::endl;
+        ReducedHandle hold(r);
+        FieldVector<double> coeffs; FieldVector<std::array<unsigned int, 32>> cells; FieldVector<unsigned int> cell_map;
+        take_reduced(r, coeffs, cells, cell_map);
+        if (verbose) std::cout << "Construction: " << coeffs.size() << " nodes kept, " << cells.size() << " cells, on the GPU in " << m_last_reduced_band_ms[6] << " ms" << std::endl;
         invalidate();
         m_nodes.push_back(std::move(coeffs)); m_cells.push_back(std::move(cells)); m_cell_map.push_back(std::move(cell_map));
+        keep_reduced(static_cast<unsigned int>(m_n_fields), hold);
         return static_cast<unsigned int>(m_n_fields++);
     }
     // new: addFunction(func, verbose, sample) followed by reduceField(id, reduce) in one library call (dg_reduced_function_create); sample /
@@ -277,11 +276,13 @@ public:
         const int rc = dg_reduced_function_create(&d, ctx.func_ptr(), &ctx, ctx.sample_ptr(), &ctx, ctx.node_ptr(), &ctx, 0, 0u, &r, m_last_reduced_function_ms);
         ctx.rethrow();
         check(rc);
+        ReducedHandle hold(r);
         FieldVector<double> coeffs; FieldVector<std::array<unsigned int, 32>> cells; FieldVector<unsigned int> cell_map;
         take_reduced(r, coeffs, cells, cell_map);
         if (verbose) std::cout << "Construction: " << coeffs.size() << " nodes kept, " << cells.size() << " cells, in " << m_last_reduced_function_ms[6] << " ms" << std::endl;
         invalidate();
         m_nodes.push_back(std::move(coeffs)); m_cells.push_back(std::move(cells)); m_cell_map.push_back(std::move(cell_map));
+        keep_reduced(static_cast<unsigned int>(m_n_fields), hold);
         return static_cast<unsigned int>(m_n_fields++);
     }
     // new: GenerateDensityMap with reduction in one library call (dg_reduced_density_map_create).  Leaves exactly what
@@ -301,22 +302,20 @@ public:
         check(dg_reduced_density_map_create(&d, m_nodes[id].data(), m_nodes[id].size(), reinterpret_cast<const std::uint32_t*>(m_cells[id].data()),
                                             m_cells[id].size(), m_cell_map[id].data(), f.smoothing_length, f.rest_density, 0u, &r[0], &r[1],
                                             m_last_reduced_density_ms));
-        struct Release { dg_reduced_band** r; ~Release() { dg_reduced_band_destroy(r[0]); dg_reduced_band_destroy(r[1]); } } release{r};
+        ReducedHandle hold0(r[0]), hold1(r[1]);
         FieldVector<double> coeffs[2];
         FieldVector<std::array<unsigned int, 32>> cells[2];
         FieldVector<unsigned int> cell_map[2];
-        for (int k = 0; k < 2; k++) {         // both copied before anything changes, so a failure leaves the grid as it was
-            std::uint64_t n_nodes = 0, n_cells = 0;
-            check(dg_reduced_band_sizes(r[k], &n_nodes, &n_cells));
-            coeffs[k].resize(n_nodes); cells[k].resize(n_cells); cell_map[k].resize(m_n_cells);
-            check(dg_reduced_band_copy(r[k], coeffs[k].data(), reinterpret_cast<std::uint32_t*>(cells[k].data()), cell_map[k].data()));
-        }
+        for (int k = 0; k < 2; k++)           // both copied before anything changes, so a failure leaves the grid as it was
+            take_reduced(r[k], coeffs[k], cells[k], cell_map[k]);
         if (verbose)
             std::cout << "Construction: density map sampled and both fields reduced on the GPU in " << m_last_reduced_density_ms[12] << " ms ("
                       << coeffs[0].size() << " SDF nodes and " << coeffs[1].size() << " density nodes kept)" << std::endl;
         invalidate();
         m_nodes[id] = std::move(coeffs[0]); m_cells[id] = std::move(cells[0]); m_cell_map[id] = std::move(cell_map[0]);
         m_nodes.push_back(std::move(coeffs[1])); m_cells.push_back(std::move(cells[1])); m_cell_map.push_back(std::move(cell_map[1]));
+        keep_reduced(id, hold0);
+        keep_reduced(static_cast<unsigned int>(m_n_fields), hold1);
         return static_cast<unsigned int>(m_n_fields++);
     }
     // appends a field from node values + the closed-form connectivity (:833-886, built on the GPU) + identity cell map (:888-891)
@@ -423,14 +422,23 @@ public:
                                       d.cell_size[k] = m_cell_size[k]; d.inv_cell_size[k] = m_inv_cell_size[k]; }
         return d;
     }
+    // the device field of field_id, made at first use: from the handle a reduced call kept for it (dg_field_create_reduced, device to device;
+    // the handle is released) or else by uploading the members (dg_field_create).  Making it synchronises the device.
     const dg_field* deviceField(unsigned int field_id) const
     {
         auto it = m_dev.find(field_id);
         if (it != m_dev.end()) return it->second;
-        const dg_grid_desc d = desc();
         dg_field* f = nullptr;
-        check(dg_field_create(&d, m_nodes.at(field_id).data(), m_nodes[field_id].size(), reinterpret_cast<const std::uint32_t*>(m_cells[field_id].data()),
-                              m_cells[field_id].size(), m_cell_map[field_id].data(), &f));
+        auto kept = m_reduced.find(field_id);
+        if (kept != m_reduced.end()) {
+            check(dg_field_create_reduced(kept->second, &f));
+            dg_reduced_band_destroy(kept->second);
+            m_reduced.erase(kept);
+        } else {
+            const dg_grid_desc d = desc();
+            check(dg_field_create(&d, m_nodes.at(field_id).data(), m_nodes[field_id].size(), reinterpret_cast<const std::uint32_t*>(m_cells[field_id].data()),
+                                  m_cells[field_id].size(), m_cell_map[field_id].data(), &f));
+        }
         m_dev[field_id] = f;
         return f;
     }
@@ -444,11 +452,29 @@ private:
     double m_last_reduced_density_ms[13] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
     double m_last_reduced_function_ms[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     mutable std::map<unsigned int, dg_field*> m_dev;
+    // the handles the reduced calls returned, kept until their field's first deviceField or the next invalidate(): a field made from a
+    // handle needs no upload.  Owned like m_dev.
+    mutable std::map<unsigned int, dg_reduced_band*> m_reduced;
 
-    // the arrays of a dg_reduced_band handle, which is destroyed
+    // owns a dg_reduced_band until keep_reduced takes it; destroys it on every other path
+    struct ReducedHandle {
+        dg_reduced_band* r;
+        explicit ReducedHandle(dg_reduced_band* p) : r(p) {}
+        ReducedHandle(const ReducedHandle&) = delete;
+        ReducedHandle& operator=(const ReducedHandle&) = delete;
+        ~ReducedHandle() { dg_reduced_band_destroy(r); }
+    };
+    void keep_reduced(unsigned int field_id, ReducedHandle& h)
+    {
+        dg_reduced_band*& slot = m_reduced[field_id];
+        dg_reduced_band_destroy(slot);
+        slot = h.r;
+        h.r = nullptr;
+    }
+
+    // the arrays of a dg_reduced_band handle (which stays with the caller)
     void take_reduced(dg_reduced_band* r, FieldVector<double>& coeffs, FieldVector<std::array<unsigned int, 32>>& cells, FieldVector<unsigned int>& cell_map) const
     {
-        struct Release { dg_reduced_band* r; ~Release() { dg_reduced_band_destroy(r); } } release{r};
         std::uint64_t n_nodes = 0, n_cells = 0;
         check(dg_reduced_band_sizes(r, &n_nodes, &n_cells));
         coeffs.resize(n_nodes); cells.resize(n_cells); cell_map.resize(m_n_cells);
@@ -456,7 +482,13 @@ private:
     }
 
     static void check(int rc) { if (rc != DG_OK) throw std::runtime_error(std::string("discregrid_b200: ") + dg_last_error()); }
-    void invalidate() { for (auto& kv : m_dev) dg_field_destroy(kv.second); m_dev.clear(); }
+    void invalidate()
+    {
+        for (auto& kv : m_dev) dg_field_destroy(kv.second);
+        m_dev.clear();
+        for (auto& kv : m_reduced) dg_reduced_band_destroy(kv.second);
+        m_reduced.clear();
+    }
     bool in_kept_cell(unsigned int field_id, Eigen::Vector3d const& x) const
     {
         if (!m_domain.contains(x)) return false;
@@ -478,10 +510,12 @@ inline void CubicLagrangeDiscreteGrid::reduceField(unsigned int field_id, Predic
                                               m_cells[field_id].size(), ctx.node_ptr(), &ctx, 0, 0u, &r, m_last_reduced_function_ms);
         ctx.rethrow();
         check(rc);
+        ReducedHandle hold(r);
         FieldVector<double> coeffs; FieldVector<std::array<unsigned int, 32>> cells; FieldVector<unsigned int> cell_map;
         take_reduced(r, coeffs, cells, cell_map);
         invalidate();
         m_nodes[field_id] = std::move(coeffs); m_cells[field_id] = std::move(cells); m_cell_map[field_id] = std::move(cell_map);
+        keep_reduced(field_id, hold);
         return;
     }
     invalidate();

@@ -385,7 +385,7 @@ int dg_mesh_info(const dg_mesh* m, uint64_t info[8])
     info[0] = m->host.n_vertices; info[1] = m->host.n_triangles; info[2] = (uint64_t)m->dev.stack_depth;
     info[3] = (uint64_t)m->host.flags;
     info[4] = m->d_spheres.bytes() + m->d_leaves.bytes() + m->d_normals.bytes() + m->d_nodes_f.bytes() + m->d_leaves_f.bytes();
-    info[5] = m->build_us; info[6] = m->upload_us; info[7] = 0;
+    info[5] = m->build_us; info[6] = m->upload_us; info[7] = (uint64_t)m->device;
     return DG_OK;
 }
 
@@ -1350,7 +1350,7 @@ int dg_field_info(const dg_field* f, uint64_t info[4])
 {
     if (!f || !info) return fail(DG_ERR_INVALID, "dg_field_info: NULL argument");
     info[0] = f->n_nodes; info[1] = f->n_cells_kept;
-    info[2] = f->d_packed.bytes() + f->d_cell_map.bytes() + f->d_tab.bytes(); info[3] = 0;
+    info[2] = f->d_packed.bytes() + f->d_cell_map.bytes() + f->d_tab.bytes(); info[3] = (uint64_t)f->device;
     return DG_OK;
 }
 
@@ -1614,6 +1614,7 @@ static int dg_reduce_field_impl(const dg_grid_desc* grid, double* nodes, uint64_
 // count per 1024 flags for the scans and the survivors' Z-curve keys for the tie-order-preserving sort; the results stay on the device in a
 // dg_reduced_band (a reduced field kept on its device) until dg_reduced_band_copy.
 struct dg_reduced_band {
+    dg_grid_desc desc;                   // the grid it was made for: dg_field_create_reduced builds its field on it
     DevBuf<double> d_nodes;
     DevBuf<unsigned> d_cells, d_cell_map;
     uint64_t n_nodes = 0, n_cells = 0, n_grid_cells = 0;
@@ -1758,6 +1759,7 @@ static int reduced_band_create_impl(const dg_mesh* m, const dg_grid_desc* grid, 
     const cudaStream_t st = nullptr;
     double ms[5] = {0, 0, 0, 0, 0};
     std::unique_ptr<dg_reduced_band> h(new dg_reduced_band());
+    h->desc = *grid;
     DG_CUDA(cudaGetDevice(&h->device));
     // ---- 1. the dense band coefficients (addFunction(func, pred), :806-817), on the device only
     DevBuf<double> d_dense;
@@ -1818,6 +1820,7 @@ static int reduced_density_map_create_impl(const dg_grid_desc* grid, const doubl
     std::unique_ptr<dg_reduced_band> r0(new dg_reduced_band()), r1(new dg_reduced_band());
     DG_CUDA(cudaGetDevice(&r0->device));
     r1->device = r0->device;
+    r0->desc = r1->desc = *grid;
     // ---- 1. upload the SDF field; flag the kept cells of its reduction (this checks the rows) and check the cell map before K2 packs
     //         through them (dg_field_create's checks); pack the SDF field for K3
     DevBuf<double> d_sdf, d_density;
@@ -2036,6 +2039,7 @@ static int reduced_function_create_impl(const dg_grid_desc* grid, dg_device_func
     double ms[5] = {0, 0, 0, 0, 0}, ms_callbacks = 0.0;
     int tie_path = 0;
     std::unique_ptr<dg_reduced_band> h(new dg_reduced_band());
+    h->desc = *grid;
     DG_CUDA(cudaGetDevice(&h->device));
     CallStreamSync st;
     if (int rc = call_stream(st.s)) return rc;
@@ -2077,6 +2081,7 @@ static int reduce_field_device_impl(const dg_grid_desc* grid, const double* node
     double ms[5] = {0, 0, 0, 0, 0}, ms_callbacks = 0.0;
     int tie_path = 0;
     std::unique_ptr<dg_reduced_band> h(new dg_reduced_band());
+    h->desc = *grid;
     DG_CUDA(cudaGetDevice(&h->device));
     CallStreamSync st;
     if (int rc = call_stream(st.s)) return rc;
@@ -2119,6 +2124,27 @@ int dg_reduced_band_copy(const dg_reduced_band* h, double* nodes, uint32_t* cell
 int dg_reduced_band_destroy(dg_reduced_band* h)
 {
     delete h;
+    return DG_OK;
+}
+
+// dg_field_create of the handle's own arrays, device to device: K2's pack reads the handle's rows and nodes, the cell map is copied.  The
+// library made the rows and the cell map, so dg_field_create's host checks have nothing to find.
+int dg_field_create_reduced(const dg_reduced_band* h, dg_field** out)
+{
+    static const char* who = "dg_field_create_reduced";
+    if (!out) return fail(DG_ERR_INVALID, "%s: out is NULL", who);
+    *out = nullptr;
+    if (!h) return fail(DG_ERR_INVALID, "%s: handle is NULL", who);
+    dg_field* f = nullptr;
+    if (int rc = field_common(&h->desc, h->n_nodes, out, f)) return rc;
+    std::unique_ptr<dg_field> own(f);
+    if (int rc = check_handle_device(h->device, who)) return rc;
+    f->n_nodes = h->n_nodes; f->n_cells_kept = h->n_cells;
+    DG_CUDA(f->d_cell_map.alloc(h->n_grid_cells));
+    if (h->n_grid_cells) DG_CUDA(cudaMemcpyAsync(f->d_cell_map.p, h->d_cell_map.p, h->n_grid_cells * sizeof(unsigned), cudaMemcpyDeviceToDevice, nullptr));
+    if (int rc = field_finish(f, h->d_nodes.p, h->d_cells.p, nullptr)) return rc;
+    DG_CUDA(cudaDeviceSynchronize());
+    *out = own.release();
     return DG_OK;
 }
 

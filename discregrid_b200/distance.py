@@ -3,7 +3,8 @@
 Same surface -- construct from a TriangleMesh or from (vertices, triangles), signed_distance / unsigned_distance
 returning Result(distance, nearest_point, nearest_entity, triangle_id) -- but batched: the argument is an (n, 3)
 array of points (a single point is promoted) and each Result field is an array.  All queries run in the sm_90a
-kernel of csrc/k1_sdf.cu; there is no host implementation.
+kernel of csrc/k1_sdf.cu; there is no host implementation.  Points given as a float64 CUDA tensor stay on the device and the
+Result holds CUDA tensors.
 """
 import ctypes as C
 from collections import namedtuple
@@ -12,6 +13,7 @@ from enum import IntEnum
 import numpy as np
 
 from . import _capi as capi
+from . import _device
 from .mesh import TriangleMesh
 
 
@@ -91,7 +93,29 @@ class TriangleMeshDistance:
                                                   capi.ptr(vert, capi.F64P)))
         return tri, edge, vert
 
+    @property
+    def device(self):
+        """the CUDA device the mesh lives on (the library's current device when it was constructed)"""
+        a = (C.c_uint64 * 8)()
+        capi.check(capi.lib.dg_mesh_info(self.handle, a))
+        return int(a[7])
+
+    def _query_device(self, points, signed):
+        """the CUDA-tensor route: dg_mesh_distance_device on torch's current stream, asynchronous like a torch op"""
+        import torch
+        x = _device.points(points, self.device, "signed_distance" if signed else "unsigned_distance")
+        n = len(x)
+        dist = torch.empty(n, dtype=torch.float64, device=x.device)
+        near = torch.empty((n, 3), dtype=torch.float64, device=x.device)
+        ent = torch.empty(n, dtype=torch.int32, device=x.device)
+        tri = torch.empty(n, dtype=torch.int32, device=x.device)
+        capi.check(capi.lib.dg_mesh_distance_device(self.handle, x.data_ptr(), n, int(signed), dist.data_ptr(), near.data_ptr(), ent.data_ptr(),
+                                                    tri.data_ptr(), _device.stream(x)))
+        return Result(dist, near, ent, tri)
+
     def _query(self, points, signed):
+        if _device.is_device_query(points):
+            return self._query_device(points, signed)
         x = np.ascontiguousarray(points, dtype=np.float64).reshape(-1, 3)
         n = len(x)
         dist = np.empty(n); near = np.empty((n, 3)); ent = np.empty(n, np.int32); tri = np.empty(n, np.int32)
@@ -100,9 +124,14 @@ class TriangleMeshDistance:
         return Result(dist, near, ent, tri)
 
     def signed_distance(self, points):      # :269-314
+        """points: (n, 3) or (3,).  A numpy array (or anything numpy converts, CPU tensors included) goes through the host pipeline and
+        returns numpy arrays.  A float64 torch tensor on the mesh's CUDA device stays there: the query runs on torch's current stream,
+        asynchronously, and the Result holds CUDA tensors (distance float64 (n,), nearest_point float64 (n, 3), nearest_entity and
+        triangle_id int32 (n,)) with the same bits as the host route."""
         return self._query(points, True)
 
     def unsigned_distance(self, points):    # :316-334
+        """as signed_distance, unsigned"""
         return self._query(points, False)
 
 

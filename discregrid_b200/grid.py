@@ -19,7 +19,11 @@ that save()/load() stay byte-compatible with the reference's .cdf/.cdm files
                                          -> dg_reduce_field_device (your predicate on the GPU, then reduceField's passes there)
   addReducedFunction(DeviceFunction, DeviceSamplePredicate, DeviceNodePredicate)
                                          -> dg_reduced_function_create (addFunction + reduceField, the dense field kept on the GPU)
-  interpolate(field_id, x[, gradient])   -> dg_interpolate_batch (K2, csrc/k2_interp.cu), batched over x
+  interpolate(field_id, x[, gradient])   -> dg_interpolate_batch (K2, csrc/k2_interp.cu), batched over x; a float64 CUDA tensor x
+                                            -> dg_interpolate_batch_device on torch's current stream (CUDA tensors out, autograd in x)
+
+The reduced calls keep the handle they get from the library until the field's first device use, which builds the interpolation
+field from it on the device (dg_field_create_reduced) instead of uploading the host copy again.
 
 The reference's addFunction takes an opaque std::function.  The two functor types the reference's own tools build are recognised
 and run on the library's kernels; a function of your own runs as your own GPU code when wrapped in DeviceFunction (and its
@@ -33,6 +37,7 @@ import struct
 import numpy as np
 
 from . import _capi as capi
+from . import _device
 from .distance import MeshDistanceBand, MeshSignedDistance
 
 
@@ -51,7 +56,10 @@ class DeviceFunction:
     they get DBL_MAX anyway.  values: float64 tensor (n,) on the same device.  Both tensors view the library's buffers (no copy) and are only
     valid during the call.  fn runs on the library's stream (torch.cuda.ExternalStream), which first waits for the torch stream that was current
     when the grid method was called, so fn sees every tensor computed before the call; plain torch operations inside fn are ordered with the
-    library's own work."""
+    library's own work.  So are the library's own queries on CUDA tensors, which run on torch's current stream: fn may be a function of a
+    mesh or of an existing field, e.g. lambda x, k: md.signed_distance(x).distance or lambda x, k: other.interpolate(0, x) - r.  A field
+    used inside fn should have its device field before the call (one interpolate on it is enough): making it synchronises the device, and
+    inside fn that would stall every chunk's queued work."""
 
     def __init__(self, fn):
         if not callable(fn):
@@ -169,8 +177,8 @@ class _DeviceCallbacks:
         return cb
 
 
-def _copy_reduced(h, n_grid_cells):
-    """the (nodes, cells, cell map) of a dg_reduced_band handle, which is destroyed"""
+def _copy_reduced(h, n_grid_cells, keep=False):
+    """the (nodes, cells, cell map) of a dg_reduced_band handle, which is destroyed unless keep is set"""
     try:
         n_nodes, n_cells = C.c_uint64(), C.c_uint64()
         capi.check(capi.lib.dg_reduced_band_sizes(h, C.byref(n_nodes), C.byref(n_cells)))
@@ -178,7 +186,47 @@ def _copy_reduced(h, n_grid_cells):
         capi.check(capi.lib.dg_reduced_band_copy(h, capi.ptr(f[0], capi.F64P), capi.ptr(f[1], capi.U32P), capi.ptr(f[2], capi.U32P)))
         return f
     finally:
-        capi.lib.dg_reduced_band_destroy(h)
+        if not keep:
+            capi.lib.dg_reduced_band_destroy(h)
+
+
+def _copy_kept(handles, n_grid_cells):
+    """the (nodes, cells, cell map) of each dg_reduced_band handle; the handles are kept for the grid's first _device_field, or all
+    destroyed when a copy fails"""
+    try:
+        return [_copy_reduced(h, n_grid_cells, keep=True) for h in handles]
+    except BaseException:
+        for h in handles:
+            capi.lib.dg_reduced_band_destroy(h)
+        raise
+
+
+_INTERPOLATE = None
+
+
+def _interpolate_function():
+    """the autograd Function of interpolate on CUDA tensors: phi(x) with d phi / d x = K2's gradient, first order only.  Made at first use:
+    torch is only imported by callers that pass tensors."""
+    global _INTERPOLATE
+    if _INTERPOLATE is None:
+        import torch
+        from torch.autograd.function import once_differentiable
+
+        class Interpolate(torch.autograd.Function):
+            @staticmethod
+            def forward(ctx, x, run):
+                phi, grad = run(x, True)
+                ctx.mark_non_differentiable(grad)
+                ctx.save_for_backward(grad)
+                return phi, grad
+
+            @staticmethod
+            @once_differentiable
+            def backward(ctx, grad_phi, _grad_grad):
+                (grad,) = ctx.saved_tensors
+                return grad_phi[:, None] * grad, None
+        _INTERPOLATE = Interpolate
+    return _INTERPOLATE
 
 
 def grid_desc(domain_min, domain_max, resolution, cell_size=None, inv_cell_size=None):
@@ -208,6 +256,7 @@ class CubicLagrangeDiscreteGrid:
         self.m_nodes, self.m_cells, self.m_cell_map = [], [], []
         self.m_n_fields = 0
         self._fields = {}          # field_id -> device handle (cache; invalidated by addFunction/load/reduceField)
+        self._reduced = {}         # field_id -> the dg_reduced_band its reduced call returned, until its first _device_field (or invalidation)
         self._desc = None
         if isinstance(domain_or_filename, str):
             self.load(domain_or_filename)
@@ -320,7 +369,12 @@ class CubicLagrangeDiscreteGrid:
     def addReducedBandField(self, func, pred, verbose=False):
         """addFunction(func, verbose, pred) followed by reduceField(id, always true), in one GPU call (dg_reduced_band_create): the field
         holds exactly what those two calls leave, but only the survivors and the cell map ever reach the host.  func: MeshSignedDistance,
-        pred: MeshDistanceBand over the same TriangleMeshDistance.  Returns the field id."""
+        pred: MeshDistanceBand over the same TriangleMeshDistance.  Returns the field id.
+        The library's handle on the device copy of the result is kept: the field's first interpolate (or any other device use) builds its
+        interpolation field from it on the device and then releases it, with no host round trip.  Until then, or until the grid's device
+        fields are invalidated (addFunction, reduceField, load, ...), the handle's arrays stay held in GPU memory -- for the 512^3 bunny band
+        (49.4 M nodes, 6.28 M cells) 0.40 GB of nodes, 0.80 GB of rows and 0.54 GB of cell map.  The same holds for addReducedFunction,
+        addReducedDensityMap (both fields) and reduceField with a DeviceNodePredicate."""
         if not isinstance(func, MeshSignedDistance) or not isinstance(pred, MeshDistanceBand):
             raise TypeError("addReducedBandField takes a MeshSignedDistance and a MeshDistanceBand")
         if pred.md is not func.md:
@@ -329,26 +383,19 @@ class CubicLagrangeDiscreteGrid:
         self.last_reduced_band_ms = np.zeros(7)
         capi.check(capi.lib.dg_reduced_band_create(func.md.handle, C.byref(self._desc), func.sign, pred.band, 0, C.byref(h),
                                                    capi.ptr(self.last_reduced_band_ms, capi.F64P)))
-        try:
-            n_nodes, n_cells = C.c_uint64(), C.c_uint64()
-            capi.check(capi.lib.dg_reduced_band_sizes(h, C.byref(n_nodes), C.byref(n_cells)))
-            coeffs = np.empty(n_nodes.value)
-            cells = np.empty((n_cells.value, 32), np.uint32)
-            cmap = np.empty(self.m_n_cells, np.uint32)
-            capi.check(capi.lib.dg_reduced_band_copy(h, capi.ptr(coeffs, capi.F64P), capi.ptr(cells, capi.U32P), capi.ptr(cmap, capi.U32P)))
-        finally:
-            capi.lib.dg_reduced_band_destroy(h)
+        coeffs, cells, cmap = _copy_kept([h], self.m_n_cells)[0]
         if verbose:
             print(f"Construction: {len(coeffs)} of {self.nNodes()} nodes kept in {self.last_reduced_band_ms[6]:.1f} ms on the GPU")
         self.m_nodes.append(coeffs); self.m_cells.append(cells); self.m_cell_map.append(cmap)
         self.m_n_fields += 1
+        self._keep_reduced(self.m_n_fields - 1, h)
         return self.m_n_fields - 1
 
     def addReducedFunction(self, func, sample_pred=None, reduce_pred=None, verbose=False):
         """addFunction(func, verbose, sample_pred) followed by reduceField(id, reduce_pred), in one call (dg_reduced_function_create): the
         field holds exactly what those two calls leave, but the dense values stay on the GPU; only the survivors and the cell map reach the
         host.  func: DeviceFunction; sample_pred: DeviceSamplePredicate or None; reduce_pred: DeviceNodePredicate or None (always true).
-        Returns the field id."""
+        Returns the field id.  The result's device copy is kept for the field's first interpolate, as in addReducedBandField."""
         if not isinstance(func, DeviceFunction) or not isinstance(sample_pred, (DeviceSamplePredicate, type(None))) \
                 or not isinstance(reduce_pred, (DeviceNodePredicate, type(None))):
             raise TypeError("addReducedFunction takes a DeviceFunction, a DeviceSamplePredicate or None and a DeviceNodePredicate or None")
@@ -357,19 +404,21 @@ class CubicLagrangeDiscreteGrid:
         cb = _DeviceCallbacks(func=func, sample=sample_pred, node=reduce_pred)
         cb.check(capi.lib.dg_reduced_function_create(C.byref(self._desc), cb.func, None, cb.sample, None, cb.node, None, 0, 0, C.byref(h),
                                                      capi.ptr(self.last_reduced_function_ms, capi.F64P)))
-        coeffs, cells, cmap = _copy_reduced(h, self.m_n_cells)
+        coeffs, cells, cmap = _copy_kept([h], self.m_n_cells)[0]
         if verbose:
             print(f"Construction: {len(coeffs)} of {self.nNodes()} nodes kept in {self.last_reduced_function_ms[6]:.1f} ms")
         self._invalidate()
         self.m_nodes.append(coeffs); self.m_cells.append(cells); self.m_cell_map.append(cmap)
         self.m_n_fields += 1
+        self._keep_reduced(self.m_n_fields - 1, h)
         return self.m_n_fields - 1
 
     def addReducedDensityMap(self, func):
         """GenerateDensityMap with reduction in one GPU call (dg_reduced_density_map_create): leaves exactly what
         addFunction(func) followed by reduceField(func.field_id, p0) and reduceField(new_id, p1) leave, with the tool's predicates
         p0(x, v) = -6h < v + cell_diag & v - cell_diag < 2h and p1(x, v) = 0 <= v <= 3 rho0 (main.cpp:139-140).  The SDF field is replaced by
-        its reduction and the reduced density field is appended; the dense density field never reaches the host.  Returns the new field id."""
+        its reduction and the reduced density field is appended; the dense density field never reaches the host.  Returns the new field id.
+        The device copies of both results are kept for the fields' first interpolate, as in addReducedBandField."""
         if not isinstance(func, DensityMapFunction):
             raise TypeError("addReducedDensityMap takes a DensityMapFunction")
         if func.no_reduction:
@@ -385,21 +434,13 @@ class CubicLagrangeDiscreteGrid:
         capi.check(capi.lib.dg_reduced_density_map_create(C.byref(self._desc), capi.ptr(nodes, capi.F64P), len(nodes), capi.ptr(cells, capi.U32P),
                                                           len(cells), capi.ptr(cmap, capi.U32P), func.h, func.rho0, 0, C.byref(r[0]), C.byref(r[1]),
                                                           capi.ptr(self.last_reduced_density_ms, capi.F64P)))
-        out = []
-        try:
-            for h in r:
-                n_nodes, n_cells = C.c_uint64(), C.c_uint64()
-                capi.check(capi.lib.dg_reduced_band_sizes(h, C.byref(n_nodes), C.byref(n_cells)))
-                f = (np.empty(n_nodes.value), np.empty((n_cells.value, 32), np.uint32), np.empty(self.m_n_cells, np.uint32))
-                capi.check(capi.lib.dg_reduced_band_copy(h, capi.ptr(f[0], capi.F64P), capi.ptr(f[1], capi.U32P), capi.ptr(f[2], capi.U32P)))
-                out.append(f)
-        finally:
-            for h in r:
-                capi.lib.dg_reduced_band_destroy(h)
+        out = _copy_kept(r, self.m_n_cells)
         self._invalidate()
         self.m_nodes[fid], self.m_cells[fid], self.m_cell_map[fid] = out[0]
         self.m_nodes.append(out[1][0]); self.m_cells.append(out[1][1]); self.m_cell_map.append(out[1][2])
         self.m_n_fields += 1
+        self._keep_reduced(fid, r[0])
+        self._keep_reduced(self.m_n_fields - 1, r[1])
         return self.m_n_fields - 1
 
     def addSampledFunction(self, coeffs):
@@ -420,7 +461,8 @@ class CubicLagrangeDiscreteGrid:
     def reduceField(self, field_id, pred):
         """Sparsifies a field.  pred(x[n,3], values[n]) -> bool[n] is the reference's Predicate, vectorised; nodes, cells and the
         cell map end up exactly as the reference leaves them (dg_reduce_field).  A DeviceNodePredicate runs on the GPU instead, on
-        positions made there, and so does the whole reduction (dg_reduce_field_device)."""
+        positions made there, and so does the whole reduction (dg_reduce_field_device); its device copy of the result is kept for the
+        field's first interpolate, as in addReducedBandField."""
         if isinstance(pred, DeviceNodePredicate):
             nodes = np.ascontiguousarray(self.m_nodes[field_id], np.float64)
             cells = np.ascontiguousarray(self.m_cells[field_id], np.uint32)
@@ -428,9 +470,10 @@ class CubicLagrangeDiscreteGrid:
             cb = _DeviceCallbacks(node=pred)
             cb.check(capi.lib.dg_reduce_field_device(C.byref(self._desc), capi.ptr(nodes, capi.F64P), len(nodes), capi.ptr(cells, capi.U32P),
                                                      len(cells), cb.node, None, 0, 0, C.byref(h), None))
-            out = _copy_reduced(h, self.m_n_cells)
+            out = _copy_kept([h], self.m_n_cells)[0]
             self._invalidate()
             self.m_nodes[field_id], self.m_cells[field_id], self.m_cell_map[field_id] = out
+            self._keep_reduced(field_id, h)
             return
         nodes = np.ascontiguousarray(self.m_nodes[field_id], np.float64).copy()
         keep = np.asarray(pred(self.nodePositions(0, len(nodes)), nodes), bool) & (nodes != np.finfo(np.float64).max)   # :1073
@@ -445,18 +488,35 @@ class CubicLagrangeDiscreteGrid:
 
     # ------------------------------------------------------------------ device field cache
     def _device_field(self, field_id):
+        """the device field of field_id, made at first use: from the reduced handle the field's reduced call kept (dg_field_create_reduced,
+        device to device; the handle is released) or else by uploading the host members (dg_field_create).  Creating it synchronises the
+        device."""
         if field_id not in self._fields:
-            nodes, cells, cmap = self.m_nodes[field_id], self.m_cells[field_id], self.m_cell_map[field_id]
             h = C.c_void_p()
-            capi.check(capi.lib.dg_field_create(C.byref(self._desc), capi.ptr(nodes, capi.F64P), len(nodes),
-                                                capi.ptr(cells, capi.U32P), len(cells), capi.ptr(cmap, capi.U32P), C.byref(h)))
+            r = self._reduced.get(field_id)
+            if r is not None:
+                capi.check(capi.lib.dg_field_create_reduced(r, C.byref(h)))
+                capi.lib.dg_reduced_band_destroy(self._reduced.pop(field_id))
+            else:
+                nodes, cells, cmap = self.m_nodes[field_id], self.m_cells[field_id], self.m_cell_map[field_id]
+                capi.check(capi.lib.dg_field_create(C.byref(self._desc), capi.ptr(nodes, capi.F64P), len(nodes),
+                                                    capi.ptr(cells, capi.U32P), len(cells), capi.ptr(cmap, capi.U32P), C.byref(h)))
             self._fields[field_id] = h
         return self._fields[field_id]
+
+    def _keep_reduced(self, field_id, h):
+        """keeps the handle a reduced call returned for field_id, so that the field's first _device_field needs no upload"""
+        old = self._reduced.pop(field_id, None)
+        if old is not None:
+            capi.lib.dg_reduced_band_destroy(old)
+        self._reduced[field_id] = h
 
     def _invalidate(self):
         for h in self._fields.values():
             capi.lib.dg_field_destroy(h)
-        self._fields = {}
+        for h in self._reduced.values():
+            capi.lib.dg_reduced_band_destroy(h)
+        self._fields, self._reduced = {}, {}
 
     def __del__(self):
         try:
@@ -467,16 +527,42 @@ class CubicLagrangeDiscreteGrid:
     # ------------------------------------------------------------------ interpolate (cubic_lagrange_discrete_grid.cpp:977-1063)
     def interpolate(self, field_id_or_x, x=None, gradient=False):
         """interpolate(x) == interpolate(0, x) (discrete_grid.hpp:38-41).  x: (n, 3).  Returns phi[n], or
-        (phi[n], grad[n,3]) when gradient=True.  Out-of-domain / removed cell / missing coefficient -> DBL_MAX, grad 0."""
+        (phi[n], grad[n,3]) when gradient=True.  Out-of-domain / removed cell / missing coefficient -> DBL_MAX, grad 0.
+        A numpy array (or a CPU tensor) goes through the host pipeline and gives numpy arrays.  A float64 torch tensor (n, 3) or (3,) on
+        the field's CUDA device stays there: the query runs on torch's current stream, asynchronously, and phi / grad are CUDA tensors with
+        the bits of the host route.  When x requires grad (and grad mode is on), phi is differentiable in x, first order only:
+        d phi / d x is K2's gradient, the reference's derivative of the interpolant (0 at DBL_MAX).  The returned grad is not differentiable."""
         if x is None:
             field_id, x = 0, field_id_or_x
         else:
             field_id = field_id_or_x
+        if _device.is_device_query(x):
+            return self._interpolate_device(field_id, x, gradient)
         x = np.ascontiguousarray(x, np.float64).reshape(-1, 3)
         phi = np.empty(len(x))
         grad = np.empty((len(x), 3)) if gradient else None
         capi.check(capi.lib.dg_interpolate_batch(self._device_field(field_id), capi.ptr(x, capi.F64P), len(x),
                                                  capi.ptr(phi, capi.F64P), capi.ptr(grad, capi.F64P)))
+        return (phi, grad) if gradient else phi
+
+    def _interpolate_device(self, field_id, x, gradient):
+        """the CUDA-tensor route: dg_interpolate_batch_device on torch's current stream"""
+        import torch
+        h = self._device_field(field_id)
+        info = (C.c_uint64 * 4)()
+        capi.check(capi.lib.dg_field_info(h, info))
+        x = _device.points(x, int(info[3]), "interpolate")
+
+        def run(xc, with_grad):
+            phi = torch.empty(len(xc), dtype=torch.float64, device=xc.device)
+            grad = torch.empty((len(xc), 3), dtype=torch.float64, device=xc.device) if with_grad else None
+            capi.check(capi.lib.dg_interpolate_batch_device(h, xc.data_ptr(), len(xc), phi.data_ptr(), None if grad is None else grad.data_ptr(),
+                                                            _device.stream(xc)))
+            return phi, grad
+        if x.requires_grad and torch.is_grad_enabled():
+            phi, grad = _interpolate_function().apply(x, run)
+        else:
+            phi, grad = run(x, gradient)
         return (phi, grad) if gradient else phi
 
     # ------------------------------------------------------------------ save / load (cubic_lagrange_discrete_grid.cpp:678-778)

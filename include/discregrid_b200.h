@@ -113,7 +113,7 @@ DG_API int dg_mesh_create(const double* vertices, uint64_t n_vertices, const uin
 DG_API int dg_mesh_destroy(dg_mesh* mesh);
 /* info[0]=n_vertices, [1]=n_triangles, [2]=max stack depth, [3]=watertight flags (bit0: edge with one
  * triangle, bit1: edge with >2 triangles -- the two warnings of TriangleMeshDistance.h:422-438),
- * [4]=device bytes, [5]=host build microseconds, [6]=upload microseconds */
+ * [4]=device bytes, [5]=host build microseconds, [6]=upload microseconds, [7]=the CUDA device the mesh lives on */
 DG_API int dg_mesh_info(const dg_mesh* mesh, uint64_t info[8]);
 /* Test/diagnostic: copies the host-built tree in the reference's node numbering (pre-order; left == -1 marks
  * a leaf whose `right` is the triangle id).  spheres: n_nodes x 8 (cl.xyz, rl, cr.xyz, rr), kids: n_nodes x 2.
@@ -225,7 +225,7 @@ DG_API int dg_field_create(const dg_grid_desc* grid, const double* nodes, uint64
 /* same, coefficient array already on the device (e.g. straight out of dg_sample_sdf_device); unreduced only */
 DG_API int dg_field_create_device(const dg_grid_desc* grid, const double* d_nodes, uint64_t n_nodes, void* stream, dg_field** out);
 DG_API int dg_field_destroy(dg_field* field);
-/* info[0]=n_nodes, [1]=n_cells_kept, [2]=device bytes */
+/* info[0]=n_nodes, [1]=n_cells_kept, [2]=device bytes, [3]=the CUDA device the field lives on */
 DG_API int dg_field_info(const dg_field* field, uint64_t info[4]);
 
 /* Batched CubicLagrangeDiscreteGrid::interpolate(field_id, x, gradient*) (cubic_lagrange_discrete_grid.cpp:977-1063;
@@ -289,6 +289,13 @@ DG_API int dg_reduced_band_create(const dg_mesh* mesh, const dg_grid_desc* grid,
 DG_API int dg_reduced_band_sizes(const dg_reduced_band* result, uint64_t* n_nodes, uint64_t* n_cells);
 DG_API int dg_reduced_band_copy(const dg_reduced_band* result, double* nodes, uint32_t* cells, uint32_t* cell_map);
 DG_API int dg_reduced_band_destroy(dg_reduced_band* result);
+/* An interpolation field (the packed layout of dg_field_create) made from the reduced field held by a dg_reduced_band handle
+ * (dg_reduced_band_create, dg_reduced_density_map_create, dg_reduced_function_create, dg_reduce_field_device), entirely on the
+ * handle's device: nothing is copied to or from the host and the rows are not re-checked (the library made them).  The field has the
+ * grid the handle was made for, and dg_field_info gives what it gives for dg_field_create of the handle's dg_reduced_band_copy.
+ * Synchronous: when it returns, the field does not depend on the handle, which may be destroyed.  The handle must live on the current
+ * device (DG_ERR_INVALID otherwise).  A handle with no kept cell gives a field whose every query returns DBL_MAX. */
+DG_API int dg_field_create_reduced(const dg_reduced_band* r, dg_field** out);
 
 /* ---- reduced density map: GenerateDensityMap with reduction in one call -----------------------------------------------------------
  * GenerateDensityMap with reduction (cmd/generate_density_map/main.cpp:117-147) in one call:
