@@ -183,6 +183,7 @@ struct dg_field {
     DevBuf<unsigned> d_cell_map;
     DevBuf<double2> d_tab;
     uint64_t n_nodes = 0, n_cells_kept = 0;
+    double coeff_max = 0.0;      // k3_coeff_max of the packed coefficients: whether K3 may skip points outside the kernel support
     int device = 0;
 };
 
@@ -1276,6 +1277,7 @@ static int field_finish(dg_field* f, const double* d_nodes, const unsigned* d_ce
     if (e == cudaSuccess) e = f->d_tab.alloc(f->dev.g.n[0] + f->dev.g.n[1] + f->dev.g.n[2]);
     if (e == cudaSuccess) { e = k2_launch_pack(f->dev.g, d_nodes, d_cells, f->n_cells_kept, f->d_packed.p, stream); g_launches.fetch_add(1); }
     if (e == cudaSuccess) { e = k2_launch_axis_tables(f->dev.g, f->d_tab.p, stream); g_launches.fetch_add(1); }
+    if (e == cudaSuccess) { e = k3_coeff_max(f->d_packed.p, 32 * f->n_cells_kept, &f->coeff_max, stream); g_launches.fetch_add(1); }
     if (e != cudaSuccess) return fail(e == cudaErrorMemoryAllocation ? DG_ERR_NOMEM : DG_ERR_CUDA, "dg_field_create: %s", cudaGetErrorString(e));
     f->dev.packed = f->d_packed.p;
     f->dev.cell_map = f->d_cell_map.p;
@@ -1500,7 +1502,7 @@ int dg_density_map_device(const dg_field* f, double h, double rho0, int no_reduc
     if (!(h > 0.0)) return fail(DG_ERR_INVALID, "dg_density_map: smoothing length must be > 0");
     if (l_end > l_begin && !d_out) return fail(DG_ERR_INVALID, "dg_density_map: output is NULL");
     if (int rc = check_handle_device(f->device, "dg_density_map")) return rc;
-    DG_LAUNCH(k3_launch_density(f->dev, h, rho0, no_reduction, l_begin, l_end - l_begin, d_out, (cudaStream_t)stream));
+    DG_LAUNCH(k3_launch_density(f->dev, f->coeff_max, h, rho0, no_reduction, l_begin, l_end - l_begin, d_out, (cudaStream_t)stream));
     return DG_OK;
 }
 
@@ -1851,7 +1853,7 @@ static int reduced_density_map_create_impl(const dg_grid_desc* grid, const doubl
     ms[0] += clock.lap();
     // ---- 2. addFunction(density_func, verbose, pred) (main.cpp:96-133): K3 over every node, predicate on
     DG_CUDA(d_density.alloc(n));
-    DG_LAUNCH(k3_launch_density(f->dev, h, rho0, 0, 0, n, d_density.p, st));
+    DG_LAUNCH(k3_launch_density(f->dev, f->coeff_max, h, rho0, 0, 0, n, d_density.p, st));
     DG_CUDA(cudaStreamSynchronize(st));
     ms[1] = clock.lap();
     // ---- 3. the packed SDF field is not needed any more: free it before reducing anything

@@ -13,10 +13,25 @@
 // The 4096-term sum is sequential in the reference, so for bit-exact parity one lane owns one node and walks
 // the 4096 points in order; parallelism comes from the 10^8 nodes.  Everything that does not depend on the
 // node is tabulated on the host with the reference's operation order: the 16 offsets c0*xi+c1 per axis, the
-// 16 weights, and W at the 4096 points (constant / global memory).  Points with W == 0 (outside the kernel
-// support, ~48 % of the cube) contribute exactly +0 to a non-negative accumulator and are skipped -- valid for
-// fields whose coefficients are finite or the DBL_MAX sentinel.  The 32 adjacent nodes of a warp sample 32
+// 16 weights, and W at the 4096 points (constant / global memory).  The 32 adjacent nodes of a warp sample 32
 // adjacent points at every step, i.e. one to three cells, so the 256-byte coefficient blocks are L1 hits.
+//
+// Points with W == 0 (outside the kernel support, ~48 % of the cube) add wijk * (gamma * 0).  That is +-0, which
+// leaves the accumulator unchanged (it starts at +0 and every term is >= 0), only while gamma is finite; the
+// reference adds NaN where gamma = 1 - d/h is +inf (d/h overflowed to -inf) or NaN (d is NaN), and a field may
+// hold anything (dg_field_create does not look at values, a .cdf may hold NaN, inf or -DBL_MAX).  So the
+// skipping kernel (SKIP_ZERO_W) runs only when gamma is finite at every point by construction:
+//   * M = max |c| over the field's packed coefficients c != DBL_MAX, with M = +inf if one of them is NaN or
+//     +-inf (k3_coeff_max, once per field).  A cell holding a DBL_MAX coefficient interpolates to DBL_MAX
+//     whatever its other terms are, and d = DBL_MAX > h gives gamma = 0, or 1 - DBL_MAX/inf = 1 for h = inf.
+//   * Otherwise d = sum_j c_j N_j(X) over a cell's 32 coefficients with X in [-1, 1]^3 up to rounding, and
+//     sum_j |N_j| <= 8 there: the 8 corner functions facc (1+-x)(1+-y)(1+-z) with |facc| <= 19/64 sum to at
+//     most 8 * 19/64 < 2.4 (the products sum to 8); the 8 edge functions along x, 9/64 (1-x^2)(1+-3x)(1+-y)(1+-z),
+//     to 9/64 * 4 * (1-x^2) * 2 max(1, 3|x|) <= 9/64 * 4 * 4/sqrt(3) < 1.3, likewise along y and z.  Total < 6.3.
+//     Each product and partial sum is then below 8 M (1 + 1e-14), so with 64 M < DBL_MAX every partial sum
+//     and d are finite, and |d / h| <= 8 M / h < DBL_MAX when 64 M / h < DBL_MAX: gamma is finite.
+// k3_launch_density takes M and picks the instantiation; a field that fails the bound (or h too small for
+// it) samples all 4096 points as the reference does.
 #include "dg_device.cuh"
 #include "k3_density.h"
 #include "fast_div.h"
@@ -28,9 +43,11 @@
 #define K3_FAST_DIV 1
 #endif
 
+#include <algorithm>
 #include <cfloat>
 #include <climits>
 #include <cmath>
+#include <cstring>
 #include <vector>
 
 namespace dgb {
@@ -119,6 +136,7 @@ __device__ __forceinline__ double interp_value(const FieldDev& f, double x, doub
                                    // no spills (6 -> 80 registers and 8 B of spill stores, 8 -> 64 registers and 144 B).  H100 80GB HBM3
                                    // capped at 400 W, 128^3 bunny field: 4 / 5 / 6 / 8 -> 380 / 372-380 / 381-383 / 500 ms
 #endif
+template <bool SKIP_ZERO_W>
 __global__ void __launch_bounds__(128, K3_MIN_BLOCKS)
 density_map_kernel(FieldDev f, QuadParams qp, const double* __restrict__ Wtab, int no_reduction, unsigned l_begin,
                    unsigned long long count, double* __restrict__ out)
@@ -149,7 +167,7 @@ density_map_kernel(FieldDev f, QuadParams qp, const double* __restrict__ Wtab, i
 #pragma unroll 1
             for (int k = 0; k < 16; k++) {
                 const double W = __ldg(wrow + k);
-                if (W == 0.0) continue;                              // contributes exactly +0 (see header)
+                if (SKIP_ZERO_W && W == 0.0) continue;               // contributes exactly +0 (see header)
                 const double wijk = wij * qp.w[k];
                 const double d = interp_value(f, sx, sy, z + qp.off[k]);
 #if K3_FAST_DIV
@@ -169,7 +187,48 @@ density_map_kernel(FieldDev f, QuadParams qp, const double* __restrict__ Wtab, i
     out[idx] = qp.rho0 * res;                                        // main.cpp:111
 }
 
+// M of the header: the bit patterns of |c| for c != DBL_MAX, maximised with atomicMax.  Non-negative doubles order like their bits, and
+// |NaN| (exponent all ones, mantissa != 0) and +inf come out above every finite value.
+__global__ void __launch_bounds__(256)
+coeff_max_kernel(const double* __restrict__ packed, unsigned long long n, unsigned long long* __restrict__ out)
+{
+    unsigned long long m = 0;
+    const unsigned long long stride = (unsigned long long)gridDim.x * blockDim.x;
+#pragma unroll 4
+    for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+        const double c = __ldg(packed + i);
+        const unsigned long long b = (unsigned long long)__double_as_longlong(fabs(c));
+        if (c != DBL_MAX && b > m) m = b;
+    }
+    if (m) atomicMax(out, m);
+}
+
 }  // namespace
+
+cudaError_t k3_coeff_max(const double* d_packed, uint64_t n, double* out, cudaStream_t stream)
+{
+    const unsigned blocks = (unsigned)std::min<uint64_t>((n + 255) / 256, 1024), nb = blocks ? blocks : 1;
+    unsigned long long bits = 0;
+#ifdef DG_EMU
+    DG_KERNEL_LAUNCH(coeff_max_kernel, nb, 256, 0, stream, d_packed, (unsigned long long)n, &bits);
+#else
+    unsigned long long* d_bits = nullptr;
+    cudaError_t e = cudaMallocAsync(reinterpret_cast<void**>(&d_bits), sizeof bits, stream);
+    if (e != cudaSuccess) return e;
+    e = cudaMemsetAsync(d_bits, 0, sizeof bits, stream);
+    if (e == cudaSuccess) {
+        DG_KERNEL_LAUNCH(coeff_max_kernel, nb, 256, 0, stream, d_packed, (unsigned long long)n, d_bits);
+        e = DG_AFTER_LAUNCH();
+    }
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&bits, d_bits, sizeof bits, cudaMemcpyDeviceToHost, stream);
+    cudaFreeAsync(d_bits, stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
+    if (e != cudaSuccess) return e;
+#endif
+    if (bits > 0x7ff0000000000000ull) bits = 0x7ff0000000000000ull;    // NaN -> +inf
+    std::memcpy(out, &bits, sizeof bits);
+    return cudaSuccess;
+}
 
 // Host tables.  This TU is compiled without FP contraction on the host side as well (x86-64 baseline has no FMA;
 // -ffp-contract=off is passed explicitly), so these match the reference's CPU arithmetic bit for bit.
@@ -180,10 +239,15 @@ double k3_cell_diag(const GridDev& g)
     return std::sqrt((g.cell[0] * g.cell[0] + g.cell[1] * g.cell[1]) + g.cell[2] * g.cell[2]);
 }
 
-cudaError_t k3_launch_density(const FieldDev& f, double h, double rho0, int no_reduction, uint64_t l_begin, uint64_t count,
-                              double* d_out, cudaStream_t stream)
+cudaError_t k3_launch_density(const FieldDev& f, double coeff_max, double h, double rho0, int no_reduction, uint64_t l_begin,
+                              uint64_t count, double* d_out, cudaStream_t stream)
 {
     if (count == 0) return cudaSuccess;
+    // the bound of the header: W == 0 points may be skipped when 64 M and 64 M / h are finite (h > 0 is the caller's to check; h = +inf
+    // passes: every point then lies outside the domain, see the header)
+    const double m64 = 64.0 * coeff_max;
+    const bool skip_zero_w = (m64 < DBL_MAX) && (m64 / h < DBL_MAX);
+    const auto kernel = skip_zero_w ? density_map_kernel<true> : density_map_kernel<false>;
     QuadParams qp;
     // integrate(): c0 = 0.5 * diagonal, c1 = 0.5 * (min + max) of [-h, h]^3 (gauss_quadrature.cpp:5937-5938)
     const double lo = -h, hi = h;
@@ -215,7 +279,7 @@ cudaError_t k3_launch_density(const FieldDev& f, double h, double rho0, int no_r
             }
     const unsigned blocks = (unsigned)((count + 127) / 128);
 #ifdef DG_EMU
-    DG_KERNEL_LAUNCH(density_map_kernel, blocks, 128, 0, stream, f, qp, W.data(), no_reduction, (unsigned)l_begin, (unsigned long long)count, d_out);
+    DG_KERNEL_LAUNCH(kernel, blocks, 128, 0, stream, f, qp, W.data(), no_reduction, (unsigned)l_begin, (unsigned long long)count, d_out);
     return cudaSuccess;
 #else
     double* d_W = nullptr;
@@ -224,7 +288,7 @@ cudaError_t k3_launch_density(const FieldDev& f, double h, double rho0, int no_r
     e = cudaMemcpyAsync(d_W, W.data(), 4096 * sizeof(double), cudaMemcpyHostToDevice, stream);
     if (e == cudaSuccess) {
         // the pageable source is staged synchronously by the runtime, so W may go out of scope afterwards
-        DG_KERNEL_LAUNCH(density_map_kernel, blocks, 128, 0, stream, f, qp, d_W, no_reduction, (unsigned)l_begin, (unsigned long long)count, d_out);
+        DG_KERNEL_LAUNCH(kernel, blocks, 128, 0, stream, f, qp, d_W, no_reduction, (unsigned)l_begin, (unsigned long long)count, d_out);
         e = DG_AFTER_LAUNCH();
     }
     cudaFreeAsync(d_W, stream);

@@ -7,6 +7,9 @@
 namespace dgb {
 // GenerateDensityMap's cell_diag = cellSize().norm() (main.cpp:117): the value K3's predicate uses, and the SDF field's reduceField with it
 double k3_cell_diag(const GridDev& g);
-cudaError_t k3_launch_density(const FieldDev& f, double h, double rho0, int no_reduction, uint64_t l_begin, uint64_t count,
-                              double* d_out, cudaStream_t stream);
+// max |c| over the n packed coefficients c != DBL_MAX, +inf if one of them is NaN or +-inf; synchronises `stream`
+cudaError_t k3_coeff_max(const double* d_packed, uint64_t n, double* out, cudaStream_t stream);
+// coeff_max: k3_coeff_max of f's packed coefficients (it decides whether points outside the kernel support may be skipped)
+cudaError_t k3_launch_density(const FieldDev& f, double coeff_max, double h, double rho0, int no_reduction, uint64_t l_begin,
+                              uint64_t count, double* d_out, cudaStream_t stream);
 }

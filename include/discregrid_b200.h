@@ -222,7 +222,8 @@ DG_API int dg_build_cells(const uint32_t resolution[3], uint64_t c_begin, uint64
  * (:888-891).  After reduceField() pass the reduced arrays (cell_map entries UINT32_MAX = removed cell). */
 DG_API int dg_field_create(const dg_grid_desc* grid, const double* nodes, uint64_t n_nodes, const uint32_t* cells,
                     uint64_t n_cells_kept, const uint32_t* cell_map, dg_field** out);
-/* same, coefficient array already on the device (e.g. straight out of dg_sample_sdf_device); unreduced only */
+/* same, coefficient array already on the device (e.g. straight out of dg_sample_sdf_device); unreduced only.  Returns once the
+ * field is built on `stream` (it reads one fact about the coefficients back: see dg_density_map) */
 DG_API int dg_field_create_device(const dg_grid_desc* grid, const double* d_nodes, uint64_t n_nodes, void* stream, dg_field** out);
 DG_API int dg_field_destroy(dg_field* field);
 /* info[0]=n_nodes, [1]=n_cells_kept, [2]=device bytes, [3]=the CUDA device the field lives on */
@@ -242,7 +243,9 @@ DG_API int dg_shape_functions(const double* xi, uint64_t n, double* N, double* d
  * replaces addFunction(density_func, verbose, pred) of cmd/generate_density_map/main.cpp:96-133 with
  * GaussQuadrature::integrate(p=30 -> 16^3 points, gauss_quadrature.cpp:5927-5960) and CubicKernel::W
  * (sph_kernel.hpp:22-42) over nodes [l_begin, l_end) of the grid of `sdf` (its field 0):
- * out = DBL_MAX where the predicate rejects (unless no_reduction), 0 where dist > 2h, else rho0 * integral. */
+ * out = DBL_MAX where the predicate rejects (unless no_reduction), 0 where dist > 2h, else rho0 * integral.
+ * Quadrature points outside the kernel support are skipped only where that is exact, which the field's creation decides from its
+ * coefficients: a field holding NaN, +-inf or magnitudes near DBL_MAX (or an h too small for them) gets the reference's NaN. */
 DG_API int dg_density_map(const dg_field* sdf, double h, double rho0, int no_reduction, uint64_t l_begin, uint64_t l_end, double* out_host);
 DG_API int dg_density_map_device(const dg_field* sdf, double h, double rho0, int no_reduction, uint64_t l_begin, uint64_t l_end,
                           double* d_out, void* stream);

@@ -13,6 +13,7 @@ struct EmuField {
     double* packed = nullptr;
     std::vector<double2> tab;
     std::vector<unsigned> cell_map;
+    double coeff_max = 0.0;
     ~EmuField() { std::free(packed); }
 };
 bool to_grid(const double* gd, const uint32_t* res, GridDev& g)
@@ -41,6 +42,7 @@ void* emu_field_create(const double* gd, const uint32_t* res, const double* node
     if (cell_map) f->cell_map.assign(cell_map, cell_map + n_cells);
     if (k2_launch_pack(f->dev.g, nodes, cells, n_cells_kept, f->packed, nullptr) != cudaSuccess) { delete f; return nullptr; }
     if (k2_launch_axis_tables(f->dev.g, f->tab.data(), nullptr) != cudaSuccess) { delete f; return nullptr; }
+    if (k3_coeff_max(f->packed, 32 * n_cells_kept, &f->coeff_max, nullptr) != cudaSuccess) { delete f; return nullptr; }
     f->dev.packed = f->packed; f->dev.tab = f->tab.data(); f->dev.cell_map = cell_map ? f->cell_map.data() : nullptr;
     return f;
 }
@@ -52,7 +54,8 @@ int emu_interpolate(void* h, const double* x, uint64_t n, double* phi, double* g
 int emu_shape_functions(const double* xi, uint64_t n, double* N, double* dN) { return (int)k2_launch_shape_functions(xi, n, N, dN, nullptr); }
 int emu_density_map(void* h, double hh, double rho0, int no_reduction, uint64_t l_begin, uint64_t l_end, double* out)
 {
-    return (int)k3_launch_density(((EmuField*)h)->dev, hh, rho0, no_reduction, l_begin, l_end - l_begin, out, nullptr);
+    const EmuField* f = (EmuField*)h;
+    return (int)k3_launch_density(f->dev, f->coeff_max, hh, rho0, no_reduction, l_begin, l_end - l_begin, out, nullptr);
 }
 
 }  // extern "C"

@@ -25,7 +25,25 @@ CASES = {
     # dense band field: DBL_MAX wherever the distance exceeds the band, so K3's predicate and both reductions meet the sentinel
     "band_dragon_12_inverted": dict(sdf="ref_band_dragon_12_inverted.cdf", h_diag=0.5, rho0=1000.0, ties=False),
     "aniso": dict(sdf="ref_aniso_field.cdf", h_diag=0.5, rho0=1000.0, ties=True),
+    # a sphere SDF with one -DBL_MAX coefficient (made by make_inputs): d / h overflows to -inf near it, gamma = +inf, and the quadrature
+    # points outside the kernel support add inf * 0 = NaN -- the reference's density is NaN there
+    "minus_dbl_max": dict(sdf="ref_density_minus_dbl_max_sdf.cdf", h_diag=0.35, rho0=1000.0, ties=False),
 }
+
+
+def make_inputs():
+    """the SDF inputs that are not made by another script: a sphere SDF on a 4^3 grid over [0, 2]^3 with node 126 (an x-edge node) set to -DBL_MAX"""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    from oracle_api import Oracle
+    from make_reduce_golden import write_cdf
+    orc = Oracle()
+    gd, r = orc.grid_desc([0.0, 0.0, 0.0], [2.0, 2.0, 2.0], (4, 4, 4))
+    cells = orc.build_cells(r)
+    x = orc.node_positions(gd, r, 0, int(cells.max()) + 1)
+    v = np.linalg.norm(x - np.array([1.0, 0.9, 1.1]), axis=1) - 0.6
+    v[126] = -np.finfo(np.float64).max
+    write_cdf(os.path.join(HERE, CASES["minus_dbl_max"]["sdf"]), gd[0:3], gd[3:6], r, gd[6:9], gd[9:12], v, cells,
+              np.arange(len(cells), dtype=np.uint32))
 
 
 def read_grid(path):
@@ -59,6 +77,7 @@ def sdf_field_tie_flag(g, h):
 
 
 def main():
+    make_inputs()
     meta = {}
     for name, case in CASES.items():
         src = os.path.join(HERE, case["sdf"])
