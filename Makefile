@@ -24,7 +24,7 @@ CPPBIN   := build/bin
 CPPFLAGS := -std=c++11 -O2 -ffp-contract=off -I$(EIGEN3_INCLUDE_DIR) -Icpp/include -Iinclude
 CPPLINK  := -Ldiscregrid_b200/lib -ldiscregrid_b200 -Wl,-rpath,'$$ORIGIN/../../discregrid_b200/lib'
 CPPHDRS  := $(wildcard cpp/include/Discregrid/* cpp/include/Discregrid/*/*) include/discregrid_b200.h
-cpp: $(CPPBIN)/GenerateSDF $(CPPBIN)/GenerateDensityMap $(CPPBIN)/DiscreteFieldToBitmap $(CPPBIN)/facade_check $(CPPBIN)/bvh_host_check $(CPPBIN)/reduce_facade_check $(CPPBIN)/sort_replay_check $(CPPBIN)/fast_div_check $(CPPBIN)/libk1emu.so $(CPPBIN)/libk1emu_knobs.so $(CPPBIN)/libk1emu_wave.so $(CPPBIN)/libk1emu_perlane.so $(CPPBIN)/libk1emu_packet.so $(CPPBIN)/libk1emu_band.so $(CPPBIN)/libk1emu_band_perlane.so $(CPPBIN)/libk23emu.so $(CPPBIN)/libk23emu_knobs.so $(CPPBIN)/libdgemu.so $(CPPBIN)/libk4emu.so $(CPPBIN)/device_function_check $(CPPBIN)/device_query_check
+cpp: $(CPPBIN)/GenerateSDF $(CPPBIN)/GenerateDensityMap $(CPPBIN)/DiscreteFieldToBitmap $(CPPBIN)/facade_check $(CPPBIN)/bvh_host_check $(CPPBIN)/reduce_facade_check $(CPPBIN)/sort_replay_check $(CPPBIN)/fast_div_check $(CPPBIN)/libk1emu.so $(CPPBIN)/libk1emu_knobs.so $(CPPBIN)/libk1emu_wave.so $(CPPBIN)/libk1emu_perlane.so $(CPPBIN)/libk1emu_packet.so $(CPPBIN)/libk1emu_band.so $(CPPBIN)/libk1emu_band_perlane.so $(CPPBIN)/libk23emu.so $(CPPBIN)/libk23emu_knobs.so $(CPPBIN)/libk2hemu.so $(CPPBIN)/libdgemu.so $(CPPBIN)/libk4emu.so $(CPPBIN)/device_function_check $(CPPBIN)/device_query_check $(CPPBIN)/hessian_check
 $(CPPBIN)/DiscreteFieldToBitmap: cpp/cmd/discrete_field_to_bitmap.cpp $(CPPHDRS) $(LIB)
 	@mkdir -p $(CPPBIN)
 	$(HOSTCXX) $(CPPFLAGS) $< -o $@ $(CPPLINK)
@@ -68,6 +68,11 @@ $(CPPBIN)/libk23emu.so: $(K23EMU_DEP)
 $(CPPBIN)/libk23emu_knobs.so: $(K23EMU_DEP)
 	@mkdir -p $(CPPBIN)
 	$(HOSTCXX) -std=c++17 -O2 -ffp-contract=off -fPIC -shared -DK3_FAST_DIV=0 -I$(CUDA_INC) -Itests/emu -I$(SRC) $(K23EMU_SRC) -o $@ -lpthread
+# the same with K2's Hessian mode exposed (emu_interpolate_hessian)
+K2HEMU_SRC := tests/emu/k2_emu.cpp tests/emu/k2_hessian_emu.cpp
+$(CPPBIN)/libk2hemu.so: $(K23EMU_DEP) tests/emu/k2_hessian_emu.cpp
+	@mkdir -p $(CPPBIN)
+	$(HOSTCXX) -std=c++17 -O2 -ffp-contract=off -fPIC -shared -I$(CUDA_INC) -Itests/emu -I$(SRC) $(K2HEMU_SRC) -o $@ -lpthread
 # test library: the WHOLE product library with every kernel emulated and the CUDA runtime stubbed on host memory -- lets the Python-level
 # and tool-level `-m gpu` tests be rehearsed on the CPU (tests/test_gpu_rehearsal.py); never loaded by the product
 DGEMU_SRC := tests/emu/dgapi_emu.cpp tests/emu/k1_emu.cpp tests/emu/k2_emu.cpp tests/emu/k3_emu.cpp tests/emu/k4_emu.cpp tests/emu/cudart_stub.cpp \
@@ -99,6 +104,10 @@ $(CPPBIN)/device_function_check: tests/cpp/device_function_check.cpp $(CPPHDRS) 
 	$(HOSTCXX) $(CPPFLAGS) -I$(CUDA_INC) $< -o $@ $(CPPLINK) -L$(CUDA_LIB) -lcudart_static -ldl -lrt -lpthread
 # test binary: the facade's reduced calls feed interpolate from the kept handle; it defines its own dg_field_create, which refuses
 $(CPPBIN)/device_query_check: tests/cpp/device_query_check.cpp $(CPPHDRS) $(LIB)
+	@mkdir -p $(CPPBIN)
+	$(HOSTCXX) $(CPPFLAGS) $< -o $@ $(CPPLINK)
+# test binary: the facade's batched Hessian overload on a grid file, for comparison with the Python route
+$(CPPBIN)/hessian_check: tests/cpp/hessian_check.cpp $(CPPHDRS) $(LIB)
 	@mkdir -p $(CPPBIN)
 	$(HOSTCXX) $(CPPFLAGS) $< -o $@ $(CPPLINK)
 oracle/liboracle.so:

@@ -14,6 +14,7 @@
 //   addReducedFunction(DeviceFunction, DeviceSamplePredicate*, DeviceNodePredicate*)
 //                                            -> dg_reduced_function_create (both calls in one, the dense field kept on the GPU)
 //   interpolate(field, x, grad*)             -> dg_interpolate_batch (K2), also batched: interpolate(field, n, x, phi, grad)
+//   interpolate(field, n, x, phi, grad, hess) -> dg_interpolate_hessian_batch (K2's Hessian mode; not in the reference)
 //   connectivity table of addFunction        -> dg_build_cells  (GPU)  replaces the serial loop :833-886
 //
 // m_nodes / m_cells / m_cell_map hold exactly what the reference would have produced, so save()/load() stay
@@ -345,6 +346,12 @@ public:
     void interpolate(unsigned int field_id, std::size_t n, const double* x, double* phi, double* grad = nullptr) const
     {
         check(dg_interpolate_batch(deviceField(field_id), x, n, phi, grad));
+    }
+    // batched value + gradient + Hessian (new, beyond the reference): phi = n, grad = n x 3 (the bits of the form above), hess = n x 3 x 3
+    // row-major and exactly symmetric, all three required (dg_interpolate_hessian_batch)
+    void interpolate(unsigned int field_id, std::size_t n, const double* x, double* phi, double* grad, double* hess) const
+    {
+        check(dg_interpolate_hessian_batch(deviceField(field_id), x, n, phi, grad, hess));
     }
 
     // ---- split API (:901-975): shape functions on the GPU (dg_shape_functions), index algebra on the host

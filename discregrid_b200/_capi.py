@@ -98,6 +98,8 @@ SIGNATURES = {
     "dg_field_info": (C.c_int, [_vp, _u64p]),
     "dg_interpolate_batch": (C.c_int, [_vp, _dp, C.c_uint64, _dp, _dp]),
     "dg_interpolate_batch_device": (C.c_int, [_vp, _vp, C.c_uint64, _vp, _vp, _vp]),
+    "dg_interpolate_hessian_batch": (C.c_int, [_vp, _dp, C.c_uint64, _dp, _dp, _dp]),
+    "dg_interpolate_hessian_batch_device": (C.c_int, [_vp, _vp, C.c_uint64, _vp, _vp, _vp, _vp]),
     "dg_shape_functions": (C.c_int, [_dp, C.c_uint64, _dp, _dp]),
     "dg_density_map": (C.c_int, [_vp, C.c_double, C.c_double, C.c_int, C.c_uint64, C.c_uint64, _dp]),
     "dg_reduce_field": (C.c_int, [_gp, _dp, C.c_uint64, C.POINTER(C.c_uint8), _u32p, C.c_uint64, _u32p, C.c_uint32, _u64p, _u64p, _dp]),

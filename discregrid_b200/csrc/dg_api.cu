@@ -1365,6 +1365,15 @@ int dg_interpolate_batch_device(const dg_field* f, const double* d_x, uint64_t n
     return DG_OK;
 }
 
+int dg_interpolate_hessian_batch_device(const dg_field* f, const double* d_x, uint64_t n, double* d_phi, double* d_grad, double* d_hess, void* stream)
+{
+    if (!f) return fail(DG_ERR_INVALID, "dg_interpolate_hessian_batch: field is NULL");
+    if (n && (!d_x || !d_phi || !d_grad || !d_hess)) return fail(DG_ERR_INVALID, "dg_interpolate_hessian_batch: x / phi / grad / hess is NULL");
+    if (int rc = check_handle_device(f->device, "dg_interpolate_hessian_batch")) return rc;
+    DG_LAUNCH(k2_launch_interpolate(f->dev, d_x, n, d_phi, d_grad, (cudaStream_t)stream, d_hess));
+    return DG_OK;
+}
+
 // Host-buffer path of K2: a three-slot pipeline.  Each slot owns device buffers for one chunk of queries, a stream and an event;
 // chunk c runs H2D -> kernel -> D2H on slot c % 3, so the uploads, kernels and downloads of neighbouring chunks overlap on the two
 // DMA directions of the link.  Caller memory that is already page-locked (cudaMallocHost / cudaHostRegister / torch pin_memory) is
@@ -1379,18 +1388,20 @@ struct InterpPool {
     uint64_t cap = 0;                                            // queries per slot currently allocated
     double* d_x[kSlots] = {}; double* d_phi[kSlots] = {}; double* d_grad[kSlots] = {};
     double* h_in[kSlots] = {}; double* h_out[kSlots] = {};       // pinned staging (allocated on first pageable call)
+    double* d_hess[kSlots] = {}; double* h_hess[kSlots] = {};    // Hessian outputs and their pinned staging (first Hessian call only)
     cudaStream_t st[kSlots] = {}; cudaEvent_t done[kSlots] = {};
     void release()
     {
         for (int i = 0; i < kSlots; i++) {
             if (d_x[i]) cudaFree(d_x[i]); if (d_phi[i]) cudaFree(d_phi[i]); if (d_grad[i]) cudaFree(d_grad[i]);
             if (h_in[i]) cudaFreeHost(h_in[i]); if (h_out[i]) cudaFreeHost(h_out[i]);
+            if (d_hess[i]) cudaFree(d_hess[i]); if (h_hess[i]) cudaFreeHost(h_hess[i]);
             if (st[i]) cudaStreamDestroy(st[i]); if (done[i]) cudaEventDestroy(done[i]);
-            d_x[i] = d_phi[i] = d_grad[i] = h_in[i] = h_out[i] = nullptr; st[i] = nullptr; done[i] = nullptr;
+            d_x[i] = d_phi[i] = d_grad[i] = h_in[i] = h_out[i] = d_hess[i] = h_hess[i] = nullptr; st[i] = nullptr; done[i] = nullptr;
         }
         cap = 0;
     }
-    cudaError_t prepare(uint64_t chunk, bool need_stage_in, bool need_stage_out)
+    cudaError_t prepare(uint64_t chunk, bool need_stage_in, bool need_stage_out, bool need_hess)
     {
         int dev = 0;
         cudaError_t e = cudaGetDevice(&dev);
@@ -1411,6 +1422,8 @@ struct InterpPool {
         for (int i = 0; i < kSlots && e == cudaSuccess; i++) {
             if (need_stage_in && !h_in[i]) e = cudaMallocHost(reinterpret_cast<void**>(&h_in[i]), cap * 3 * sizeof(double));
             if (e == cudaSuccess && need_stage_out && !h_out[i]) e = cudaMallocHost(reinterpret_cast<void**>(&h_out[i]), cap * 4 * sizeof(double));
+            if (e == cudaSuccess && need_hess && !d_hess[i]) e = cudaMalloc(reinterpret_cast<void**>(&d_hess[i]), cap * 9 * sizeof(double));
+            if (e == cudaSuccess && need_hess && need_stage_out && !h_hess[i]) e = cudaMallocHost(reinterpret_cast<void**>(&h_hess[i]), cap * 9 * sizeof(double));
         }
         if (e != cudaSuccess) release();
         return e;
@@ -1432,7 +1445,8 @@ void threaded_copy(void* dst, const void* src, size_t bytes, unsigned nt)
 }
 }  // namespace
 
-static int dg_interpolate_batch_impl(const dg_field* f, const double* x, uint64_t n, double* phi, double* grad)
+// hess (nullable; grad must then be given too) selects K2's Hessian mode; its buffers join the pool at the first call that passes it
+static int dg_interpolate_batch_impl(const dg_field* f, const double* x, uint64_t n, double* phi, double* grad, double* hess = nullptr)
 {
     if (!f) return fail(DG_ERR_INVALID, "dg_interpolate_batch: field is NULL");
     if (n == 0) return DG_OK;
@@ -1441,8 +1455,8 @@ static int dg_interpolate_batch_impl(const dg_field* f, const double* x, uint64_
     std::lock_guard<std::mutex> lock(g_ipool.mu);
     constexpr int S = InterpPool::kSlots;
     const uint64_t chunk = std::min<uint64_t>(InterpPool::kChunk, n);
-    const bool x_direct = is_pinned_host(x), out_direct = is_pinned_host(phi) && is_pinned_host(grad);
-    DG_CUDA(g_ipool.prepare(std::max<uint64_t>(chunk, g_ipool.cap), !x_direct, !out_direct));
+    const bool x_direct = is_pinned_host(x), out_direct = is_pinned_host(phi) && is_pinned_host(grad) && is_pinned_host(hess);
+    DG_CUDA(g_ipool.prepare(std::max<uint64_t>(chunk, g_ipool.cap), !x_direct, !out_direct, hess != nullptr));
     const unsigned nt = std::max(1u, std::min(4u, host_threads() / 4));      // copy threads of the staged (pageable) path, started per chunk
     const uint64_t n_chunks = (n + chunk - 1) / chunk;
     auto unstage = [&](uint64_t c) {                      // results of chunk c: pinned staging -> caller memory
@@ -1450,6 +1464,7 @@ static int dg_interpolate_batch_impl(const dg_field* f, const double* x, uint64_
         const double* src = g_ipool.h_out[c % S];
         threaded_copy(phi + off, src, cnt * sizeof(double), nt);
         if (grad) threaded_copy(grad + 3 * off, src + g_ipool.cap, 3 * cnt * sizeof(double), nt);
+        if (hess) threaded_copy(hess + 9 * off, g_ipool.h_hess[c % S], 9 * cnt * sizeof(double), nt);
     };
     for (uint64_t c = 0; c < n_chunks; c++) {
         const int s = (int)(c % S);
@@ -1461,11 +1476,14 @@ static int dg_interpolate_batch_impl(const dg_field* f, const double* x, uint64_
         const double* src = x + 3 * off;
         if (!x_direct) { threaded_copy(g_ipool.h_in[s], src, 3 * cnt * sizeof(double), nt); src = g_ipool.h_in[s]; }
         DG_CUDA(cudaMemcpyAsync(g_ipool.d_x[s], src, 3 * cnt * sizeof(double), cudaMemcpyHostToDevice, g_ipool.st[s]));
-        DG_LAUNCH(k2_launch_interpolate(f->dev, g_ipool.d_x[s], cnt, g_ipool.d_phi[s], grad ? g_ipool.d_grad[s] : nullptr, g_ipool.st[s]));
+        DG_LAUNCH(k2_launch_interpolate(f->dev, g_ipool.d_x[s], cnt, g_ipool.d_phi[s], grad ? g_ipool.d_grad[s] : nullptr, g_ipool.st[s],
+                                        hess ? g_ipool.d_hess[s] : nullptr));
         double* dst_phi = out_direct ? phi + off : g_ipool.h_out[s];
         double* dst_grad = out_direct ? grad + 3 * off : g_ipool.h_out[s] + g_ipool.cap;
         DG_CUDA(cudaMemcpyAsync(dst_phi, g_ipool.d_phi[s], cnt * sizeof(double), cudaMemcpyDeviceToHost, g_ipool.st[s]));
         if (grad) DG_CUDA(cudaMemcpyAsync(dst_grad, g_ipool.d_grad[s], 3 * cnt * sizeof(double), cudaMemcpyDeviceToHost, g_ipool.st[s]));
+        if (hess) DG_CUDA(cudaMemcpyAsync(out_direct ? hess + 9 * off : g_ipool.h_hess[s], g_ipool.d_hess[s], 9 * cnt * sizeof(double),
+                                          cudaMemcpyDeviceToHost, g_ipool.st[s]));
         DG_CUDA(cudaEventRecord(g_ipool.done[s], g_ipool.st[s]));
     }
     for (uint64_t c = (n_chunks > (uint64_t)S ? n_chunks - S : 0); c < n_chunks; c++) {
@@ -2195,6 +2213,12 @@ int dg_add_function_sdf_multi(dg_mesh_group* grp, const dg_grid_desc* grid, doub
 int dg_interpolate_batch(const dg_field* f, const double* x, uint64_t n, double* phi, double* grad)
 {
     return guarded("dg_interpolate_batch", [&]() { return dg_interpolate_batch_impl(f, x, n, phi, grad); });
+}
+
+int dg_interpolate_hessian_batch(const dg_field* f, const double* x, uint64_t n, double* phi, double* grad, double* hess)
+{
+    if (n && (!phi || !grad || !hess)) return fail(DG_ERR_INVALID, "dg_interpolate_hessian_batch: phi / grad / hess is NULL");
+    return guarded("dg_interpolate_hessian_batch", [&]() { return dg_interpolate_batch_impl(f, x, n, phi, grad, hess); });
 }
 
 int dg_reduce_field(const dg_grid_desc* grid, double* nodes, uint64_t n_nodes, const uint8_t* keep_node, uint32_t* cells, uint64_t n_cells_in,

@@ -20,6 +20,21 @@
 // The per-axis reference-cell maps c0 = 2/denom, c1 = (hi+lo)/denom (:1000-1002) depend only on the cell
 // index along that axis; they are tabulated once per field with the reference's exact operation order, which
 // removes six fp64 divisions per query without changing a bit.
+//
+// Hessian mode (interpolate_kernel<true, true>; the reference has no Hessian, so this contract is the library's own).  phi and grad
+// are computed by the same expressions in the same order as the gradient mode and have its bits.  Notation as in the code: X, Y, Z = xi,
+// Lx = 1 + sx*X (_1mx / _1px), and so on.  The second derivatives of the 32 shape functions, in xi:
+//   corner (sx, sy, sz), N = F*Lx*Ly*Lz/64 with F = 9(X^2+Y^2+Z^2) - 19, scale 1/64:
+//     d2/dX2  = (18*(1 + 3*sx*X)) * (Ly*Lz)                       (18 * _1m3x / _1p3x, times mymz ...)
+//     d2/dXdY = (sy*xsA + sx*(18Y*Ly)) * Lz                        (xsA = 18X + sx*A, the gradient's xmA / xpA)
+//     d2/dXdZ = (sz*xsA + sx*(18Z*Lz)) * Ly,   d2/dYdZ = (sz*ysB + sy*(18Z*Lz)) * Lx,   d2/dY2, d2/dZ2 by permutation
+//   x-edge (s, sy, sz), N = (9/64)*P*Ly*Lz with P = (1-X^2)(1+3sX) (Xm / Xp), P' = mX / pX, P'' = -2 - 18sX, scale 9/64:
+//     d2/dX2 = P''*(Ly*Lz),  d2/dXdY = (sy*P')*Lz,  d2/dXdZ = (sz*P')*Ly,  d2/dYdZ = (sy*sz)*P,  d2/dY2 = d2/dZ2 = 0
+//   y- and z-edges by permutation.  A sign s* is applied as an exact negation, never as a product.
+// Each entry h_ab accumulates h = h + c_j * (d2 * scale) over j = 0..31 in the order of the value sum, skipping the structural zeros
+// (a diagonal entry sums the 8 corners and the 8 edges along its axis, a mixed entry all 32): adding c_j * 0 would turn an infinite
+// coefficient into NaN and could flip the sign of a zero.  Then H_ab = (h_ab * c0_a) * c0_b, computed once for a < b and stored at
+// [a][b] and [b][a] of the row-major hess[n][3][3].  Sentinels as in the gradient mode, with all nine entries +0.0.
 #include "dg_device.cuh"
 #include "k2_interp.h"
 #include "dg_launch.h"
@@ -111,12 +126,14 @@ __global__ void axis_tables_kernel(GridDev g, double2* __restrict__ tab)
     tab[idx] = make_double2(2.0 / denom, (hi + lo) / denom);
 }
 
-template <bool GRAD>
+// <false, false>: value; <true, false>: value + gradient; <true, true>: value + gradient + Hessian (see the header comment)
+template <bool GRAD, bool HESS>
 __global__ void __launch_bounds__(K2_THREADS)
 interpolate_kernel(GridDev g, const double* __restrict__ packed, const unsigned* __restrict__ cell_map /*nullable*/,
                    const double2* __restrict__ tab, const double* __restrict__ xq, unsigned long long n,
-                   double* __restrict__ phi_out, double* __restrict__ grad_out)
+                   double* __restrict__ phi_out, double* __restrict__ grad_out, double* __restrict__ hess_out)
 {
+    static_assert(GRAD || !HESS, "the Hessian mode also computes the gradient");
     __shared__ __align__(16) unsigned char stage[K2_WARPS][32 * K2_SLOT_BYTES];
     __shared__ __align__(8) unsigned long long bars[K2_WARPS];
 
@@ -181,6 +198,15 @@ interpolate_kernel(GridDev g, const double* __restrict__ packed, const unsigned*
         mY = -_3m9y2 - _2y; pY = _3m9y2 - _2y; Ym = _1my2 * _1m3y; Yp = _1my2 * _1p3y;                    // :518-521
         mZ = -_3m9z2 - _2z; pZ = _3m9z2 - _2z; Zm = _1mz2 * _1m3z; Zp = _1mz2 * _1p3z;                    // :547-550
     }
+    // Hessian-mode temporaries: 18(1 -+ 3X) of the corners' d2/dX2, 18X*(1 -+ X) of their mixed terms, P'' = -2 -+ 18X of the x-edges
+    double d2xm = 0, d2xp = 0, d2ym = 0, d2yp = 0, d2zm = 0, d2zp = 0, x18m = 0, x18p = 0, y18m = 0, y18p = 0, z18m = 0, z18p = 0,
+           ddXm = 0, ddXp = 0, ddYm = 0, ddYp = 0, ddZm = 0, ddZp = 0;
+    if (HESS) {
+        const double _18x = 18.0 * X, _18y = 18.0 * Y, _18z = 18.0 * Z;
+        d2xm = 18.0 * _1m3x; d2xp = 18.0 * _1p3x; d2ym = 18.0 * _1m3y; d2yp = 18.0 * _1p3y; d2zm = 18.0 * _1m3z; d2zp = 18.0 * _1p3z;
+        x18m = _18x * _1mx; x18p = _18x * _1px; y18m = _18y * _1my; y18p = _18y * _1py; z18m = _18z * _1mz; z18p = _18z * _1pz;
+        ddXm = -2.0 + _18x; ddXp = -2.0 - _18x; ddYm = -2.0 + _18y; ddYp = -2.0 - _18y; ddZm = -2.0 + _18z; ddZp = -2.0 - _18z;
+    }
 
     // ---- wait for the warp's 32 blocks
     mbar_wait(bar, 0);
@@ -203,66 +229,119 @@ interpolate_kernel(GridDev g, const double* __restrict__ packed, const unsigned*
         phi = phi + c_ * (n);                                                \
         if (GRAD) { g0 = g0 + c_ * ((dx) * (9.0 / 64.0)); g1 = g1 + c_ * ((dy) * (9.0 / 64.0)); g2 = g2 + c_ * ((dz) * (9.0 / 64.0)); } \
     }
+    // Hessian terms of one node, given by its signs (m = -1, p = +1); an edge's own axis sign is S.  Structural zeros are not added.
+    double hxx = 0.0, hxy = 0.0, hxz = 0.0, hyy = 0.0, hyz = 0.0, hzz = 0.0;
+#define DG_SG_m(v) (-(v))
+#define DG_SG_p(v) (v)
+#define DG_SG2_mm(v) (v)
+#define DG_SG2_mp(v) (-(v))
+#define DG_SG2_pm(v) (-(v))
+#define DG_SG2_pp(v) (v)
+#define DG_CORNER_H(cj, SX, SY, SZ)                                                                                   \
+    if (HESS) {                                                                                                       \
+        const double c_ = (cj);                                                                                       \
+        hxx = hxx + c_ * ((d2x##SX * SY##y##SZ##z) * 0.015625);                                                       \
+        hyy = hyy + c_ * ((d2y##SY * SX##x##SZ##z) * 0.015625);                                                       \
+        hzz = hzz + c_ * ((d2z##SZ * SX##x##SY##y) * 0.015625);                                                       \
+        hxy = hxy + c_ * (((DG_SG_##SY(x##SX##A) + DG_SG_##SX(y18##SY)) * _1##SZ##z) * 0.015625);                    \
+        hxz = hxz + c_ * (((DG_SG_##SZ(x##SX##A) + DG_SG_##SX(z18##SZ)) * _1##SY##y) * 0.015625);                    \
+        hyz = hyz + c_ * (((DG_SG_##SZ(y##SY##B) + DG_SG_##SY(z18##SZ)) * _1##SX##x) * 0.015625);                    \
+    }
+#define DG_XEDGE_H(cj, S, SY, SZ)                                                                                     \
+    if (HESS) {                                                                                                       \
+        const double c_ = (cj);                                                                                       \
+        hxx = hxx + c_ * ((ddX##S * SY##y##SZ##z) * (9.0 / 64.0));                                                    \
+        hxy = hxy + c_ * ((DG_SG_##SY(S##X) * _1##SZ##z) * (9.0 / 64.0));                                             \
+        hxz = hxz + c_ * ((DG_SG_##SZ(S##X) * _1##SY##y) * (9.0 / 64.0));                                             \
+        hyz = hyz + c_ * (DG_SG2_##SY##SZ(X##S) * (9.0 / 64.0));                                                      \
+    }
+#define DG_YEDGE_H(cj, SX, S, SZ)                                                                                     \
+    if (HESS) {                                                                                                       \
+        const double c_ = (cj);                                                                                       \
+        hyy = hyy + c_ * ((ddY##S * SX##x##SZ##z) * (9.0 / 64.0));                                                    \
+        hxy = hxy + c_ * ((DG_SG_##SX(S##Y) * _1##SZ##z) * (9.0 / 64.0));                                             \
+        hxz = hxz + c_ * (DG_SG2_##SX##SZ(Y##S) * (9.0 / 64.0));                                                      \
+        hyz = hyz + c_ * ((DG_SG_##SZ(S##Y) * _1##SX##x) * (9.0 / 64.0));                                             \
+    }
+#define DG_ZEDGE_H(cj, SX, SY, S)                                                                                     \
+    if (HESS) {                                                                                                       \
+        const double c_ = (cj);                                                                                       \
+        hzz = hzz + c_ * ((ddZ##S * SX##x##SY##y) * (9.0 / 64.0));                                                    \
+        hxy = hxy + c_ * (DG_SG2_##SX##SY(Z##S) * (9.0 / 64.0));                                                      \
+        hxz = hxz + c_ * ((DG_SG_##SX(S##Z) * _1##SY##y) * (9.0 / 64.0));                                             \
+        hyz = hyz + c_ * ((DG_SG_##SY(S##Z) * _1##SX##x) * (9.0 / 64.0));                                             \
+    }
     double2 c;
     // corners (:389-396, :462-485)
     c = cb[0];
-    DG_CORNER(c.x, facc * mxmy * _1mz, xmA * mymz, mxmz * ymB, mxmy * zmC)
-    DG_CORNER(c.y, facc * pxmy * _1mz, xpA * mymz, pxmz * ymB, pxmy * zmC)
+    DG_CORNER(c.x, facc * mxmy * _1mz, xmA * mymz, mxmz * ymB, mxmy * zmC) DG_CORNER_H(c.x, m, m, m)
+    DG_CORNER(c.y, facc * pxmy * _1mz, xpA * mymz, pxmz * ymB, pxmy * zmC) DG_CORNER_H(c.y, p, m, m)
     c = cb[1];
-    DG_CORNER(c.x, facc * mxpy * _1mz, xmA * pymz, mxmz * ypB, mxpy * zmC)
-    DG_CORNER(c.y, facc * pxpy * _1mz, xpA * pymz, pxmz * ypB, pxpy * zmC)
+    DG_CORNER(c.x, facc * mxpy * _1mz, xmA * pymz, mxmz * ypB, mxpy * zmC) DG_CORNER_H(c.x, m, p, m)
+    DG_CORNER(c.y, facc * pxpy * _1mz, xpA * pymz, pxmz * ypB, pxpy * zmC) DG_CORNER_H(c.y, p, p, m)
     c = cb[2];
-    DG_CORNER(c.x, facc * mxmy * _1pz, xmA * mypz, mxpz * ymB, mxmy * zpC)
-    DG_CORNER(c.y, facc * pxmy * _1pz, xpA * mypz, pxpz * ymB, pxmy * zpC)
+    DG_CORNER(c.x, facc * mxmy * _1pz, xmA * mypz, mxpz * ymB, mxmy * zpC) DG_CORNER_H(c.x, m, m, p)
+    DG_CORNER(c.y, facc * pxmy * _1pz, xpA * mypz, pxpz * ymB, pxmy * zpC) DG_CORNER_H(c.y, p, m, p)
     c = cb[3];
-    DG_CORNER(c.x, facc * mxpy * _1pz, xmA * pypz, mxpz * ypB, mxpy * zpC)
-    DG_CORNER(c.y, facc * pxpy * _1pz, xpA * pypz, pxpz * ypB, pxpy * zpC)
+    DG_CORNER(c.x, facc * mxpy * _1pz, xmA * pypz, mxpz * ypB, mxpy * zpC) DG_CORNER_H(c.x, m, p, p)
+    DG_CORNER(c.y, facc * pxpy * _1pz, xpA * pypz, pxpz * ypB, pxpy * zpC) DG_CORNER_H(c.y, p, p, p)
     // x edges (:403-410, :493-516)
     c = cb[4];
-    DG_EDGE(c.x, fxm * mymz, mX * mymz, -Xm * _1mz, -Xm * _1my)
-    DG_EDGE(c.y, fxp * mymz, pX * mymz, -Xp * _1mz, -Xp * _1my)
+    DG_EDGE(c.x, fxm * mymz, mX * mymz, -Xm * _1mz, -Xm * _1my) DG_XEDGE_H(c.x, m, m, m)
+    DG_EDGE(c.y, fxp * mymz, pX * mymz, -Xp * _1mz, -Xp * _1my) DG_XEDGE_H(c.y, p, m, m)
     c = cb[5];
-    DG_EDGE(c.x, fxm * mypz, mX * mypz, -Xm * _1pz, Xm * _1my)
-    DG_EDGE(c.y, fxp * mypz, pX * mypz, -Xp * _1pz, Xp * _1my)
+    DG_EDGE(c.x, fxm * mypz, mX * mypz, -Xm * _1pz, Xm * _1my) DG_XEDGE_H(c.x, m, m, p)
+    DG_EDGE(c.y, fxp * mypz, pX * mypz, -Xp * _1pz, Xp * _1my) DG_XEDGE_H(c.y, p, m, p)
     c = cb[6];
-    DG_EDGE(c.x, fxm * pymz, mX * pymz, Xm * _1mz, -Xm * _1py)
-    DG_EDGE(c.y, fxp * pymz, pX * pymz, Xp * _1mz, -Xp * _1py)
+    DG_EDGE(c.x, fxm * pymz, mX * pymz, Xm * _1mz, -Xm * _1py) DG_XEDGE_H(c.x, m, p, m)
+    DG_EDGE(c.y, fxp * pymz, pX * pymz, Xp * _1mz, -Xp * _1py) DG_XEDGE_H(c.y, p, p, m)
     c = cb[7];
-    DG_EDGE(c.x, fxm * pypz, mX * pypz, Xm * _1pz, Xm * _1py)
-    DG_EDGE(c.y, fxp * pypz, pX * pypz, Xp * _1pz, Xp * _1py)
+    DG_EDGE(c.x, fxm * pypz, mX * pypz, Xm * _1pz, Xm * _1py) DG_XEDGE_H(c.x, m, p, p)
+    DG_EDGE(c.y, fxp * pypz, pX * pypz, Xp * _1pz, Xp * _1py) DG_XEDGE_H(c.y, p, p, p)
     // y edges (:415-422, :522-545)
     c = cb[8];
-    DG_EDGE(c.x, fym * mxmz, -Ym * _1mz, mY * mxmz, -Ym * _1mx)
-    DG_EDGE(c.y, fyp * mxmz, -Yp * _1mz, pY * mxmz, -Yp * _1mx)
+    DG_EDGE(c.x, fym * mxmz, -Ym * _1mz, mY * mxmz, -Ym * _1mx) DG_YEDGE_H(c.x, m, m, m)
+    DG_EDGE(c.y, fyp * mxmz, -Yp * _1mz, pY * mxmz, -Yp * _1mx) DG_YEDGE_H(c.y, m, p, m)
     c = cb[9];
-    DG_EDGE(c.x, fym * pxmz, Ym * _1mz, mY * pxmz, -Ym * _1px)
-    DG_EDGE(c.y, fyp * pxmz, Yp * _1mz, pY * pxmz, -Yp * _1px)
+    DG_EDGE(c.x, fym * pxmz, Ym * _1mz, mY * pxmz, -Ym * _1px) DG_YEDGE_H(c.x, p, m, m)
+    DG_EDGE(c.y, fyp * pxmz, Yp * _1mz, pY * pxmz, -Yp * _1px) DG_YEDGE_H(c.y, p, p, m)
     c = cb[10];
-    DG_EDGE(c.x, fym * mxpz, -Ym * _1pz, mY * mxpz, Ym * _1mx)
-    DG_EDGE(c.y, fyp * mxpz, -Yp * _1pz, pY * mxpz, Yp * _1mx)
+    DG_EDGE(c.x, fym * mxpz, -Ym * _1pz, mY * mxpz, Ym * _1mx) DG_YEDGE_H(c.x, m, m, p)
+    DG_EDGE(c.y, fyp * mxpz, -Yp * _1pz, pY * mxpz, Yp * _1mx) DG_YEDGE_H(c.y, m, p, p)
     c = cb[11];
-    DG_EDGE(c.x, fym * pxpz, Ym * _1pz, mY * pxpz, Ym * _1px)
-    DG_EDGE(c.y, fyp * pxpz, Yp * _1pz, pY * pxpz, Yp * _1px)
+    DG_EDGE(c.x, fym * pxpz, Ym * _1pz, mY * pxpz, Ym * _1px) DG_YEDGE_H(c.x, p, m, p)
+    DG_EDGE(c.y, fyp * pxpz, Yp * _1pz, pY * pxpz, Yp * _1px) DG_YEDGE_H(c.y, p, p, p)
     // z edges (:427-434, :551-574)
     c = cb[12];
-    DG_EDGE(c.x, fzm * mxmy, -Zm * _1my, -Zm * _1mx, mZ * mxmy)
-    DG_EDGE(c.y, fzp * mxmy, -Zp * _1my, -Zp * _1mx, pZ * mxmy)
+    DG_EDGE(c.x, fzm * mxmy, -Zm * _1my, -Zm * _1mx, mZ * mxmy) DG_ZEDGE_H(c.x, m, m, m)
+    DG_EDGE(c.y, fzp * mxmy, -Zp * _1my, -Zp * _1mx, pZ * mxmy) DG_ZEDGE_H(c.y, m, m, p)
     c = cb[13];
-    DG_EDGE(c.x, fzm * mxpy, -Zm * _1py, Zm * _1mx, mZ * mxpy)
-    DG_EDGE(c.y, fzp * mxpy, -Zp * _1py, Zp * _1mx, pZ * mxpy)
+    DG_EDGE(c.x, fzm * mxpy, -Zm * _1py, Zm * _1mx, mZ * mxpy) DG_ZEDGE_H(c.x, m, p, m)
+    DG_EDGE(c.y, fzp * mxpy, -Zp * _1py, Zp * _1mx, pZ * mxpy) DG_ZEDGE_H(c.y, m, p, p)
     c = cb[14];
-    DG_EDGE(c.x, fzm * pxmy, Zm * _1my, -Zm * _1px, mZ * pxmy)
-    DG_EDGE(c.y, fzp * pxmy, Zp * _1my, -Zp * _1px, pZ * pxmy)
+    DG_EDGE(c.x, fzm * pxmy, Zm * _1my, -Zm * _1px, mZ * pxmy) DG_ZEDGE_H(c.x, p, m, m)
+    DG_EDGE(c.y, fzp * pxmy, Zp * _1my, -Zp * _1px, pZ * pxmy) DG_ZEDGE_H(c.y, p, m, p)
     c = cb[15];
-    DG_EDGE(c.x, fzm * pxpy, Zm * _1py, Zm * _1px, mZ * pxpy)
-    DG_EDGE(c.y, fzp * pxpy, Zp * _1py, Zp * _1px, pZ * pxpy)
+    DG_EDGE(c.x, fzm * pxpy, Zm * _1py, Zm * _1px, mZ * pxpy) DG_ZEDGE_H(c.x, p, p, m)
+    DG_EDGE(c.y, fzp * pxpy, Zp * _1py, Zp * _1px, pZ * pxpy) DG_ZEDGE_H(c.y, p, p, p)
 #undef DG_CORNER
 #undef DG_EDGE
+#undef DG_CORNER_H
+#undef DG_XEDGE_H
+#undef DG_YEDGE_H
+#undef DG_ZEDGE_H
+#undef DG_SG_m
+#undef DG_SG_p
+#undef DG_SG2_mm
+#undef DG_SG2_mp
+#undef DG_SG2_pm
+#undef DG_SG2_pp
 
     if (!live) return;
     if (!valid || missing) {                        // sentinel paths (:981-982, :993-994, :1015-1018, :1050-1054)
         phi_out[q] = DBL_MAX;
         if (GRAD) { grad_out[3 * q] = 0.0; grad_out[3 * q + 1] = 0.0; grad_out[3 * q + 2] = 0.0; }
+        if (HESS) { for (int k = 0; k < 9; k++) hess_out[9 * q + k] = 0.0; }
         return;
     }
     phi_out[q] = phi;
@@ -270,6 +349,14 @@ interpolate_kernel(GridDev g, const double* __restrict__ packed, const unsigned*
         grad_out[3 * q] = g0 * tx.x;
         grad_out[3 * q + 1] = g1 * ty.x;
         grad_out[3 * q + 2] = g2 * tz.x;
+    }
+    if (HESS) {                                     // d2/dx_a dx_b = (h_ab * c0_a) * c0_b, one value for [a][b] and [b][a]
+        const double Hxx = (hxx * tx.x) * tx.x, Hxy = (hxy * tx.x) * ty.x, Hxz = (hxz * tx.x) * tz.x;
+        const double Hyy = (hyy * ty.x) * ty.x, Hyz = (hyz * ty.x) * tz.x, Hzz = (hzz * tz.x) * tz.x;
+        double* h = hess_out + 9 * q;
+        h[0] = Hxx; h[1] = Hxy; h[2] = Hxz;
+        h[3] = Hxy; h[4] = Hyy; h[5] = Hyz;
+        h[6] = Hxz; h[7] = Hyz; h[8] = Hzz;
     }
 }
 
@@ -367,14 +454,17 @@ cudaError_t k2_launch_axis_tables(const GridDev& g, double2* d_tab, cudaStream_t
 }
 
 cudaError_t k2_launch_interpolate(const FieldDev& f, const double* d_x, uint64_t n, double* d_phi, double* d_grad,
-                                  cudaStream_t stream)
+                                  cudaStream_t stream, double* d_hess)
 {
     if (n == 0) return cudaSuccess;
+    if (d_hess && !d_grad) return cudaErrorInvalidValue;
     const unsigned blocks = (unsigned)((n + K2_THREADS - 1) / K2_THREADS);
-    if (d_grad)
-        DG_KERNEL_LAUNCH((interpolate_kernel<true>), blocks, K2_THREADS, 0, stream, f.g, f.packed, f.cell_map, f.tab, d_x, (unsigned long long)n, d_phi, d_grad);
+    if (d_hess)
+        DG_KERNEL_LAUNCH((interpolate_kernel<true, true>), blocks, K2_THREADS, 0, stream, f.g, f.packed, f.cell_map, f.tab, d_x, (unsigned long long)n, d_phi, d_grad, d_hess);
+    else if (d_grad)
+        DG_KERNEL_LAUNCH((interpolate_kernel<true, false>), blocks, K2_THREADS, 0, stream, f.g, f.packed, f.cell_map, f.tab, d_x, (unsigned long long)n, d_phi, d_grad, nullptr);
     else
-        DG_KERNEL_LAUNCH((interpolate_kernel<false>), blocks, K2_THREADS, 0, stream, f.g, f.packed, f.cell_map, f.tab, d_x, (unsigned long long)n, d_phi, nullptr);
+        DG_KERNEL_LAUNCH((interpolate_kernel<false, false>), blocks, K2_THREADS, 0, stream, f.g, f.packed, f.cell_map, f.tab, d_x, (unsigned long long)n, d_phi, nullptr, nullptr);
     return DG_AFTER_LAUNCH();
 }
 

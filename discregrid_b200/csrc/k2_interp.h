@@ -18,8 +18,9 @@ struct FieldDev {                   // device-resident field (see k2_interp.cu f
 cudaError_t k2_launch_pack(const GridDev& g, const double* d_nodes, const unsigned* d_cells, uint64_t n_cells_kept,
                            double* d_packed, cudaStream_t stream);
 cudaError_t k2_launch_axis_tables(const GridDev& g, double2* d_tab, cudaStream_t stream);
+// d_grad nullable (value only); d_hess nullable, and when given d_grad must be too: the Hessian mode, hess[n][3][3] row-major
 cudaError_t k2_launch_interpolate(const FieldDev& f, const double* d_x, uint64_t n, double* d_phi, double* d_grad,
-                                  cudaStream_t stream);
+                                  cudaStream_t stream, double* d_hess = nullptr);
 cudaError_t k2_launch_shape_functions(const double* d_xi, uint64_t n, double* d_N, double* d_dN, cudaStream_t stream);
 
 }  // namespace dgb

@@ -21,6 +21,7 @@ that save()/load() stay byte-compatible with the reference's .cdf/.cdm files
                                          -> dg_reduced_function_create (addFunction + reduceField, the dense field kept on the GPU)
   interpolate(field_id, x[, gradient])   -> dg_interpolate_batch (K2, csrc/k2_interp.cu), batched over x; a float64 CUDA tensor x
                                             -> dg_interpolate_batch_device on torch's current stream (CUDA tensors out, autograd in x)
+  interpolate(field_id, x, hessian=True) -> dg_interpolate_hessian_batch[_device] (K2's Hessian mode; second-order autograd in x)
 
 The reduced calls keep the handle they get from the library until the field's first device use, which builds the interpolation
 field from it on the device (dg_field_create_reduced) instead of uploading the host copy again.
@@ -227,6 +228,43 @@ def _interpolate_function():
                 return grad_phi[:, None] * grad, None
         _INTERPOLATE = Interpolate
     return _INTERPOLATE
+
+
+_INTERPOLATE_HESSIAN = None
+
+
+def _interpolate_hessian_function():
+    """the autograd Function of interpolate(..., hessian=True) on CUDA tensors: one kernel launch gives phi, grad and hess.  phi is
+    differentiable to second order and grad to first order: phi's backward multiplies by the grad *output* (saved as an output, so a
+    create_graph backward reaches grad's own backward), and grad's backward is einsum('na,nab->nb', v, hess).  hess has no derivative:
+    a gradient that reaches it -- from a loss on hess, or from differentiating grad's backward, i.e. a third derivative of phi -- raises
+    RuntimeError rather than being taken as zero."""
+    global _INTERPOLATE_HESSIAN
+    if _INTERPOLATE_HESSIAN is None:
+        import torch
+
+        class InterpolateHessian(torch.autograd.Function):
+            @staticmethod
+            def forward(ctx, x, run):
+                phi, grad, hess = run(x)
+                ctx.set_materialize_grads(False)
+                ctx.save_for_backward(grad, hess)
+                return phi, grad, hess
+
+            @staticmethod
+            def backward(ctx, grad_phi, grad_grad, grad_hess):
+                if grad_hess is not None:
+                    raise RuntimeError("interpolate: the Hessian has no derivative (third derivatives of the interpolant are not provided)")
+                grad, hess = ctx.saved_tensors
+                dx = None
+                if grad_phi is not None:
+                    dx = grad_phi[:, None] * grad
+                if grad_grad is not None:
+                    v = torch.einsum("na,nab->nb", grad_grad, hess)
+                    dx = v if dx is None else dx + v
+                return dx, None
+        _INTERPOLATE_HESSIAN = InterpolateHessian
+    return _INTERPOLATE_HESSIAN
 
 
 def grid_desc(domain_min, domain_max, resolution, cell_size=None, inv_cell_size=None):
@@ -525,21 +563,35 @@ class CubicLagrangeDiscreteGrid:
             pass
 
     # ------------------------------------------------------------------ interpolate (cubic_lagrange_discrete_grid.cpp:977-1063)
-    def interpolate(self, field_id_or_x, x=None, gradient=False):
+    def interpolate(self, field_id_or_x, x=None, gradient=False, hessian=False):
         """interpolate(x) == interpolate(0, x) (discrete_grid.hpp:38-41).  x: (n, 3).  Returns phi[n], or
         (phi[n], grad[n,3]) when gradient=True.  Out-of-domain / removed cell / missing coefficient -> DBL_MAX, grad 0.
         A numpy array (or a CPU tensor) goes through the host pipeline and gives numpy arrays.  A float64 torch tensor (n, 3) or (3,) on
         the field's CUDA device stays there: the query runs on torch's current stream, asynchronously, and phi / grad are CUDA tensors with
         the bits of the host route.  When x requires grad (and grad mode is on), phi is differentiable in x, first order only:
-        d phi / d x is K2's gradient, the reference's derivative of the interpolant (0 at DBL_MAX).  The returned grad is not differentiable."""
+        d phi / d x is K2's gradient, the reference's derivative of the interpolant (0 at DBL_MAX).  The returned grad is not differentiable.
+
+        hessian=True (beyond the reference) returns (phi[n], grad[n,3], hess[n,3,3]) from one pass of K2's Hessian mode: phi and grad have
+        the bits of gradient=True, hess is the exactly symmetric second derivative of the interpolant in x (+0.0 where phi is DBL_MAX).
+        The interpolant is only C0 across cell faces, so on a face hess is that of the cell the point is assigned to.  On CUDA tensors
+        that require grad, phi is differentiable to second order and grad to first order (its vector-Jacobian product is
+        einsum('na,nab->nb', v, hess)), so torch.autograd.grad(..., create_graph=True) works on phi; hess has no derivative, and a
+        gradient that reaches it (a third derivative of phi) raises RuntimeError."""
         if x is None:
             field_id, x = 0, field_id_or_x
         else:
             field_id = field_id_or_x
         if _device.is_device_query(x):
+            if hessian:
+                return self._interpolate_hessian_device(field_id, x)
             return self._interpolate_device(field_id, x, gradient)
         x = np.ascontiguousarray(x, np.float64).reshape(-1, 3)
         phi = np.empty(len(x))
+        if hessian:
+            grad, hess = np.empty((len(x), 3)), np.empty((len(x), 3, 3))
+            capi.check(capi.lib.dg_interpolate_hessian_batch(self._device_field(field_id), capi.ptr(x, capi.F64P), len(x), capi.ptr(phi, capi.F64P),
+                                                             capi.ptr(grad, capi.F64P), capi.ptr(hess, capi.F64P)))
+            return phi, grad, hess
         grad = np.empty((len(x), 3)) if gradient else None
         capi.check(capi.lib.dg_interpolate_batch(self._device_field(field_id), capi.ptr(x, capi.F64P), len(x),
                                                  capi.ptr(phi, capi.F64P), capi.ptr(grad, capi.F64P)))
@@ -564,6 +616,25 @@ class CubicLagrangeDiscreteGrid:
         else:
             phi, grad = run(x, gradient)
         return (phi, grad) if gradient else phi
+
+    def _interpolate_hessian_device(self, field_id, x):
+        """the CUDA-tensor route of hessian=True: dg_interpolate_hessian_batch_device on torch's current stream"""
+        import torch
+        h = self._device_field(field_id)
+        info = (C.c_uint64 * 4)()
+        capi.check(capi.lib.dg_field_info(h, info))
+        x = _device.points(x, int(info[3]), "interpolate")
+
+        def run(xc):
+            phi = torch.empty(len(xc), dtype=torch.float64, device=xc.device)
+            grad = torch.empty((len(xc), 3), dtype=torch.float64, device=xc.device)
+            hess = torch.empty((len(xc), 3, 3), dtype=torch.float64, device=xc.device)
+            capi.check(capi.lib.dg_interpolate_hessian_batch_device(h, xc.data_ptr(), len(xc), phi.data_ptr(), grad.data_ptr(), hess.data_ptr(),
+                                                                    _device.stream(xc)))
+            return phi, grad, hess
+        if x.requires_grad and torch.is_grad_enabled():
+            return _interpolate_hessian_function().apply(x, run)
+        return run(x)
 
     # ------------------------------------------------------------------ save / load (cubic_lagrange_discrete_grid.cpp:678-778)
     def save(self, filename):

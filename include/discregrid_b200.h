@@ -235,6 +235,13 @@ DG_API int dg_field_info(const dg_field* field, uint64_t info[4]);
  * -> phi = DBL_MAX and grad = 0 exactly as the reference. */
 DG_API int dg_interpolate_batch(const dg_field* field, const double* x, uint64_t n, double* phi, double* grad);
 DG_API int dg_interpolate_batch_device(const dg_field* field, const double* d_x, uint64_t n, double* d_phi, double* d_grad, void* stream);
+/* Value, gradient and Hessian in one pass (beyond the reference, which has no Hessian): phi[n] and grad[n x 3] have the bits of
+ * dg_interpolate_batch with a gradient; hess[n x 3 x 3] is the row-major Hessian in x, exactly symmetric (the numerical contract is
+ * in k2_interp.cu).  Sentinel points get phi = DBL_MAX, grad = 0 and hess = +0.0.  phi, grad and hess are all required when n > 0.
+ * The _device form takes device pointers and runs on `stream` (a cudaStream_t; NULL = legacy default stream), asynchronously. */
+DG_API int dg_interpolate_hessian_batch(const dg_field* field, const double* x, uint64_t n, double* phi, double* grad, double* hess);
+DG_API int dg_interpolate_hessian_batch_device(const dg_field* field, const double* d_x, uint64_t n, double* d_phi, double* d_grad, double* d_hess,
+                                               void* stream);
 /* shape_function_ (cubic_lagrange_discrete_grid.cpp:339-580) for n reference-cell points xi[n x 3]:
  * N[n x 32], dN[n x 32 x 3] (nullable). */
 DG_API int dg_shape_functions(const double* xi, uint64_t n, double* N, double* dN);
