@@ -1,10 +1,13 @@
 // GenerateSDF -- same command line and output as the reference tool (cmd/generate_sdf/main.cpp:28-130), sampling on the GPU.
-//   GenerateSDF [-r "nx ny nz"] [-d "minx miny minz maxx maxy maxz"] [-i] [-o out.cdf] [--gpus N] [--band W [--no-reduction]] input.obj
+//   GenerateSDF [-r "nx ny nz"] [-d "minx miny minz maxx maxy maxz"] [-i] [-o out.cdf] [--gpus N] [--band W [--no-reduction]]
+//               [--sign pseudonormal|winding] input.obj
 // --gpus N (new, SURVEY 5 "same flags + --gpus N"): the node loop is dealt to N GPUs of this node (dg_add_function_sdf_multi); same file.
 // --band W (new): a narrow-band field -- addFunction(func, verbose, pred) with pred(x) = |distance(x)| <= W (world units), DBL_MAX
 //   elsewhere, then reduceField with an always-true predicate (drops the DBL_MAX nodes and the cells without a kept node), as
 //   GenerateDensityMap does (cmd/generate_density_map/main.cpp:119-147) -- both in one call (addReducedBandField), so that only the reduced
 //   field reaches the host.  --no-reduction keeps the dense field (addFunction with the band predicate).  One GPU only.
+// --sign pseudonormal|winding (new): where the distances take their sign from.  pseudonormal (default) is the reference's rule, right for
+//   closed manifold meshes; winding uses the generalized winding number (inside iff w > 0.5) for open or non-manifold meshes.  One GPU only.
 // The one functional change against the reference source: the functor handed to addFunction is the recognisable
 // MeshSignedDistanceFunction instead of an anonymous lambda (main.cpp:94-102).
 #include <Discregrid/All>
@@ -22,6 +25,7 @@ int main(int argc, char* argv[])
     bool invert = false;
     int n_gpus = 1;
     bool use_band = false, no_reduction = false;
+    std::string sign_mode = "pseudonormal";
     double band = 0.0;
     for (int a = 1; a < argc; a++) {
         const std::string s = argv[a];
@@ -31,6 +35,7 @@ int main(int argc, char* argv[])
                          "  -r, --resolution \"nx ny nz\"   -d, --domain \"minx miny minz maxx maxy maxz\"   -i, --invert   -o, --output file.cdf   --gpus N\n"
                          "  --band W   keep only nodes within distance W of the surface (others DBL_MAX), then reduce the field\n"
                          "  --no-reduction   with --band: keep the dense field (no reduceField)\n"
+                         "  --sign pseudonormal|winding   sign from the pseudonormal (default; closed meshes) or the generalized winding number\n"
                          "Example: GenerateSDF -r \"50 50 50\" dragon.obj" << std::endl;
             return 0;
         } else if (s == "-r" || s == "--resolution") { std::istringstream is(next()); is >> resolution[0] >> resolution[1] >> resolution[2]; }
@@ -40,11 +45,14 @@ int main(int argc, char* argv[])
         else if (s == "--gpus") n_gpus = std::atoi(next().c_str());
         else if (s == "--band") { use_band = true; band = std::strtod(next().c_str(), nullptr); }
         else if (s == "--no-reduction") no_reduction = true;
+        else if (s == "--sign") sign_mode = next();
         else filename = s;
     }
     if (filename.empty()) { std::cout << "ERROR: No input mesh given." << std::endl; return 1; }
     if (!std::ifstream(filename).good()) { std::cerr << "ERROR: Input file does not exist!" << std::endl; return 1; }
     if (use_band && n_gpus > 1) { std::cerr << "ERROR: --band runs on one GPU; it cannot be combined with --gpus " << n_gpus << std::endl; return 1; }
+    if (sign_mode != "pseudonormal" && sign_mode != "winding") { std::cerr << "ERROR: --sign must be pseudonormal or winding" << std::endl; return 1; }
+    if (sign_mode == "winding" && n_gpus > 1) { std::cerr << "ERROR: --sign winding runs on one GPU; it cannot be combined with --gpus " << n_gpus << std::endl; return 1; }
     if (use_band && !(band >= 0.0)) { std::cerr << "ERROR: --band needs a width >= 0" << std::endl; return 1; }
     try {
         std::cout << "Load mesh...";
@@ -53,6 +61,7 @@ int main(int argc, char* argv[])
         std::cout << "Set up data structures...";
         Discregrid::TriangleMeshDistance md(mesh);
         if (n_gpus > 1) md.useGpus(n_gpus);
+        if (sign_mode == "winding") md.setSignMode(Discregrid::SignMode::Winding);
         std::cout << "DONE" << std::endl;
 
         AlignedBox3d domain;

@@ -19,6 +19,9 @@
 namespace Discregrid {
 
 enum class NearestEntity { V0, V1, V2, E01, E12, E02, F };
+// new: where signed distances take their sign from.  Pseudonormal is the reference's rule (right for closed manifold meshes only); Winding
+// takes it from the generalized winding number (inside iff w > 0.5), which also holds for open and non-manifold meshes.  One GPU only.
+enum class SignMode { Pseudonormal = DG_SIGN_PSEUDONORMAL, Winding = DG_SIGN_WINDING };
 
 template <typename FLOAT>
 class Vec3r {
@@ -87,15 +90,41 @@ public:
         if (n_gpus > 1 && dg_mesh_group_create(m_mesh, n_gpus, nullptr, &m_group) != DG_OK) throw std::runtime_error(std::string("TriangleMeshDistance: ") + dg_last_error());
     }
     dg_mesh_group* group() const { return m_group; }
+    // new: the sign mode of signed_distance and of the grid calls built on it (MeshSignedDistanceFunction, MeshDistanceBandPredicate);
+    // beta >= 1 or infinity (the exact sum).  Not to be called while another thread uses this object.  The winding mode runs on one GPU:
+    // it throws after useGpus(n > 1), and useGpus(n > 1) throws in it.
+    void setSignMode(SignMode mode, double beta = 2.0)
+    {
+        require();
+        if (mode == SignMode::Winding && m_group) throw std::runtime_error("TriangleMeshDistance: the winding sign mode runs on one GPU; it is not available after useGpus(n > 1)");
+        if (dg_mesh_set_sign_mode(m_mesh, (int)mode, beta) != DG_OK) throw std::runtime_error(std::string("TriangleMeshDistance: ") + dg_last_error());
+        m_sign_mode = mode;
+    }
+    SignMode signMode() const { return m_sign_mode; }
+    // new: generalized winding number at a point (1 inside a closed surface, 0 outside), or at n points (xyzxyz) into w[n]
+    template <typename IndexableVector3double> double winding_number(const IndexableVector3double& p, double beta = 2.0) const
+    {
+        const double x[3] = {(double)p[0], (double)p[1], (double)p[2]};
+        double w = 0.0;
+        winding_number(x, 1, &w, beta);
+        return w;
+    }
+    void winding_number(const double* points, size_t n, double* w, double beta = 2.0) const
+    {
+        require();
+        if (dg_mesh_winding_number(m_mesh, points, n, beta, w) != DG_OK) throw std::runtime_error(std::string("TriangleMeshDistance: ") + dg_last_error());
+    }
 
 private:
     dg_mesh* m_mesh = nullptr;
     dg_mesh_group* m_group = nullptr;
+    SignMode m_sign_mode = SignMode::Pseudonormal;
     void require() const { if (!m_mesh) throw std::runtime_error("DistanceTriangleMesh error: not constructed."); }
     void upload(const std::vector<double>& V, const std::vector<uint32_t>& F)
     {
         if (m_group) { dg_mesh_group_destroy(m_group); m_group = nullptr; }
         if (m_mesh) { dg_mesh_destroy(m_mesh); m_mesh = nullptr; }
+        m_sign_mode = SignMode::Pseudonormal;
         if (F.empty()) throw std::runtime_error("DistanceTriangleMesh error: Empty triangle list.");
         if (dg_mesh_create(V.data(), V.size() / 3, F.data(), F.size() / 3, &m_mesh) != DG_OK) throw std::runtime_error(std::string("TriangleMeshDistance: ") + dg_last_error());
     }

@@ -13,6 +13,7 @@ LIB_PATH = os.environ.get("DISCREGRID_B200_LIB") or os.path.join(_HERE, "lib", "
 
 DG_OK, DG_ERR_INVALID, DG_ERR_NO_DEVICE, DG_ERR_CUDA, DG_ERR_NOMEM, DG_ERR_SELFTEST, DG_ERR_IO, DG_ERR_CALLBACK = 0, -1, -2, -3, -4, -5, -6, -7
 DBL_MAX = 1.7976931348623157e308
+DG_SIGN_PSEUDONORMAL, DG_SIGN_WINDING = 0, 1
 UINT32_MAX = 0xFFFFFFFF
 
 
@@ -72,6 +73,9 @@ SIGNATURES = {
     "dg_mesh_info": (C.c_int, [_vp, _u64p]),
     "dg_mesh_tree": (C.c_int, [_vp, _dp, _i32p]),
     "dg_mesh_pseudonormals": (C.c_int, [_vp, _dp, _dp, _dp]),
+    "dg_mesh_set_sign_mode": (C.c_int, [_vp, C.c_int, C.c_double]),
+    "dg_mesh_winding_number": (C.c_int, [_vp, _dp, C.c_uint64, C.c_double, _dp]),
+    "dg_mesh_winding_number_device": (C.c_int, [_vp, _vp, C.c_uint64, C.c_double, _vp, _vp]),
     "dg_mesh_distance": (C.c_int, [_vp, _dp, C.c_uint64, C.c_int, _dp, _dp, _i32p, _i32p]),
     "dg_mesh_distance_device": (C.c_int, [_vp, _vp, C.c_uint64, C.c_int, _vp, _vp, _vp, _vp, _vp]),
     "dg_sample_sdf": (C.c_int, [_vp, _gp, C.c_double, C.c_uint64, C.c_uint64, _dp]),

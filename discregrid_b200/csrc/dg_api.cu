@@ -39,6 +39,7 @@
 #include "k2_interp.h"
 #include "k3_density.h"
 #include "k4_reduce.h"
+#include "k5_winding.h"
 #include "reduce_field.h"
 #include "obj_reader.h"
 
@@ -174,6 +175,14 @@ struct dg_mesh {
     DeviceBvh dev;
     int device = 0;
     uint64_t build_us = 0, upload_us = 0;
+    // sign mode (dg_mesh_set_sign_mode) and the winding-number records of K5, built and uploaded at their first use
+    int sign_mode = DG_SIGN_PSEUDONORMAL;
+    double beta = 2.0;
+    mutable std::mutex wind_mu;
+    mutable bool wind_ready = false;
+    mutable DevBuf<WindLeaf> d_wind_leaves;
+    mutable DevBuf<WindClusterPair> d_wind_clusters;
+    mutable WindDev wind;
 };
 
 struct dg_field {
@@ -386,6 +395,10 @@ int dg_mesh_info(const dg_mesh* m, uint64_t info[8])
     info[0] = m->host.n_vertices; info[1] = m->host.n_triangles; info[2] = (uint64_t)m->dev.stack_depth;
     info[3] = (uint64_t)m->host.flags;
     info[4] = m->d_spheres.bytes() + m->d_leaves.bytes() + m->d_normals.bytes() + m->d_nodes_f.bytes() + m->d_leaves_f.bytes();
+    {
+        std::lock_guard<std::mutex> lock(m->wind_mu);
+        info[4] += m->d_wind_leaves.bytes() + m->d_wind_clusters.bytes();      // 0 until the winding records are first used
+    }
     info[5] = m->build_us; info[6] = m->upload_us; info[7] = (uint64_t)m->device;
     return DG_OK;
 }
@@ -412,12 +425,100 @@ int dg_mesh_pseudonormals(const dg_mesh* m, double* tri, double* edge, double* v
     return DG_OK;
 }
 
+// ------------------------------------------------------------------------------------------------ K5: winding numbers, the winding sign mode
+static int check_beta(double beta, const char* who)
+{
+    if (!(beta >= 1.0)) return fail(DG_ERR_INVALID, "%s: beta must be >= 1 or +inf (got %g)", who, beta);     // below 1 or NaN
+    return DG_OK;
+}
+
+// the mesh's K5 records on its device, built (host threads) and uploaded at the first call; later calls only read them
+static int winding_dev(const dg_mesh* m, const WindDev*& out, const char* who)
+{
+    std::lock_guard<std::mutex> lock(m->wind_mu);
+    if (!m->wind_ready) {
+        const uint64_t nT = m->host.n_triangles;
+        if (m->dev.stack_depth > K5_MAX_STACK) return fail(DG_ERR_INVALID, "%s: tree too deep for the winding walk", who);
+        RawVec<WindLeaf> leaves;
+        RawVec<WindClusterPair> clusters;
+        try { build_winding_records(m->host, leaves, clusters); }
+        catch (const std::bad_alloc&) { return fail(DG_ERR_NOMEM, "%s: out of host memory", who); }
+        DevBuf<WindLeaf> dl;
+        DevBuf<WindClusterPair> dc;
+        DG_CUDA(dl.alloc(nT));
+        DG_CUDA(dc.alloc(nT));
+        DG_CUDA(cudaMemcpy(dl.p, leaves.data(), nT * sizeof(WindLeaf), cudaMemcpyHostToDevice));
+        DG_CUDA(cudaMemcpy(dc.p, clusters.data(), nT * sizeof(WindClusterPair), cudaMemcpyHostToDevice));
+        std::swap(m->d_wind_leaves.p, dl.p); std::swap(m->d_wind_leaves.n, dl.n);
+        std::swap(m->d_wind_clusters.p, dc.p); std::swap(m->d_wind_clusters.n, dc.n);
+        m->wind.leaves = m->d_wind_leaves.p; m->wind.clusters = m->d_wind_clusters.p;
+        m->wind.n_tri = (int)nT; m->wind.stack_depth = m->dev.stack_depth;
+        m->wind_ready = true;
+    }
+    out = &m->wind;
+    return DG_OK;
+}
+
+static int refuse_winding(const dg_mesh* m, const char* who)
+{
+    if (m && m->sign_mode == DG_SIGN_WINDING)
+        return fail(DG_ERR_INVALID, "%s: the mesh is in the winding sign mode, which runs on one GPU only (dg_sample_sdf_device, dg_add_function_sdf, "
+                    "dg_reduced_band_create ...); set DG_SIGN_PSEUDONORMAL for the multi-GPU and sharded entry points", who);
+    return DG_OK;
+}
+
+int dg_mesh_set_sign_mode(dg_mesh* m, int mode, double beta)
+{
+    if (!m) return fail(DG_ERR_INVALID, "dg_mesh_set_sign_mode: mesh is NULL (not constructed)");
+    if (mode != DG_SIGN_PSEUDONORMAL && mode != DG_SIGN_WINDING) return fail(DG_ERR_INVALID, "dg_mesh_set_sign_mode: unknown mode %d", mode);
+    if (int rc = check_beta(beta, "dg_mesh_set_sign_mode")) return rc;
+    m->sign_mode = mode;
+    m->beta = beta;
+    return DG_OK;
+}
+
+int dg_mesh_winding_number_device(const dg_mesh* m, const double* d_x, uint64_t n, double beta, double* d_w, void* stream)
+{
+    if (!m) return fail(DG_ERR_INVALID, "dg_mesh_winding_number: mesh is NULL (not constructed)");
+    if (int rc = check_beta(beta, "dg_mesh_winding_number")) return rc;
+    if (n && (!d_x || !d_w)) return fail(DG_ERR_INVALID, "dg_mesh_winding_number: points or output is NULL");
+    if (int rc = check_handle_device(m->device, "dg_mesh_winding_number")) return rc;
+    if (n == 0) return DG_OK;
+    const WindDev* wd = nullptr;
+    if (int rc = winding_dev(m, wd, "dg_mesh_winding_number")) return rc;
+    DG_LAUNCH(k5_launch_winding(*wd, d_x, n, beta, d_w, (cudaStream_t)stream));
+    return DG_OK;
+}
+
+int dg_mesh_winding_number(const dg_mesh* m, const double* x, uint64_t n, double beta, double* w)
+{
+    if (!m) return fail(DG_ERR_INVALID, "dg_mesh_winding_number: mesh is NULL (not constructed)");
+    if (int rc = check_beta(beta, "dg_mesh_winding_number")) return rc;
+    if (n == 0) return DG_OK;
+    if (!x || !w) return fail(DG_ERR_INVALID, "dg_mesh_winding_number: points or output is NULL");
+    DevBuf<double> d_x, d_w;
+    DG_CUDA(d_x.alloc(3 * n));
+    DG_CUDA(d_w.alloc(n));
+    DG_CUDA(cudaMemcpy(d_x.p, x, 3 * n * sizeof(double), cudaMemcpyHostToDevice));
+    if (int rc = dg_mesh_winding_number_device(m, d_x.p, n, beta, d_w.p, nullptr)) return rc;
+    DG_CUDA(cudaMemcpy(w, d_w.p, n * sizeof(double), cudaMemcpyDeviceToHost));
+    DG_CUDA(cudaDeviceSynchronize());
+    return DG_OK;
+}
+
 int dg_mesh_distance_device(const dg_mesh* m, const double* d_pts, uint64_t n, int is_signed, double* d_dist, double* d_near,
                             int32_t* d_ent, int32_t* d_tri, void* stream)
 {
     if (!m) return fail(DG_ERR_INVALID, "dg_mesh_distance: mesh is NULL (not constructed)");
     if (n && !d_pts) return fail(DG_ERR_INVALID, "dg_mesh_distance: points is NULL");
     if (int rc = check_handle_device(m->device, "dg_mesh_distance")) return rc;
+    if (is_signed && m->sign_mode == DG_SIGN_WINDING) {       // the unsigned query, then the sign from w (k5_winding.cu)
+        const WindDev* wd = nullptr;
+        if (int rc = winding_dev(m, wd, "dg_mesh_distance")) return rc;
+        DG_LAUNCH(k1_launch_distance(m->dev, d_pts, n, 0, d_dist, d_near, d_ent, d_tri, (cudaStream_t)stream));
+        if (d_dist) DG_LAUNCH(k5_launch_sign_points(*wd, d_pts, n, m->beta, d_dist, (cudaStream_t)stream));
+        return DG_OK;
+    }
     DG_LAUNCH(k1_launch_distance(m->dev, d_pts, n, is_signed, d_dist, d_near, d_ent, d_tri, (cudaStream_t)stream));
     return DG_OK;
 }
@@ -465,6 +566,13 @@ int dg_sample_sdf_device(const dg_mesh* m, const dg_grid_desc* grid, double sign
     if (int rc = check_range(grid, l_begin, l_end, g, "dg_sample_sdf")) return rc;
     if (l_end > l_begin && !d_out) return fail(DG_ERR_INVALID, "dg_sample_sdf: output is NULL");
     if (int rc = check_handle_device(m->device, "dg_sample_sdf")) return rc;
+    if (m->sign_mode == DG_SIGN_WINDING) {      // K1 with sign = +1, then the node pass of k5_winding.cu
+        const WindDev* wd = nullptr;
+        if (int rc = winding_dev(m, wd, "dg_sample_sdf")) return rc;
+        DG_LAUNCH(k1_launch_sample_nodes(m->dev, g, 1.0, l_begin, l_end - l_begin, d_out, (cudaStream_t)stream));
+        DG_LAUNCH(k5_launch_sign_nodes(*wd, g, sign, INFINITY, m->beta, l_begin, l_end - l_begin, d_out, (cudaStream_t)stream));
+        return DG_OK;
+    }
     DG_LAUNCH(k1_launch_sample_nodes(m->dev, g, sign, l_begin, l_end - l_begin, d_out, (cudaStream_t)stream));
     return DG_OK;
 }
@@ -488,18 +596,22 @@ int dg_sample_sdf_band_device(const dg_mesh* m, const dg_grid_desc* grid, double
     if (int rc = check_handle_device(m->device, "dg_sample_sdf_band")) return rc;
     if (l_end == l_begin) return DG_OK;
     const cudaStream_t st = (cudaStream_t)stream;
+    const WindDev* wd = nullptr;
+    if (m->sign_mode == DG_SIGN_WINDING) { if (int rc = winding_dev(m, wd, "dg_sample_sdf_band")) return rc; }
+    const double k1_sign = wd ? 1.0 : sign;     // winding mode: K1 with sign = +1, then the node pass
     const size_t bytes = k1_band_scratch_bytes(g, l_begin, l_end - l_begin);
     void* scratch = nullptr;
 #ifdef DG_EMU
     DG_CUDA(cudaMalloc(&scratch, bytes));
-    const cudaError_t e = k1_launch_sample_nodes_band(m->dev, g, sign, band, l_begin, l_end - l_begin, d_out, scratch, st);
+    const cudaError_t e = k1_launch_sample_nodes_band(m->dev, g, k1_sign, band, l_begin, l_end - l_begin, d_out, scratch, st);
     cudaFree(scratch);
 #else
     DG_CUDA(cudaMallocAsync(&scratch, bytes, st));
-    const cudaError_t e = k1_launch_sample_nodes_band(m->dev, g, sign, band, l_begin, l_end - l_begin, d_out, scratch, st);
+    const cudaError_t e = k1_launch_sample_nodes_band(m->dev, g, k1_sign, band, l_begin, l_end - l_begin, d_out, scratch, st);
     cudaFreeAsync(scratch, st);
 #endif
     DG_LAUNCH(e);
+    if (wd) DG_LAUNCH(k5_launch_sign_nodes(*wd, g, sign, band, m->beta, l_begin, l_end - l_begin, d_out, st));
     return DG_OK;
 }
 
@@ -614,11 +726,15 @@ static int sample_sdf_host_locked(const dg_mesh* m, const GridDev& g, double sig
             const uint64_t b = c * chunk, cnt = (b + chunk <= n) ? chunk : n - b;
             band_bytes = std::max(band_bytes, k1_band_scratch_bytes(g, l_begin + b, cnt));
         }
+    const WindDev* wd = nullptr;             // winding mode: every chunk is K1 with sign = +1, then the node pass of k5_winding.cu
+    if (m->sign_mode == DG_SIGN_WINDING) { if (int rc = winding_dev(m, wd, "dg_sample_sdf")) return rc; }
+    const double k1_sign = wd ? 1.0 : sign;
     DG_CUDA(g_pool.prepare(n, n_chunks, band_bytes));
     for (uint64_t c = 0; c < n_chunks; c++) {
         const uint64_t b = c * chunk, cnt = (b + chunk <= n) ? chunk : n - b;
-        if (band) DG_LAUNCH(k1_launch_sample_nodes_band(m->dev, g, sign, *band, l_begin + b, cnt, g_pool.d_out + b, g_pool.band_scratch[c & 1], g_pool.s_k[c & 1]));
-        else DG_LAUNCH(k1_launch_sample_nodes(m->dev, g, sign, l_begin + b, cnt, g_pool.d_out + b, g_pool.s_k[c & 1]));
+        if (band) DG_LAUNCH(k1_launch_sample_nodes_band(m->dev, g, k1_sign, *band, l_begin + b, cnt, g_pool.d_out + b, g_pool.band_scratch[c & 1], g_pool.s_k[c & 1]));
+        else DG_LAUNCH(k1_launch_sample_nodes(m->dev, g, k1_sign, l_begin + b, cnt, g_pool.d_out + b, g_pool.s_k[c & 1]));
+        if (wd) DG_LAUNCH(k5_launch_sign_nodes(*wd, g, sign, band ? *band : INFINITY, m->beta, l_begin + b, cnt, g_pool.d_out + b, g_pool.s_k[c & 1]));
         DG_CUDA(cudaEventRecord(g_pool.chunk_ev[c], g_pool.s_k[c & 1]));
     }
     return drain_to_host_locked(g_pool.d_out, n, chunk, out_host, copier);
@@ -929,6 +1045,7 @@ int dg_mesh_group_create(const dg_mesh* mesh, int n_gpus, const int* devices, dg
     if (!out) return fail(DG_ERR_INVALID, "dg_mesh_group_create: out is NULL");
     *out = nullptr;
     if (!mesh) return fail(DG_ERR_INVALID, "dg_mesh_group_create: mesh is NULL (not constructed)");
+    if (int rc = refuse_winding(mesh, "dg_mesh_group_create")) return rc;
     if (int rc = require_device()) return rc;
     const int have = dg_device_count();
     if (n_gpus < 1 || n_gpus > 16 || n_gpus > have) return fail(DG_ERR_INVALID, "dg_mesh_group_create: n_gpus = %d, but 1..min(16, %d visible devices) are possible", n_gpus, have);
@@ -990,6 +1107,7 @@ static int dg_add_function_sdf_multi_impl(dg_mesh_group* grp, const dg_grid_desc
                               uint32_t* cell_map_host, double* timings_ms)
 {
     if (!grp) return fail(DG_ERR_INVALID, "dg_add_function_sdf_multi: group is NULL");
+    if (int rc = refuse_winding(grp->parts[0], "dg_add_function_sdf_multi")) return rc;
     GridDev g;
     uint64_t n_nodes = 0;
     if (grid && dg_grid_num_nodes(grid->resolution, &n_nodes)) return DG_ERR_INVALID;
@@ -1065,6 +1183,7 @@ static int dg_add_function_sdf_multi_impl(dg_mesh_group* grp, const dg_grid_desc
 int dg_sample_sdf_multi_device(dg_mesh_group* grp, const dg_grid_desc* grid, double sign, double* const* d_out)
 {
     if (!grp || !d_out) return fail(DG_ERR_INVALID, "dg_sample_sdf_multi_device: NULL argument");
+    if (int rc = refuse_winding(grp->parts[0], "dg_sample_sdf_multi_device")) return rc;
     GridDev g;
     uint64_t n_nodes = 0;
     if (grid && dg_grid_num_nodes(grid->resolution, &n_nodes)) return DG_ERR_INVALID;
@@ -1141,6 +1260,7 @@ int dg_slab_ranges(const dg_grid_desc* grid, uint32_t part, uint32_t n_parts, ui
 int dg_sample_sdf_slab_device(const dg_mesh* m, const dg_grid_desc* grid, double sign, uint32_t part, uint32_t n_parts, double* d_full, void* stream)
 {
     if (!m) return fail(DG_ERR_INVALID, "dg_sample_sdf_slab: mesh is NULL (not constructed)");
+    if (int rc = refuse_winding(m, "dg_sample_sdf_slab")) return rc;
     GridDev g; const char* why = "";
     if (!grid_to_dev(grid, g, &why)) return fail(DG_ERR_INVALID, "dg_sample_sdf_slab: %s", why);
     if (n_parts == 0 || part >= n_parts || !d_full) return fail(DG_ERR_INVALID, "dg_sample_sdf_slab: bad part / n_parts / output");
@@ -1176,6 +1296,7 @@ int dg_interleaved_node_slots(const dg_grid_desc* grid, uint32_t n_parts, uint64
 int dg_sample_sdf_interleaved_device(const dg_mesh* m, const dg_grid_desc* grid, double sign, uint32_t part, uint32_t n_parts, double* d_slot, void* stream)
 {
     if (!m) return fail(DG_ERR_INVALID, "dg_sample_sdf_interleaved: mesh is NULL (not constructed)");
+    if (int rc = refuse_winding(m, "dg_sample_sdf_interleaved")) return rc;
     GridDev g; const char* why = "";
     if (!grid_to_dev(grid, g, &why)) return fail(DG_ERR_INVALID, "dg_sample_sdf_interleaved: %s", why);
     InterleavedLayout L;

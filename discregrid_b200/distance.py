@@ -49,6 +49,7 @@ class TriangleMeshDistance:
         h = C.c_void_p()
         capi.check(capi.lib.dg_mesh_create(capi.ptr(V, capi.F64P), len(V), capi.ptr(F, capi.U32P), len(F), C.byref(h)))
         self._h = h
+        self._sign_mode = "pseudonormal"
         self.n_vertices, self.n_triangles = len(V), len(F)
         return self
 
@@ -99,6 +100,40 @@ class TriangleMeshDistance:
         a = (C.c_uint64 * 8)()
         capi.check(capi.lib.dg_mesh_info(self.handle, a))
         return int(a[7])
+
+    def set_sign_mode(self, mode, beta=2.0):
+        """Where signed distances take their sign from (beyond the reference).  "pseudonormal" (the default) is the reference's rule, the
+        angle-weighted pseudonormal at the nearest entity, which is right only for closed manifold meshes.  "winding" takes it from the
+        generalized winding number: inside iff winding_number(x, beta) > 0.5, which holds for open, non-manifold and self-intersecting
+        meshes too.  signed_distance, MeshSignedDistance, MeshDistanceBand and the grid calls built on them follow the mode; multi-GPU
+        sampling refuses the winding mode.  beta >= 1 or inf (exact).  Not to be called while another thread queries this mesh."""
+        modes = {"pseudonormal": capi.DG_SIGN_PSEUDONORMAL, "winding": capi.DG_SIGN_WINDING}
+        if mode not in modes:
+            raise ValueError(f"sign mode must be 'pseudonormal' or 'winding' (got {mode!r})")
+        capi.check(capi.lib.dg_mesh_set_sign_mode(self.handle, modes[mode], float(beta)))
+        self._sign_mode = mode
+        return self
+
+    @property
+    def sign_mode(self):
+        return getattr(self, "_sign_mode", "pseudonormal")
+
+    def winding_number(self, points, beta=2.0):
+        """Generalized winding number w(x) of the mesh (Barill et al. 2018) at points (n, 3) or (3,): 1 inside a closed surface, 0 outside,
+        fractional near holes.  Clusters of triangles farther than beta times their radius are summed by a far-field expansion; beta = inf
+        sums every triangle exactly.  A numpy array returns a numpy array; a float64 CUDA tensor on the mesh's device returns a CUDA tensor,
+        computed on torch's current stream with the same bits."""
+        beta = float(beta)
+        if _device.is_device_query(points):
+            import torch
+            x = _device.points(points, self.device, "winding_number")
+            w = torch.empty(len(x), dtype=torch.float64, device=x.device)
+            capi.check(capi.lib.dg_mesh_winding_number_device(self.handle, x.data_ptr(), len(x), beta, w.data_ptr(), _device.stream(x)))
+            return w
+        x = np.ascontiguousarray(points, dtype=np.float64).reshape(-1, 3)
+        w = np.empty(len(x))
+        capi.check(capi.lib.dg_mesh_winding_number(self.handle, capi.ptr(x, capi.F64P), len(x), beta, capi.ptr(w, capi.F64P)))
+        return w
 
     def _query_device(self, points, signed):
         """the CUDA-tensor route: dg_mesh_distance_device on torch's current stream, asynchronous like a torch op"""

@@ -131,6 +131,29 @@ DG_API int dg_mesh_distance_device(const dg_mesh* mesh, const double* d_points, 
                             double* d_distance, double* d_nearest_point, int32_t* d_nearest_entity,
                             int32_t* d_triangle_id, void* stream);
 
+/* ---- sign modes and generalized winding numbers (K5, k5_winding.cu; beyond the reference) -----------------------------------------
+ * The reference signs every distance with the angle-weighted pseudonormal at the nearest entity (TriangleMeshDistance.h:269-308), which is
+ * right only for closed manifold meshes (dg_mesh_info[3] reports open and non-manifold edges).  The winding mode takes the sign from the
+ * generalized winding number w(x) instead (Barill et al. 2018): inside iff w > 0.5.  w is the sum of the triangles' solid angles / 4 pi,
+ * evaluated over the mesh's sphere tree with a far-field expansion for clusters farther than beta times their radius; the numerical
+ * contract (operation order, the library's own atan2, the fold order) is stated in k5_winding.cu.  beta >= 1 or +inf (exact sum over all
+ * triangles); NaN or < 1: DG_ERR_INVALID.  The default beta is 2.
+ *   dg_mesh_set_sign_mode: DG_SIGN_PSEUDONORMAL (the default, the reference's rule) or DG_SIGN_WINDING, with the beta the signed entry
+ *       points then use.  Must not be called while another call uses the same mesh.  In the winding mode these single-GPU entry points take
+ *       the sign from w: dg_mesh_distance[_device] with is_signed (nearest point, entity and triangle id are those of the unsigned query),
+ *       dg_sample_sdf[_device], dg_add_function_sdf, dg_sample_sdf_band_device, dg_add_function_sdf_band, dg_reduced_band_create: K1 runs
+ *       with sign = +1 and a node pass writes sign * (w > 0.5 ? -d : d); the DBL_MAX sentinels are those of the pseudonormal mode.
+ *       dg_mesh_group_create, dg_add_function_sdf_multi, dg_sample_sdf_multi_device and the slab / interleaved entry points refuse a mesh in
+ *       the winding mode (DG_ERR_INVALID).
+ *   dg_mesh_winding_number[_device]: w[n] for points x[n x 3], host arrays or device pointers on `stream`.
+ * The winding records (the vertices per triangle in leaf order, 72 B, and a 256-byte cluster pair per internal node) are built on the host
+ * and uploaded at their first use; a mesh that never uses them allocates nothing more. */
+#define DG_SIGN_PSEUDONORMAL 0   /* the reference's rule; default */
+#define DG_SIGN_WINDING      1
+DG_API int dg_mesh_set_sign_mode(dg_mesh* mesh, int mode, double beta);
+DG_API int dg_mesh_winding_number(const dg_mesh* mesh, const double* x, uint64_t n, double beta, double* w);
+DG_API int dg_mesh_winding_number_device(const dg_mesh* mesh, const double* d_x, uint64_t n, double beta, double* d_w, void* stream);
+
 /* ---- K1: addFunction node loop with the GenerateSDF functor -------------------------------------------
  * replaces the hot loop cubic_lagrange_discrete_grid.cpp:806-817 with
  * func = sign * md.signed_distance(x).distance (cmd/generate_sdf/main.cpp:97,101; sign = -1 for --invert):
