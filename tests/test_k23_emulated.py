@@ -103,13 +103,20 @@ def test_interpolate_fuzz_against_reference_class():
     """a short run of tools/k2_fuzz.py: random anisotropic grids and fields (DBL_MAX sentinels, reduced fields, +-1e308 / -DBL_MAX / NaN /
     +-inf / subnormal / -0.0 coefficients, no kept cell or one), queries on cell faces / max faces / domain corners / outside / non-finite and
     runs of live lanes between dead ones, prefix counts around the warp and block sizes -- emulated interpolate kernel == the reference class
-    (the oracle where oracle/_ref is not built), value, gradient and value-only, bit for bit"""
+    (the oracle where oracle/_ref is not built), value, gradient and value-only, bit for bit.  Then the same fields and queries in K2's
+    Hessian mode (build/bin/libk2hemu.so): phi and grad the gradient mode's bits, hess the restatement's (tests/hessian_ref.py), exactly
+    symmetric, +0.0 at DBL_MAX"""
     import subprocess
     import sys
     if not os.path.exists(LIBS[0]):
         pytest.skip("needs build/bin/libk23emu.so")
     r = subprocess.run([sys.executable, os.path.join(ROOT, "tools", "k2_fuzz.py"), "24", "5"], capture_output=True, text=True, timeout=900)
     assert r.returncode == 0 and "0 mismatches" in r.stdout, r.stdout[-2000:] + r.stderr[-2000:]
+    hemu = os.path.join(ROOT, "build", "bin", "libk2hemu.so")
+    if os.path.exists(hemu):
+        r = subprocess.run([sys.executable, os.path.join(ROOT, "tools", "k2_fuzz.py"), "36", "5", hemu, "hessian"], capture_output=True, text=True,
+                           timeout=900)
+        assert r.returncode == 0 and "36 fields" in r.stdout and " 0 mismatches" in r.stdout, r.stdout[-2000:] + r.stderr[-2000:]
 
 
 def test_density_map_fuzz_against_oracle(emu):

@@ -325,3 +325,159 @@ def test_refusals(emu):
         emu.lib.dg_mesh_group_destroy(grp)
     emu.lib.dg_mesh_destroy(h)
     emu.lib.dg_mesh_destroy(h2)
+
+
+# ---------------------------------------------------------------------------------------------------------------- tools/k5_fuzz.py, short runs
+def _k5_fuzz():
+    import sys
+    sys.path.insert(0, os.path.join(ROOT, "tools"))
+    import k5_fuzz
+    return k5_fuzz
+
+
+def test_k5_fuzz_short_run(k5):
+    """a short run of tools/k5_fuzz.py on the emulated K5: tree sizes around powers of two, tie-rich meshes (w exactly 1/2, 1/4, 1/8) and a
+    zero-area subtree, scales 10^-300 .. 10^300, NaN / inf vertices and queries, every branch of k5_atan2, beta = 1, 2, 3.5, inf and
+    prefix counts around the warp and block sizes -- bit for bit with the restatement"""
+    f = _k5_fuzz()
+    be = f.EmuK5(K5EMU)
+    msgs = []
+    sizes = [1, 2, 3, 7, 8, 9, 63, 64, 65, 255, 256, 257]
+    runs = [f.run_cases(be, f.tree_cases(0, sizes), betas=(2.0, math.inf), counts=f.COUNTS, log=msgs.append, max_points=40),
+            f.run_cases(be, f.tie_cases(14, 3), log=msgs.append, max_points=120),
+            f.run_cases(be, f.scale_cases(0, (-300, -150, -24, -6, 0, 9, 17, 150, 300)), betas=(2.0, math.inf), log=msgs.append, max_points=60),
+            f.run_cases(be, f.nonfinite_cases(), betas=f.BETAS, counts=(33, 129), log=msgs.append),
+            f.run_cases(be, f.atan2_cases(), betas=(2.0, math.inf), log=msgs.append)]
+    assert sum(r[2] for r in runs) == 0, "\n".join(msgs[:10])
+    assert sum(r[0] for r in runs) > 150 and sum(r[1] for r in runs) > 50000
+
+
+def test_k5_fuzz_atan2_cases_take_every_branch():
+    """the one-triangle cases reach every branch of k5_atan2, and |det/den| lands exactly one ulp below and at or one ulp above each of
+    7/16, 11/16, 19/16, 39/16 with den of either sign"""
+    f = _k5_fuzz()
+    seen = f.atan2_coverage(f.atan2_cases())
+    assert f.ATAN2_BRANCHES <= seen
+    assert all(f"{t}+-ulp,{s}" in seen for t in f.ATAN2_BOUNDS for s in ("den>0", "den<0"))
+
+
+def test_zero_area_case_has_a_zero_area_subtree(k5):
+    f = _k5_fuzz()
+    V, F, _ = f.zero_area_case(np.random.default_rng(0))
+    e = EmuWinding(k5, V, F)
+    assert f.has_zero_area_subtree(V, F, e.order.astype(np.int64))
+
+
+def test_stack_canary_fails_a_launch_one_entry_short(k5):
+    """a perfect tree (T = 2^k) is walked with exactly stack_depth deferred entries: with one entry less the walk writes past the launch's
+    shared memory, which the emulation's canary turns into a failed launch; with the tree's own depth the same launch succeeds"""
+    f = _k5_fuzz()
+    k5.emu_winding_number_with_depth.argtypes = [VP, DP, C.c_uint64, C.c_double, C.c_int, DP]
+    k5.emu_winding_stack_depth.argtypes = [VP]
+    for T in (8, 64, 1024):
+        V, F = f.soup(np.random.default_rng(T), T)
+        e = EmuWinding(k5, V, F)
+        depth = k5.emu_winding_stack_depth(e.h)
+        assert depth == int(math.log2(T))
+        p = wr.query_points(V, 40, seed=1)
+        w = np.empty(len(p))
+        assert k5.emu_winding_number_with_depth(e.h, P(p), len(p), math.inf, depth, P(w)) == 0
+        assert bits_equal(w, wr.exact_w(e.leaves, p))
+        assert k5.emu_winding_number_with_depth(e.h, P(p), len(p), math.inf, depth - 1, P(w)) != 0
+
+
+def test_records_and_w_with_an_infinite_vertex(k5):
+    """regression: with an infinite vertex a subtree's p~ is +-inf, so every |v - p~|^2 is inf or NaN; r_c is the max over the others (the
+    fold from 0 skips NaN), here inf -- the restatement took np.max (NaN), then max(0.0, NaN) = 0 and made such clusters far"""
+    f = _k5_fuzz()
+    case = next(c for c in f.nonfinite_cases() if c[0] == "awkward 9 x1 vertex inf")
+    _, V, F, x = case
+    e = EmuWinding(k5, V, F)
+    rec = wr.Records(V, F, e.order)
+    assert bits_equal(e.clusters, rec.as_array())
+    assert np.isinf(e.clusters[..., 15]).any()
+    for beta in f.BETAS:
+        assert f.same(e.w(x, beta), rec.w(x, beta)).all(), beta
+
+
+# ---------------------------------------------------------------------------------------------------------------- accuracy of the exact sum
+U = 2.0 ** -53
+
+
+def exact_sum_bound(tris, p):
+    """first-order bound on |w - w*| for the exact sum (beta = inf) at points p, from the operation count of the contract; w* is the sum of
+    the exact solid angles of the same fp64 inputs.  Per term, with a, b, c = v - x (relative error u each) and first-order error terms:
+      det = (ax kx + ay ky) + az kz:  |d det| <= 8u Pdet,  Pdet = sum of |a_i b_j c_k| over the six products of the cross and dot products
+      den = ((|a||b||c| + (a.b)|c|) + (b.c)|a|) + (c.a)|b|:  |d den| <= 16u Pden,  Pden = |a||b||c| + P_ab |c| + P_bc |a| + P_ca |b|,
+          P_ab = sum |a_i b_i| (|u| carries 3.5u, a.b 5u, each product u, the three additions 3u, 2u, u)
+      theta = atan2(det, den):  |d theta| <= (|d det| |den| + |d den| |det|) / (det^2 + den^2) + 4u |theta|  (k5_atan2: 2 ulp)
+      Omega = 2 theta exactly.
+    The fold adds u |S_k| per addition (k = 2 .. T), the division by FOUR_PI (4 pi (1 + d), |d| <= u) 2u |w|.  So
+      |w - w*| <= u [ sum_t 2 (kappa_t + 4 |theta_t|) + sum_k |S_k| ] / 4 pi + 2u |w|,   kappa_t = (8 Pdet |den| + 16 Pden |det|) / (det^2 + den^2)
+    -> (w, bound, kappa (n, T), partial sums (n, T))"""
+    v = tris[None, :, :]
+    a = [v[..., i] - p[:, i:i + 1] for i in range(3)]
+    b = [v[..., 3 + i] - p[:, i:i + 1] for i in range(3)]
+    c = [v[..., 6 + i] - p[:, i:i + 1] for i in range(3)]
+    A = lambda x: np.abs(x)
+    pdet = (A(a[0]) * (A(b[1] * c[2]) + A(b[2] * c[1])) + A(a[1]) * (A(b[2] * c[0]) + A(b[0] * c[2])) + A(a[2]) * (A(b[0] * c[1]) + A(b[1] * c[0])))
+    n = lambda x: np.sqrt(x[0] * x[0] + x[1] * x[1] + x[2] * x[2])
+    la, lb, lc = n(a), n(b), n(c)
+    pab = sum(A(a[i] * b[i]) for i in range(3)); pbc = sum(A(b[i] * c[i]) for i in range(3)); pca = sum(A(c[i] * a[i]) for i in range(3))
+    pden = la * lb * lc + pab * lc + pbc * la + pca * lb
+    det, den = wr.det_den(tris, p)
+    kappa = (8.0 * pdet * np.abs(den) + 16.0 * pden * np.abs(det)) / (det * det + den * den)
+    theta = wr.atan2(det, den)
+    partial = np.cumsum(2.0 * theta, axis=1)
+    w = wr.exact_w(tris, p)
+    bound = U * ((2.0 * (kappa + 4.0 * np.abs(theta))).sum(1) + np.abs(partial[:, 1:]).sum(1)) / (4 * math.pi) + 2.0 * U * np.abs(w)
+    return w, bound, kappa, partial
+
+
+def exact_w_mp(tris, p, dps=40):
+    """sum over the triangles of 2 atan2(det, den) / 4 pi at `dps` digits, from the same fp64 vertices and points"""
+    import mpmath as mp
+    mp.mp.dps = dps
+    out = []
+    T = [[[mp.mpf(float(t[3 * k + d])) for d in range(3)] for k in range(3)] for t in tris]
+    for x in p:
+        X = [mp.mpf(float(v)) for v in x]
+        S = []
+        for v0, v1, v2 in T:
+            a = [v0[d] - X[d] for d in range(3)]; b = [v1[d] - X[d] for d in range(3)]; c = [v2[d] - X[d] for d in range(3)]
+            la, lb, lc = (mp.sqrt(u[0] ** 2 + u[1] ** 2 + u[2] ** 2) for u in (a, b, c))
+            det = a[0] * (b[1] * c[2] - b[2] * c[1]) + a[1] * (b[2] * c[0] - b[0] * c[2]) + a[2] * (b[0] * c[1] - b[1] * c[0])
+            dot = lambda u, q: u[0] * q[0] + u[1] * q[1] + u[2] * q[2]
+            den = la * lb * lc + dot(a, b) * lc + dot(b, c) * la + dot(c, a) * lb
+            S.append(2 * mp.atan2(det, den))
+        out.append(mp.fsum(S) / (4 * mp.pi))
+    return out
+
+
+ACCURACY_MESHES = [("box", 200), ("torus", 12), ("open_torus", 12), ("soup", 200), ("open_bunny_200", 60)]
+
+
+@pytest.mark.parametrize("name,n_points", ACCURACY_MESHES)
+def test_exact_sum_accuracy_against_mpmath(k5, orc, name, n_points):
+    """the exact sum (beta = inf; the device returns these bits, see test_gpu_winding.py) against 2 atan2(det, den) / 4 pi summed at 40
+    digits from the same fp64 inputs, at points at least 1e-3 of the mesh extent from the surface: within exact_sum_bound, whose
+    coefficients come from the operation count, not from this data"""
+    pytest.importorskip("mpmath")
+    if name == "open_bunny_200":
+        V, F = mesh("open_bunny_small")
+        F = np.ascontiguousarray(F[:200])
+    else:
+        V, F = mesh(name)
+    e = EmuWinding(k5, V, F)
+    ext = float(np.linalg.norm(V.max(0) - V.min(0)))
+    p = wr.query_points(V, 6 * n_points, seed=17, near=2 * n_points)
+    d = orc.mesh(V, F).distance(p, signed=False)[0]
+    p = np.ascontiguousarray(p[d >= 1e-3 * ext][:n_points])
+    assert len(p) >= n_points // 2
+    w, bound, _kappa, _ = exact_sum_bound(e.leaves, p)
+    assert bits_equal(e.w(p, math.inf), w)
+    ref = exact_w_mp(e.leaves, p)
+    err = np.array([abs(float(r - wi)) for r, wi in zip(ref, w.tolist())])
+    assert (err <= bound).all(), (float((err / bound).max()), float(err.max()))
+    print(f"{name}: T = {len(F)}, {len(p)} points, max |w - w*| = {err.max():.3g} = {err.max() / U:.1f} u, "
+          f"max bound {bound.max() / U:.0f} u, max err / bound = {(err / bound).max():.3g}")

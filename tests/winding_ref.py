@@ -58,18 +58,25 @@ def atan2(y, x):
     return out
 
 
-def solid_angles(tris, p):
-    """exact terms: tris (T, 9) [v0 v1 v2], p (n, 3) -> (n, T)"""
+def det_den(tris, p):
+    """the two arguments of the exact term's atan2: tris (T, 9) [v0 v1 v2], p (n, 3) -> det (n, T), den (n, T)"""
     v = tris[None, :, :]
     px, py, pz = p[:, 0:1], p[:, 1:2], p[:, 2:3]
-    ax, ay, az = v[..., 0] - px, v[..., 1] - py, v[..., 2] - pz
-    bx, by, bz = v[..., 3] - px, v[..., 4] - py, v[..., 5] - pz
-    cx, cy, cz = v[..., 6] - px, v[..., 7] - py, v[..., 8] - pz
-    la = np.sqrt(ax * ax + ay * ay + az * az); lb = np.sqrt(bx * bx + by * by + bz * bz); lc = np.sqrt(cx * cx + cy * cy + cz * cz)
-    kx, ky, kz = by * cz - bz * cy, bz * cx - bx * cz, bx * cy - by * cx
-    det = ax * kx + ay * ky + az * kz
-    ab = ax * bx + ay * by + az * bz; bc = bx * cx + by * cy + bz * cz; ca = cx * ax + cy * ay + cz * az
-    den = la * lb * lc + ab * lc + bc * la + ca * lb
+    with np.errstate(all="ignore"):
+        ax, ay, az = v[..., 0] - px, v[..., 1] - py, v[..., 2] - pz
+        bx, by, bz = v[..., 3] - px, v[..., 4] - py, v[..., 5] - pz
+        cx, cy, cz = v[..., 6] - px, v[..., 7] - py, v[..., 8] - pz
+        la = np.sqrt(ax * ax + ay * ay + az * az); lb = np.sqrt(bx * bx + by * by + bz * bz); lc = np.sqrt(cx * cx + cy * cy + cz * cz)
+        kx, ky, kz = by * cz - bz * cy, bz * cx - bx * cz, bx * cy - by * cx
+        det = ax * kx + ay * ky + az * kz
+        ab = ax * bx + ay * by + az * bz; bc = bx * cx + by * cy + bz * cz; ca = cx * ax + cy * ay + cz * az
+        den = la * lb * lc + ab * lc + bc * la + ca * lb
+    return det, den
+
+
+def solid_angles(tris, p):
+    """exact terms: tris (T, 9) [v0 v1 v2], p (n, 3) -> (n, T)"""
+    det, den = det_den(tris, p)
     return 2.0 * atan2(det, den)
 
 
@@ -112,8 +119,12 @@ class Records:
         s["M"] = [(L["M"][3 * j + k] + (L["p"][j] - s["p"][j]) * L["N"][k]) + (R["M"][3 * j + k] + (R["p"][j] - s["p"][j]) * R["N"][k])
                   for j in range(3) for k in range(3)]
         vv = self.leaves[b:e].reshape(-1, 3)
-        d = vv - np.array(s["p"])
-        r2 = max(0.0, float(np.max(d[:, 0] * d[:, 0] + d[:, 1] * d[:, 1] + d[:, 2] * d[:, 2])))
+        with np.errstate(all="ignore"):
+            d = vv - np.array(s["p"])
+            d2 = d[:, 0] * d[:, 0] + d[:, 1] * d[:, 1] + d[:, 2] * d[:, 2]
+        # the max is the fold r2 = (r2 < d2) ? d2 : r2 from 0.0: a NaN d2 compares false and is skipped (np.fmax), where np.max would
+        # return NaN.  Matters for meshes with non-finite vertices: p~ = +-inf gives r_c = inf, not 0
+        r2 = float(np.fmax.reduce(d2, initial=0.0))
         self.clusters[idx][side] = (s["p"], s["N"], s["M"], math.sqrt(r2))
         return s
 

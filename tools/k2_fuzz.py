@@ -6,10 +6,14 @@ kept cell or exactly one.  Queries sit on cell faces, the max faces (the cell-in
 runs of 1, 2 and 3 live lanes between runs of lanes that issue no real copy (out of domain, NaN, removed cell, missing coefficient), at
 counts around the warp and block sizes.  Value + gradient and value-only, bit for bit (any NaN equal to any NaN).
 
-usage: tools/k2_fuzz.py [rounds=60] [seed=0] [lib=build/bin/libk23emu.so]
-  lib  a build of tests/emu (libk23emu*.so: the K2 translation unit compiled for the CPU, its TMA staging a plain copy), or `dg`: the
-       product library through its C-ABI (dg_field_create, dg_interpolate_batch), i.e. the CUDA kernels -- needs a GPU
-The functions are shared with tests/test_k23_emulated.py and tests/test_gpu_k23_fuzz.py."""
+usage: tools/k2_fuzz.py [rounds=60] [seed=0] [lib=build/bin/libk23emu.so] [gradient|hessian]
+  lib      a build of tests/emu (libk23emu*.so: the K2 translation unit compiled for the CPU, its TMA staging a plain copy), or `dg`: the
+           product library through its C-ABI (dg_field_create, dg_interpolate_batch), i.e. the CUDA kernels -- needs a GPU
+  hessian  K2's Hessian mode (interpolate_kernel<true, true>; build/bin/libk2hemu.so or `dg`: dg_interpolate_hessian_batch) on the same
+           fields and queries: phi and grad are the gradient mode's bits, hess the bits of the numpy restatement of its contract
+           (tests/hessian_ref.py), exactly symmetric, and +0.0 in all nine entries wherever phi is DBL_MAX
+The functions are shared with tests/test_k23_emulated.py, tests/test_k2_hessian_emulated.py, tests/test_gpu_k23_fuzz.py and
+tests/test_gpu_winding_hessian_fuzz.py."""
 import ctypes as C
 import os
 import sys
@@ -76,6 +80,8 @@ class EmuK2:
         lib.emu_field_destroy.argtypes = [C.c_void_p]
         lib.emu_interpolate.argtypes = [C.c_void_p, dp, C.c_uint64, dp, dp]
         lib.emu_density_map.argtypes = [C.c_void_p, C.c_double, C.c_double, C.c_int, C.c_uint64, C.c_uint64, dp]
+        if hasattr(lib, "emu_interpolate_hessian"):
+            lib.emu_interpolate_hessian.argtypes = [C.c_void_p, dp, C.c_uint64, dp, dp, dp]
 
     def field(self, gd, r, nodes, cells, cmap):
         keep = (gd, r, np.ascontiguousarray(nodes, np.float64), np.ascontiguousarray(cells, np.uint32), np.ascontiguousarray(cmap, np.uint32))
@@ -91,6 +97,12 @@ class EmuK2:
         phi = np.full(n, -1.0); g = np.full((n, 3), -1.0) if grad else None
         assert self.lib.emu_interpolate(f[0], _p(x, dp), n, _p(phi, dp), _p(g, dp)) == 0
         return phi, g
+
+    def hessian(self, f, x):
+        n = len(x)
+        phi, g, h = np.full(n, -1.0), np.full((n, 3), -1.0), np.full((n, 3, 3), -1.0)
+        assert self.lib.emu_interpolate_hessian(f[0], _p(x, dp), n, _p(phi, dp), _p(g, dp), _p(h, dp)) == 0
+        return phi, g, h
 
     def density(self, f, h, rho0, no_reduction, l0, l1):
         out = np.full(l1 - l0, -1.0)
@@ -124,6 +136,12 @@ class DgK2:
         phi = np.full(n, -1.0); g = np.full((n, 3), -1.0) if grad else None
         self.capi.check(self.lib.dg_interpolate_batch(f[0], _p(x, dp), n, _p(phi, dp), _p(g, dp)))
         return phi, g
+
+    def hessian(self, f, x):
+        n = len(x)
+        phi, g, h = np.full(n, -1.0), np.full((n, 3), -1.0), np.full((n, 3, 3), -1.0)
+        self.capi.check(self.lib.dg_interpolate_hessian_batch(f[0], _p(x, dp), n, _p(phi, dp), _p(g, dp), _p(h, dp)))
+        return phi, g, h
 
     def density(self, f, h, rho0, no_reduction, l0, l1):
         out = np.full(l1 - l0, -1.0)
@@ -252,8 +270,50 @@ def queries(rng, gd, r, nodes, cells, cmap):
     return np.ascontiguousarray(np.concatenate(xs), np.float64)
 
 
-def check_field(be, ref, f, gd, r, nodes, cells, cmap, x, label, counts=COUNTS):
-    """value + gradient and value-only at the full count and at the prefix counts -> (queries checked, mismatches, first mismatch)"""
+def restate(gd, r, nodes, cells, cmap, x, chunk=1 << 20):
+    """tests/hessian_ref.py's restatement of the Hessian on a k2_fuzz field, in chunks of queries"""
+    from hessian_ref import restate_hessian        # only the Hessian mode needs it: importing k2_fuzz does not
+    return np.concatenate([restate_hessian(gd[0:3], gd[3:6], gd[6:9], gd[9:12], r, nodes, cells, cmap, x[i:i + chunk])
+                           for i in range(0, len(x), chunk)] or [np.zeros((0, 3, 3))])
+
+
+def hessian_ok(phi, grad, hess, phi_g, grad_g, want_hess):
+    """per query: the Hessian mode's phi and grad are the gradient mode's bits, hess the restatement's (any NaN equal to any NaN), exactly
+    symmetric (the same bits at [a][b] and [b][a], NaN payloads included), and +0.0 in all nine entries where phi is DBL_MAX"""
+    hb = hess.reshape(-1, 3, 3).view(np.uint64)
+    sym = (hb == hb.transpose(0, 2, 1)).all((1, 2))
+    zero = ~(phi == DBL_MAX) | ~hb.any((1, 2))
+    return same(phi, phi_g) & same(grad, grad_g).all(1) & same(hess, want_hess).all((1, 2)) & sym & zero
+
+
+def check_hessian(be, f, gd, r, nodes, cells, cmap, x, label, counts=COUNTS):
+    """the Hessian mode at the full count and at the prefix counts -> (queries checked, mismatches, first mismatch)"""
+    phi_g, grad_g = be.interpolate(f, x, True)
+    want = restate(gd, r, nodes, cells, cmap, x)
+    phi, grad, hess = be.hessian(f, x)
+    ok = hessian_ok(phi, grad, hess, phi_g, grad_g, want)
+    total, bad, first = len(x), int((~ok).sum()), None
+    if bad:
+        i = int(np.nonzero(~ok)[0][0])
+        first = (f"MISMATCH {label} hessian x={x[i]!r}: phi {phi[i]!r} vs {phi_g[i]!r}, grad {grad[i]} vs {grad_g[i]}, "
+                 f"hess {hess[i].tolist()} vs {want[i].tolist()}")
+    for c in counts:
+        if c > len(x):
+            continue
+        p, g, h = be.hessian(f, x[:c])
+        okc = same(p, phi[:c]) & same(g, grad[:c]).all(1) & same(h, hess[:c]).all((1, 2))
+        total += c
+        if not okc.all():
+            bad += int((~okc).sum())
+            first = first or f"MISMATCH {label} hessian count {c}: first bad query {int(np.nonzero(~okc)[0][0])}"
+    return total, bad, first
+
+
+def check_field(be, ref, f, gd, r, nodes, cells, cmap, x, label, counts=COUNTS, mode="gradient"):
+    """value + gradient and value-only at the full count and at the prefix counts -> (queries checked, mismatches, first mismatch);
+    mode "hessian": check_hessian"""
+    if mode == "hessian":
+        return check_hessian(be, f, gd, r, nodes, cells, cmap, x, label, counts)
     want_phi, want_grad = ref.interpolate(gd, r, nodes, cells, cmap, x, True)
     want_only = ref.interpolate(gd, r, nodes, cells, cmap, x, False)[0]
     phi, grad = be.interpolate(f, x, True)
@@ -276,20 +336,20 @@ def check_field(be, ref, f, gd, r, nodes, cells, cmap, x, label, counts=COUNTS):
     return total, bad, first
 
 
-def run(be, rounds, seed, log=print):
-    """-> (fields, queries checked, mismatches)"""
+def run(be, rounds, seed, log=print, mode="gradient"):
+    """-> (fields, queries checked, mismatches); mode: "gradient" (value + gradient and value-only against the reference) or "hessian" """
     rng = np.random.default_rng(seed)
     orc = Oracle()
     tmp = tempfile.mkdtemp(prefix="k2_fuzz_")
     ref = Reference(tmp)
-    log(f"backend {be.name}, reference: {ref.name}")
+    log(f"backend {be.name}, {mode} mode, reference: {ref.name if mode == 'gradient' else 'tests/hessian_ref.py'}")
     total = bad = 0
     for k in range(rounds):
         gd, r, nodes, cells, cmap, label = make_field(orc, rng, k, tmp)
         x = queries(rng, gd, r, nodes, cells, cmap)
         f = be.field(gd, r, nodes, cells, cmap)
         try:
-            n, b, msg = check_field(be, ref, f, gd, r, nodes, cells, cmap, x, label)
+            n, b, msg = check_field(be, ref, f, gd, r, nodes, cells, cmap, x, label, mode=mode)
         finally:
             be.destroy(f)
         total += n; bad += b
@@ -297,7 +357,7 @@ def run(be, rounds, seed, log=print):
     return rounds, total, bad
 
 
-def run_many(be, n_queries=4 << 20, seed=0, log=print):
+def run_many(be, n_queries=4 << 20, seed=0, log=print, mode="gradient"):
     """one field of every kind of lane and n_queries queries in one call (many warps with copies in flight) -> (queries, mismatches)"""
     rng = np.random.default_rng(seed)
     orc = Oracle()
@@ -311,6 +371,18 @@ def run_many(be, n_queries=4 << 20, seed=0, log=print):
     base = queries(rng, gd, r, nodes, cells, cmap)
     x = np.ascontiguousarray(base[rng.integers(len(base), size=n_queries)] + np.where(rng.random((n_queries, 1)) < 0.5, 0.0,
                                                                                       1e-3 * rng.standard_normal((n_queries, 3))))
+    if mode == "hessian":
+        f = be.field(gd, r, nodes, cells, cmap)
+        try:
+            phi_g, grad_g = be.interpolate(f, x, True)
+            phi, grad, hess = be.hessian(f, x)
+        finally:
+            be.destroy(f)
+        ok = hessian_ok(phi, grad, hess, phi_g, grad_g, restate(gd, r, nodes, cells, cmap, x))
+        if not ok.all():
+            i = int(np.nonzero(~ok)[0][0])
+            log(f"MISMATCH {n_queries} queries, hessian: query {i} x={x[i]!r}: hess {hess[i].tolist()}")
+        return n_queries, int((~ok).sum())
     want_phi, want_grad = ref.interpolate(gd, r, nodes, cells, cmap, x, True)
     want_only = ref.interpolate(gd, r, nodes, cells, cmap, x, False)[0]
     f = be.field(gd, r, nodes, cells, cmap)
@@ -329,8 +401,9 @@ def run_many(be, n_queries=4 << 20, seed=0, log=print):
 def main(argv):
     rounds = int(argv[1]) if len(argv) > 1 else 60
     seed = int(argv[2]) if len(argv) > 2 else 0
-    lib = argv[3] if len(argv) > 3 else os.path.join(ROOT, "build", "bin", "libk23emu.so")
-    fields, total, bad = run(backend(lib), rounds, seed)
+    mode = argv[4] if len(argv) > 4 else "gradient"
+    lib = argv[3] if len(argv) > 3 else os.path.join(ROOT, "build", "bin", "libk2hemu.so" if mode == "hessian" else "libk23emu.so")
+    fields, total, bad = run(backend(lib), rounds, seed, mode=mode)
     print(f"{fields} fields, {total} queries, {bad} mismatches")
     return 1 if bad else 0
 
