@@ -15,6 +15,7 @@
 //                                            -> dg_reduced_function_create (both calls in one, the dense field kept on the GPU)
 //   interpolate(field, x, grad*)             -> dg_interpolate_batch (K2), also batched: interpolate(field, n, x, phi, grad)
 //   interpolate(field, n, x, phi, grad, hess) -> dg_interpolate_hessian_batch (K2's Hessian mode; not in the reference)
+//   isosurface(field, iso, subdivisions)     -> dg_isosurface_create (K6: the level set as a TriangleMesh; not in the reference)
 //   connectivity table of addFunction        -> dg_build_cells  (GPU)  replaces the serial loop :833-886
 //
 // m_nodes / m_cells / m_cell_map hold exactly what the reference would have produced, so save()/load() stay
@@ -352,6 +353,21 @@ public:
     void interpolate(unsigned int field_id, std::size_t n, const double* x, double* phi, double* grad, double* hess) const
     {
         check(dg_interpolate_hessian_batch(deviceField(field_id), x, n, phi, grad, hess));
+    }
+    // the level set {phi = iso} of a field by marching tetrahedra on a lattice that subdivides every cell `subdivisions` times (new, beyond
+    // the reference; contract in k6_isosurface.cu): outward-oriented triangles for an SDF, coincident vertices not welded
+    TriangleMesh isosurface(unsigned int field_id, double iso = 0.0, unsigned int subdivisions = 1) const
+    {
+        dg_isosurface* s = nullptr;
+        check(dg_isosurface_create(deviceField(field_id), iso, subdivisions, &s, nullptr));
+        std::uint64_t nv = 0, nt = 0;
+        dg_isosurface_sizes(s, &nv, &nt);
+        std::vector<double> v(3 * nv);
+        std::vector<std::uint32_t> t(3 * nt);
+        const int rc = dg_isosurface_copy(s, v.data(), t.data());
+        dg_isosurface_destroy(s);
+        check(rc);
+        return TriangleMesh(v.data(), t.data(), (std::size_t)nv, (std::size_t)nt);
     }
 
     // ---- split API (:901-975): shape functions on the GPU (dg_shape_functions), index algebra on the host

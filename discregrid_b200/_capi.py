@@ -113,6 +113,11 @@ SIGNATURES = {
     "dg_reduced_band_copy": (C.c_int, [_vp, _dp, _u32p, _u32p]),
     "dg_reduced_band_destroy": (C.c_int, [_vp]),
     "dg_field_create_reduced": (C.c_int, [_vp, C.POINTER(_vp)]),
+    "dg_isosurface_create": (C.c_int, [_vp, C.c_double, C.c_uint32, C.POINTER(_vp), _dp]),
+    "dg_isosurface_sizes": (C.c_int, [_vp, _u64p, _u64p]),
+    "dg_isosurface_copy": (C.c_int, [_vp, _dp, _u32p]),
+    "dg_isosurface_copy_device": (C.c_int, [_vp, _vp, _vp, _vp]),
+    "dg_isosurface_destroy": (C.c_int, [_vp]),
     "dg_reduced_density_map_create": (C.c_int, [_gp, _dp, C.c_uint64, _u32p, C.c_uint64, _u32p, C.c_double, C.c_double, C.c_uint32,
                                                  C.POINTER(_vp), C.POINTER(_vp), _dp]),
     "dg_add_function_device": (C.c_int, [_gp, DEVICE_FUNCTION, _vp, DEVICE_SAMPLE_PREDICATE, _vp, C.c_uint64, _dp, _u32p, _u32p, _dp]),

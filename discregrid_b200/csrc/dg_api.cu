@@ -40,6 +40,7 @@
 #include "k3_density.h"
 #include "k4_reduce.h"
 #include "k5_winding.h"
+#include "k6_isosurface.h"
 #include "reduce_field.h"
 #include "obj_reader.h"
 
@@ -2286,6 +2287,132 @@ int dg_field_create_reduced(const dg_reduced_band* h, dg_field** out)
     if (int rc = field_finish(f, h->d_nodes.p, h->d_cells.p, nullptr)) return rc;
     DG_CUDA(cudaDeviceSynchronize());
     *out = own.release();
+    return DG_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ K6: level sets (marching tetrahedra)
+// The mesh stays on the field's device in the handle until dg_isosurface_copy[_device].
+struct dg_isosurface {
+    DevBuf<double> d_vertices;
+    DevBuf<unsigned> d_triangles;
+    uint64_t n_vertices = 0, n_triangles = 0;
+    int device = 0;
+};
+
+// values, classify, scans, emit (k6_isosurface.cu); each stage ends with a synchronise.  Device memory: 8 B per lattice point of values,
+// 7 B per point of edge flags, 1 B per lattice cell of counts, 1/8 B per point of chunk ranks, the tile arrays, one chunk of positions
+// (24 B x min(Np, 2^24)), then 24 B per vertex and 12 B per triangle of output.
+static int isosurface_create_impl(const dg_field* f, double iso, uint32_t s, dg_isosurface** out, double* timings_ms)
+{
+    static const char* who = "dg_isosurface_create";
+    if (!out) return fail(DG_ERR_INVALID, "%s: out is NULL", who);
+    *out = nullptr;
+    if (!f) return fail(DG_ERR_INVALID, "%s: field is NULL", who);
+    if (!std::isfinite(iso)) return fail(DG_ERR_INVALID, "%s: iso must be finite (got %g)", who, iso);
+    if (s == 0 || s > K6_MAX_SUBDIVISIONS) return fail(DG_ERR_INVALID, "%s: subdivisions must be 1..%u (got %u)", who, K6_MAX_SUBDIVISIONS, s);
+    uint64_t np = 0;
+    const K6Lattice L = k6_lattice(f->dev.g, s, np);
+    if (np >= (1ull << 31))
+        return fail(DG_ERR_INVALID, "%s: the lattice of %llu points (%u x %u x %u) has 2^31 points or more; use fewer subdivisions", who,
+                    (unsigned long long)np, L.np[0], L.np[1], L.np[2]);
+    if (int rc = check_handle_device(f->device, who)) return rc;
+    const uint64_t n_cells = (uint64_t)(L.np[0] - 1) * (L.np[1] - 1) * (L.np[2] - 1);
+    const uint64_t n_edges = 7 * np, tile = k6_tile();
+    StageClock clock;
+    const auto t_start = clock.t0;
+    const cudaStream_t st = nullptr;
+    double ms[4] = {0, 0, 0, 0};
+    std::unique_ptr<dg_isosurface> h(new dg_isosurface());
+    h->device = f->device;
+    // ---- values: lattice positions per chunk, K2 value-only
+    DevBuf<double> d_values;
+    DG_CUDA(d_values.alloc(np));
+    {
+        DevBuf<double> d_x;
+        const uint64_t chunk = std::min<uint64_t>(np, K6_CHUNK);
+        DG_CUDA(d_x.alloc(3 * chunk));
+        for (uint64_t b = 0; b < np; b += chunk) {
+            const uint64_t n = std::min(chunk, np - b);
+            DG_LAUNCH(k6_launch_positions(L, b, n, d_x.p, st));
+            DG_LAUNCH(k2_launch_interpolate(f->dev, d_x.p, n, d_values.p + b, nullptr, st));
+        }
+        DG_CUDA(cudaStreamSynchronize(st));
+    }
+    ms[0] = clock.lap();
+    // ---- classify: triangle count per lattice cell, flags of the crossing edges (rounded up to whole 32-edge chunks, which emit reads)
+    DevBuf<unsigned char> d_count, d_flags;
+    DG_CUDA(d_count.alloc(n_cells));
+    DG_CUDA(d_flags.alloc((n_edges + 31) / 32 * 32));
+    DG_CUDA(cudaMemsetAsync(d_flags.p, 0, d_flags.bytes(), st));
+    DG_LAUNCH(k6_launch_classify(L, d_values.p, iso, d_count.p, d_flags.p, st));
+    DG_CUDA(cudaStreamSynchronize(st));
+    ms[1] = clock.lap();
+    // ---- scans: triangles per tile of cells, vertices per tile of edges; both totals must fit the uint32 indices of the output
+    DevBuf<unsigned> d_tri_tile, d_edge_tile;
+    DG_CUDA(d_tri_tile.alloc((n_cells + tile - 1) / tile));
+    DG_CUDA(d_edge_tile.alloc((n_edges + tile - 1) / tile));
+    uint64_t n_tri = 0, n_vert = 0;
+    DG_LAUNCH(k6_scan_counts(d_count.p, n_cells, d_tri_tile.p, n_tri, st));
+    DG_LAUNCH(k4_scan_flags(d_flags.p, n_edges, d_edge_tile.p, n_vert, st));
+    if (n_vert >= (1ull << 32)) return fail(DG_ERR_INVALID, "%s: %llu vertices do not fit uint32 indices; use fewer subdivisions", who, (unsigned long long)n_vert);
+    if (n_tri >= (1ull << 32)) return fail(DG_ERR_INVALID, "%s: %llu triangles do not fit uint32 counts; use fewer subdivisions", who, (unsigned long long)n_tri);
+    ms[2] = clock.lap();
+    // ---- emit: vertices at their ranks (and the rank of every 32-edge chunk), then the triangles
+    if (n_vert) {
+        DevBuf<unsigned> d_chunk;
+        DG_CUDA(d_chunk.alloc((n_edges + 31) / 32));
+        DG_CUDA(h->d_vertices.alloc(3 * n_vert));
+        DG_CUDA(h->d_triangles.alloc(3 * n_tri));
+        DG_LAUNCH(k6_launch_vertices(L, d_values.p, iso, d_flags.p, n_edges, d_edge_tile.p, d_chunk.p, h->d_vertices.p, st));
+        DG_LAUNCH(k6_launch_triangles(L, d_values.p, iso, d_count.p, d_tri_tile.p, d_flags.p, d_chunk.p, h->d_triangles.p, st));
+        DG_CUDA(cudaStreamSynchronize(st));
+    }
+    h->n_vertices = n_vert; h->n_triangles = n_tri;
+    ms[3] = clock.lap();
+    if (timings_ms) {
+        for (int k = 0; k < 4; k++) timings_ms[k] = ms[k];
+        timings_ms[4] = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_start).count();
+    }
+    *out = h.release();
+    return DG_OK;
+}
+
+int dg_isosurface_create(const dg_field* field, double iso, uint32_t subdivisions, dg_isosurface** out, double* timings_ms)
+{
+    return guarded("dg_isosurface_create", [&]() { return isosurface_create_impl(field, iso, subdivisions, out, timings_ms); });
+}
+
+int dg_isosurface_sizes(const dg_isosurface* s, uint64_t* n_vertices, uint64_t* n_triangles)
+{
+    if (!s || !n_vertices || !n_triangles) return fail(DG_ERR_INVALID, "dg_isosurface_sizes: NULL argument");
+    *n_vertices = s->n_vertices; *n_triangles = s->n_triangles;
+    return DG_OK;
+}
+
+int dg_isosurface_copy(const dg_isosurface* s, double* vertices, uint32_t* triangles)
+{
+    if (!s) return fail(DG_ERR_INVALID, "dg_isosurface_copy: handle is NULL");
+    if ((!vertices && s->n_vertices) || (!triangles && s->n_triangles)) return fail(DG_ERR_INVALID, "dg_isosurface_copy: NULL output");
+    if (int rc = check_handle_device(s->device, "dg_isosurface_copy")) return rc;
+    if (s->n_vertices) DG_CUDA(cudaMemcpy(vertices, s->d_vertices.p, 3 * s->n_vertices * sizeof(double), cudaMemcpyDeviceToHost));
+    if (s->n_triangles) DG_CUDA(cudaMemcpy(triangles, s->d_triangles.p, 3 * s->n_triangles * sizeof(unsigned), cudaMemcpyDeviceToHost));
+    return DG_OK;
+}
+
+int dg_isosurface_copy_device(const dg_isosurface* s, double* d_vertices, uint32_t* d_triangles, void* stream)
+{
+    if (!s) return fail(DG_ERR_INVALID, "dg_isosurface_copy_device: handle is NULL");
+    if ((!d_vertices && s->n_vertices) || (!d_triangles && s->n_triangles)) return fail(DG_ERR_INVALID, "dg_isosurface_copy_device: NULL output");
+    if (int rc = check_handle_device(s->device, "dg_isosurface_copy_device")) return rc;
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (s->n_vertices) DG_CUDA(cudaMemcpyAsync(d_vertices, s->d_vertices.p, 3 * s->n_vertices * sizeof(double), cudaMemcpyDeviceToDevice, st));
+    if (s->n_triangles) DG_CUDA(cudaMemcpyAsync(d_triangles, s->d_triangles.p, 3 * s->n_triangles * sizeof(unsigned), cudaMemcpyDeviceToDevice, st));
+    return DG_OK;
+}
+
+int dg_isosurface_destroy(dg_isosurface* s)
+{
+    delete s;
     return DG_OK;
 }
 

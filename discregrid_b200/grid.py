@@ -636,6 +636,45 @@ class CubicLagrangeDiscreteGrid:
             return _interpolate_hessian_function().apply(x, run)
         return run(x)
 
+    # ------------------------------------------------------------------ level sets (beyond the reference)
+    def isosurface(self, field_id=0, iso=0.0, subdivisions=1, device=False):
+        """The level set {phi = iso} of a field as a triangle mesh: marching tetrahedra on a lattice that subdivides every grid cell
+        `subdivisions` times (1..16), on the field's GPU (dg_isosurface_create; the contract is in csrc/k6_isosurface.cu and DESIGN §3).
+        The lattice values are the bits interpolate() returns there; points where it returns DBL_MAX or a non-finite value (outside the
+        domain, removed cells of a reduced field) are invalid, and tetrahedra touching them emit nothing.  Triangles are oriented from the
+        negative to the non-negative side (outward for an SDF); coincident vertices are not welded, so the mesh is closed by vertex ids.
+        Returns (vertices float64 (n, 3), triangles uint32 (m, 3)) as numpy arrays -- the layout TriangleMeshDistance takes.  With
+        device=True they are CUDA tensors on the field's device, filled on torch's current stream, with triangles as torch.int32 (same
+        values; 2^31 vertices or more are refused on this route).  A reduced field's kept device handle is used without a host round trip.
+        Stage times (values, classify, scans, emit, total; ms) are left in last_isosurface_ms."""
+        h = self._device_field(field_id)
+        s = C.c_void_p()
+        self.last_isosurface_ms = np.zeros(5)
+        capi.check(capi.lib.dg_isosurface_create(h, float(iso), int(subdivisions), C.byref(s), capi.ptr(self.last_isosurface_ms, capi.F64P)))
+        try:
+            nv, nt = C.c_uint64(), C.c_uint64()
+            capi.check(capi.lib.dg_isosurface_sizes(s, C.byref(nv), C.byref(nt)))
+            nv, nt = nv.value, nt.value
+            if not device:
+                V = np.empty((nv, 3)); T = np.empty((nt, 3), np.uint32)
+                capi.check(capi.lib.dg_isosurface_copy(s, capi.ptr(V, capi.F64P), capi.ptr(T, capi.U32P)))
+                return V, T
+            import torch
+            if nv >= 2 ** 31:
+                raise ValueError(f"isosurface: {nv} vertices do not fit the int32 indices of the device route; use device=False")
+            info = (C.c_uint64 * 4)()
+            capi.check(capi.lib.dg_field_info(h, info))
+            dev = torch.device("cpu") if capi.EMULATED else torch.device("cuda", int(info[3]))
+            V = torch.empty((nv, 3), dtype=torch.float64, device=dev)
+            T = torch.empty((nt, 3), dtype=torch.int32, device=dev)
+            st = _device.stream(V)
+            capi.check(capi.lib.dg_isosurface_copy_device(s, V.data_ptr(), T.data_ptr(), st))
+            if not capi.EMULATED:
+                torch.cuda.current_stream(dev).synchronize()          # the copies read the handle, released below
+            return V, T
+        finally:
+            capi.lib.dg_isosurface_destroy(s)
+
     # ------------------------------------------------------------------ save / load (cubic_lagrange_discrete_grid.cpp:678-778)
     def save(self, filename):
         d = self._desc

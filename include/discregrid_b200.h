@@ -330,6 +330,26 @@ DG_API int dg_reduced_band_destroy(dg_reduced_band* result);
  * device (DG_ERR_INVALID otherwise).  A handle with no kept cell gives a field whose every query returns DBL_MAX. */
 DG_API int dg_field_create_reduced(const dg_reduced_band* r, dg_field** out);
 
+/* ---- level sets: the surface {phi = iso} of a field as a triangle mesh (not in the reference) -------------------------------------------
+ * Marching tetrahedra on a lattice that subdivides every grid cell `subdivisions` times; the lattice values are the bits of the value-only
+ * dg_interpolate_batch.  The full contract -- lattice, validity (finite and != DBL_MAX; a point in a removed cell of a reduced field is
+ * invalid), the Kuhn split, the case table and orientation (normals from the negative to the non-negative side: outward for an SDF), vertex
+ * arithmetic and the order of vertices and triangles -- is stated in discregrid_b200/csrc/k6_isosurface.cu and DESIGN.md section 3.
+ * Coincident vertices are not welded; no normals are output.  One GPU (the field's), synchronous on the legacy default stream.  The result
+ * stays on the device in the handle until dg_isosurface_copy[_device]; vertices[n_vertices x 3] and triangles[n_triangles x 3] (0-based
+ * indices, the layout dg_mesh_create takes).  A field with no kept cell, or an iso above or below every value, gives 0 / 0.
+ *   iso: finite (NaN or +-inf: DG_ERR_INVALID).  subdivisions: 1..16.  A lattice of 2^31 points or more, and a result of 2^32 vertices or
+ *       triangles or more, are refused (DG_ERR_INVALID), the lattice before anything is allocated.  The field must live on the current device.
+ *   timings_ms: NULL or 5 doubles = ms of values, classify, scans, emit, total.  Every stage ends with a device synchronise.
+ *   dg_isosurface_copy / _copy_device: outputs may be NULL only when their count is 0.  _copy_device is asynchronous on `stream`; let it
+ *       finish before dg_isosurface_destroy. */
+typedef struct dg_isosurface dg_isosurface;
+DG_API int dg_isosurface_create(const dg_field* field, double iso, uint32_t subdivisions, dg_isosurface** out, double* timings_ms);
+DG_API int dg_isosurface_sizes(const dg_isosurface* s, uint64_t* n_vertices, uint64_t* n_triangles);
+DG_API int dg_isosurface_copy(const dg_isosurface* s, double* vertices, uint32_t* triangles);
+DG_API int dg_isosurface_copy_device(const dg_isosurface* s, double* d_vertices, uint32_t* d_triangles, void* stream);
+DG_API int dg_isosurface_destroy(dg_isosurface* s);
+
 /* ---- reduced density map: GenerateDensityMap with reduction in one call -----------------------------------------------------------
  * GenerateDensityMap with reduction (cmd/generate_density_map/main.cpp:117-147) in one call:
  *   id = addFunction(density_func, verbose, pred);  reduceField(0, p0);  reduceField(id, p1);
