@@ -16,6 +16,7 @@
 //   interpolate(field, x, grad*)             -> dg_interpolate_batch (K2), also batched: interpolate(field, n, x, phi, grad)
 //   interpolate(field, n, x, phi, grad, hess) -> dg_interpolate_hessian_batch (K2's Hessian mode; not in the reference)
 //   isosurface(field, iso, subdivisions)     -> dg_isosurface_create (K6: the level set as a TriangleMesh; not in the reference)
+//   raycast(field, n, o, d, iso, t0, t1, ...) -> dg_field_raycast (K7: first crossings along rays and segments; not in the reference)
 //   connectivity table of addFunction        -> dg_build_cells  (GPU)  replaces the serial loop :833-886
 //
 // m_nodes / m_cells / m_cell_map hold exactly what the reference would have produced, so save()/load() stay
@@ -368,6 +369,14 @@ public:
         dg_isosurface_destroy(s);
         check(rc);
         return TriangleMesh(v.data(), t.data(), (std::size_t)nv, (std::size_t)nt);
+    }
+    // the first crossing of {phi = iso} along n rays (new, beyond the reference; contract in k7_raycast.cu): origins and directions n x 3,
+    // t in [t_min, t_max] (a segment x0 -> x1 is the ray (x0, x1 - x0) on [0, 1]); outputs t_lo, t_hi (the bracket) and status = DG_RAY_MISS /
+    // DG_RAY_ENTER / DG_RAY_LEAVE, all n (dg_field_raycast)
+    void raycast(unsigned int field_id, std::size_t n, const double* origins, const double* directions, double iso, double t_min, double t_max,
+                 double* t_lo, double* t_hi, std::int32_t* status) const
+    {
+        check(dg_field_raycast(deviceField(field_id), origins, directions, n, iso, t_min, t_max, t_lo, t_hi, status));
     }
 
     // ---- split API (:901-975): shape functions on the GPU (dg_shape_functions), index algebra on the host

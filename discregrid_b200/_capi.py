@@ -14,6 +14,7 @@ LIB_PATH = os.environ.get("DISCREGRID_B200_LIB") or os.path.join(_HERE, "lib", "
 DG_OK, DG_ERR_INVALID, DG_ERR_NO_DEVICE, DG_ERR_CUDA, DG_ERR_NOMEM, DG_ERR_SELFTEST, DG_ERR_IO, DG_ERR_CALLBACK = 0, -1, -2, -3, -4, -5, -6, -7
 DBL_MAX = 1.7976931348623157e308
 DG_SIGN_PSEUDONORMAL, DG_SIGN_WINDING = 0, 1
+DG_RAY_MISS, DG_RAY_ENTER, DG_RAY_LEAVE = 0, 1, 2
 UINT32_MAX = 0xFFFFFFFF
 
 
@@ -118,6 +119,8 @@ SIGNATURES = {
     "dg_isosurface_copy": (C.c_int, [_vp, _dp, _u32p]),
     "dg_isosurface_copy_device": (C.c_int, [_vp, _vp, _vp, _vp]),
     "dg_isosurface_destroy": (C.c_int, [_vp]),
+    "dg_field_raycast": (C.c_int, [_vp, _dp, _dp, C.c_uint64, C.c_double, C.c_double, C.c_double, _dp, _dp, _i32p]),
+    "dg_field_raycast_device": (C.c_int, [_vp, _vp, _vp, C.c_uint64, C.c_double, C.c_double, C.c_double, _vp, _vp, _vp, _vp]),
     "dg_reduced_density_map_create": (C.c_int, [_gp, _dp, C.c_uint64, _u32p, C.c_uint64, _u32p, C.c_double, C.c_double, C.c_uint32,
                                                  C.POINTER(_vp), C.POINTER(_vp), _dp]),
     "dg_add_function_device": (C.c_int, [_gp, DEVICE_FUNCTION, _vp, DEVICE_SAMPLE_PREDICATE, _vp, C.c_uint64, _dp, _u32p, _u32p, _dp]),

@@ -41,6 +41,7 @@
 #include "k4_reduce.h"
 #include "k5_winding.h"
 #include "k6_isosurface.h"
+#include "k7_raycast.h"
 #include "reduce_field.h"
 #include "obj_reader.h"
 
@@ -2414,6 +2415,59 @@ int dg_isosurface_destroy(dg_isosurface* s)
 {
     delete s;
     return DG_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ K7: ray casts
+static int raycast_check(const dg_field* f, const void* o, const void* d, uint64_t n, double iso, double t_min, double t_max, const void* t_lo,
+                         const void* t_hi, const void* status, const char* who)
+{
+    if (!f) return fail(DG_ERR_INVALID, "%s: field is NULL", who);
+    if (n && (!o || !d || !t_lo || !t_hi || !status)) return fail(DG_ERR_INVALID, "%s: origins / directions / t_lo / t_hi / status is NULL", who);
+    if (!std::isfinite(iso)) return fail(DG_ERR_INVALID, "%s: iso must be finite (got %g)", who, iso);
+    if (std::isnan(t_min) || std::isnan(t_max)) return fail(DG_ERR_INVALID, "%s: t_min and t_max must not be NaN", who);
+    if (t_min > t_max) return fail(DG_ERR_INVALID, "%s: t_min > t_max (%g > %g)", who, t_min, t_max);
+    return check_handle_device(f->device, who);
+}
+
+int dg_field_raycast_device(const dg_field* f, const double* d_o, const double* d_d, uint64_t n, double iso, double t_min, double t_max,
+                            double* d_t_lo, double* d_t_hi, int32_t* d_status, void* stream)
+{
+    if (int rc = raycast_check(f, d_o, d_d, n, iso, t_min, t_max, d_t_lo, d_t_hi, d_status, "dg_field_raycast_device")) return rc;
+    if (n) DG_LAUNCH(k7_launch_raycast(f->dev, d_o, d_d, n, iso, t_min, t_max, d_t_lo, d_t_hi, d_status, (cudaStream_t)stream));
+    return DG_OK;
+}
+
+// host arrays: chunks of 2^20 rays (64 MiB of device buffers) uploaded, cast and downloaded in turn on the legacy default stream
+static int raycast_host_impl(const dg_field* f, const double* o, const double* d, uint64_t n, double iso, double t_min, double t_max,
+                             double* t_lo, double* t_hi, int32_t* status)
+{
+    static const char* who = "dg_field_raycast";
+    if (int rc = raycast_check(f, o, d, n, iso, t_min, t_max, t_lo, t_hi, status, who)) return rc;
+    if (n == 0) return DG_OK;
+    const uint64_t chunk = std::min<uint64_t>(n, 1ull << 20);
+    DevBuf<double> d_o, d_d, d_lo, d_hi;
+    DevBuf<int32_t> d_st;
+    DG_CUDA(d_o.alloc(3 * chunk));
+    DG_CUDA(d_d.alloc(3 * chunk));
+    DG_CUDA(d_lo.alloc(chunk));
+    DG_CUDA(d_hi.alloc(chunk));
+    DG_CUDA(d_st.alloc(chunk));
+    for (uint64_t b = 0; b < n; b += chunk) {
+        const uint64_t c = std::min(chunk, n - b);
+        DG_CUDA(cudaMemcpy(d_o.p, o + 3 * b, 3 * c * sizeof(double), cudaMemcpyHostToDevice));
+        DG_CUDA(cudaMemcpy(d_d.p, d + 3 * b, 3 * c * sizeof(double), cudaMemcpyHostToDevice));
+        DG_LAUNCH(k7_launch_raycast(f->dev, d_o.p, d_d.p, c, iso, t_min, t_max, d_lo.p, d_hi.p, d_st.p, nullptr));
+        DG_CUDA(cudaMemcpy(t_lo + b, d_lo.p, c * sizeof(double), cudaMemcpyDeviceToHost));
+        DG_CUDA(cudaMemcpy(t_hi + b, d_hi.p, c * sizeof(double), cudaMemcpyDeviceToHost));
+        DG_CUDA(cudaMemcpy(status + b, d_st.p, c * sizeof(int32_t), cudaMemcpyDeviceToHost));
+    }
+    return DG_OK;
+}
+
+int dg_field_raycast(const dg_field* f, const double* o, const double* d, uint64_t n, double iso, double t_min, double t_max, double* t_lo,
+                     double* t_hi, int32_t* status)
+{
+    return guarded("dg_field_raycast", [&]() { return raycast_host_impl(f, o, d, n, iso, t_min, t_max, t_lo, t_hi, status); });
 }
 
 int dg_obj_read(const char* path, double** vertices, uint64_t* n_vertices, uint32_t** triangles, uint64_t* n_triangles)

@@ -22,6 +22,7 @@ that save()/load() stay byte-compatible with the reference's .cdf/.cdm files
   interpolate(field_id, x[, gradient])   -> dg_interpolate_batch (K2, csrc/k2_interp.cu), batched over x; a float64 CUDA tensor x
                                             -> dg_interpolate_batch_device on torch's current stream (CUDA tensors out, autograd in x)
   interpolate(field_id, x, hessian=True) -> dg_interpolate_hessian_batch[_device] (K2's Hessian mode; second-order autograd in x)
+  raycast(field_id, origins, directions) -> dg_field_raycast[_device] (K7: first crossings of a level set along rays and segments)
 
 The reduced calls keep the handle they get from the library until the field's first device use, which builds the interpolation
 field from it on the device (dg_field_create_reduced) instead of uploading the host copy again.
@@ -674,6 +675,43 @@ class CubicLagrangeDiscreteGrid:
             return V, T
         finally:
             capi.lib.dg_isosurface_destroy(s)
+
+    def raycast(self, field_id, origins, directions, iso=0.0, t_min=0.0, t_max=math.inf):
+        """The first crossing of {phi = iso} along rays x(t) = origin + t * direction, t in [t_min, t_max] clipped to the domain, on the
+        field's GPU (dg_field_raycast; the contract is in csrc/k7_raycast.cu and DESIGN §3).  The crossing is isolated cell by cell with
+        Bernstein bounds of the interpolant along the line, so features thinner than any step are not missed, on any field (SDF, density
+        map, reduced band, user function).  A segment x0 -> x1 (continuous collision detection of a step) is raycast(f, x0, x1 - x0,
+        t_min=0, t_max=1).  The values along the ray are the bits interpolate() returns there; DBL_MAX and non-finite values (outside the
+        domain, removed cells) are never crossed.
+        Returns (t_lo, t_hi, status): the final bisection bracket and DG_RAY_ENTER (1: phi(x(t_lo)) >= iso > phi(x(t_hi))), DG_RAY_LEAVE (2:
+        the reverse; a ray that starts inside reports its first LEAVE) or DG_RAY_MISS (0, with t_lo = t_hi = inf).  numpy inputs (n, 3)
+        give numpy arrays (float64, float64, int32).  float64 CUDA tensors (n, 3) on the field's device stay there: the cast runs on
+        torch's current stream and returns CUDA tensors.  Not differentiable.  A reduced field's kept device handle is used directly."""
+        h = self._device_field(field_id)
+        iso, t_min, t_max = float(iso), float(t_min), float(t_max)
+        if _device.is_device_query(origins) or _device.is_device_query(directions):
+            import torch
+            info = (C.c_uint64 * 4)()
+            capi.check(capi.lib.dg_field_info(h, info))
+            o = _device.points(origins, int(info[3]), "raycast")
+            d = _device.points(directions, int(info[3]), "raycast")
+            if o.shape != d.shape:
+                raise ValueError(f"raycast: origins {tuple(o.shape)} and directions {tuple(d.shape)} differ in shape")
+            n = len(o)
+            t_lo = torch.empty(n, dtype=torch.float64, device=o.device)
+            t_hi = torch.empty(n, dtype=torch.float64, device=o.device)
+            status = torch.empty(n, dtype=torch.int32, device=o.device)
+            capi.check(capi.lib.dg_field_raycast_device(h, o.data_ptr(), d.data_ptr(), n, iso, t_min, t_max, t_lo.data_ptr(), t_hi.data_ptr(),
+                                                        status.data_ptr(), _device.stream(o)))
+            return t_lo, t_hi, status
+        o = np.ascontiguousarray(origins, np.float64).reshape(-1, 3)
+        d = np.ascontiguousarray(directions, np.float64).reshape(-1, 3)
+        if o.shape != d.shape:
+            raise ValueError(f"raycast: origins {o.shape} and directions {d.shape} differ in shape")
+        t_lo, t_hi, status = np.empty(len(o)), np.empty(len(o)), np.empty(len(o), np.int32)
+        capi.check(capi.lib.dg_field_raycast(h, capi.ptr(o, capi.F64P), capi.ptr(d, capi.F64P), len(o), iso, t_min, t_max,
+                                             capi.ptr(t_lo, capi.F64P), capi.ptr(t_hi, capi.F64P), capi.ptr(status, capi.I32P)))
+        return t_lo, t_hi, status
 
     # ------------------------------------------------------------------ save / load (cubic_lagrange_discrete_grid.cpp:678-778)
     def save(self, filename):

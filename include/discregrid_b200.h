@@ -350,6 +350,25 @@ DG_API int dg_isosurface_copy(const dg_isosurface* s, double* vertices, uint32_t
 DG_API int dg_isosurface_copy_device(const dg_isosurface* s, double* d_vertices, uint32_t* d_triangles, void* stream);
 DG_API int dg_isosurface_destroy(dg_isosurface* s);
 
+/* ---- ray casts: the first crossing of {phi = iso} along rays and segments (not in the reference) -----------------------------------------
+ * For each ray i (origin origins[3 i..], direction directions[3 i..]) and t in [t_min, t_max] clipped to the domain: the first crossing of
+ * the level set, isolated cell by cell with Bernstein bounds of the interpolant's restriction to the line, so a feature thinner than any step
+ * is not missed.  The values along the ray are the bits of the value-only dg_interpolate_batch; the full contract (clip, segments, samples,
+ * pruning, descent, bisection) is stated in discregrid_b200/csrc/k7_raycast.cu and DESIGN.md section 3.  A segment x0 -> x1 is the ray
+ * (x0, x1 - x0) with t_min = 0, t_max = 1.
+ *   t_lo[i], t_hi[i]: the final bisection bracket; status[i] = DG_RAY_ENTER when phi(x(t_lo)) >= iso > phi(x(t_hi)), DG_RAY_LEAVE for the
+ *       reverse (a ray that starts inside reports its first LEAVE), DG_RAY_MISS with t_lo = t_hi = +inf when no crossing is found.
+ *   iso: finite.  t_min <= t_max, neither NaN (either may be infinite).  Arrays may be NULL only when n is 0.  The field must live on the
+ *       current device.  Otherwise DG_ERR_INVALID.
+ *   dg_field_raycast: host arrays, synchronous.  dg_field_raycast_device: device arrays, asynchronous on `stream`. */
+#define DG_RAY_MISS  0
+#define DG_RAY_ENTER 1
+#define DG_RAY_LEAVE 2
+DG_API int dg_field_raycast(const dg_field* field, const double* origins, const double* directions, uint64_t n, double iso, double t_min,
+                            double t_max, double* t_lo, double* t_hi, int32_t* status);
+DG_API int dg_field_raycast_device(const dg_field* field, const double* d_origins, const double* d_directions, uint64_t n, double iso,
+                                   double t_min, double t_max, double* d_t_lo, double* d_t_hi, int32_t* d_status, void* stream);
+
 /* ---- reduced density map: GenerateDensityMap with reduction in one call -----------------------------------------------------------
  * GenerateDensityMap with reduction (cmd/generate_density_map/main.cpp:117-147) in one call:
  *   id = addFunction(density_func, verbose, pred);  reduceField(0, p0);  reduceField(id, p1);
