@@ -101,6 +101,22 @@ public:
         m_sign_mode = mode;
     }
     SignMode signMode() const { return m_sign_mode; }
+    // new: moves the vertices (the count of the construction) and refits the tree, pseudonormals and winding records on the GPU; the
+    // triangles and the tree's leaf order stay, so construct again after large deformations.  Not to be called while another thread uses
+    // this object.  The multi-GPU replicas would go stale: it throws after useGpus(n > 1).
+    template <typename IndexableVector3double> void refit(const std::vector<IndexableVector3double>& vertices)
+    {
+        std::vector<double> V(3 * vertices.size());
+        for (size_t i = 0; i < vertices.size(); i++) for (int k = 0; k < 3; k++) V[3 * i + k] = (double)vertices[i][k];
+        refit_check();
+        if (dg_mesh_refit(m_mesh, V.data(), vertices.size()) != DG_OK) throw std::runtime_error(std::string("TriangleMeshDistance: ") + dg_last_error());
+    }
+    // the same from n_vertices x 3 doubles in the mesh's device memory, read on `stream` (cudaStream_t) after the work queued there
+    void refit(const double* d_vertices, size_t n_vertices, void* stream = nullptr)
+    {
+        refit_check();
+        if (dg_mesh_refit_device(m_mesh, d_vertices, n_vertices, stream) != DG_OK) throw std::runtime_error(std::string("TriangleMeshDistance: ") + dg_last_error());
+    }
     // new: generalized winding number at a point (1 inside a closed surface, 0 outside), or at n points (xyzxyz) into w[n]
     template <typename IndexableVector3double> double winding_number(const IndexableVector3double& p, double beta = 2.0) const
     {
@@ -120,6 +136,11 @@ private:
     dg_mesh_group* m_group = nullptr;
     SignMode m_sign_mode = SignMode::Pseudonormal;
     void require() const { if (!m_mesh) throw std::runtime_error("DistanceTriangleMesh error: not constructed."); }
+    void refit_check() const
+    {
+        require();
+        if (m_group) throw std::runtime_error("TriangleMeshDistance: refit is not available after useGpus(n > 1): the replicas on the other GPUs would go stale");
+    }
     void upload(const std::vector<double>& V, const std::vector<uint32_t>& F)
     {
         if (m_group) { dg_mesh_group_destroy(m_group); m_group = nullptr; }

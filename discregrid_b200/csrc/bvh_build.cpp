@@ -1,6 +1,7 @@
 // See bvh_build.h.  Compiled with -ffp-contract=off: every expression below must round exactly like the
 // reference's x86-64 build (no FMA), because these values feed bit-exact device comparisons.
 #include "bvh_build.h"
+#include "bvh_records.h"
 #include "sort_replay.h"
 
 #include <algorithm>
@@ -44,14 +45,10 @@ struct Builder {
     {
         { int cur = max_depth.load(std::memory_order_relaxed); while (depth > cur && !max_depth.compare_exchange_weak(cur, depth)) {} }
         const int n = e - b;
-        if (n == 1) {
+        if (n == 1) {                                        // bvh_records.h, shared with the device refit
             const P3 a = vert(order[b], 0), bb = vert(order[b], 1), c = vert(order[b], 2);
-            const P3 s = (a + bb) + c;
-            const P3 ctr = {s.x / 3.0, s.y / 3.0, s.z / 3.0};
-            sr = std::max(std::max(len(a - ctr), len(bb - ctr)), len(c - ctr));
-            sc[0] = ctr.x; sc[1] = ctr.y; sc[2] = ctr.z;
-            box[0] = std::min(std::min(a.x, bb.x), c.x); box[1] = std::min(std::min(a.y, bb.y), c.y); box[2] = std::min(std::min(a.z, bb.z), c.z);
-            box[3] = std::max(std::max(a.x, bb.x), c.x); box[4] = std::max(std::max(a.y, bb.y), c.y); box[5] = std::max(std::max(a.z, bb.z), c.z);
+            make_leaf_sphere(&a.x, &bb.x, &c.x, sc, sr);
+            make_leaf_box(&a.x, &bb.x, &c.x, box);
             return;
         }
         double top[3] = {-DBL_MAX, -DBL_MAX, -DBL_MAX}, bot[3] = {DBL_MAX, DBL_MAX, DBL_MAX};
@@ -209,16 +206,7 @@ bool build_host_bvh(const double* Vd, uint64_t nV, const uint32_t* F, uint64_t n
             const int id = out.order[pos];
             const uint32_t* t = F + 3 * (size_t)id;
             const P3 v0 = V[t[0]], v1 = V[t[1]], v2 = V[t[2]];
-            const P3 e0 = v1 - v0, e1 = v2 - v0;                            // TriangleMeshDistance.h:567-568
-            LeafRecord& L = out.leaves[pos];
-            L.v0[0] = v0.x; L.v0[1] = v0.y; L.v0[2] = v0.z;
-            L.e0[0] = e0.x; L.e0[1] = e0.y; L.e0[2] = e0.z;
-            L.e1[0] = e1.x; L.e1[1] = e1.y; L.e1[2] = e1.z;
-            L.a00 = dot3(e0, e0); L.a01 = dot3(e0, e1); L.a11 = dot3(e1, e1);  // :569-571
-            L.det = std::abs(L.a00 * L.a11 - L.a01 * L.a01);                   // :575
-            L.inv_det = 1 / L.det;                                            // :675
-            L.denom = L.a00 - 2 * L.a01 + L.a11;                              // :693,740,792
-            L.tri_id = id; L._pad = 0;
+            make_leaf_record(&v0.x, &v1.x, &v2.x, id, out.leaves[pos]);      // TriangleMeshDistance.h:567-575 (bvh_records.h)
             PseudoNormals& N = out.normals[pos];
             const P3 src[7] = {pv[t[0]], pv[t[1]], pv[t[2]], pe[3 * id + 0], pe[3 * id + 1], pe[3 * id + 2], pt[id]};
             for (int k = 0; k < 7; k++) { N.n[k][0] = src[k].x; N.n[k][1] = src[k].y; N.n[k][2] = src[k].z; }
@@ -240,41 +228,19 @@ bool build_host_bvh(const double* Vd, uint64_t nV, const uint32_t* F, uint64_t n
         out.spheres_f.resize(nT);
         out.boxes_f.resize(nT);
         // child boxes are rounded outward so that the fp32 box contains the fp64 one
-        auto down = [](double v) { float f = (float)v; return ((double)f > v) ? std::nextafterf(f, -INFINITY) : f; };
-        auto up = [](double v) { float f = (float)v; return ((double)f < v) ? std::nextafterf(f, INFINITY) : f; };
         parallel_for(nT, [&](uint64_t m0, uint64_t m1) {
             for (uint64_t m = m0; m < m1; m++) {
-                const SpherePair& sp = out.spheres[m];
-                SpherePairF& f = out.spheres_f[m];
-                for (int d = 0; d < 3; d++) { f.lc[d] = (float)(sp.lc[d] - out.center[d]); f.rc[d] = (float)(sp.rc[d] - out.center[d]); }
-                f.lr = (float)sp.lr; f.rr = (float)sp.rr;
+                make_sphere_shadow(out.spheres[m], out.center, out.spheres_f[m]);
                 BoxPairF& q = out.boxes_f[m];
                 if (m == 0) { std::memset(&q, 0, sizeof q); continue; }
-                const double* bx = &out.boxes[12 * m];
-                for (int d = 0; d < 3; d++) {
-                    q.l_lo[d] = down(bx[d] - out.center[d]); q.l_hi[d] = up(bx[3 + d] - out.center[d]);
-                    q.r_lo[d] = down(bx[6 + d] - out.center[d]); q.r_hi[d] = up(bx[9 + d] - out.center[d]);
-                }
+                make_box_shadow(&out.boxes[12 * m], out.center, q);
             }
         });
         RawVec<double>().swap(out.boxes);
         // fp32 triangle shadows in leaf order (all products formed in fp64, then rounded once)
         if (with_leaf_shadow) out.leaves_f.resize(nT);
         if (with_leaf_shadow) parallel_for(nT, [&](uint64_t p0, uint64_t p1) {
-            for (uint64_t pos = p0; pos < p1; pos++) {
-                const LeafRecord& L = out.leaves[pos];
-                LeafF& f = out.leaves_f[pos];
-                double e2[3], n3[3];
-                for (int d = 0; d < 3; d++) { f.v0[d] = (float)(L.v0[d] - out.center[d]); f.e0[d] = (float)L.e0[d]; f.e1[d] = (float)L.e1[d]; e2[d] = L.e1[d] - L.e0[d]; }
-                n3[0] = L.e0[1] * L.e1[2] - L.e0[2] * L.e1[1]; n3[1] = L.e0[2] * L.e1[0] - L.e0[0] * L.e1[2]; n3[2] = L.e0[0] * L.e1[1] - L.e0[1] * L.e1[0];
-                f.d00 = (float)L.a00; f.d01 = (float)L.a01; f.d11 = (float)L.a11; f.d22 = (float)(e2[0] * e2[0] + e2[1] * e2[1] + e2[2] * e2[2]);
-                // UNIT normal: the filter's (w.n)^2 then scales like a squared distance and stays a normal fp32 number wherever the filter runs
-                // (e0 x e1 scales like length^2, so with it (w.n)^2 overflows fp32 for meshes of size ~1e6 and goes subnormal at ~1e-7).  Zero
-                // area (or a non-finite mesh): n = 0, i.e. no plane bound.  The max-component scaling keeps n.n clear of fp64 under/overflow.
-                const double s = std::max(std::fabs(n3[0]), std::max(std::fabs(n3[1]), std::fabs(n3[2])));
-                const double len = (s > 0 && std::isfinite(s)) ? s * std::sqrt((n3[0] / s) * (n3[0] / s) + (n3[1] / s) * (n3[1] / s) + (n3[2] / s) * (n3[2] / s)) : 0.0;
-                for (int d = 0; d < 3; d++) f.n[d] = (len > 0) ? (float)(n3[d] / len) : 0.f;
-            }
+            for (uint64_t pos = p0; pos < p1; pos++) make_leaf_shadow(out.leaves[pos], out.center, out.leaves_f[pos]);
         });
     }
 

@@ -12,6 +12,7 @@
 #include <cstdlib>
 #include <algorithm>
 #include <cstring>
+#include <limits>
 #include <memory>
 #include <mutex>
 #include <new>
@@ -42,6 +43,7 @@
 #include "k5_winding.h"
 #include "k6_isosurface.h"
 #include "k7_raycast.h"
+#include "k8_refit.h"
 #include "reduce_field.h"
 #include "obj_reader.h"
 
@@ -185,7 +187,34 @@ struct dg_mesh {
     mutable DevBuf<WindLeaf> d_wind_leaves;
     mutable DevBuf<WindClusterPair> d_wind_clusters;
     mutable WindDev wind;
+    // dg_mesh_refit (k8_refit.cu): topology tables and scratch, allocated at the first refit and kept
+    std::atomic<int> borrows{0};            // live dg_mesh_group's whose replicas copy this mesh's records
+    bool failed = false;                    // a refit stopped after it had started to write records
+    bool refit_ready = false;               // the tables below are allocated and uploaded
+    bool refit_done = false;                // the records are those of a refit: d_V holds the positions, host V and pseudonormals are stale
+    std::vector<uint32_t> refit_levels;     // RefitTopoHost::level_begin
+    DevBuf<double> d_V;                     // [nV][3] the positions of the last refit
+    DevBuf<uint32_t> d_F, d_f_leaf, d_inc_begin, d_inc;
+    DevBuf<int32_t> d_order;
+    DevBuf<RefitNodeRef> d_nodes;
+    DevBuf<RefitSums> d_sums;
+    DevBuf<RefitBounds> d_part;
+    DevBuf<double> d_bounds, d_pn_tri, d_angle, d_pn_vert, d_pn_edge;
+    size_t refit_bytes() const
+    {
+        return d_V.bytes() + d_F.bytes() + d_f_leaf.bytes() + d_inc_begin.bytes() + d_inc.bytes() + d_order.bytes() + d_nodes.bytes() +
+               d_sums.bytes() + d_part.bytes() + d_bounds.bytes() + d_pn_tri.bytes() + d_angle.bytes() + d_pn_vert.bytes() + d_pn_edge.bytes();
+    }
 };
+
+// every call on a mesh whose refit failed half way refuses it (its records are a mix of two vertex sets); NULL is left to the caller's check
+static int mesh_usable(const dg_mesh* m, const char* who)
+{
+    if (m && m->failed)
+        return fail(DG_ERR_INVALID, "%s: a refit of this mesh failed after it had started to write the records; the mesh is unusable "
+                    "(dg_mesh_destroy it and create it again)", who);
+    return DG_OK;
+}
 
 struct dg_field {
     dg_grid_desc desc;
@@ -393,10 +422,12 @@ int dg_mesh_destroy(dg_mesh* m)
 
 int dg_mesh_info(const dg_mesh* m, uint64_t info[8])
 {
+    if (int rc = mesh_usable(m, "dg_mesh_info")) return rc;
     if (!m || !info) return fail(DG_ERR_INVALID, "dg_mesh_info: NULL argument");
     info[0] = m->host.n_vertices; info[1] = m->host.n_triangles; info[2] = (uint64_t)m->dev.stack_depth;
     info[3] = (uint64_t)m->host.flags;
     info[4] = m->d_spheres.bytes() + m->d_leaves.bytes() + m->d_normals.bytes() + m->d_nodes_f.bytes() + m->d_leaves_f.bytes();
+    info[4] += m->refit_bytes();                                            // 0 until the first dg_mesh_refit
     {
         std::lock_guard<std::mutex> lock(m->wind_mu);
         info[4] += m->d_wind_leaves.bytes() + m->d_wind_clusters.bytes();      // 0 until the winding records are first used
@@ -407,6 +438,7 @@ int dg_mesh_info(const dg_mesh* m, uint64_t info[8])
 
 int dg_mesh_tree(const dg_mesh* m, double* spheres, int32_t* kids)
 {
+    if (int rc = mesh_usable(m, "dg_mesh_tree")) return rc;
     if (!m) return fail(DG_ERR_INVALID, "dg_mesh_tree: mesh is NULL");
     // the sphere pairs were released after upload: read them back from the device
     HostBvh tmp;
@@ -421,10 +453,43 @@ int dg_mesh_tree(const dg_mesh* m, double* spheres, int32_t* kids)
 int dg_mesh_pseudonormals(const dg_mesh* m, double* tri, double* edge, double* vert)
 {
     if (!m) return fail(DG_ERR_INVALID, "dg_mesh_pseudonormals: mesh is NULL");
+    if (int rc = mesh_usable(m, "dg_mesh_pseudonormals")) return rc;
+    if (m->refit_done) {        // the reference's arrays rebuilt from the device's per-leaf blocks (V0 V1 V2 E01 E12 E02 F)
+        const uint64_t nT = m->host.n_triangles;
+        RawVec<PseudoNormals> blk(nT);
+        DG_CUDA(cudaMemcpy(blk.data(), m->d_normals.p, nT * sizeof(PseudoNormals), cudaMemcpyDeviceToHost));
+        if (vert) std::fill(vert, vert + 3 * m->host.n_vertices, std::numeric_limits<double>::quiet_NaN());     // no triangle uses it
+        for (uint64_t pos = 0; pos < nT; pos++) {
+            const size_t id = (size_t)m->host.order[pos];
+            const PseudoNormals& N = blk[pos];
+            for (int d = 0; d < 3; d++) {
+                if (tri) tri[3 * id + d] = N.n[6][d];
+                if (edge) for (int k = 0; k < 3; k++) edge[9 * id + 3 * k + d] = N.n[3 + k][d];
+                if (vert) for (int k = 0; k < 3; k++) vert[3 * (size_t)m->host.F[3 * id + k] + d] = N.n[k][d];
+            }
+        }
+        return DG_OK;
+    }
+    if (!m) return fail(DG_ERR_INVALID, "dg_mesh_pseudonormals: mesh is NULL");
     if (tri) std::memcpy(tri, m->host.pn_tri.data(), m->host.pn_tri.size() * sizeof(double));
     if (edge) std::memcpy(edge, m->host.pn_edge.data(), m->host.pn_edge.size() * sizeof(double));
     if (vert) std::memcpy(vert, m->host.pn_vert.data(), m->host.pn_vert.size() * sizeof(double));
     return DG_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ refit (k8_refit.cu)
+// the scratch and tables of the refit as K8 reads them; output pointers are set by the caller
+static RefitDev refit_dev(const dg_mesh* m)
+{
+    RefitDev r;
+    r.V = m->d_V.p; r.n_vertices = m->host.n_vertices;
+    r.n_tri = (int)m->host.n_triangles; r.levels = m->host.max_depth;
+    r.F = m->d_F.p; r.f_leaf = m->d_f_leaf.p; r.order = m->d_order.p; r.inc_begin = m->d_inc_begin.p; r.inc = m->d_inc.p; r.nodes = m->d_nodes.p;
+    r.sums = m->d_sums.p; r.part = m->d_part.p; r.bounds = m->d_bounds.p;
+    r.pn_tri = m->d_pn_tri.p; r.angle = m->d_angle.p; r.pn_vert = m->d_pn_vert.p; r.pn_edge = m->d_pn_edge.p;
+    r.nodef_stride = K1_NODEF_STRIDE;
+    static_assert(K1_NODEF_STRIDE <= K8_MAX_NODEF_STRIDE, "k8_pack_kernel stages at most K8_MAX_NODEF_STRIDE float4s");
+    return r;
 }
 
 // ------------------------------------------------------------------------------------------------ K5: winding numbers, the winding sign mode
@@ -438,6 +503,23 @@ static int check_beta(double beta, const char* who)
 static int winding_dev(const dg_mesh* m, const WindDev*& out, const char* who)
 {
     std::lock_guard<std::mutex> lock(m->wind_mu);
+    if (!m->wind_ready && m->refit_done) {      // the host copy of V is stale: the records of the refit positions, built by K8's kernels
+        const uint64_t nT = m->host.n_triangles;
+        if (m->dev.stack_depth > K5_MAX_STACK) return fail(DG_ERR_INVALID, "%s: tree too deep for the winding walk", who);
+        DevBuf<WindLeaf> dl;
+        DevBuf<WindClusterPair> dc;
+        DG_CUDA(dl.alloc(nT));
+        DG_CUDA(dc.alloc(nT));
+        RefitDev r = refit_dev(m);
+        r.wind_leaves = dl.p; r.wind_clusters = dc.p;
+        DG_LAUNCH(k8_launch_refit(r, m->refit_levels, false, nullptr));
+        DG_CUDA(cudaStreamSynchronize(nullptr));
+        std::swap(m->d_wind_leaves.p, dl.p); std::swap(m->d_wind_leaves.n, dl.n);
+        std::swap(m->d_wind_clusters.p, dc.p); std::swap(m->d_wind_clusters.n, dc.n);
+        m->wind.leaves = m->d_wind_leaves.p; m->wind.clusters = m->d_wind_clusters.p;
+        m->wind.n_tri = (int)nT; m->wind.stack_depth = m->dev.stack_depth;
+        m->wind_ready = true;
+    }
     if (!m->wind_ready) {
         const uint64_t nT = m->host.n_triangles;
         if (m->dev.stack_depth > K5_MAX_STACK) return fail(DG_ERR_INVALID, "%s: tree too deep for the winding walk", who);
@@ -471,6 +553,7 @@ static int refuse_winding(const dg_mesh* m, const char* who)
 
 int dg_mesh_set_sign_mode(dg_mesh* m, int mode, double beta)
 {
+    if (int rc = mesh_usable(m, "dg_mesh_set_sign_mode")) return rc;
     if (!m) return fail(DG_ERR_INVALID, "dg_mesh_set_sign_mode: mesh is NULL (not constructed)");
     if (mode != DG_SIGN_PSEUDONORMAL && mode != DG_SIGN_WINDING) return fail(DG_ERR_INVALID, "dg_mesh_set_sign_mode: unknown mode %d", mode);
     if (int rc = check_beta(beta, "dg_mesh_set_sign_mode")) return rc;
@@ -479,8 +562,100 @@ int dg_mesh_set_sign_mode(dg_mesh* m, int mode, double beta)
     return DG_OK;
 }
 
+// topology tables (from F and the leaf order, once) and every scratch buffer: all allocated before any record is written
+static int refit_prepare(dg_mesh* m)
+{
+    if (m->refit_ready) return DG_OK;
+    const uint64_t nT = m->host.n_triangles, nV = m->host.n_vertices;
+    RefitTopoHost topo;
+    k8_build_topology(m->host, topo);
+    DG_CUDA(m->d_V.alloc(3 * nV));
+    DG_CUDA(m->d_F.alloc(3 * nT)); DG_CUDA(m->d_f_leaf.alloc(3 * nT)); DG_CUDA(m->d_order.alloc(nT));
+    DG_CUDA(m->d_inc_begin.alloc(nV + 1)); DG_CUDA(m->d_inc.alloc(3 * nT));
+    DG_CUDA(m->d_nodes.alloc(topo.nodes.size()));
+    DG_CUDA(m->d_sums.alloc(nT)); DG_CUDA(m->d_part.alloc(k8_bounds_entries(nV))); DG_CUDA(m->d_bounds.alloc(5));
+    DG_CUDA(m->d_pn_tri.alloc(3 * nT)); DG_CUDA(m->d_angle.alloc(3 * nT)); DG_CUDA(m->d_pn_vert.alloc(3 * nV)); DG_CUDA(m->d_pn_edge.alloc(9 * nT));
+    DG_CUDA(cudaMemcpy(m->d_F.p, m->host.F.data(), 3 * nT * sizeof(uint32_t), cudaMemcpyHostToDevice));
+    DG_CUDA(cudaMemcpy(m->d_f_leaf.p, topo.f_leaf.data(), 3 * nT * sizeof(uint32_t), cudaMemcpyHostToDevice));
+    DG_CUDA(cudaMemcpy(m->d_order.p, m->host.order.data(), nT * sizeof(int32_t), cudaMemcpyHostToDevice));
+    DG_CUDA(cudaMemcpy(m->d_inc_begin.p, topo.inc_begin.data(), (nV + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice));
+    DG_CUDA(cudaMemcpy(m->d_inc.p, topo.inc.data(), 3 * nT * sizeof(uint32_t), cudaMemcpyHostToDevice));
+    if (!topo.nodes.empty()) DG_CUDA(cudaMemcpy(m->d_nodes.p, topo.nodes.data(), topo.nodes.size() * sizeof(RefitNodeRef), cudaMemcpyHostToDevice));
+    m->refit_levels = topo.level_begin;
+    m->refit_ready = true;
+    return DG_OK;
+}
+
+static int refit_checks(dg_mesh* m, const void* v, uint64_t nV, const char* who)
+{
+    if (!m) return fail(DG_ERR_INVALID, "%s: mesh is NULL (not constructed)", who);
+    if (int rc = mesh_usable(m, who)) return rc;
+    if (nV && !v) return fail(DG_ERR_INVALID, "%s: vertices is NULL", who);
+    if (nV != m->host.n_vertices)
+        return fail(DG_ERR_INVALID, "%s: %llu vertices, but the mesh was built with %llu (a refit keeps the triangles; dg_mesh_create for a new topology)",
+                    who, (unsigned long long)nV, (unsigned long long)m->host.n_vertices);
+    if (int rc = check_handle_device(m->device, who)) return rc;
+    if (m->borrows.load() > 0)
+        return fail(DG_ERR_INVALID, "%s: a live dg_mesh_group replicates this mesh on other GPUs; its replicas would go stale (destroy the group first)", who);
+    return DG_OK;
+}
+
+int dg_mesh_refit_device(dg_mesh* m, const double* d_vertices, uint64_t n_vertices, void* stream)
+{
+    if (int rc = refit_checks(m, d_vertices, n_vertices, "dg_mesh_refit_device")) return rc;
+    if (d_vertices != m->d_V.p) {             // device (or managed) memory of the mesh's device: refused before anything is written
+        cudaPointerAttributes a;
+        if (cudaPointerGetAttributes(&a, d_vertices) != cudaSuccess) { cudaGetLastError(); a.type = cudaMemoryTypeUnregistered; }
+#ifndef DG_EMU
+        if ((a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged) || a.device != m->device)
+            return fail(DG_ERR_INVALID, "dg_mesh_refit_device: vertices is not device memory of the mesh's device %d (dg_mesh_refit takes a host array)",
+                        m->device);
+#endif
+    }
+    if (int rc = refit_prepare(m)) return rc;
+    const cudaStream_t st = (cudaStream_t)stream;
+    const uint64_t nV = n_vertices;
+    // from here on records are written: a CUDA error leaves the mesh failed
+    auto broken = [&](cudaError_t e, const char* what) {
+        m->failed = true;
+        return fail(e == cudaErrorMemoryAllocation ? DG_ERR_NOMEM : DG_ERR_CUDA, "dg_mesh_refit_device: %s failed: %s; the mesh is left unusable "
+                    "(dg_mesh_destroy it)", what, cudaGetErrorString(e));
+    };
+    cudaError_t e;
+    if (d_vertices != m->d_V.p && (e = cudaMemcpyAsync(m->d_V.p, d_vertices, 3 * nV * sizeof(double), cudaMemcpyDeviceToDevice, st)) != cudaSuccess)
+        return broken(e, "cudaMemcpyAsync of the vertices");
+    std::lock_guard<std::mutex> lock(m->wind_mu);
+    RefitDev r = refit_dev(m);
+    r.spheres = m->d_spheres.p; r.leaves = m->d_leaves.p; r.leaves_f = m->d_leaves_f.p; r.normals = m->d_normals.p; r.nodes_f = m->d_nodes_f.p;
+    if (m->wind_ready) { r.wind_leaves = m->d_wind_leaves.p; r.wind_clusters = m->d_wind_clusters.p; }     // else built at their first use
+    if ((e = k8_launch_refit(r, m->refit_levels, true, st)) != cudaSuccess) return broken(e, "k8_launch_refit");
+    g_launches.fetch_add(1);
+    double b[5];
+    if ((e = cudaMemcpyAsync(b, m->d_bounds.p, sizeof b, cudaMemcpyDeviceToHost, st)) != cudaSuccess) return broken(e, "cudaMemcpyAsync of the bounds");
+    if ((e = cudaStreamSynchronize(st)) != cudaSuccess) return broken(e, "cudaStreamSynchronize");
+    for (int d = 0; d < 3; d++) { m->host.center[d] = b[d]; m->dev.ctr[d] = b[d]; }
+    m->host.half_extent = b[3];
+    m->dev.half_extent = (float)m->host.half_extent * 1.0000002f;   // rounded up, as dg_mesh_create
+    m->refit_done = true;
+    return DG_OK;
+}
+
+int dg_mesh_refit(dg_mesh* m, const double* vertices, uint64_t n_vertices)
+{
+    if (int rc = refit_checks(m, vertices, n_vertices, "dg_mesh_refit")) return rc;
+    if (int rc = refit_prepare(m)) return rc;
+    const cudaError_t e = cudaMemcpy(m->d_V.p, vertices, 3 * n_vertices * sizeof(double), cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) {                   // d_V may now hold part of the new positions: out of step with the records
+        m->failed = true;
+        return fail(e == cudaErrorMemoryAllocation ? DG_ERR_NOMEM : DG_ERR_CUDA, "dg_mesh_refit: upload of the vertices failed: %s; the mesh "
+                    "is left unusable (dg_mesh_destroy it)", cudaGetErrorString(e));
+    }
+    return dg_mesh_refit_device(m, m->d_V.p, n_vertices, nullptr);
+}
+
 int dg_mesh_winding_number_device(const dg_mesh* m, const double* d_x, uint64_t n, double beta, double* d_w, void* stream)
 {
+    if (int rc = mesh_usable(m, "dg_mesh_winding_number_device")) return rc;
     if (!m) return fail(DG_ERR_INVALID, "dg_mesh_winding_number: mesh is NULL (not constructed)");
     if (int rc = check_beta(beta, "dg_mesh_winding_number")) return rc;
     if (n && (!d_x || !d_w)) return fail(DG_ERR_INVALID, "dg_mesh_winding_number: points or output is NULL");
@@ -494,6 +669,7 @@ int dg_mesh_winding_number_device(const dg_mesh* m, const double* d_x, uint64_t 
 
 int dg_mesh_winding_number(const dg_mesh* m, const double* x, uint64_t n, double beta, double* w)
 {
+    if (int rc = mesh_usable(m, "dg_mesh_winding_number")) return rc;
     if (!m) return fail(DG_ERR_INVALID, "dg_mesh_winding_number: mesh is NULL (not constructed)");
     if (int rc = check_beta(beta, "dg_mesh_winding_number")) return rc;
     if (n == 0) return DG_OK;
@@ -511,6 +687,7 @@ int dg_mesh_winding_number(const dg_mesh* m, const double* x, uint64_t n, double
 int dg_mesh_distance_device(const dg_mesh* m, const double* d_pts, uint64_t n, int is_signed, double* d_dist, double* d_near,
                             int32_t* d_ent, int32_t* d_tri, void* stream)
 {
+    if (int rc = mesh_usable(m, "dg_mesh_distance_device")) return rc;
     if (!m) return fail(DG_ERR_INVALID, "dg_mesh_distance: mesh is NULL (not constructed)");
     if (n && !d_pts) return fail(DG_ERR_INVALID, "dg_mesh_distance: points is NULL");
     if (int rc = check_handle_device(m->device, "dg_mesh_distance")) return rc;
@@ -528,6 +705,7 @@ int dg_mesh_distance_device(const dg_mesh* m, const double* d_pts, uint64_t n, i
 int dg_mesh_distance(const dg_mesh* m, const double* pts, uint64_t n, int is_signed, double* dist, double* nearp, int32_t* ent,
                      int32_t* tri)
 {
+    if (int rc = mesh_usable(m, "dg_mesh_distance")) return rc;
     if (!m) return fail(DG_ERR_INVALID, "dg_mesh_distance: mesh is NULL (not constructed)");
     if (n == 0) return DG_OK;
     if (!pts) return fail(DG_ERR_INVALID, "dg_mesh_distance: points is NULL");
@@ -563,6 +741,7 @@ static int check_range(const dg_grid_desc* grid, uint64_t b, uint64_t e, GridDev
 int dg_sample_sdf_device(const dg_mesh* m, const dg_grid_desc* grid, double sign, uint64_t l_begin, uint64_t l_end, double* d_out,
                          void* stream)
 {
+    if (int rc = mesh_usable(m, "dg_sample_sdf_device")) return rc;
     if (!m) return fail(DG_ERR_INVALID, "dg_sample_sdf: mesh is NULL (not constructed)");
     GridDev g;
     if (int rc = check_range(grid, l_begin, l_end, g, "dg_sample_sdf")) return rc;
@@ -590,6 +769,7 @@ static int check_band(double band, const char* who)
 int dg_sample_sdf_band_device(const dg_mesh* m, const dg_grid_desc* grid, double sign, double band, uint64_t l_begin, uint64_t l_end, double* d_out,
                               void* stream)
 {
+    if (int rc = mesh_usable(m, "dg_sample_sdf_band_device")) return rc;
     if (!m) return fail(DG_ERR_INVALID, "dg_sample_sdf_band: mesh is NULL (not constructed)");
     GridDev g;
     if (int rc = check_range(grid, l_begin, l_end, g, "dg_sample_sdf_band")) return rc;
@@ -888,6 +1068,7 @@ static void tables_job_copy(HostTablesJob* job, void* dst, const void* src, size
 
 int dg_sample_sdf(const dg_mesh* m, const dg_grid_desc* grid, double sign, uint64_t l_begin, uint64_t l_end, double* out_host)
 {
+    if (int rc = mesh_usable(m, "dg_sample_sdf")) return rc;
     if (!m) return fail(DG_ERR_INVALID, "dg_sample_sdf: mesh is NULL (not constructed)");
     GridDev g;
     if (int rc = check_range(grid, l_begin, l_end, g, "dg_sample_sdf")) return rc;
@@ -926,6 +1107,7 @@ int dg_sample_sdf(const dg_mesh* m, const dg_grid_desc* grid, double sign, uint6
 static int dg_add_function_sdf_impl(const dg_mesh* m, const dg_grid_desc* grid, double sign, double* nodes_host, uint32_t* cells_host, uint32_t* cell_map_host,
                         double* timings_ms, const double* band = nullptr)
 {
+    if (int rc = mesh_usable(m, "dg_add_function_sdf")) return rc;
     if (!m) return fail(DG_ERR_INVALID, "dg_add_function_sdf: mesh is NULL (not constructed)");
     if (band) { if (int rc = check_band(*band, "dg_add_function_sdf_band")) return rc; }
     GridDev g;
@@ -968,6 +1150,7 @@ struct dg_mesh_group {
     std::vector<dg_mesh*> parts;                            // parts[0] is the caller's mesh (not owned); the others are replicas
     std::vector<PerDev> dev;
     bool comms_ready = false;
+    bool borrowed = false;                                  // counted in parts[0]->borrows (dg_mesh_refit refuses while > 0)
     std::mutex mu;
 };
 
@@ -1038,12 +1221,14 @@ int dg_mesh_group_destroy(dg_mesh_group* grp)
         if (d.h_stage) cudaFreeHost(d.h_stage);
         if (i > 0 && (size_t)i < grp->parts.size()) delete grp->parts[i];
     }
+    if (grp->borrowed) grp->parts[0]->borrows.fetch_sub(1);
     delete grp;
     return DG_OK;
 }
 
 int dg_mesh_group_create(const dg_mesh* mesh, int n_gpus, const int* devices, dg_mesh_group** out)
 {
+    if (int rc = mesh_usable(mesh, "dg_mesh_group_create")) return rc;
     if (!out) return fail(DG_ERR_INVALID, "dg_mesh_group_create: out is NULL");
     *out = nullptr;
     if (!mesh) return fail(DG_ERR_INVALID, "dg_mesh_group_create: mesh is NULL (not constructed)");
@@ -1095,6 +1280,8 @@ int dg_mesh_group_create(const dg_mesh* mesh, int n_gpus, const int* devices, dg
         DG_CUDA(k1_configure(r->dev.stack_depth));
         DG_CUDA(cudaDeviceSynchronize());
     }
+    grp->parts[0]->borrows.fetch_add(1);
+    grp->borrowed = true;
     *out = grp.release();
     return DG_OK;
 }
@@ -1261,6 +1448,7 @@ int dg_slab_ranges(const dg_grid_desc* grid, uint32_t part, uint32_t n_parts, ui
 
 int dg_sample_sdf_slab_device(const dg_mesh* m, const dg_grid_desc* grid, double sign, uint32_t part, uint32_t n_parts, double* d_full, void* stream)
 {
+    if (int rc = mesh_usable(m, "dg_sample_sdf_slab_device")) return rc;
     if (!m) return fail(DG_ERR_INVALID, "dg_sample_sdf_slab: mesh is NULL (not constructed)");
     if (int rc = refuse_winding(m, "dg_sample_sdf_slab")) return rc;
     GridDev g; const char* why = "";
@@ -1297,6 +1485,7 @@ int dg_interleaved_node_slots(const dg_grid_desc* grid, uint32_t n_parts, uint64
 
 int dg_sample_sdf_interleaved_device(const dg_mesh* m, const dg_grid_desc* grid, double sign, uint32_t part, uint32_t n_parts, double* d_slot, void* stream)
 {
+    if (int rc = mesh_usable(m, "dg_sample_sdf_interleaved_device")) return rc;
     if (!m) return fail(DG_ERR_INVALID, "dg_sample_sdf_interleaved: mesh is NULL (not constructed)");
     if (int rc = refuse_winding(m, "dg_sample_sdf_interleaved")) return rc;
     GridDev g; const char* why = "";
@@ -1885,6 +2074,7 @@ static int device_reduce(const GridDev& g, const double* d_dense, uint64_t n, co
 static int reduced_band_create_impl(const dg_mesh* m, const dg_grid_desc* grid, double sign, double band, uint32_t flags, dg_reduced_band** out,
                                     double* timings_ms)
 {
+    if (int rc = mesh_usable(m, "dg_reduced_band_create")) return rc;
     static const char* who = "dg_reduced_band_create";
     if (!out) return fail(DG_ERR_INVALID, "%s: out is NULL", who);
     *out = nullptr;

@@ -114,6 +114,23 @@ class TriangleMeshDistance:
         self._sign_mode = mode
         return self
 
+    def refit(self, vertices):
+        """Moves the mesh's vertices to `vertices` (n_vertices x 3, the count of the construction) and refits every device record to
+        them: the sphere tree, the pseudonormals and, once used, the winding records (beyond the reference).  The triangles and the tree's
+        leaf order stay those of the construction, so a large deformation loosens the tree and queries slow down; construct again then.
+        A numpy array (or anything numpy converts) is uploaded first; a float64 CUDA tensor of shape (n_vertices, 3) on the mesh's device
+        is read in place, on torch's current stream after the work queued there.  Returns when the refit has finished; returns self.  Not
+        to be called while another call uses this mesh, on any stream."""
+        if _device.is_device_query(vertices):
+            x = _device.points(vertices, self.device, "refit")
+            capi.check(capi.lib.dg_mesh_refit_device(self.handle, x.data_ptr(), len(x), _device.stream(x)))
+            return self
+        V = np.ascontiguousarray(vertices, dtype=np.float64)
+        if V.ndim != 2 or V.shape[1] != 3:
+            raise ValueError(f"refit: vertices must have shape (n_vertices, 3) (got {V.shape})")
+        capi.check(capi.lib.dg_mesh_refit(self.handle, capi.ptr(V, capi.F64P), len(V)))
+        return self
+
     @property
     def sign_mode(self):
         return getattr(self, "_sign_mode", "pseudonormal")

@@ -154,6 +154,26 @@ DG_API int dg_mesh_set_sign_mode(dg_mesh* mesh, int mode, double beta);
 DG_API int dg_mesh_winding_number(const dg_mesh* mesh, const double* x, uint64_t n, double beta, double* w);
 DG_API int dg_mesh_winding_number_device(const dg_mesh* mesh, const double* d_x, uint64_t n, double beta, double* d_w, void* stream);
 
+/* ---- refit to new vertex positions (K8, k8_refit.cu; beyond the reference) ---------------------------------------------------------
+ * dg_mesh_refit replaces the mesh's vertices with `vertices` (n_vertices x 3 doubles, the count of the build) and recomputes on the device
+ * every record the kernels read: leaf records and shadows, the sphere tree's spheres and fp32 records, the bounding-box centre and half
+ * extent, the pseudonormals and, when they exist, the winding records.  The triangles and the tree's leaf order stay those of
+ * dg_mesh_create, so spheres grow with large deformations and queries slow down: rebuild with dg_mesh_create when they do.  Query
+ * results after a refit are the reference's query rule over the refit tree and pseudonormals; the numerical contract (sums bottom-up,
+ * the library's own acos for the pseudonormal angles) is stated in k8_refit.cu.  The watertight flags, the stack depth, the sign mode and
+ * beta are unchanged.
+ *   dg_mesh_refit_device: d_vertices on the mesh's device, read on `stream` after the work already queued there; returns when the refit
+ *       has finished (it reads back the centre and half extent).  No host<->device copy proportional to the mesh.
+ *   dg_mesh_refit: uploads the host array, then runs the device form.
+ * Topology tables and scratch are allocated at the first refit and kept (dg_mesh_info[4] counts them).  DG_ERR_INVALID, before anything is
+ * written: NULL mesh, NULL vertices with n_vertices > 0, n_vertices different from the build's, a mesh on another device, a mesh a live
+ * dg_mesh_group replicates.  Like dg_mesh_set_sign_mode, a refit must not overlap any other call that uses the mesh, including work queued
+ * on other streams.  A CUDA error after records have started to be written leaves the mesh failed: every later call on it except
+ * dg_mesh_destroy returns DG_ERR_INVALID.  After a refit dg_mesh_tree and dg_mesh_pseudonormals report the refit records (a vertex no
+ * triangle uses has NaN pseudonormals, as after dg_mesh_create). */
+DG_API int dg_mesh_refit(dg_mesh* mesh, const double* vertices, uint64_t n_vertices);
+DG_API int dg_mesh_refit_device(dg_mesh* mesh, const double* d_vertices, uint64_t n_vertices, void* stream);
+
 /* ---- K1: addFunction node loop with the GenerateSDF functor -------------------------------------------
  * replaces the hot loop cubic_lagrange_discrete_grid.cpp:806-817 with
  * func = sign * md.signed_distance(x).distance (cmd/generate_sdf/main.cpp:97,101; sign = -1 for --invert):
