@@ -24,7 +24,7 @@ CPPBIN   := build/bin
 CPPFLAGS := -std=c++11 -O2 -ffp-contract=off -I$(EIGEN3_INCLUDE_DIR) -Icpp/include -Iinclude
 CPPLINK  := -Ldiscregrid_b200/lib -ldiscregrid_b200 -Wl,-rpath,'$$ORIGIN/../../discregrid_b200/lib'
 CPPHDRS  := $(wildcard cpp/include/Discregrid/* cpp/include/Discregrid/*/*) include/discregrid_b200.h
-cpp: $(CPPBIN)/GenerateSDF $(CPPBIN)/GenerateDensityMap $(CPPBIN)/DiscreteFieldToBitmap $(CPPBIN)/DiscreteFieldToMesh $(CPPBIN)/facade_check $(CPPBIN)/bvh_host_check $(CPPBIN)/reduce_facade_check $(CPPBIN)/sort_replay_check $(CPPBIN)/fast_div_check $(CPPBIN)/libk1emu.so $(CPPBIN)/libk1emu_knobs.so $(CPPBIN)/libk1emu_wave.so $(CPPBIN)/libk1emu_perlane.so $(CPPBIN)/libk1emu_packet.so $(CPPBIN)/libk1emu_band.so $(CPPBIN)/libk1emu_band_perlane.so $(CPPBIN)/libk23emu.so $(CPPBIN)/libk23emu_knobs.so $(CPPBIN)/libk2hemu.so $(CPPBIN)/libk5emu.so $(CPPBIN)/libk8emu.so $(CPPBIN)/libdgemu.so $(CPPBIN)/libk4emu.so $(CPPBIN)/device_function_check $(CPPBIN)/device_query_check $(CPPBIN)/hessian_check $(CPPBIN)/winding_check $(CPPBIN)/raycast_check $(CPPBIN)/refit_check $(CPPBIN)/liborctree.so
+cpp: $(CPPBIN)/GenerateSDF $(CPPBIN)/GenerateDensityMap $(CPPBIN)/GenerateVolumeMap $(CPPBIN)/liborcvolume.so ref_volume $(CPPBIN)/DiscreteFieldToBitmap $(CPPBIN)/DiscreteFieldToMesh $(CPPBIN)/facade_check $(CPPBIN)/bvh_host_check $(CPPBIN)/reduce_facade_check $(CPPBIN)/sort_replay_check $(CPPBIN)/fast_div_check $(CPPBIN)/libk1emu.so $(CPPBIN)/libk1emu_knobs.so $(CPPBIN)/libk1emu_wave.so $(CPPBIN)/libk1emu_perlane.so $(CPPBIN)/libk1emu_packet.so $(CPPBIN)/libk1emu_band.so $(CPPBIN)/libk1emu_band_perlane.so $(CPPBIN)/libk23emu.so $(CPPBIN)/libk23emu_knobs.so $(CPPBIN)/libk3vemu.so $(CPPBIN)/libk2hemu.so $(CPPBIN)/libk5emu.so $(CPPBIN)/libk8emu.so $(CPPBIN)/libdgemu.so $(CPPBIN)/libk4emu.so $(CPPBIN)/device_function_check $(CPPBIN)/device_query_check $(CPPBIN)/hessian_check $(CPPBIN)/winding_check $(CPPBIN)/raycast_check $(CPPBIN)/refit_check $(CPPBIN)/liborctree.so
 $(CPPBIN)/DiscreteFieldToBitmap: cpp/cmd/discrete_field_to_bitmap.cpp $(CPPHDRS) $(LIB)
 	@mkdir -p $(CPPBIN)
 	$(HOSTCXX) $(CPPFLAGS) $< -o $@ $(CPPLINK)
@@ -71,6 +71,10 @@ $(CPPBIN)/libk23emu.so: $(K23EMU_DEP)
 $(CPPBIN)/libk23emu_knobs.so: $(K23EMU_DEP)
 	@mkdir -p $(CPPBIN)
 	$(HOSTCXX) -std=c++17 -O2 -ffp-contract=off -fPIC -shared -DK3_FAST_DIV=0 -I$(CUDA_INC) -Itests/emu -I$(SRC) $(K23EMU_SRC) -o $@ -lpthread
+# the same with the volume map exposed (emu_volume_map, tests/emu/k3_volume_emu.cpp)
+$(CPPBIN)/libk3vemu.so: $(K23EMU_DEP) tests/emu/k3_volume_emu.cpp
+	@mkdir -p $(CPPBIN)
+	$(HOSTCXX) -std=c++17 -O2 -ffp-contract=off -fPIC -shared -I$(CUDA_INC) -Itests/emu -I$(SRC) tests/emu/k2_emu.cpp tests/emu/k3_volume_emu.cpp -o $@ -lpthread
 # the same with K2's Hessian mode exposed (emu_interpolate_hessian)
 K2HEMU_SRC := tests/emu/k2_emu.cpp tests/emu/k2_hessian_emu.cpp
 $(CPPBIN)/libk2hemu.so: $(K23EMU_DEP) tests/emu/k2_hessian_emu.cpp
@@ -139,12 +143,22 @@ $(CPPBIN)/refit_check: tests/cpp/refit_check.cpp $(CPPHDRS) $(LIB)
 $(CPPBIN)/liborctree.so: tests/cpp/oracle_from_tree.cpp oracle/dg_oracle.cpp
 	@mkdir -p $(CPPBIN)
 	$(HOSTCXX) -std=c++11 -O3 -DNDEBUG -fopenmp -ffp-contract=off -fPIC -shared $< -o $@
+# test library: the oracle plus the volume map restated over its interpolate (orc_volume_map)
+$(CPPBIN)/liborcvolume.so: tests/cpp/volume_oracle.cpp oracle/dg_oracle.cpp
+	@mkdir -p $(CPPBIN)
+	$(HOSTCXX) -std=c++11 -O3 -DNDEBUG -fopenmp -ffp-contract=off -fPIC -shared $< -o $@
+# the reference-side volume-map generator (oracle/ref_volume_map.cpp on the reference's own sources), when the reference is present
+ref_volume:
+	$(MAKE) -C oracle -f ref_volume.mk
 oracle/liboracle.so:
 	$(MAKE) -C oracle oracle
 $(CPPBIN)/GenerateSDF: cpp/cmd/generate_sdf.cpp $(CPPHDRS) $(LIB)
 	@mkdir -p $(CPPBIN)
 	$(HOSTCXX) $(CPPFLAGS) $< -o $@ $(CPPLINK)
 $(CPPBIN)/GenerateDensityMap: cpp/cmd/generate_density_map.cpp $(CPPHDRS) $(LIB)
+	@mkdir -p $(CPPBIN)
+	$(HOSTCXX) $(CPPFLAGS) $< -o $@ $(CPPLINK)
+$(CPPBIN)/GenerateVolumeMap: cpp/cmd/generate_volume_map.cpp $(CPPHDRS) $(LIB)
 	@mkdir -p $(CPPBIN)
 	$(HOSTCXX) $(CPPFLAGS) $< -o $@ $(CPPLINK)
 $(CPPBIN)/facade_check: cpp/cmd/facade_check.cpp $(CPPHDRS) $(LIB)
@@ -168,4 +182,4 @@ oracle:
 clean:
 	rm -rf build $(LIB)
 	$(MAKE) -C oracle clean
-.PHONY: all lib cpp oracle clean
+.PHONY: all lib cpp oracle ref_volume clean

@@ -8,6 +8,8 @@
 //                                            -> dg_reduced_band_create (the same band + reduceField(always true), on the GPU)
 //   addFunction(DensityMapFunction)          -> dg_density_map  (K3)   (GenerateDensityMap's functor + predicate)
 //   addReducedDensityMap(DensityMapFunction) -> dg_reduced_density_map_create (K3 + both of GenerateDensityMap's reduceField calls, on the GPU)
+//   addFunction(VolumeMapFunction)           -> dg_volume_map   (K3's volume-map kernel: SPH boundary volumes; not in the reference)
+//   addReducedVolumeMap(VolumeMapFunction)   -> dg_reduced_volume_map_create (the volume map + reduceField(0, p0) + reduceField(id, 0 <= v))
 //   addFunction(DeviceFunction, verbose, DeviceSamplePredicate)
 //                                            -> dg_add_function_device (the caller's own GPU code on batches of node positions)
 //   reduceField(field, DeviceNodePredicate)  -> dg_reduce_field_device (the caller's predicate on the GPU, reduceField's passes there)
@@ -77,6 +79,20 @@ struct DensityMapFunction {
     double smoothing_length, rest_density;
     bool no_reduction;
     double operator()(Eigen::Vector3d const&) const { throw std::logic_error("DensityMapFunction is evaluated by addFunction on the GPU"); }
+};
+
+// The volume map of Bender et al. 2019 (SPlisHSPlasH's boundary representation) as a recognisable type: scale * the 16^3-point Gauss
+// quadrature of an inside indicator over the ball of radius h around each node, on the SDF in field sdf_field_id, with GenerateDensityMap's
+// sample predicate unless no_reduction (include/discregrid_b200.h, dg_volume_map)
+struct VolumeMapFunction {
+    const CubicLagrangeDiscreteGrid* grid;
+    unsigned int sdf_field_id;
+    double smoothing_length, scale;
+    bool no_reduction;
+    VolumeMapFunction(const CubicLagrangeDiscreteGrid* grid_, unsigned int sdf_field_id_, double smoothing_length_, double scale_ = 0.8,
+                      bool no_reduction_ = false)
+        : grid(grid_), sdf_field_id(sdf_field_id_), smoothing_length(smoothing_length_), scale(scale_), no_reduction(no_reduction_) {}
+    double operator()(Eigen::Vector3d const&) const { throw std::logic_error("VolumeMapFunction is evaluated by addFunction on the GPU"); }
 };
 
 // The caller's own GPU code as recognisable types (include/discregrid_b200.h, dg_device_function & co.): f is called once per chunk of node
@@ -229,6 +245,9 @@ public:
         if (auto const* dm = func.target<DensityMapFunction>()) {
             check(dg_density_map(dm->grid->deviceField(dm->sdf_field_id), dm->smoothing_length, dm->rest_density, dm->no_reduction ? 1 : 0,
                                  0, n_nodes, coeffs.data()));
+        } else if (auto const* vm = func.target<VolumeMapFunction>()) {
+            check(dg_volume_map(vm->grid->deviceField(vm->sdf_field_id), vm->smoothing_length, vm->scale, vm->no_reduction ? 1 : 0, 0, n_nodes,
+                                coeffs.data()));
         } else {
 #ifdef DISCREGRID_B200_ALLOW_HOST_CALLBACK
             FieldVector<double> x(3 * n_nodes);
@@ -239,7 +258,7 @@ public:
             }
 #else
             (void)pred;
-            throw std::invalid_argument("CubicLagrangeDiscreteGrid::addFunction: only MeshSignedDistanceFunction / DensityMapFunction run on the GPU "
+            throw std::invalid_argument("CubicLagrangeDiscreteGrid::addFunction: only MeshSignedDistanceFunction / DensityMapFunction / VolumeMapFunction run on the GPU "
                                         "(define DISCREGRID_B200_ALLOW_HOST_CALLBACK to have other callables invoked per node on the host)");
 #endif
         }
@@ -297,29 +316,18 @@ public:
     {
         if (f.grid != this) throw std::invalid_argument("addReducedDensityMap: the DensityMapFunction must sample this grid's own SDF field");
         if (f.no_reduction) throw std::invalid_argument("addReducedDensityMap: the DensityMapFunction has no_reduction set (use addFunction)");
-        const unsigned int id = f.sdf_field_id;
-        if (id >= m_n_fields) throw std::invalid_argument("addReducedDensityMap: no SDF field with that id");
-        if (m_cell_map[id].size() != m_n_cells) throw std::invalid_argument("addReducedDensityMap: the SDF field's cell map must cover every grid cell");
-        const dg_grid_desc d = desc();
-        dg_reduced_band* r[2] = {nullptr, nullptr};
-        check(dg_reduced_density_map_create(&d, m_nodes[id].data(), m_nodes[id].size(), reinterpret_cast<const std::uint32_t*>(m_cells[id].data()),
-                                            m_cells[id].size(), m_cell_map[id].data(), f.smoothing_length, f.rest_density, 0u, &r[0], &r[1],
-                                            m_last_reduced_density_ms));
-        ReducedHandle hold0(r[0]), hold1(r[1]);
-        FieldVector<double> coeffs[2];
-        FieldVector<std::array<unsigned int, 32>> cells[2];
-        FieldVector<unsigned int> cell_map[2];
-        for (int k = 0; k < 2; k++)           // both copied before anything changes, so a failure leaves the grid as it was
-            take_reduced(r[k], coeffs[k], cells[k], cell_map[k]);
-        if (verbose)
-            std::cout << "Construction: density map sampled and both fields reduced on the GPU in " << m_last_reduced_density_ms[12] << " ms ("
-                      << coeffs[0].size() << " SDF nodes and " << coeffs[1].size() << " density nodes kept)" << std::endl;
-        invalidate();
-        m_nodes[id] = std::move(coeffs[0]); m_cells[id] = std::move(cells[0]); m_cell_map[id] = std::move(cell_map[0]);
-        m_nodes.push_back(std::move(coeffs[1])); m_cells.push_back(std::move(cells[1])); m_cell_map.push_back(std::move(cell_map[1]));
-        keep_reduced(id, hold0);
-        keep_reduced(static_cast<unsigned int>(m_n_fields), hold1);
-        return static_cast<unsigned int>(m_n_fields++);
+        return addReducedNodeMap("addReducedDensityMap", "density", dg_reduced_density_map_create, f.sdf_field_id, f.smoothing_length,
+                                 f.rest_density, m_last_reduced_density_ms, verbose);
+    }
+    // new: the volume map with reduction in one library call (dg_reduced_volume_map_create).  Leaves exactly what
+    //   id = addFunction(f, verbose);  reduceField(f.sdf_field_id, p0);  reduceField(id, p1);
+    // leave, with GenerateDensityMap's p0 (as above) and p1(x, v) = 0 <= v.  The dense volume field never reaches the host.
+    unsigned int addReducedVolumeMap(VolumeMapFunction const& f, bool verbose = false)
+    {
+        if (f.grid != this) throw std::invalid_argument("addReducedVolumeMap: the VolumeMapFunction must sample this grid's own SDF field");
+        if (f.no_reduction) throw std::invalid_argument("addReducedVolumeMap: the VolumeMapFunction has no_reduction set (use addFunction)");
+        return addReducedNodeMap("addReducedVolumeMap", "volume", dg_reduced_volume_map_create, f.sdf_field_id, f.smoothing_length, f.scale,
+                                 m_last_reduced_volume_ms, verbose);
     }
     // appends a field from node values + the closed-form connectivity (:833-886, built on the GPU) + identity cell map (:888-891)
     unsigned int addSampledFunction(FieldVector<double> coeffs)
@@ -443,6 +451,8 @@ public:
     const double* lastReducedBandTimings() const { return m_last_reduced_band_ms; }
     // ms of the last addReducedDensityMap: upload + pack, density; cells, nodes, sort, write-back of field 0 then of field 1; tie paths; total
     const double* lastReducedDensityTimings() const { return m_last_reduced_density_ms; }
+    // ms of the last addReducedVolumeMap, in the same layout ([1] is the volume sampling)
+    const double* lastReducedVolumeTimings() const { return m_last_reduced_volume_ms; }
     // ms of the last addReducedFunction / reduceField(DeviceNodePredicate): positions + callbacks (reduceField: with the upload), cells, nodes,
     // sort, write-back; tie path (1.0 / 0.0); total; inside the callbacks
     const double* lastReducedFunctionTimings() const { return m_last_reduced_function_ms; }
@@ -476,12 +486,41 @@ public:
     }
 
 private:
+    // the shared body of addReducedDensityMap / addReducedVolumeMap: `entry` is the library's one-call route, timings its 13 stage times
+    typedef int (*ReducedNodeMapEntry)(const dg_grid_desc*, const double*, std::uint64_t, const std::uint32_t*, std::uint64_t, const std::uint32_t*,
+                                       double, double, std::uint32_t, dg_reduced_band**, dg_reduced_band**, double*);
+    unsigned int addReducedNodeMap(const char* who, const char* what, ReducedNodeMapEntry entry, unsigned int id, double h, double param,
+                                   double* timings, bool verbose)
+    {
+        if (id >= m_n_fields) throw std::invalid_argument(std::string(who) + ": no SDF field with that id");
+        if (m_cell_map[id].size() != m_n_cells) throw std::invalid_argument(std::string(who) + ": the SDF field's cell map must cover every grid cell");
+        const dg_grid_desc d = desc();
+        dg_reduced_band* r[2] = {nullptr, nullptr};
+        check(entry(&d, m_nodes[id].data(), m_nodes[id].size(), reinterpret_cast<const std::uint32_t*>(m_cells[id].data()), m_cells[id].size(),
+                    m_cell_map[id].data(), h, param, 0u, &r[0], &r[1], timings));
+        ReducedHandle hold0(r[0]), hold1(r[1]);
+        FieldVector<double> coeffs[2];
+        FieldVector<std::array<unsigned int, 32>> cells[2];
+        FieldVector<unsigned int> cell_map[2];
+        for (int k = 0; k < 2; k++)           // both copied before anything changes, so a failure leaves the grid as it was
+            take_reduced(r[k], coeffs[k], cells[k], cell_map[k]);
+        if (verbose)
+            std::cout << "Construction: " << what << " map sampled and both fields reduced on the GPU in " << timings[12] << " ms ("
+                      << coeffs[0].size() << " SDF nodes and " << coeffs[1].size() << " " << what << " nodes kept)" << std::endl;
+        invalidate();
+        m_nodes[id] = std::move(coeffs[0]); m_cells[id] = std::move(cells[0]); m_cell_map[id] = std::move(cell_map[0]);
+        m_nodes.push_back(std::move(coeffs[1])); m_cells.push_back(std::move(cells[1])); m_cell_map.push_back(std::move(cell_map[1]));
+        keep_reduced(id, hold0);
+        keep_reduced(static_cast<unsigned int>(m_n_fields), hold1);
+        return static_cast<unsigned int>(m_n_fields++);
+    }
     std::vector<FieldVector<double>> m_nodes;
     std::vector<FieldVector<std::array<unsigned int, 32>>> m_cells;
     std::vector<FieldVector<unsigned int>> m_cell_map;
     double m_last_add_function_ms[6] = {0, 0, 0, 0, 0, 0};
     double m_last_reduced_band_ms[7] = {0, 0, 0, 0, 0, 0, 0};
     double m_last_reduced_density_ms[13] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+    double m_last_reduced_volume_ms[13] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
     double m_last_reduced_function_ms[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     mutable std::map<unsigned int, dg_field*> m_dev;
     // the handles the reduced calls returned, kept until their field's first deviceField or the next invalidate(): a field made from a

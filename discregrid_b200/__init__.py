@@ -8,11 +8,11 @@ from . import _capi
 from ._capi import DiscregridError, DBL_MAX, LIB_PATH
 from .mesh import TriangleMesh, bumpy_torus, uv_sphere, box
 from .distance import TriangleMeshDistance, MeshSignedDistance, MeshDistanceBand, NearestEntity, Result
-from .grid import (CubicLagrangeDiscreteGrid, DensityMapFunction, DeviceFunction, DeviceNodePredicate, DeviceSamplePredicate, grid_desc,
+from .grid import (CubicLagrangeDiscreteGrid, DensityMapFunction, VolumeMapFunction, DeviceFunction, DeviceNodePredicate, DeviceSamplePredicate, grid_desc,
                    generate_sdf_domain)
 
 __all__ = ["TriangleMesh", "TriangleMeshDistance", "MeshSignedDistance", "MeshDistanceBand", "NearestEntity", "Result",
-           "CubicLagrangeDiscreteGrid", "DensityMapFunction", "DeviceFunction", "DeviceSamplePredicate", "DeviceNodePredicate", "grid_desc",
+           "CubicLagrangeDiscreteGrid", "DensityMapFunction", "VolumeMapFunction", "DeviceFunction", "DeviceSamplePredicate", "DeviceNodePredicate", "grid_desc",
            "generate_sdf_domain", "DiscregridError",
            "DBL_MAX", "LIB_PATH", "bumpy_torus", "uv_sphere", "box"]
 

@@ -111,6 +111,8 @@ SIGNATURES = {
     "dg_density_map": (C.c_int, [_vp, C.c_double, C.c_double, C.c_int, C.c_uint64, C.c_uint64, _dp]),
     "dg_reduce_field": (C.c_int, [_gp, _dp, C.c_uint64, C.POINTER(C.c_uint8), _u32p, C.c_uint64, _u32p, C.c_uint32, _u64p, _u64p, _dp]),
     "dg_density_map_device": (C.c_int, [_vp, C.c_double, C.c_double, C.c_int, C.c_uint64, C.c_uint64, _vp, _vp]),
+    "dg_volume_map": (C.c_int, [_vp, C.c_double, C.c_double, C.c_int, C.c_uint64, C.c_uint64, _dp]),
+    "dg_volume_map_device": (C.c_int, [_vp, C.c_double, C.c_double, C.c_int, C.c_uint64, C.c_uint64, _vp, _vp]),
     "dg_reduced_band_create": (C.c_int, [_vp, _gp, C.c_double, C.c_double, C.c_uint32, C.POINTER(_vp), _dp]),
     "dg_reduced_band_sizes": (C.c_int, [_vp, _u64p, _u64p]),
     "dg_reduced_band_copy": (C.c_int, [_vp, _dp, _u32p, _u32p]),
@@ -125,6 +127,8 @@ SIGNATURES = {
     "dg_field_raycast_device": (C.c_int, [_vp, _vp, _vp, C.c_uint64, C.c_double, C.c_double, C.c_double, _vp, _vp, _vp, _vp]),
     "dg_reduced_density_map_create": (C.c_int, [_gp, _dp, C.c_uint64, _u32p, C.c_uint64, _u32p, C.c_double, C.c_double, C.c_uint32,
                                                  C.POINTER(_vp), C.POINTER(_vp), _dp]),
+    "dg_reduced_volume_map_create": (C.c_int, [_gp, _dp, C.c_uint64, _u32p, C.c_uint64, _u32p, C.c_double, C.c_double, C.c_uint32,
+                                                C.POINTER(_vp), C.POINTER(_vp), _dp]),
     "dg_add_function_device": (C.c_int, [_gp, DEVICE_FUNCTION, _vp, DEVICE_SAMPLE_PREDICATE, _vp, C.c_uint64, _dp, _u32p, _u32p, _dp]),
     "dg_reduced_function_create": (C.c_int, [_gp, DEVICE_FUNCTION, _vp, DEVICE_SAMPLE_PREDICATE, _vp, DEVICE_NODE_PREDICATE, _vp, C.c_uint64,
                                               C.c_uint32, C.POINTER(_vp), _dp]),

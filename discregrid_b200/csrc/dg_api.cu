@@ -1849,6 +1849,40 @@ int dg_density_map(const dg_field* f, double h, double rho0, int no_reduction, u
     return DG_OK;
 }
 
+// the volume map's arguments: h finite and > 0 (c1 = 0.5 * (-inf + inf) would make every offset NaN), scale finite
+static const char* volume_args_invalid(double h, double scale)
+{
+    if (!(h > 0.0) || !std::isfinite(h)) return "smoothing length must be finite and > 0";
+    if (!std::isfinite(scale)) return "scale must be finite";
+    return nullptr;
+}
+
+int dg_volume_map_device(const dg_field* f, double h, double scale, int no_reduction, uint64_t l_begin, uint64_t l_end, double* d_out,
+                         void* stream)
+{
+    if (!f) return fail(DG_ERR_INVALID, "dg_volume_map: field is NULL");
+    GridDev g;
+    if (int rc = check_range(&f->desc, l_begin, l_end, g, "dg_volume_map")) return rc;
+    if (const char* why = volume_args_invalid(h, scale)) return fail(DG_ERR_INVALID, "dg_volume_map: %s", why);
+    if (l_end > l_begin && !d_out) return fail(DG_ERR_INVALID, "dg_volume_map: output is NULL");
+    if (int rc = check_handle_device(f->device, "dg_volume_map")) return rc;
+    DG_LAUNCH(k3_launch_volume(f->dev, h, scale, no_reduction, l_begin, l_end - l_begin, d_out, (cudaStream_t)stream));
+    return DG_OK;
+}
+
+int dg_volume_map(const dg_field* f, double h, double scale, int no_reduction, uint64_t l_begin, uint64_t l_end, double* out_host)
+{
+    if (!f) return fail(DG_ERR_INVALID, "dg_volume_map: field is NULL");
+    if (l_end < l_begin) return fail(DG_ERR_INVALID, "dg_volume_map: bad range");
+    const uint64_t n = l_end - l_begin;
+    if (n && !out_host) return fail(DG_ERR_INVALID, "dg_volume_map: output is NULL");
+    DevBuf<double> d_out;
+    DG_CUDA(d_out.alloc(n));
+    if (int rc = dg_volume_map_device(f, h, scale, no_reduction, l_begin, l_end, d_out.p, nullptr)) return rc;
+    if (n) DG_CUDA(cudaMemcpy(out_host, d_out.p, n * sizeof(double), cudaMemcpyDeviceToHost));
+    return DG_OK;
+}
+
 // reduceField with its index passes on the GPU (k4_reduce.cu); the swap-walk compaction and the tie-order-preserving sort stay on the host
 static int reduce_field_gpu(const GridDev& g, double* nodes, uint64_t n_nodes, const uint8_t* keep_node, uint32_t* cells, uint64_t n_cells_in,
                             uint32_t* cell_map, uint64_t n_cells_grid, bool force_std_sort, ReduceStats& st)
@@ -2118,13 +2152,23 @@ static int reduced_band_create_impl(const dg_mesh* m, const dg_grid_desc* grid, 
     return DG_OK;
 }
 
-// GenerateDensityMap with reduction (cmd/generate_density_map/main.cpp:117-147) on one GPU: K3 on the uploaded SDF field, then reduceField
-// of the SDF field over its own rows and of the density field over the closed-form rows, each with the tool's predicate.
-static int reduced_density_map_create_impl(const dg_grid_desc* grid, const double* sdf_nodes, uint64_t n_nodes, const uint32_t* sdf_cells,
-                                           uint64_t n_cells, const uint32_t* sdf_cell_map, double h, double rho0, uint32_t flags,
-                                           dg_reduced_band** sdf_out, dg_reduced_band** density_out, double* timings_ms)
+// What a reduced node map (GenerateDensityMap's pattern) takes from its node function: the entry point's name, the check of its
+// arguments (nullptr when they are valid), the K3 kernel that samples every node with the sample predicate on, and field 1's predicate.
+struct ReducedNodeMap {
+    const char* who;
+    const char* (*args_invalid)(double h, double param);
+    cudaError_t (*launch)(const dg_field& f, double h, double param, uint64_t n, double* d_out, cudaStream_t st);
+    K4ValuePred keep1;
+};
+
+// GenerateDensityMap with reduction (cmd/generate_density_map/main.cpp:117-147) on one GPU, for the density map and the volume map: the node
+// function (K3) on the uploaded SDF field, then reduceField of the SDF field over its own rows with the tool's predicate, and of the new
+// field over the closed-form rows with m.keep1.
+static int reduced_node_map_create_impl(const ReducedNodeMap& m, const dg_grid_desc* grid, const double* sdf_nodes, uint64_t n_nodes,
+                                        const uint32_t* sdf_cells, uint64_t n_cells, const uint32_t* sdf_cell_map, double h, double param,
+                                        uint32_t flags, dg_reduced_band** sdf_out, dg_reduced_band** density_out, double* timings_ms)
 {
-    static const char* who = "dg_reduced_density_map_create";
+    const char* who = m.who;
     if (!sdf_out || !density_out) return fail(DG_ERR_INVALID, "%s: out is NULL", who);
     *sdf_out = nullptr; *density_out = nullptr;
     GridDev g; const char* why = "";
@@ -2136,14 +2180,14 @@ static int reduced_density_map_create_impl(const dg_grid_desc* grid, const doubl
         return fail(DG_ERR_INVALID, "%s: the SDF field has %llu nodes, the grid %llu (already reduced?)", who, (unsigned long long)n_nodes,
                     (unsigned long long)n);
     if (n_cells > n_grid_cells) return fail(DG_ERR_INVALID, "%s: more cells than the grid has", who);
-    if (!(h > 0.0)) return fail(DG_ERR_INVALID, "%s: smoothing length must be > 0", who);
+    if (const char* why = m.args_invalid(h, param)) return fail(DG_ERR_INVALID, "%s: %s", who, why);
     if (flags & ~DG_REDUCE_REFERENCE_SORT) return fail(DG_ERR_INVALID, "%s: unknown flags 0x%x (only DG_REDUCE_REFERENCE_SORT)", who, flags);
     if (int rc = require_device()) return rc;
     if (int rc = ensure_selftest()) return rc;
-    // the tool's predicates (main.cpp:139-140) with their bounds computed as its lambdas compute them
+    // the tool's SDF predicate (main.cpp:139) with its bounds computed as its lambda computes them
     const double cell_diag = k3_cell_diag(g);
     const K4ValuePred sdf_pred{K4_KEEP_SDF, -6.0 * h, 2.0 * h, cell_diag};
-    const K4ValuePred density_pred{K4_KEEP_RANGE, 0.0, 3.0 * rho0, 0.0};
+    const K4ValuePred density_pred = m.keep1;
     const bool reference_sort = (flags & DG_REDUCE_REFERENCE_SORT) != 0;
     StageClock clock;
     const auto t_start = clock.t0;
@@ -2182,9 +2226,9 @@ static int reduced_density_map_create_impl(const dg_grid_desc* grid, const doubl
     if (int rc = field_finish(f.get(), d_sdf.p, d_cells.p, st)) return rc;
     DG_CUDA(cudaStreamSynchronize(st));
     ms[0] += clock.lap();
-    // ---- 2. addFunction(density_func, verbose, pred) (main.cpp:96-133): K3 over every node, predicate on
+    // ---- 2. addFunction(node_func, verbose, pred) (main.cpp:96-133): K3 over every node, predicate on
     DG_CUDA(d_density.alloc(n));
-    DG_LAUNCH(k3_launch_density(f->dev, f->coeff_max, h, rho0, 0, 0, n, d_density.p, st));
+    DG_LAUNCH(m.launch(*f, h, param, n, d_density.p, st));
     DG_CUDA(cudaStreamSynchronize(st));
     ms[1] = clock.lap();
     // ---- 3. the packed SDF field is not needed any more: free it before reducing anything
@@ -2193,7 +2237,7 @@ static int reduced_density_map_create_impl(const dg_grid_desc* grid, const doubl
     if (int rc = device_reduce(g, d_sdf.p, n, DenseRows{d_cells.p, n_cells}, d_cell_keep0.p, n_grid_cells, reference_sort, *r0, ms + 2, tie[0], clock, st))
         return rc;
     d_cell_keep0.release(); d_cells.release(); d_sdf.release();
-    // ---- 5. reduceField(1, 0 <= v && v <= 3 rho0) over the closed-form rows of the density field (addSampledFunction's cells, identity map)
+    // ---- 5. reduceField(1, keep1) over the closed-form rows of the new field (addSampledFunction's cells, identity map)
     {
         const DenseRows rows1{nullptr, n_grid_cells};
         DevBuf<unsigned char> d_cell_keep1;
@@ -2728,8 +2772,30 @@ int dg_reduced_density_map_create(const dg_grid_desc* grid, const double* sdf_no
                                   const uint32_t* sdf_cell_map, double h, double rho0, uint32_t flags, dg_reduced_band** sdf_out,
                                   dg_reduced_band** density_out, double* timings_ms)
 {
+    // GenerateDensityMap's second predicate, 0 <= v && v <= 3 rho0 (main.cpp:140)
+    const ReducedNodeMap m{"dg_reduced_density_map_create",
+                           [](double h_, double) -> const char* { return (h_ > 0.0) ? nullptr : "smoothing length must be > 0"; },
+                           [](const dg_field& f, double h_, double rho0_, uint64_t n, double* d_out, cudaStream_t st) {
+                               return k3_launch_density(f.dev, f.coeff_max, h_, rho0_, 0, 0, n, d_out, st);
+                           },
+                           K4ValuePred{K4_KEEP_RANGE, 0.0, 3.0 * rho0, 0.0}};
     return guarded("dg_reduced_density_map_create", [&]() {
-        return reduced_density_map_create_impl(grid, sdf_nodes, n_nodes, sdf_cells, n_cells, sdf_cell_map, h, rho0, flags, sdf_out, density_out, timings_ms);
+        return reduced_node_map_create_impl(m, grid, sdf_nodes, n_nodes, sdf_cells, n_cells, sdf_cell_map, h, rho0, flags, sdf_out, density_out, timings_ms);
+    });
+}
+
+int dg_reduced_volume_map_create(const dg_grid_desc* grid, const double* sdf_nodes, uint64_t n_nodes, const uint32_t* sdf_cells, uint64_t n_cells,
+                                 const uint32_t* sdf_cell_map, double h, double scale, uint32_t flags, dg_reduced_band** sdf_out,
+                                 dg_reduced_band** volume_out, double* timings_ms)
+{
+    // the volume field keeps 0 <= v (and != DBL_MAX, as every reduceField): K4_KEEP_RANGE with b = +inf
+    const ReducedNodeMap m{"dg_reduced_volume_map_create", volume_args_invalid,
+                           [](const dg_field& f, double h_, double scale_, uint64_t n, double* d_out, cudaStream_t st) {
+                               return k3_launch_volume(f.dev, h_, scale_, 0, 0, n, d_out, st);
+                           },
+                           K4ValuePred{K4_KEEP_RANGE, 0.0, INFINITY, 0.0}};
+    return guarded("dg_reduced_volume_map_create", [&]() {
+        return reduced_node_map_create_impl(m, grid, sdf_nodes, n_nodes, sdf_cells, n_cells, sdf_cell_map, h, scale, flags, sdf_out, volume_out, timings_ms);
     });
 }
 

@@ -296,4 +296,140 @@ cudaError_t k3_launch_density(const FieldDev& f, double coeff_max, double h, dou
 #endif
 }
 
+// ================================================================================================ volume map
+// The volume map of Bender et al. 2019 ("Volume Maps: An Implicit Boundary Representation for SPH", MIG 2019), in 3D and in fp64, as
+// SPlisHSPlasH generates it with Discregrid's addFunction over an SDF grid.  The reference has no volume map; this is the library's contract,
+// written in the reference's own building blocks (DESIGN section 3, "Volume map"):
+//   d(y)           : interpolate(sdf, y), the bits of interp_value above (DBL_MAX outside the domain, in a removed cell, or where a
+//                    coefficient is missing)
+//   pred(x)        : GenerateDensityMap's sample predicate (main.cpp:119-133), unless no_reduction: clamp x into the domain,
+//                    dd = d(clamp(x)); reject (DBL_MAX, :817) if dd == DBL_MAX, else keep iff -6h < dd + cell_diag && dd - cell_diag < 2h
+//   volume(x)      : 0.0 if d(x) > (1.0 + 1.0) * h, else s * GaussQuadrature::integrate(g, [-h, h]^3, p = 30) with the order of
+//                    gauss_quadrature.cpp:5927-5960: 16^3 points, i outermost, res += wijk * g(c0 * xi + c1), res *= c0.prod()
+//   g(xi)          : 0.0 if (xi.x^2 + xi.y^2) + xi.z^2 > h * h (Eigen's squaredNorm; d is not evaluated), else gamma(d(x + xi)) with
+//                    x + xi formed per component, as K3's x + off[i]
+//   gamma(delta)   : 1.0 if delta <= 0; W((delta, 0, 0)) / W_zero if delta < h; 0.0 otherwise (DBL_MAX and NaN included).  W is
+//                    sph_kernel.hpp:22-42's CubicKernel with radius h, W_zero = W(0) = k.
+// Two consequences the kernel uses:
+//   * The skip is exact.  The reference returns 0.0 for an offset outside the ball without interpolating, and wijk * 0.0 = +0 leaves
+//     the accumulator (which starts at +0) unchanged whatever it holds.  So the points outside the ball are simply not visited; no
+//     bound on the coefficients like K3's SKIP_ZERO_W is needed.
+//   * The ball test, the offsets and wijk = (wi * wj) * wk depend on h alone.  The host tabulates the points inside the ball once per
+//     call, in quadrature order (1008 of 4096 at h = 1; rounding at the sphere can change the count with h, so it is not a constant),
+//     and the kernel walks that flat list with no branch on the ball.  All 32 lanes of a warp read the same entry at each step.
+// rl = sqrt((delta * delta + 0 * 0) + 0 * 0) is sqrt(delta * delta): delta * delta >= +0, and adding +0 to it changes no bit.
+
+namespace {
+
+struct VolumeParams {
+    double h, two_h, six_h_neg, scale, c0prod, cell_diag, k, w_zero;
+};
+
+#ifndef K3V_MIN_BLOCKS
+#define K3V_MIN_BLOCKS 5           // blocks of 128 threads per SM the register allocation must allow; ptxas for sm_90a: see DESIGN section 4
+#endif
+__global__ void __launch_bounds__(128, K3V_MIN_BLOCKS)
+volume_map_kernel(FieldDev f, VolumeParams vp, const double2* __restrict__ pts, unsigned n_pts, int no_reduction, unsigned l_begin,
+                  unsigned long long count, double* __restrict__ out)
+{
+    const unsigned long long idx = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= count) return;
+    double x, y, z;
+    node_position(f.g, l_begin + (unsigned)idx, x, y, z);
+    if (!no_reduction) {                                            // GenerateDensityMap's predicate, main.cpp:119-133
+        const double cx = fmin(fmax(x, f.g.mn[0]), f.g.mx[0]);
+        const double cy = fmin(fmax(y, f.g.mn[1]), f.g.mx[1]);
+        const double cz = fmin(fmax(z, f.g.mn[2]), f.g.mx[2]);
+        const double d = interp_value(f, cx, cy, cz);
+        const bool keep = (d != DBL_MAX) && (vp.six_h_neg < d + vp.cell_diag) && (d - vp.cell_diag < vp.two_h);
+        if (!keep) { out[idx] = DBL_MAX; return; }
+    }
+    const double dist = interp_value(f, x, y, z);
+    if (dist > vp.two_h) { out[idx] = 0.0; return; }
+    double res = 0.0;
+#pragma unroll 1
+    for (unsigned p = 0; p < n_pts; p++) {
+        const double2 a = __ldg(pts + 2 * p), b = __ldg(pts + 2 * p + 1);    // (xi.x, xi.y), (xi.z, wijk)
+        const double d = interp_value(f, x + a.x, y + a.y, z + b.x);
+        double gam = 0.0;
+        if (d <= 0.0) gam = 1.0;
+        else if (d < vp.h) {                                        // W((d, 0, 0)) / W_zero, sph_kernel.hpp:22-42
+            const double rl = sqrt(d * d);
+            const double q = rl / vp.h;
+            double W = 0.0;
+            if (q <= 1.0) {
+                if (q <= 0.5) { const double q2 = q * q, q3 = q2 * q; W = vp.k * (6.0 * q3 - 6.0 * q2 + 1.0); }
+                else { const double m = 1.0 - q; W = vp.k * (2.0 * m * m * m); }
+            }
+            gam = W / vp.w_zero;
+        }
+        res = res + b.y * gam;                                      // gauss_quadrature.cpp:5954
+    }
+    res = res * vp.c0prod;                                          // :5958
+    out[idx] = vp.scale * res;
+}
+
+}  // namespace
+
+// The points of the 16^3 rule inside the ball of radius h, in quadrature order: (xi.x, xi.y, xi.z, wijk) each.  Host arithmetic without
+// contraction, with the reference's expressions (gauss_quadrature.cpp:5937-5954, Eigen's squaredNorm (a0 + a1) + a2).
+std::vector<double> k3_volume_points(double h)
+{
+    const double lo = -h, hi = h;
+    const double c0 = 0.5 * (hi - lo), c1 = 0.5 * (lo + hi);
+    double off[16];
+    for (int i = 0; i < 16; i++) off[i] = c0 * GA16[i] + c1;
+    const double hh = h * h;
+    std::vector<double> pts;
+    pts.reserve(4 * 1100);
+    for (int i = 0; i < 16; i++) {
+        const double wi = GW16[i];
+        for (int j = 0; j < 16; j++) {
+            const double wij = wi * GW16[j];
+            for (int k = 0; k < 16; k++) {
+                const double wijk = wij * GW16[k];
+                if ((off[i] * off[i] + off[j] * off[j]) + off[k] * off[k] > hh) continue;
+                pts.push_back(off[i]); pts.push_back(off[j]); pts.push_back(off[k]); pts.push_back(wijk);
+            }
+        }
+    }
+    return pts;
+}
+
+cudaError_t k3_launch_volume(const FieldDev& f, double h, double scale, int no_reduction, uint64_t l_begin, uint64_t count, double* d_out,
+                             cudaStream_t stream)
+{
+    if (count == 0) return cudaSuccess;
+    const std::vector<double> pts = k3_volume_points(h);
+    const unsigned n_pts = (unsigned)(pts.size() / 4);
+    VolumeParams vp;
+    const double c0 = 0.5 * (h - (-h));
+    vp.h = h; vp.two_h = (1.0 + 1.0) * h; vp.six_h_neg = -6.0 * h; vp.scale = scale;
+    vp.c0prod = c0 * c0 * c0;                                       // Eigen prod(): (c0*c0)*c0
+    vp.cell_diag = k3_cell_diag(f.g);
+    // CubicKernel::setRadius (sph_kernel.hpp:10-20): k = 8/(pi h^3), W_zero = W(0) = k * (6*0 - 6*0 + 1)
+    const double pi = static_cast<double>(M_PI);
+    const double h3 = h * h * h;
+    vp.k = 8.0 / (pi * h3);
+    vp.w_zero = vp.k * (6.0 * 0.0 - 6.0 * 0.0 + 1.0);
+    const unsigned blocks = (unsigned)((count + 127) / 128);
+    const double2* h_pts = reinterpret_cast<const double2*>(pts.data());
+#ifdef DG_EMU
+    DG_KERNEL_LAUNCH(volume_map_kernel, blocks, 128, 0, stream, f, vp, h_pts, n_pts, no_reduction, (unsigned)l_begin, (unsigned long long)count, d_out);
+    return cudaSuccess;
+#else
+    const size_t bytes = pts.size() * sizeof(double);
+    double2* d_pts = nullptr;
+    cudaError_t e = cudaMallocAsync(reinterpret_cast<void**>(&d_pts), bytes ? bytes : sizeof(double2), stream);
+    if (e != cudaSuccess) return e;
+    if (bytes) e = cudaMemcpyAsync(d_pts, h_pts, bytes, cudaMemcpyHostToDevice, stream);   // pageable: staged before the call returns
+    if (e == cudaSuccess) {
+        DG_KERNEL_LAUNCH(volume_map_kernel, blocks, 128, 0, stream, f, vp, d_pts, n_pts, no_reduction, (unsigned)l_begin, (unsigned long long)count, d_out);
+        e = DG_AFTER_LAUNCH();
+    }
+    cudaFreeAsync(d_pts, stream);
+    return e;
+#endif
+}
+
 }  // namespace dgb

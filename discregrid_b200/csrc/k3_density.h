@@ -1,6 +1,7 @@
 // Launch interface of the K3 kernel (k3_density.cu): GenerateDensityMap's per-node function.
 #pragma once
 #include <cstdint>
+#include <vector>
 #include <cuda_runtime.h>
 #include "k2_interp.h"
 
@@ -12,4 +13,10 @@ cudaError_t k3_coeff_max(const double* d_packed, uint64_t n, double* out, cudaSt
 // coeff_max: k3_coeff_max of f's packed coefficients (it decides whether points outside the kernel support may be skipped)
 cudaError_t k3_launch_density(const FieldDev& f, double coeff_max, double h, double rho0, int no_reduction, uint64_t l_begin,
                               uint64_t count, double* d_out, cudaStream_t stream);
+// the volume map (contract in k3_density.cu): scale * the quadrature of the inside indicator over the ball of radius h, per node.
+// h finite and > 0, scale finite: the caller's to check
+cudaError_t k3_launch_volume(const FieldDev& f, double h, double scale, int no_reduction, uint64_t l_begin, uint64_t count, double* d_out,
+                             cudaStream_t stream);
+// the volume map's quadrature points inside the ball of radius h, in quadrature order: (xi.x, xi.y, xi.z, wijk) per point
+std::vector<double> k3_volume_points(double h);
 }

@@ -13,6 +13,8 @@ that save()/load() stay byte-compatible with the reference's .cdf/.cdm files
   addFunction(DensityMapFunction, pred)  -> dg_density_map       (K3, csrc/k3_density.cu)
   addReducedDensityMap(DensityMapFunction)
                                          -> dg_reduced_density_map_create (K3, then both of GenerateDensityMap's reduceField calls, on the GPU)
+  addFunction(VolumeMapFunction)         -> dg_volume_map        (K3's volume-map kernel: SPH boundary volumes, not in the reference)
+  addReducedVolumeMap(VolumeMapFunction) -> dg_reduced_volume_map_create (the volume map, then reduceField(0, p0) and reduceField(id, 0 <= v))
   addFunction(DeviceFunction, pred=DeviceSamplePredicate)
                                          -> dg_add_function_device (your torch code on batches of node positions made on the GPU)
   reduceField(field_id, DeviceNodePredicate)
@@ -49,6 +51,15 @@ class DensityMapFunction:
 
     def __init__(self, sdf_field_id=0, smoothing_length=0.1, rest_density=1000.0, no_reduction=False):
         self.field_id, self.h, self.rho0, self.no_reduction = sdf_field_id, float(smoothing_length), float(rest_density), bool(no_reduction)
+
+
+class VolumeMapFunction:
+    """The volume map of Bender et al. 2019 (SPlisHSPlasH's boundary representation) as a recognisable function for addFunction:
+    scale * the 16^3-point Gauss quadrature of an inside indicator gamma(d(x + xi)) over the ball |xi| <= h, on the SDF in field
+    `sdf_field_id`, with GenerateDensityMap's sample predicate unless no_reduction (contract: DESIGN section 3, "Volume map")."""
+
+    def __init__(self, sdf_field_id=0, smoothing_length=0.1, scale=0.8, no_reduction=False):
+        self.field_id, self.h, self.scale, self.no_reduction = sdf_field_id, float(smoothing_length), float(scale), bool(no_reduction)
 
 
 class DeviceFunction:
@@ -400,8 +411,12 @@ class CubicLagrangeDiscreteGrid:
             coeffs = np.empty(self.nNodes())
             capi.check(capi.lib.dg_density_map(self._device_field(func.field_id), func.h, func.rho0, int(func.no_reduction), 0,
                                                len(coeffs), capi.ptr(coeffs, capi.F64P)))
+        elif isinstance(func, VolumeMapFunction):
+            coeffs = np.empty(self.nNodes())
+            capi.check(capi.lib.dg_volume_map(self._device_field(func.field_id), func.h, func.scale, int(func.no_reduction), 0,
+                                              len(coeffs), capi.ptr(coeffs, capi.F64P)))
         else:
-            raise TypeError("addFunction runs on the GPU and only accepts MeshSignedDistance, DensityMapFunction or DeviceFunction; "
+            raise TypeError("addFunction runs on the GPU and only accepts MeshSignedDistance, DensityMapFunction, VolumeMapFunction or DeviceFunction; "
                             "wrap a function of your own that runs on the GPU (e.g. torch operations) in DeviceFunction")
         return self.addSampledFunction(coeffs)
 
@@ -462,17 +477,33 @@ class CubicLagrangeDiscreteGrid:
             raise TypeError("addReducedDensityMap takes a DensityMapFunction")
         if func.no_reduction:
             raise TypeError("addReducedDensityMap: the DensityMapFunction has no_reduction set (use addFunction)")
-        fid = func.field_id
+        self.last_reduced_density_ms = np.zeros(13)
+        return self._add_reduced_node_map("addReducedDensityMap", capi.lib.dg_reduced_density_map_create, func.field_id, func.h, func.rho0,
+                                          self.last_reduced_density_ms)
+
+    def addReducedVolumeMap(self, func):
+        """The volume map with reduction in one GPU call (dg_reduced_volume_map_create): leaves exactly what addFunction(func) followed by
+        reduceField(func.field_id, p0) and reduceField(new_id, p1) leave, with GenerateDensityMap's p0 (as in addReducedDensityMap) and
+        p1(x, v) = 0 <= v.  The SDF field is replaced by its reduction and the reduced volume field is appended; the dense volume field never
+        reaches the host.  Returns the new field id.  The device copies of both results are kept for the fields' first interpolate."""
+        if not isinstance(func, VolumeMapFunction):
+            raise TypeError("addReducedVolumeMap takes a VolumeMapFunction")
+        if func.no_reduction:
+            raise TypeError("addReducedVolumeMap: the VolumeMapFunction has no_reduction set (use addFunction)")
+        self.last_reduced_volume_ms = np.zeros(13)
+        return self._add_reduced_node_map("addReducedVolumeMap", capi.lib.dg_reduced_volume_map_create, func.field_id, func.h, func.scale,
+                                          self.last_reduced_volume_ms)
+
+    def _add_reduced_node_map(self, who, entry, fid, h, param, timings):
+        """the shared body of addReducedDensityMap / addReducedVolumeMap: `entry` is the library's one-call route"""
         nodes = np.ascontiguousarray(self.m_nodes[fid], np.float64)
         cells = np.ascontiguousarray(self.m_cells[fid], np.uint32)
         cmap = np.ascontiguousarray(self.m_cell_map[fid], np.uint32)
         if len(cmap) != self.m_n_cells:
-            raise ValueError("addReducedDensityMap: the SDF field's cell map must cover every grid cell")
+            raise ValueError(f"{who}: the SDF field's cell map must cover every grid cell")
         r = (C.c_void_p(), C.c_void_p())
-        self.last_reduced_density_ms = np.zeros(13)
-        capi.check(capi.lib.dg_reduced_density_map_create(C.byref(self._desc), capi.ptr(nodes, capi.F64P), len(nodes), capi.ptr(cells, capi.U32P),
-                                                          len(cells), capi.ptr(cmap, capi.U32P), func.h, func.rho0, 0, C.byref(r[0]), C.byref(r[1]),
-                                                          capi.ptr(self.last_reduced_density_ms, capi.F64P)))
+        capi.check(entry(C.byref(self._desc), capi.ptr(nodes, capi.F64P), len(nodes), capi.ptr(cells, capi.U32P), len(cells),
+                         capi.ptr(cmap, capi.U32P), h, param, 0, C.byref(r[0]), C.byref(r[1]), capi.ptr(timings, capi.F64P)))
         out = _copy_kept(r, self.m_n_cells)
         self._invalidate()
         self.m_nodes[fid], self.m_cells[fid], self.m_cell_map[fid] = out[0]

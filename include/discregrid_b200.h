@@ -300,6 +300,19 @@ DG_API int dg_density_map(const dg_field* sdf, double h, double rho0, int no_red
 DG_API int dg_density_map_device(const dg_field* sdf, double h, double rho0, int no_reduction, uint64_t l_begin, uint64_t l_end,
                           double* d_out, void* stream);
 
+/* ---- K3: volume map (Bender et al. 2019, "Volume Maps: An Implicit Boundary Representation for SPH"; not in the reference) ----------
+ * The SPH boundary volume of an SDF, as SPlisHSPlasH builds it with addFunction over the SDF grid, in 3D and in fp64, over nodes
+ * [l_begin, l_end) of the grid of `sdf` (any field: dense or reduced).  With d(y) = interpolate(sdf, y):
+ *   out = DBL_MAX where GenerateDensityMap's sample predicate rejects the node (unless no_reduction), 0 where d(x) > 2h, else
+ *   scale * GaussQuadrature::integrate(g, [-h, h]^3, p = 30) (16^3 points, the reference's order), with g(xi) = 0 outside the ball
+ *   |xi| <= h and gamma(d(x + xi)) inside it; gamma(t) = 1 for t <= 0, W((t, 0, 0)) / W(0) for t < h (CubicKernel, radius h), 0 otherwise
+ *   (DBL_MAX and NaN included).
+ * The full contract is in k3_density.cu and DESIGN section 3.  h must be finite and > 0 and scale finite (else DG_ERR_INVALID), the range
+ * inside the grid's nodes, out non-NULL when the range is not empty.  The _device form writes d_out on `stream` and returns at once. */
+DG_API int dg_volume_map(const dg_field* sdf, double h, double scale, int no_reduction, uint64_t l_begin, uint64_t l_end, double* out_host);
+DG_API int dg_volume_map_device(const dg_field* sdf, double h, double scale, int no_reduction, uint64_t l_begin, uint64_t l_end,
+                                double* d_out, void* stream);
+
 /* ---- reduceField (SURVEY 8f, N3) -------------------------------------------------------------------
  * replaces the body of CubicLagrangeDiscreteGrid::reduceField (cubic_lagrange_discrete_grid.cpp:1065-1174) after the predicate has
  * been evaluated: keep_node[l] != 0 <=> pred(x_l, c_l) && c_l != DBL_MAX (:1069-1074).  Rewrites IN PLACE, exactly as the
@@ -411,6 +424,17 @@ DG_API int dg_reduced_density_map_create(const dg_grid_desc* grid, const double*
                                          const uint32_t* sdf_cells, uint64_t n_cells, const uint32_t* sdf_cell_map,
                                          double h, double rho0, uint32_t flags,
                                          dg_reduced_band** sdf_out, dg_reduced_band** density_out, double* timings_ms);
+
+/* ---- reduced volume map: the volume map with reduction in one call ------------------------------------------------------------------
+ * What a volume-map generator that reduces its fields as GenerateDensityMap does leaves, in one call:
+ *   id = addFunction(volume_func, verbose, pred);  reduceField(0, p0);  reduceField(id, p1);
+ * with volume_func and pred those of dg_volume_map (no_reduction = 0), p0 GenerateDensityMap's (above) and p1(x, v) = 0 <= v (which,
+ * as in every reduceField, also drops DBL_MAX).  Arguments, outputs, rules and timings_ms (13 doubles; [1] is the volume sampling) are
+ * those of dg_reduced_density_map_create, with scale in place of rho0: h finite and > 0, scale finite, else DG_ERR_INVALID. */
+DG_API int dg_reduced_volume_map_create(const dg_grid_desc* grid, const double* sdf_nodes, uint64_t n_nodes,
+                                        const uint32_t* sdf_cells, uint64_t n_cells, const uint32_t* sdf_cell_map,
+                                        double h, double scale, uint32_t flags,
+                                        dg_reduced_band** sdf_out, dg_reduced_band** volume_out, double* timings_ms);
 
 /* ---- user functions on the GPU: addFunction(func, verbose, pred) and reduceField(id, pred) with batched device callbacks ----------------
  * The reference's addFunction and reduceField take any callable.  These entry points take the caller's OWN GPU code instead, as batched

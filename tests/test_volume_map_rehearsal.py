@@ -1,0 +1,24 @@
+"""tests/test_gpu_volume_map.py rehearsed on the CPU: the volume-map GPU tests (C-ABI, Python methods, GenerateVolumeMap and the
+reference-side generator on the fixtures, the oracle on dense, reduced and non-finite SDFs) run against build/bin/libdgemu.so -- the whole
+library with every kernel emulated (tests/emu) -- so that their Python- and tool-level logic is checked without a GPU.  The CUDA-tensor
+route and the full-size bunny runs are left to the GPU."""
+import os
+import subprocess
+import sys
+
+import pytest
+
+from conftest import ROOT
+
+EMU = os.path.join(ROOT, "build", "bin", "libdgemu.so")
+
+
+def test_gpu_volume_map_tests_pass_on_the_emulated_library():
+    if not os.path.exists(EMU):
+        pytest.skip("build/bin/libdgemu.so not built (make cpp)")
+    env = dict(os.environ, DISCREGRID_B200_LIB=EMU, LD_PRELOAD=EMU, DG_ALLOW_EMULATED_LIBRARY="1")
+    r = subprocess.run([sys.executable, "-m", "pytest", "-m", "gpu", "-q", "-x", "-k", "not full_size and not tensor", "-p", "no:cacheprovider",
+                        "tests/test_gpu_volume_map.py"], cwd=ROOT, env=env, capture_output=True, text=True, timeout=1500)
+    tail = (r.stdout + r.stderr)[-3000:]
+    assert r.returncode == 0, tail
+    assert " passed" in r.stdout and "failed" not in r.stdout, tail
