@@ -130,6 +130,24 @@ public:
         require();
         if (dg_mesh_winding_number(m_mesh, points, n, beta, w) != DG_OK) throw std::runtime_error(std::string("TriangleMeshDistance: ") + dg_last_error());
     }
+    // new: the first hit of n rays (origins, directions: xyzxyz) on the triangles, t in [t_min, t_max] (a segment x0 -> x1 is the ray
+    // (x0, x1 - x0) on [0, 1]); outputs t, triangle_id, barycentric (3 per ray; may be NULL) and status = DG_RAY_MISS / DG_RAY_ENTER /
+    // DG_RAY_LEAVE, all n (dg_mesh_raycast; contract in k9_mesh_raycast.cu).  Runs on the mesh's GPU, also after useGpus(n > 1).
+    void raycast(size_t n, const double* origins, const double* directions, double t_min, double t_max, double* t, int32_t* triangle_id,
+                 double* barycentric, int32_t* status) const
+    {
+        require();
+        if (dg_mesh_raycast(m_mesh, origins, directions, n, t_min, t_max, t, triangle_id, barycentric, status) != DG_OK)
+            throw std::runtime_error(std::string("TriangleMeshDistance: ") + dg_last_error());
+    }
+    // the same on arrays in the mesh's device memory, asynchronous on `stream` (cudaStream_t)
+    void raycast(size_t n, const double* d_origins, const double* d_directions, double t_min, double t_max, double* d_t, int32_t* d_triangle_id,
+                 double* d_barycentric, int32_t* d_status, void* stream) const
+    {
+        require();
+        if (dg_mesh_raycast_device(m_mesh, d_origins, d_directions, n, t_min, t_max, d_t, d_triangle_id, d_barycentric, d_status, stream) != DG_OK)
+            throw std::runtime_error(std::string("TriangleMeshDistance: ") + dg_last_error());
+    }
 
 private:
     dg_mesh* m_mesh = nullptr;

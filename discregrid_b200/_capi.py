@@ -79,6 +79,8 @@ SIGNATURES = {
     "dg_mesh_winding_number_device": (C.c_int, [_vp, _vp, C.c_uint64, C.c_double, _vp, _vp]),
     "dg_mesh_refit": (C.c_int, [_vp, _dp, C.c_uint64]),
     "dg_mesh_refit_device": (C.c_int, [_vp, _vp, C.c_uint64, _vp]),
+    "dg_mesh_raycast": (C.c_int, [_vp, _dp, _dp, C.c_uint64, C.c_double, C.c_double, _dp, _i32p, _dp, _i32p]),
+    "dg_mesh_raycast_device": (C.c_int, [_vp, _vp, _vp, C.c_uint64, C.c_double, C.c_double, _vp, _vp, _vp, _vp, _vp]),
     "dg_mesh_distance": (C.c_int, [_vp, _dp, C.c_uint64, C.c_int, _dp, _dp, _i32p, _i32p]),
     "dg_mesh_distance_device": (C.c_int, [_vp, _vp, C.c_uint64, C.c_int, _vp, _vp, _vp, _vp, _vp]),
     "dg_sample_sdf": (C.c_int, [_vp, _gp, C.c_double, C.c_uint64, C.c_uint64, _dp]),

@@ -44,6 +44,7 @@
 #include "k6_isosurface.h"
 #include "k7_raycast.h"
 #include "k8_refit.h"
+#include "k9_mesh_raycast.h"
 #include "reduce_field.h"
 #include "obj_reader.h"
 
@@ -2702,6 +2703,68 @@ int dg_field_raycast(const dg_field* f, const double* o, const double* d, uint64
                      double* t_hi, int32_t* status)
 {
     return guarded("dg_field_raycast", [&]() { return raycast_host_impl(f, o, d, n, iso, t_min, t_max, t_lo, t_hi, status); });
+}
+
+// ------------------------------------------------------------------------------------------------ K9: ray casts on a mesh
+static int mesh_raycast_check(const dg_mesh* m, const void* o, const void* d, uint64_t n, double t_min, double t_max, const void* t,
+                              const void* id, const void* status, const char* who)
+{
+    if (!m) return fail(DG_ERR_INVALID, "%s: mesh is NULL (not constructed)", who);
+    if (int rc = mesh_usable(m, who)) return rc;
+    if (n && (!o || !d || !t || !id || !status)) return fail(DG_ERR_INVALID, "%s: origins / directions / t / triangle_id / status is NULL", who);
+    if (std::isnan(t_min) || std::isnan(t_max)) return fail(DG_ERR_INVALID, "%s: t_min and t_max must not be NaN", who);
+    if (t_min > t_max) return fail(DG_ERR_INVALID, "%s: t_min > t_max (%g > %g)", who, t_min, t_max);
+    if (m->dev.stack_depth > K9_MAX_STACK) return fail(DG_ERR_INVALID, "%s: tree too deep for the ray walk", who);
+    return check_handle_device(m->device, who);
+}
+
+int dg_mesh_raycast_device(const dg_mesh* m, const double* d_o, const double* d_d, uint64_t n, double t_min, double t_max, double* d_t,
+                           int32_t* d_id, double* d_bary, int32_t* d_status, void* stream)
+{
+    static const char* who = "dg_mesh_raycast_device";
+    if (int rc = mesh_raycast_check(m, d_o, d_d, n, t_min, t_max, d_t, d_id, d_status, who)) return rc;
+    if (n == 0) return DG_OK;
+    const WindDev* wd = nullptr;
+    if (int rc = winding_dev(m, wd, who)) return rc;
+    DG_LAUNCH(k9_launch_mesh_raycast(m->dev, *wd, d_o, d_d, n, t_min, t_max, d_t, d_id, d_bary, d_status, (cudaStream_t)stream));
+    return DG_OK;
+}
+
+// host arrays: chunks of 2^20 rays uploaded, cast and downloaded in turn on the legacy default stream
+static int mesh_raycast_host_impl(const dg_mesh* m, const double* o, const double* d, uint64_t n, double t_min, double t_max, double* t,
+                                  int32_t* id, double* bary, int32_t* status)
+{
+    static const char* who = "dg_mesh_raycast";
+    if (int rc = mesh_raycast_check(m, o, d, n, t_min, t_max, t, id, status, who)) return rc;
+    if (n == 0) return DG_OK;
+    const WindDev* wd = nullptr;
+    if (int rc = winding_dev(m, wd, who)) return rc;
+    const uint64_t chunk = std::min<uint64_t>(n, 1ull << 20);
+    DevBuf<double> d_o, d_d, d_t, d_b;
+    DevBuf<int32_t> d_id, d_st;
+    DG_CUDA(d_o.alloc(3 * chunk));
+    DG_CUDA(d_d.alloc(3 * chunk));
+    DG_CUDA(d_t.alloc(chunk));
+    DG_CUDA(d_id.alloc(chunk));
+    DG_CUDA(d_st.alloc(chunk));
+    if (bary) DG_CUDA(d_b.alloc(3 * chunk));
+    for (uint64_t b = 0; b < n; b += chunk) {
+        const uint64_t c = std::min(chunk, n - b);
+        DG_CUDA(cudaMemcpy(d_o.p, o + 3 * b, 3 * c * sizeof(double), cudaMemcpyHostToDevice));
+        DG_CUDA(cudaMemcpy(d_d.p, d + 3 * b, 3 * c * sizeof(double), cudaMemcpyHostToDevice));
+        DG_LAUNCH(k9_launch_mesh_raycast(m->dev, *wd, d_o.p, d_d.p, c, t_min, t_max, d_t.p, d_id.p, bary ? d_b.p : nullptr, d_st.p, nullptr));
+        DG_CUDA(cudaMemcpy(t + b, d_t.p, c * sizeof(double), cudaMemcpyDeviceToHost));
+        DG_CUDA(cudaMemcpy(id + b, d_id.p, c * sizeof(int32_t), cudaMemcpyDeviceToHost));
+        DG_CUDA(cudaMemcpy(status + b, d_st.p, c * sizeof(int32_t), cudaMemcpyDeviceToHost));
+        if (bary) DG_CUDA(cudaMemcpy(bary + 3 * b, d_b.p, 3 * c * sizeof(double), cudaMemcpyDeviceToHost));
+    }
+    return DG_OK;
+}
+
+int dg_mesh_raycast(const dg_mesh* m, const double* o, const double* d, uint64_t n, double t_min, double t_max, double* t, int32_t* id,
+                    double* bary, int32_t* status)
+{
+    return guarded("dg_mesh_raycast", [&]() { return mesh_raycast_host_impl(m, o, d, n, t_min, t_max, t, id, bary, status); });
 }
 
 int dg_obj_read(const char* path, double** vertices, uint64_t* n_vertices, uint32_t** triangles, uint64_t* n_triangles)

@@ -7,6 +7,7 @@ kernel of csrc/k1_sdf.cu; there is no host implementation.  Points given as a fl
 Result holds CUDA tensors.
 """
 import ctypes as C
+import math
 from collections import namedtuple
 from enum import IntEnum
 
@@ -151,6 +152,39 @@ class TriangleMeshDistance:
         w = np.empty(len(x))
         capi.check(capi.lib.dg_mesh_winding_number(self.handle, capi.ptr(x, capi.F64P), len(x), beta, capi.ptr(w, capi.F64P)))
         return w
+
+    def raycast(self, origins, directions, t_min=0.0, t_max=math.inf):
+        """The first hit of each ray on the mesh's triangles (beyond the reference; dg_mesh_raycast, contract in csrc/k9_mesh_raycast.cu and
+        DESIGN §3).  origins and directions (n, 3) or (3,); t in [t_min, t_max].  A segment x0 -> x1 (continuous collision detection of a
+        step against a deforming mesh: refit, then cast) is raycast(x0, x1 - x0, 0.0, 1.0).  The test is watertight: a ray through a shared
+        edge or vertex is not lost.  Returns (t, triangle_id, barycentric, status): the least t (the lower id wins a tie), the original
+        triangle index, the weights (n, 3) of that triangle's vertices 0, 1, 2, and DG_RAY_ENTER (1: crossing from the outside of an
+        outward-oriented mesh) or DG_RAY_LEAVE (2); a miss gives DG_RAY_MISS (0), t = inf, id -1 and NaN weights.  numpy inputs return numpy
+        arrays; float64 CUDA tensors on the mesh's device stay there and the cast runs on torch's current stream.  No autograd."""
+        t_min, t_max = float(t_min), float(t_max)
+        if _device.is_device_query(origins) or _device.is_device_query(directions):
+            import torch
+            o = _device.points(origins, self.device, "raycast")
+            d = _device.points(directions, self.device, "raycast")
+            if o.shape != d.shape:
+                raise ValueError(f"raycast: origins {tuple(o.shape)} and directions {tuple(d.shape)} differ in shape")
+            n = len(o)
+            t = torch.empty(n, dtype=torch.float64, device=o.device)
+            tid = torch.empty(n, dtype=torch.int32, device=o.device)
+            bary = torch.empty((n, 3), dtype=torch.float64, device=o.device)
+            st = torch.empty(n, dtype=torch.int32, device=o.device)
+            capi.check(capi.lib.dg_mesh_raycast_device(self.handle, o.data_ptr(), d.data_ptr(), n, t_min, t_max, t.data_ptr(), tid.data_ptr(),
+                                                       bary.data_ptr(), st.data_ptr(), _device.stream(o)))
+            return t, tid, bary, st
+        o = np.ascontiguousarray(origins, dtype=np.float64).reshape(-1, 3)
+        d = np.ascontiguousarray(directions, dtype=np.float64).reshape(-1, 3)
+        if o.shape != d.shape:
+            raise ValueError(f"raycast: origins {o.shape} and directions {d.shape} differ in shape")
+        n = len(o)
+        t = np.empty(n); tid = np.empty(n, np.int32); bary = np.empty((n, 3)); st = np.empty(n, np.int32)
+        capi.check(capi.lib.dg_mesh_raycast(self.handle, capi.ptr(o, capi.F64P), capi.ptr(d, capi.F64P), n, t_min, t_max, capi.ptr(t, capi.F64P),
+                                            capi.ptr(tid, capi.I32P), capi.ptr(bary, capi.F64P), capi.ptr(st, capi.I32P)))
+        return t, tid, bary, st
 
     def _query_device(self, points, signed):
         """the CUDA-tensor route: dg_mesh_distance_device on torch's current stream, asynchronous like a torch op"""

@@ -402,6 +402,27 @@ DG_API int dg_field_raycast(const dg_field* field, const double* origins, const 
 DG_API int dg_field_raycast_device(const dg_field* field, const double* d_origins, const double* d_directions, uint64_t n, double iso,
                                    double t_min, double t_max, double* d_t_lo, double* d_t_hi, int32_t* d_status, void* stream);
 
+/* ---- ray casts on a mesh: the first hit of rays and segments on the triangles themselves (not in the reference) --------------------
+ * For each ray i (origin origins[3 i..], direction directions[3 i..]) and t in [t_min, t_max]: the triangle hit first, by the watertight
+ * ray/triangle test of Woop, Benthin and Wald (JCGT 2013) in fp64 on the vertices as given, with two conditions that reject hits off a
+ * triangle for rays lying in its plane.  The full contract is stated in discregrid_b200/csrc/k9_mesh_raycast.cu and DESIGN.md section 3.
+ * A ray through a shared edge or vertex of a closed mesh is not lost between its triangles.  A segment x0 -> x1 is the ray (x0, x1 - x0)
+ * with t_min = 0, t_max = 1.  A ray misses if its origin or direction is not finite, or its direction is 0.
+ *   t[i]: the least accepted t (the lower triangle id wins a tie; -0.0 == +0.0); triangle_id[i]: the original triangle index;
+ *       barycentric[3 i..]: the weights of vertices 0, 1, 2 of that triangle (may be NULL); status[i] = DG_RAY_ENTER when the ray crosses
+ *       the triangle from the side a ray enters a closed, outward-oriented mesh from, DG_RAY_LEAVE otherwise.  A miss: DG_RAY_MISS, t = +inf,
+ *       triangle_id = -1, barycentric NaN.  The result does not depend on the traversal: it equals a loop over every triangle, bit for bit.
+ *   t_min <= t_max, neither NaN (either may be infinite).  Arrays other than barycentric may be NULL only when n is 0.  The mesh must live on
+ *       the current device and not be left unusable by a failed refit.  Otherwise DG_ERR_INVALID, before anything is written.
+ *   The vertices are read from the winding-number records (dg_mesh_winding_number): the first call on a mesh builds them (328 B per
+ *   triangle) and returns after their upload.  Either sign mode; a mesh that a dg_mesh_group borrows may be cast; after dg_mesh_refit the
+ *   cast sees the refit positions.  One GPU, the mesh's.
+ *   dg_mesh_raycast: host arrays, synchronous.  dg_mesh_raycast_device: device arrays, asynchronous on `stream`. */
+DG_API int dg_mesh_raycast(const dg_mesh* mesh, const double* origins, const double* directions, uint64_t n, double t_min, double t_max,
+                           double* t, int32_t* triangle_id, double* barycentric, int32_t* status);
+DG_API int dg_mesh_raycast_device(const dg_mesh* mesh, const double* d_origins, const double* d_directions, uint64_t n, double t_min,
+                                  double t_max, double* d_t, int32_t* d_triangle_id, double* d_barycentric, int32_t* d_status, void* stream);
+
 /* ---- reduced density map: GenerateDensityMap with reduction in one call -----------------------------------------------------------
  * GenerateDensityMap with reduction (cmd/generate_density_map/main.cpp:117-147) in one call:
  *   id = addFunction(density_func, verbose, pred);  reduceField(0, p0);  reduceField(id, p1);
