@@ -24,7 +24,7 @@ CPPBIN   := build/bin
 CPPFLAGS := -std=c++11 -O2 -ffp-contract=off -I$(EIGEN3_INCLUDE_DIR) -Icpp/include -Iinclude
 CPPLINK  := -Ldiscregrid_b200/lib -ldiscregrid_b200 -Wl,-rpath,'$$ORIGIN/../../discregrid_b200/lib'
 CPPHDRS  := $(wildcard cpp/include/Discregrid/* cpp/include/Discregrid/*/*) include/discregrid_b200.h
-cpp: $(CPPBIN)/GenerateSDF $(CPPBIN)/GenerateDensityMap $(CPPBIN)/GenerateVolumeMap $(CPPBIN)/liborcvolume.so ref_volume $(CPPBIN)/DiscreteFieldToBitmap $(CPPBIN)/DiscreteFieldToMesh $(CPPBIN)/facade_check $(CPPBIN)/bvh_host_check $(CPPBIN)/reduce_facade_check $(CPPBIN)/sort_replay_check $(CPPBIN)/fast_div_check $(CPPBIN)/libk1emu.so $(CPPBIN)/libk1emu_knobs.so $(CPPBIN)/libk1emu_wave.so $(CPPBIN)/libk1emu_perlane.so $(CPPBIN)/libk1emu_packet.so $(CPPBIN)/libk1emu_band.so $(CPPBIN)/libk1emu_band_perlane.so $(CPPBIN)/libk23emu.so $(CPPBIN)/libk23emu_knobs.so $(CPPBIN)/libk3vemu.so $(CPPBIN)/libk2hemu.so $(CPPBIN)/libk5emu.so $(CPPBIN)/libk8emu.so $(CPPBIN)/libk9emu.so $(CPPBIN)/libk9emu_nocull.so $(CPPBIN)/libdgemu.so $(CPPBIN)/libk4emu.so $(CPPBIN)/device_function_check $(CPPBIN)/device_query_check $(CPPBIN)/hessian_check $(CPPBIN)/winding_check $(CPPBIN)/raycast_check $(CPPBIN)/refit_check $(CPPBIN)/mesh_raycast_check $(CPPBIN)/liborctree.so
+cpp: $(CPPBIN)/GenerateSDF $(CPPBIN)/GenerateDensityMap $(CPPBIN)/GenerateVolumeMap $(CPPBIN)/liborcvolume.so ref_volume $(CPPBIN)/DiscreteFieldToBitmap $(CPPBIN)/DiscreteFieldToMesh $(CPPBIN)/facade_check $(CPPBIN)/bvh_host_check $(CPPBIN)/reduce_facade_check $(CPPBIN)/sort_replay_check $(CPPBIN)/fast_div_check $(CPPBIN)/libk1emu.so $(CPPBIN)/libk1emu_perlane.so $(CPPBIN)/libk1emu_band.so $(CPPBIN)/libk1emu_band_perlane.so $(CPPBIN)/libk23emu.so $(CPPBIN)/libk3vemu.so $(CPPBIN)/libk2hemu.so $(CPPBIN)/libk5emu.so $(CPPBIN)/libk8emu.so $(CPPBIN)/libk9emu.so $(CPPBIN)/libk9emu_nocull.so $(CPPBIN)/libdgemu.so $(CPPBIN)/libk4emu.so $(CPPBIN)/device_function_check $(CPPBIN)/device_query_check $(CPPBIN)/hessian_check $(CPPBIN)/winding_check $(CPPBIN)/raycast_check $(CPPBIN)/refit_check $(CPPBIN)/mesh_raycast_check $(CPPBIN)/liborctree.so
 $(CPPBIN)/DiscreteFieldToBitmap: cpp/cmd/discrete_field_to_bitmap.cpp $(CPPHDRS) $(LIB)
 	@mkdir -p $(CPPBIN)
 	$(HOSTCXX) $(CPPFLAGS) $< -o $@ $(CPPLINK)
@@ -34,27 +34,17 @@ $(CPPBIN)/DiscreteFieldToMesh: cpp/cmd/discrete_field_to_mesh.cpp $(CPPHDRS) $(L
 $(CPPBIN)/bvh_host_check: tests/cpp/bvh_host_check.cpp $(SRC)/bvh_build.cpp $(SRC)/host_threads.cpp $(SRC)/sort_replay.cpp $(SRC)/sort_replay.h $(SRC)/bvh_build.h
 	@mkdir -p $(CPPBIN)
 	$(HOSTCXX) $(CXXFLAGS) -fvisibility=default tests/cpp/bvh_host_check.cpp $(SRC)/bvh_build.cpp $(SRC)/host_threads.cpp $(SRC)/sort_replay.cpp -o $@ -lpthread
-# test libraries: the K1 translation unit (kernels + launchers) compiled for the CPU by tests/emu -- default knobs, and the prepared
-# the knobs that are ON by default (redux vote, per-array brick shape) switched off, so that both settings stay checked
+# test libraries: the K1 translation unit (kernels + launchers) compiled for the CPU by tests/emu -- the product's build (packet walk)
+# and the per-lane node loop (K1_PACKET=0), the independent walk the packet walk is compared against
 K1EMU_SRC := tests/emu/k1_emu.cpp $(SRC)/bvh_build.cpp $(SRC)/host_threads.cpp $(SRC)/sort_replay.cpp
 K1EMU_DEP := $(K1EMU_SRC) tests/emu/cuda_emu.h $(SRC)/k1_sdf.cu $(HDRS)
 CUDA_INC  ?= /usr/local/cuda/include
 $(CPPBIN)/libk1emu.so: $(K1EMU_DEP)
 	@mkdir -p $(CPPBIN)
 	$(HOSTCXX) -std=c++17 -O2 -ffp-contract=off -fPIC -shared -I$(CUDA_INC) -Itests/emu -I$(SRC) $(K1EMU_SRC) -o $@ -lpthread
-$(CPPBIN)/libk1emu_knobs.so: $(K1EMU_DEP)
-	@mkdir -p $(CPPBIN)
-	$(HOSTCXX) -std=c++17 -O2 -ffp-contract=off -fPIC -shared -DK1_PACKET=0 -DK1_VOTE_REDUX=0 -DK1_BRICK_AUTO=0 -I$(CUDA_INC) -Itests/emu -I$(SRC) $(K1EMU_SRC) -o $@ -lpthread
-# the wavefront node-loop kernel (K1_WAVE=1) and the per-lane one (K1_WAVE=0), whichever is not the default build, stay checked
-$(CPPBIN)/libk1emu_wave.so: $(K1EMU_DEP)
-	@mkdir -p $(CPPBIN)
-	$(HOSTCXX) -std=c++17 -O2 -ffp-contract=off -fPIC -shared -DK1_WAVE=1 -I$(CUDA_INC) -Itests/emu -I$(SRC) $(K1EMU_SRC) -o $@ -lpthread
-$(CPPBIN)/libk1emu_packet.so: $(K1EMU_DEP)
-	@mkdir -p $(CPPBIN)
-	$(HOSTCXX) -std=c++17 -O2 -ffp-contract=off -fPIC -shared -DK1_PACKET=1 -I$(CUDA_INC) -Itests/emu -I$(SRC) $(K1EMU_SRC) -o $@ -lpthread
 $(CPPBIN)/libk1emu_perlane.so: $(K1EMU_DEP)
 	@mkdir -p $(CPPBIN)
-	$(HOSTCXX) -std=c++17 -O2 -ffp-contract=off -fPIC -shared -DK1_WAVE=0 -DK1_PACKET=0 -I$(CUDA_INC) -Itests/emu -I$(SRC) $(K1EMU_SRC) -o $@ -lpthread
+	$(HOSTCXX) -std=c++17 -O2 -ffp-contract=off -fPIC -shared -DK1_PACKET=0 -I$(CUDA_INC) -Itests/emu -I$(SRC) $(K1EMU_SRC) -o $@ -lpthread
 # the narrow-band launcher (classifier + band node loop) on top of the same TU: packet walk (default) and per-lane walk
 K1BAND_SRC := tests/emu/k1_band_emu.cpp $(SRC)/bvh_build.cpp $(SRC)/host_threads.cpp $(SRC)/sort_replay.cpp
 $(CPPBIN)/libk1emu_band.so: $(K1EMU_DEP) tests/emu/k1_band_emu.cpp
@@ -68,9 +58,6 @@ K23EMU_DEP := $(K23EMU_SRC) tests/emu/cuda_emu.h $(SRC)/k2_interp.cu $(SRC)/k3_d
 $(CPPBIN)/libk23emu.so: $(K23EMU_DEP)
 	@mkdir -p $(CPPBIN)
 	$(HOSTCXX) -std=c++17 -O2 -ffp-contract=off -fPIC -shared -I$(CUDA_INC) -Itests/emu -I$(SRC) $(K23EMU_SRC) -o $@ -lpthread
-$(CPPBIN)/libk23emu_knobs.so: $(K23EMU_DEP)
-	@mkdir -p $(CPPBIN)
-	$(HOSTCXX) -std=c++17 -O2 -ffp-contract=off -fPIC -shared -DK3_FAST_DIV=0 -I$(CUDA_INC) -Itests/emu -I$(SRC) $(K23EMU_SRC) -o $@ -lpthread
 # the same with the volume map exposed (emu_volume_map, tests/emu/k3_volume_emu.cpp)
 $(CPPBIN)/libk3vemu.so: $(K23EMU_DEP) tests/emu/k3_volume_emu.cpp
 	@mkdir -p $(CPPBIN)

@@ -94,7 +94,7 @@ struct alignas(128) LeafRecord {
 static_assert(sizeof(LeafRecord) == 128, "LeafRecord must be 128 bytes");
 
 // fp32 shadow of a triangle (relative to HostBvh::center), used only to REJECT leaf tests that provably cannot be accepted
-// (k1_sdf.cu, leaf filter): v0, e0, e1, |e0|^2, e0.e1, |e1|^2, |e1-e0|^2, n = unit normal (e0 x e1) / |e0 x e1| (0 for zero area).
+// (k1_sdf.cu, leaf_lower_bound): v0, e0, e1, |e0|^2, e0.e1, |e1|^2, |e1-e0|^2, n = unit normal (e0 x e1) / |e0 x e1| (0 for zero area).
 // Never contributes a value to the result.
 struct alignas(64) LeafF {
     float v0[3], e0[3], e1[3];

@@ -367,7 +367,7 @@ int dg_mesh_create(const double* V, uint64_t nV, const uint32_t* F, uint64_t nT,
     const auto t0 = std::chrono::steady_clock::now();
     const char* why = "";
     try {
-        if (!build_host_bvh(V, nV, F, nT, m->host, &why, K1_NEEDS_LEAF_SHADOW != 0)) { delete m; return fail(DG_ERR_INVALID, "dg_mesh_create: %s", why); }
+        if (!build_host_bvh(V, nV, F, nT, m->host, &why, true)) { delete m; return fail(DG_ERR_INVALID, "dg_mesh_create: %s", why); }
     } catch (const std::bad_alloc&) { delete m; return fail(DG_ERR_NOMEM, "dg_mesh_create: out of host memory"); }
     const auto t1 = std::chrono::steady_clock::now();
     m->build_us = (uint64_t)std::chrono::duration_cast<std::chrono::microseconds>(t1 - t0).count();
@@ -379,11 +379,9 @@ int dg_mesh_create(const double* V, uint64_t nV, const uint32_t* F, uint64_t nT,
     DG_CUDA_M(m->d_leaves.alloc(nT));
     DG_CUDA_M(m->d_normals.alloc(nT));
     DG_CUDA_M(m->d_nodes_f.alloc(nT * K1_NODEF_STRIDE));
-#if K1_NEEDS_LEAF_SHADOW
     DG_CUDA_M(m->d_leaves_f.alloc(nT));
     DG_CUDA_M(cudaMemcpy(m->d_leaves_f.p, m->host.leaves_f.data(), nT * sizeof(LeafF), cudaMemcpyHostToDevice));
     m->dev.leaves_f = m->d_leaves_f.p;
-#endif
     DG_CUDA_M(cudaMemcpy(m->d_spheres.p, m->host.spheres.data(), nT * sizeof(SpherePair), cudaMemcpyHostToDevice));
     DG_CUDA_M(cudaMemcpy(m->d_leaves.p, m->host.leaves.data(), nT * sizeof(LeafRecord), cudaMemcpyHostToDevice));
     DG_CUDA_M(cudaMemcpy(m->d_normals.p, m->host.normals.data(), nT * sizeof(PseudoNormals), cudaMemcpyHostToDevice));
@@ -1273,11 +1271,9 @@ int dg_mesh_group_create(const dg_mesh* mesh, int n_gpus, const int* devices, dg
         DG_CUDA(cudaMemcpyPeer(r->d_nodes_f.p, r->device, mesh->d_nodes_f.p, mesh->device, nT * K1_NODEF_STRIDE * sizeof(float4)));
         r->dev = mesh->dev;
         r->dev.spheres = r->d_spheres.p; r->dev.leaves = r->d_leaves.p; r->dev.normals = r->d_normals.p; r->dev.nodes_f = r->d_nodes_f.p;
-#if K1_NEEDS_LEAF_SHADOW
         DG_CUDA(r->d_leaves_f.alloc(nT));
         DG_CUDA(cudaMemcpyPeer(r->d_leaves_f.p, r->device, mesh->d_leaves_f.p, mesh->device, nT * sizeof(LeafF)));
         r->dev.leaves_f = r->d_leaves_f.p;
-#endif
         DG_CUDA(k1_configure(r->dev.stack_depth));
         DG_CUDA(cudaDeviceSynchronize());
     }
@@ -1421,15 +1417,15 @@ int dg_sample_sdf_multi_device(dg_mesh_group* grp, const dg_grid_desc* grid, dou
     return DG_OK;
 }
 
-// plane ranges of part `part` of `n_parts`: boundaries fall on even plane indices (a brick spans K1_BRICK_S = 2 planes)
+// plane ranges of part `part` of `n_parts`: whole plane pairs, so boundaries fall on even plane indices
 static void slab_planes(const GridDev& g, uint32_t part, uint32_t n_parts, unsigned pb[4], unsigned pe[4])
 {
     const unsigned Ds[4] = {g.n[2] + 1, g.n[2] + 1, g.n[0] + 1, g.n[1] + 1};
     for (int a = 0; a < 4; a++) {
-        const uint64_t groups = (Ds[a] + K1_BRICK_S - 1) / K1_BRICK_S;
+        const uint64_t groups = (Ds[a] + 1) / 2;
         const uint64_t q0 = groups * part / n_parts, q1 = groups * (part + 1) / n_parts;
-        pb[a] = (unsigned)std::min<uint64_t>(q0 * K1_BRICK_S, Ds[a]);
-        pe[a] = (unsigned)std::min<uint64_t>(q1 * K1_BRICK_S, Ds[a]);
+        pb[a] = (unsigned)std::min<uint64_t>(q0 * 2, Ds[a]);
+        pe[a] = (unsigned)std::min<uint64_t>(q1 * 2, Ds[a]);
     }
 }
 

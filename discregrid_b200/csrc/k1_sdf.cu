@@ -24,7 +24,7 @@
 // Structure of this file: tri_dist2 (leaf test) -> finish_query (nearest point + sign) -> leaf_lower_bound (certified fp32
 // triangle bound) -> nearest_triangle (the warp-synchronous per-lane traversal: NODE / LEAF / POP phases, fp32 interval
 // filter, exact-preserving shortcuts) -> nearest_triangle_packet -> the two kernels (grid nodes in bricks of 32; arbitrary points) -> launchers.
-// Tuning knobs and the variants are listed in k1_sdf.h.
+// The tuning constants are listed in k1_sdf.h.
 #include "dg_device.cuh"
 #include "bvh_build.h"
 #include "k1_sdf.h"
@@ -35,17 +35,10 @@
 #include <algorithm>
 
 #include "dg_launch.h"       // DG_KERNEL_LAUNCH: <<<>>> on the device, fibers under tests/emu (DG_EMU)
-#if K1_BRICK_AUTO
 #define SEG_BF(S) (1u << (S).lf)
 #define SEG_BM(S) (1u << (S).lm)
 #define SEG_BS(S) (32u >> ((S).lf + (S).lm))
 #define LAY_BS(L, a) (32u >> ((L).lf[a] + (L).lm[a]))
-#else
-#define SEG_BF(S) ((unsigned)K1_BRICK_F)
-#define SEG_BM(S) ((unsigned)K1_BRICK_M)
-#define SEG_BS(S) ((unsigned)K1_BRICK_S)
-#define LAY_BS(L, a) ((unsigned)K1_BRICK_S)
-#endif
 #ifdef DG_EMU
 #define DG_EMU_COUNT(i) (dg_emu::g_counters[(i)]++)        // event counters of the emulation (tests/emu, tools): nothing on the device
 #define DG_EMU_ADD(i, v) (dg_emu::g_counters[(i)] += (unsigned long long)(v))
@@ -111,55 +104,27 @@ __device__ __forceinline__ double tri_dist2(const LeafRecord* __restrict__ rec,
     const int ent_r2 = (tmp1_2 > tmp0_2) ? ((numer_2 >= denom) ? 1 : 4) : ((tmp1_2 <= 0) ? 2 : ((b1 >= 0) ? 0 : 5));   // :690-731
     const int ent_r6 = (tmp1_6 > tmp0_6) ? ((numer_6 >= denom) ? 2 : 4) : ((tmp1_6 <= 0) ? 1 : ((b0 >= 0) ? 0 : 3));   // :737-778
     const int ent_r1 = (numer_1 <= 0) ? 2 : ((numer_1 >= denom) ? 1 : 4);                                               // :783-808
-    // `pin` = empty asm that makes a value opaque: the compiler must materialise it there and cannot specialise the code
-    // that follows per outcome (left alone it re-creates ~20 divergent branches, three of them with their own division).
-    // K1_LEAF_MODE 0: plain C (compiler's branches); 1: everything straight-line (every lane pays division + quadratic form);
-    // 2: predicate-only classification, then ONE guarded block with the division and ONE with the quadratic form.
-#if K1_LEAF_MODE && !defined(DG_EMU)
-#define DG_PIN_I(v) asm volatile("" : "+r"(v))
-#define DG_PIN_D(v) asm volatile("" : "+d"(v))
-#else
-#define DG_PIN_I(v)
-#define DG_PIN_D(v)
-#endif
+    // The compiler places the branches of what follows.  Forcing it straight-line (every lane pays the division and the quadratic form),
+    // or into one guarded block for the division and one for the quadratic form, was measured slower.
     int ent = lower ? (sneg ? (tneg ? ent_r4 : chain_b1) : (tneg ? chain_b0 : 6))
                     : (sneg ? ent_r2 : (tneg ? ent_r6 : ent_r1));
-    DG_PIN_I(ent);
     const bool region6 = !lower && !sneg && tneg;
     const double numer = sneg ? numer_2 : (tneg ? numer_6 : numer_1);  // only read when ent == 4 (upper regions)
 
     // ---- one division for the three edge outcomes
     double num = (ent == 3) ? -b0 : ((ent == 5) ? -b1 : ((ent == 4) ? numer : 0.0));
     double den = (ent == 3) ? a00 : ((ent == 5) ? a11 : ((ent == 4) ? denom : 1.0));
-    DG_PIN_D(num); DG_PIN_D(den);
-    double q = 0.0;
-#if K1_LEAF_MODE == 2
-    if (ent >= 3 && ent <= 5)
-#endif
-    {
-        q = num / den;
-    }
-    DG_PIN_D(q);
+    double q = num / den;
     // ---- (s, t) of the nearest point
     const double sF = s0 * inv_det, tF = t0 * inv_det;                 // :675-677 (read when ent == 6)
     const double omq = 1 - q;                                          // :705, :752, :804 (read when ent == 4)
     double s = (ent == 6) ? sF : ((ent == 4) ? (region6 ? omq : q) : ((ent == 1) ? 1.0 : ((ent == 3) ? q : 0.0)));
     double t = (ent == 6) ? tF : ((ent == 4) ? (region6 ? q : omq) : ((ent == 2) ? 1.0 : ((ent == 5) ? q : 0.0)));
-    DG_PIN_D(s); DG_PIN_D(t);
     // ---- d2
-    double quad = 0.0;
-#if K1_LEAF_MODE == 2
-    if (ent == 4 || ent == 6)
-#endif
-    {
-        quad = s * (a00 * s + a01 * t + 2 * b0) + t * (a01 * s + a11 * t + 2 * b1) + c;   // :678, :706, :753, :805
-    }
+    double quad = s * (a00 * s + a01 * t + 2 * b0) + t * (a01 * s + a11 * t + 2 * b1) + c;   // :678, :706, :753, :805
     double dv1 = a00 + 2 * b0 + c, dv2 = a11 + 2 * b1 + c;            // :594, :616
     double de1 = b0 * q + c, de2 = b1 * q + c;                         // :600, :622
-    DG_PIN_D(quad); DG_PIN_D(dv1); DG_PIN_D(dv2); DG_PIN_D(de1); DG_PIN_D(de2);
     double d2 = (ent == 6 || ent == 4) ? quad : ((ent == 0) ? c : ((ent == 1) ? dv1 : ((ent == 2) ? dv2 : ((ent == 3) ? de1 : de2))));
-#undef DG_PIN_I
-#undef DG_PIN_D
     if (d2 < 0) d2 = 0;                                                // :812-816
     s_out = s; t_out = t; ent_out = ent;
     return d2;
@@ -208,7 +173,7 @@ __device__ __forceinline__ double sphere_dist(double px, double py, double pz, d
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// FP32 INTERVAL FILTER (K1_FILTER).  The traversal only needs the sphere distances for three yes/no questions:
+// FP32 INTERVAL FILTER.  The traversal only needs the sphere distances for three yes/no questions:
 // which child is nearer (:542), is a child nearer than the best so far (:545-557).  Both are decided from an fp32 shadow
 // of the spheres whenever the fp32 interval [d_f - E, d_f + E] -- which provably contains the reference's fp64 value -- lies
 // entirely on one side; otherwise (ties, near-ties: a few per thousand) the lane recomputes that node in fp64 exactly as the
@@ -242,14 +207,6 @@ struct MeshDev {
     int n_tri;
 };
 
-#if K1_PREFETCH
-#ifdef DG_EMU
-__device__ __forceinline__ void prefetch_l1(const void*) {}
-#else
-__device__ __forceinline__ void prefetch_l1(const void* p) { asm volatile("prefetch.global.L1 [%0];" ::"l"(p)); }
-#endif
-#endif
-
 __device__ __forceinline__ float sqrt_approx(float x)
 {
 #ifdef DG_EMU
@@ -262,7 +219,7 @@ __device__ __forceinline__ float sqrt_approx(float x)
 }
 
 
-// LEAF FILTER (K1_LEAF_FILTER): certified fp32 LOWER bound of the distance from the query to a triangle.
+// LEAF BOUND of the packet walk: certified fp32 LOWER bound of the distance from the query to a triangle.
 //   * distance to each of the three closed edges (clamped parameter => an actual point of the edge, so each value is an upper
 //     bound of that edge's true distance up to rounding; their minimum is the true distance whenever the closest point is on the
 //     boundary, i.e. whenever the projection of the query falls outside the triangle);
@@ -277,7 +234,8 @@ __device__ __forceinline__ float sqrt_approx(float x)
 // need it).  A zero normal (zero area) gives plane2 = 0: no plane bound.
 // The caller rejects the leaf only if bound > best_hi + 2E (same slack accounting as the box skip).  On bunny/dragon this rejects
 // 83-90 % of the leaf tests; the rest (accepted ones, ties, near misses) take the exact fp64 test.  Prototype with 0 invalid
-// rejections in 3 M leaf tests: see DESIGN.md.
+// rejections in 3 M leaf tests: see DESIGN.md.  The per-lane walk does not use it: there, as a phase of its own, it cost more
+// iterations than the fp64 tests it saved.
 __device__ __forceinline__ float dot3f(float ax, float ay, float az, float bx, float by, float bz) { return fmaf(az, bz, fmaf(ay, by, ax * bx)); }
 
 __device__ __forceinline__ float leaf_lower_bound(const LeafF* __restrict__ rec, float qx, float qy, float qz, float E)
@@ -334,7 +292,7 @@ __device__ __forceinline__ float leaf_lower_bound(const LeafF* __restrict__ rec,
 __device__ __forceinline__ QueryResult nearest_triangle(const MeshDev& M, bool alive, double px, double py, double pz,
                                                         unsigned* stack_rng, float* stack_d, int stride)
 {
-    enum { NODE = 0, LEAF = 1, POP = 2, DONE = 3, LEAFX = 4 };     // LEAF: filter pending; LEAFX: exact fp64 test needed
+    enum { NODE = 0, LEAF = 1, POP = 2, DONE = 3 };
     const int n_tri = M.n_tri;
     QueryResult res;
     res.dist = DBL_MAX; res.s = 0; res.t = 0; res.pos = -1; res.entity = 0;
@@ -347,7 +305,7 @@ __device__ __forceinline__ QueryResult nearest_triangle(const MeshDev& M, bool a
     // outside the budget's range (below 2^-40 or beyond ~1e18) the filter is off for this query: E = inf leaves every test undecided
     const float E = filter_slack(Mq);
     const float E2 = E + E;
-    // BOX SKIP (K1_BOX_SKIP).  A subtree may be skipped when visiting it provably changes nothing: no triangle in it can be
+    // BOX SKIP.  A subtree may be skipped when visiting it provably changes nothing: no triangle in it can be
     // accepted, i.e. every d2 the reference would compute there is >= best_sq.  With L = (fp32 distance to the subtree's
     // outward-rounded box) - E <= true distance to every triangle, the reference's d2 >= L^2 - 240 eps64 R^2 (fp64 rounding of
     // its formula, R <= 7 Mq) and best_sq <= best^2 (1 + 2^-53): both slacks are below E * best once best >= 1e-6 Mq, so
@@ -355,28 +313,17 @@ __device__ __forceinline__ QueryResult nearest_triangle(const MeshDev& M, bool a
     // The running best only shrinks, so a subtree found hopeless stays hopeless and its deferred re-test can be dropped too.
     const float tiny_best = 1.0e-6f * Mq;
     float skip_sq = __int_as_float(0x7f800000);              // (best_hi + 2E)^2 rounded up; +inf = never skip
-    float skip_lin = __int_as_float(0x7f800000);             // best_hi + 2E rounded up
     int b = 0, e = n_tri, depth = 0, sp = 0;
     int state = alive ? ((n_tri == 1) ? LEAF : NODE) : DONE;
     for (;;) {
-#if K1_VOTE_REDUX && !K1_LEAF_FILTER && !K1_NODE_REPEAT
-        // one warp-wide integer sum carries the three lane counts (8 bits each: NODE | LEAF << 8 | POP << 16; DONE adds nothing)
+        // one warp-wide integer sum carries the three lane counts (8 bits each: NODE | LEAF << 8 | POP << 16; DONE adds nothing), which
+        // costs less than ballots and popcounts: the loop head is ~19 % of the issued instructions
         const unsigned tally = __reduce_add_sync(0xffffffffu, (state < DONE) ? (1u << (8 * state)) : 0u);
         if (tally == 0u) break;                                                // every lane DONE
         const int w_node = K1_NODE_WEIGHT * (int)(tally & 0xffu), w_pop = K1_POP_WEIGHT * (int)(tally >> 16);
-        const int w_leaff = 0;
-        const int w_leafx = K1_LEAF_WEIGHT * (int)((tally >> 8) & 0xffu);
-        const unsigned bit0 = 0u, bit1 = 0u, bit2 = 0u; (void)bit0; (void)bit1; (void)bit2;
-#else
-        // three ballots carry the 3-bit state of all 32 lanes
-        const unsigned bit0 = __ballot_sync(0xffffffffu, state & 1), bit1 = __ballot_sync(0xffffffffu, state & 2);
-        const unsigned bit2 = K1_LEAF_FILTER ? __ballot_sync(0xffffffffu, state & 4) : 0u;
-        if ((bit0 & bit1) == 0xffffffffu) break;                               // every lane DONE
-        const int w_node = K1_NODE_WEIGHT * __popc(~(bit0 | bit1 | bit2)), w_pop = K1_POP_WEIGHT * __popc(~bit0 & bit1);
-        const int w_leaff = K1_LEAF_FILTER ? K1_LEAFF_WEIGHT * __popc(bit0 & ~bit1) : 0;
-        const int w_leafx = K1_LEAF_WEIGHT * __popc(K1_LEAF_FILTER ? bit2 : (bit0 & ~bit1));
-#endif
-        const int w_max = max(max(w_node, w_pop), max(w_leaff, w_leafx));
+        const int w_leaf = K1_LEAF_WEIGHT * (int)((tally >> 8) & 0xffu);
+        // (max with 0 changes no value, but without it the loop head compiles to other instructions than the timed ones)
+        const int w_max = max(max(w_node, w_pop), max(0, w_leaf));
         DG_EMU_COUNT(0);
         if (w_pop == w_max) {
             if (state == POP) {
@@ -389,7 +336,7 @@ __device__ __forceinline__ QueryResult nearest_triangle(const MeshDev& M, bool a
                     const float df = stack_d[sp * stride];
                     bool visit = (df + E < best_lo);                           // certainly d < best
                     const bool skip = (df - E >= best_hi);                     // certainly d >= best
-                    if (!K1_FILTER || !(visit || skip)) {                      // undecided in fp32: the reference's fp64 value
+                    if (!(visit || skip)) {                                    // undecided in fp32: the reference's fp64 value
                         DG_EMU_COUNT(6);
                         const unsigned r = stack_rng[sp * stride];
                         const int rb = (int)(r & 0x01ffffffu), rd = (int)((r >> 25) & 31u);
@@ -403,7 +350,6 @@ __device__ __forceinline__ QueryResult nearest_triangle(const MeshDev& M, bool a
                         const unsigned r = stack_rng[sp * stride];
                         const int rb = (int)(r & 0x01ffffffu), rd = (int)((r >> 25) & 31u);
                         const int re = rb + (n_tri >> rd) + (int)((r >> 30) & 1u);
-#if K1_BOX_SKIP
                         {   // the best has usually shrunk since this sibling was deferred: box test against the current best
                             // the child's box sits in two of the record's three box quads (l_lo.xyz l_hi.x | l_hi.yz r_lo.xy | r_lo.z r_hi.xyz): two
                             // 16-byte loads instead of six scalar ones (fewer L1 tag requests)
@@ -415,7 +361,6 @@ __device__ __forceinline__ QueryResult nearest_triangle(const MeshDev& M, bool a
                             const float gx = fmaxf(fmaxf(lox - qx, qx - hix), 0.f), gy = fmaxf(fmaxf(loy - qy, qy - hiy), 0.f), gz = fmaxf(fmaxf(loz - qz, qz - hiz), 0.f);
                             if (__fmaf_rd(gz, gz, __fmaf_rd(gy, gy, __fmul_rd(gx, gx))) > skip_sq) { DG_EMU_COUNT(7); continue; }   // visiting it could not change anything
                         }
-#endif
                         b = rb; depth = rd; e = re;
                         state = (e - b == 1) ? LEAF : NODE;
                         break;
@@ -423,30 +368,17 @@ __device__ __forceinline__ QueryResult nearest_triangle(const MeshDev& M, bool a
                 }
             }
         } else if (w_node == w_max) {
-#if K1_NODE_REPEAT
-          // consecutive node steps are the common case (about three internal levels per leaf): stay in this phase, without
-          // re-voting the full state, while the lanes still sitting at an internal node remain at least half of the lanes that ran
-          int n_run = __popc(~(bit0 | bit1 | bit2));
-          for (int rep = 0;; rep++) {
-#endif
             if (state == NODE) {                                                // internal (:537-561)
                 DG_EMU_COUNT(1);
                 const int m = (b + e) >> 1;
                 bool left_first, go_first, go_second = false, defer = true;
                 float d_second_f;
                 bool decided = false;
-#if K1_FILTER
                 {
                     const float4* f4 = M.nodes_f + (size_t)m * K1_NODEF_STRIDE;
                     const float4 l4 = __ldg(f4), r4 = __ldg(f4 + 1);
-#if K1_PREFETCH
-                    // whichever child is entered next, its record is needed by the very next step of this lane: pull both into L1 now
-                    if (m - b == 1) prefetch_l1(M.leaves + b); else prefetch_l1(M.nodes_f + (size_t)((b + m) >> 1) * K1_NODEF_STRIDE);
-                    if (e - m == 1) prefetch_l1(M.leaves + m); else prefetch_l1(M.nodes_f + (size_t)((m + e) >> 1) * K1_NODEF_STRIDE);
-#endif
-#if K1_BOX_SKIP && K1_EARLY_BOX
+                    // the box loads go out with the sphere loads (latency), not after the sphere decision that may need them
                     const float4 b0 = __ldg(f4 + 2), b1 = __ldg(f4 + 3), b2 = __ldg(f4 + 4);   // l_lo.xyz l_hi.x | l_hi.yz r_lo.xy | r_lo.z r_hi.xyz
-#endif
                     const float lx = qx - l4.x, ly = qy - l4.y, lz = qz - l4.z;
                     const float rx = qx - r4.x, ry = qy - r4.y, rz = qz - r4.z;
                     const float dl = sqrt_approx(fmaf(lz, lz, fmaf(ly, ly, lx * lx))) - l4.w;
@@ -461,11 +393,7 @@ __device__ __forceinline__ QueryResult nearest_triangle(const MeshDev& M, bool a
                     // a sibling that is already certainly not nearer than the best can never pass its re-test (best only
                     // shrinks): the reference would pop it and skip it (:549/:557), so it is not stacked at all
                     defer = !(d_second_f - E >= best_hi);
-#if K1_BOX_SKIP
                     if (decided && go_first) {
-#if !K1_EARLY_BOX
-                        const float4 b0 = __ldg(f4 + 2), b1 = __ldg(f4 + 3), b2 = __ldg(f4 + 4);   // l_lo.xyz l_hi.x | l_hi.yz r_lo.xy | r_lo.z r_hi.xyz
-#endif
                         const float lgx = fmaxf(fmaxf(b0.x - qx, qx - b0.w), 0.f), lgy = fmaxf(fmaxf(b0.y - qy, qy - b1.x), 0.f),
                                     lgz = fmaxf(fmaxf(b0.z - qz, qz - b1.y), 0.f);
                         const float rgx = fmaxf(fmaxf(b1.z - qx, qx - b2.y), 0.f), rgy = fmaxf(fmaxf(b1.w - qy, qy - b2.z), 0.f),
@@ -485,9 +413,7 @@ __device__ __forceinline__ QueryResult nearest_triangle(const MeshDev& M, bool a
                             }                                   // undecided re-test: simply do not use the shortcut
                         }
                     }
-#endif
                 }
-#endif
                 if (!decided) {                                                 // fp64, exactly the reference
                     DG_EMU_COUNT(2);
                     const double* sp8 = reinterpret_cast<const double*>(M.spheres + m);
@@ -500,9 +426,8 @@ __device__ __forceinline__ QueryResult nearest_triangle(const MeshDev& M, bool a
                     go_first = d_first < best;                                                // :545 / :554
                     go_second = !go_first && (d_second < best);     // only reachable through NaNs; kept for fidelity (:549 / :557)
                     d_second_f = (float)d_second;                   // |rounding| <= 2^-24 |d| << E: the stored value stays a valid filter input
-                    defer = K1_SKIP_HOPELESS ? (d_second < best) : true;
+                    defer = (d_second < best);
                 }
-                if (!K1_SKIP_HOPELESS) defer = true;
                 depth++;
                 if (go_first) {                        // visit first now; second is re-tested when popped (:545-551)
                     if (defer) {
@@ -520,20 +445,8 @@ __device__ __forceinline__ QueryResult nearest_triangle(const MeshDev& M, bool a
                     state = POP;
                 }
             }
-#if K1_NODE_REPEAT
-            if (rep + 1 >= K1_NODE_REPEAT) break;
-            const int n_still = __popc(__ballot_sync(0xffffffffu, state == NODE));
-            if (2 * n_still < n_run || n_still == 0) break;
-            n_run = n_still;
-          }
-#endif
-        } else if (K1_LEAF_FILTER && w_leaff == w_max) {
-            if (state == LEAF) {
-                const float lb = leaf_lower_bound(M.leaves_f + b, qx, qy, qz, E);
-                state = (lb > skip_lin) ? POP : LEAFX;      // certainly not acceptable: the reference's test would fail
-            }
         } else {
-            if (state == (K1_LEAF_FILTER ? LEAFX : LEAF)) {                     // leaf (:517-534)
+            if (state == LEAF) {                                                // leaf (:517-534)
                 double s, t; int ent;
                 DG_EMU_COUNT(3);
                 const double d2 = tri_dist2(M.leaves + b, px, py, pz, s, t, ent);
@@ -542,8 +455,7 @@ __device__ __forceinline__ QueryResult nearest_triangle(const MeshDev& M, bool a
                     best = sqrt(d2);
                     best_sq = best * best;
                     best_lo = __double2float_rd(best); best_hi = __double2float_ru(best);
-                    { const float th = __fadd_ru(best_hi, E2); const bool ok = best_lo >= tiny_best;
-                      skip_sq = (K1_BOX_SKIP && ok) ? __fmul_ru(th, th) : __int_as_float(0x7f800000); skip_lin = ok ? th : __int_as_float(0x7f800000); }
+                    { const float th = __fadd_ru(best_hi, E2); skip_sq = (best_lo >= tiny_best) ? __fmul_ru(th, th) : __int_as_float(0x7f800000); }
                     res.s = s; res.t = t; res.pos = b; res.entity = ent;
                 }
                 state = POP;
@@ -572,7 +484,7 @@ __device__ __forceinline__ QueryResult nearest_triangle(const MeshDev& M, bool a
 //        here in fp64 exactly as the reference does (ref_visits_first).
 // So the packet walk only has to (a) evaluate, with the reference's own fp64 leaf test, every triangle whose v could be <= m (1 + 1e-6)
 // -- subtrees and leaves are dropped only by the CERTIFIED fp32 bounds of the box skip (true distance > best_hi + 2E  =>  v > m (1 + 2e-6),
-// error budget at K1_BOX_SKIP above) -- (b) keep the K1_PKT_K smallest values near the minimum with their leaf position, the largest ancestor
+// error budget at BOX SKIP above) -- (b) keep the K1_PKT_K smallest values near the minimum with their leaf position, the largest ancestor
 // certificate of any of them, and the smallest value it did not keep, (c) form C, check (i) and (ii), order C by (iii) and replay the reference's
 // accept rule.  A lane for which any check fails (on-surface queries below tiny_best, more than K1_PKT_K near-ties, a sphere that is tight
 // to within E, non-finite input) is walked again by nearest_triangle() -- the per-lane reference-order traversal above -- so the result is
@@ -821,8 +733,8 @@ extern __shared__ __align__(16) unsigned char k1_smem[];
 
 // addFunction node loop: out[l - l_begin] = sign * signed_distance(indexToNodePosition(l)).distance.
 // Thread mapping: the node array is four row-major 3-D arrays (vertices, x-, y-, z-edge nodes; K1Segment).  A warp
-// owns a 4 x 4 x 2 brick (fast x mid x slow) of one of them and a 128-thread block four bricks side by side along the
-// fast axis, so the 32 queries of a warp are spatial neighbours: they visit nearly the same tree nodes (L1 hits) and
+// owns a brick of 32 nodes (fast x mid x slow, shaped per array: k1_sdf.h) of one of them and a block K1_THREADS / 32 bricks
+// side by side along the fast axis, so the 32 queries of a warp are spatial neighbours: they visit nearly the same tree nodes (L1 hits) and
 // take similar numbers of steps.  Whole slow-planes are covered; nodes outside [l_begin, l_end) are masked.
 // BAND = true is the narrow-band form (sdf_sample_nodes_band_kernel): same walk, same replay, same fallback; only the block id comes from the
 // classifier's list and the epilogue keeps the value where |distance| <= band and writes DBL_MAX elsewhere.
@@ -842,17 +754,10 @@ __device__ __forceinline__ void sample_nodes_body(MeshDev mesh, const PseudoNorm
     const unsigned tf = t % S.tiles_f; t /= S.tiles_f;
     const unsigned tm = t % S.tiles_m; const unsigned ts = t / S.tiles_m;
     const unsigned lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
-#if K1_BRICK_AUTO
     const unsigned f = tf * (SEG_BF(S) * (unsigned)(K1_THREADS / 32)) + warp * SEG_BF(S) + (lane & (SEG_BF(S) - 1u));
     const unsigned m = tm * SEG_BM(S) + ((lane >> S.lf) & (SEG_BM(S) - 1u));
     const unsigned lane_s = lane >> (S.lf + S.lm);
     const unsigned sl = S.s0 + ts * S.pl_stride * SEG_BS(S) + lane_s;
-#else
-    const unsigned f = tf * (unsigned)(K1_BRICK_F * (K1_THREADS / 32)) + warp * (unsigned)K1_BRICK_F + (lane % K1_BRICK_F);
-    const unsigned m = tm * (unsigned)K1_BRICK_M + ((lane / K1_BRICK_F) % K1_BRICK_M);
-    const unsigned lane_s = lane / (K1_BRICK_F * K1_BRICK_M);
-    const unsigned sl = S.s0 + ts * S.pl_stride * (unsigned)K1_BRICK_S + lane_s;
-#endif
     const unsigned l = S.l_base + (sl * S.Dm + m) * S.Df + f;
     const bool alive = (f < S.Df) && (m < S.Dm) && (sl < S.s1) && (l >= w.l_begin) && (l < w.l_end);
 
@@ -912,64 +817,9 @@ sdf_sample_nodes_band_kernel(MeshDev mesh, const PseudoNormals* __restrict__ nor
     sample_nodes_body<true>(mesh, normals, stack_depth, g, w, sign, out, list[blockIdx.x], band);
 }
 
-#if K1_WAVE
-// =====================================================================================================================================
-// WAVEFRONT VARIANT OF THE NODE-LOOP KERNEL (K1_WAVE): persistent warps, queries decoupled from lanes, warp-ballot compaction.
-//
-// The per-lane kernel above keeps one query per lane for its whole walk; every iteration only the lanes whose query sits in the voted
-// phase do work (unequal walk lengths x phases out of step leave many lanes idle).  Here a WARP owns a pool of
-// K1_WAVE_SLOTS query slots in shared memory; every iteration it counts the slots per phase (one redux.sync), picks the fullest phase,
-// COMPACTS the slots of that phase onto lanes 0..n-1 (two ballots, a rank, a 32-entry work list in shared memory) and runs that phase's
-// straight-line block with (nearly) all lanes busy.  Slots whose query finished are refilled from the next brick of grid nodes (a
-// global atomic hands out bricks), so warps are persistent and there is no per-brick tail.  Each query still walks the tree in the
-// reference's own order with its own stack (shared memory, [depth][slot]) and its own running best: the arithmetic that reaches the
-// output is exactly that of the per-lane kernel -- only WHICH lane executes a step changes.  Stack entries are the packed range only
-// (4 bytes): the deferred sibling's fp32 sphere distance is recomputed from its parent's record when it is popped (the box test reads
-// that record anyway).
-// Slot state (SoA, per warp): meta (depth | sp | phase | entity, 4-byte stride: the home lanes' phase reads are conflict-free) | BE = {b, e} |
-// pos | Q = {qx, qy, qz, E} | B = {best_lo, best_hi, skip_sq, tiny_best} | best | p | s, t | out
-// =====================================================================================================================================
-enum { WP_NODE = 0, WP_LEAF = 1, WP_POP = 2, WP_FIN = 3, WP_EMPTY = 4, WP_LEAFX = 5 };     // K1_LEAF_FILTER: LEAF = fp32 filter pending, LEAFX = exact test due
-constexpr int WS = K1_WAVE_SLOTS;
-static_assert(WS == 64, "two home slots per lane");
-
-struct WaveSmem {
-    int* meta; int2* BE; int* pos; float4* Q; float4* B; double* best; double* px; double* py; double* pz; double* s; double* t; unsigned* out; unsigned* stack; unsigned* wl;
-};
-__host__ __device__ inline size_t wave_bytes_per_warp(int stack_depth) { return (size_t)WS * (16 + 16 + 16 + 8 + 24 + 16 + 4 + 4 * (size_t)stack_depth) + 64 * sizeof(unsigned); }
-
-__device__ __forceinline__ WaveSmem wave_carve(unsigned char* base, int stack_depth)
-{
-    WaveSmem w;
-    w.Q = reinterpret_cast<float4*>(base); base += WS * 16;
-    w.B = reinterpret_cast<float4*>(base); base += WS * 16;
-    w.best = reinterpret_cast<double*>(base); base += WS * 8;
-    w.px = reinterpret_cast<double*>(base); base += WS * 8;
-    w.py = reinterpret_cast<double*>(base); base += WS * 8;
-    w.pz = reinterpret_cast<double*>(base); base += WS * 8;
-    w.s = reinterpret_cast<double*>(base); base += WS * 8;
-    w.t = reinterpret_cast<double*>(base); base += WS * 8;
-    w.BE = reinterpret_cast<int2*>(base); base += WS * 8;
-    w.meta = reinterpret_cast<int*>(base); base += WS * 4;
-    w.pos = reinterpret_cast<int*>(base); base += WS * 4;
-    w.out = reinterpret_cast<unsigned*>(base); base += WS * 4;
-    w.stack = reinterpret_cast<unsigned*>(base); base += (size_t)WS * 4 * stack_depth;
-    w.wl = reinterpret_cast<unsigned*>(base);
-    return w;
-}
-
-#ifdef DG_EMU
-inline void dg_syncwarp() { dg_emu::collective_wait(0u); }
-#else
-__device__ __forceinline__ void dg_syncwarp() { __syncwarp(); }
-#endif
-
-__device__ __forceinline__ int wave_meta(int depth, int sp, int phase, int ent) { return depth | (sp << 8) | (phase << 16) | (ent << 20); }
-#endif  // K1_WAVE
-
-// grid node of lane `ln` of brick unit `unit` (= 2 * block + warp of the per-lane kernel's launch geometry): position, output index.
-// Used by the wavefront kernel and by the narrow-band classifier.
-__device__ __forceinline__ bool wave_brick_node(const GridDev& g, const K1Work& w, unsigned unit, unsigned ln, double& px, double& py, double& pz, unsigned& out_idx)
+// grid node of lane `ln` of brick unit `unit` (= K1_THREADS / 32 * block + warp of the node-loop kernel's launch geometry): position,
+// output index.  Used by the narrow-band classifier.
+__device__ __forceinline__ bool brick_node(const GridDev& g, const K1Work& w, unsigned unit, unsigned ln, double& px, double& py, double& pz, unsigned& out_idx)
 {
     const unsigned this_block = unit / (unsigned)(K1_THREADS / 32), warp = unit % (unsigned)(K1_THREADS / 32);
     int sg = 0;
@@ -979,17 +829,10 @@ __device__ __forceinline__ bool wave_brick_node(const GridDev& g, const K1Work& 
     unsigned t = this_block - S.block_begin;
     const unsigned tf = t % S.tiles_f; t /= S.tiles_f;
     const unsigned tm = t % S.tiles_m; const unsigned ts = t / S.tiles_m;
-#if K1_BRICK_AUTO
     const unsigned f = tf * (SEG_BF(S) * (unsigned)(K1_THREADS / 32)) + warp * SEG_BF(S) + (ln & (SEG_BF(S) - 1u));
     const unsigned m = tm * SEG_BM(S) + ((ln >> S.lf) & (SEG_BM(S) - 1u));
     const unsigned lane_s = ln >> (S.lf + S.lm);
     const unsigned sl = S.s0 + ts * S.pl_stride * SEG_BS(S) + lane_s;
-#else
-    const unsigned f = tf * (unsigned)(K1_BRICK_F * (K1_THREADS / 32)) + warp * (unsigned)K1_BRICK_F + (ln % K1_BRICK_F);
-    const unsigned m = tm * (unsigned)K1_BRICK_M + ((ln / K1_BRICK_F) % K1_BRICK_M);
-    const unsigned lane_s = ln / (K1_BRICK_F * K1_BRICK_M);
-    const unsigned sl = S.s0 + ts * S.pl_stride * (unsigned)K1_BRICK_S + lane_s;
-#endif
     const unsigned l = S.l_base + (sl * S.Dm + m) * S.Df + f;
     const bool alive = (f < S.Df) && (m < S.Dm) && (sl < S.s1) && (l >= w.l_begin) && (l < w.l_end);
     unsigned i, j, k;
@@ -1008,247 +851,6 @@ __device__ __forceinline__ bool wave_brick_node(const GridDev& g, const K1Work& 
     out_idx = w.compact ? S.out_base + ((ts * SEG_BS(S) + lane_s) * S.Dm + m) * S.Df + f : l - w.l_begin;
     return alive;
 }
-
-#if K1_WAVE
-__global__ void __launch_bounds__(K1_THREADS, K1_WAVE_MIN_BLOCKS)
-sdf_sample_nodes_wave_kernel(MeshDev M, const PseudoNormals* __restrict__ normals, int stack_depth, GridDev g, K1Work w, unsigned n_units, double sign,
-                             double* __restrict__ out, unsigned* __restrict__ unit_counter)
-{
-    const unsigned lane = threadIdx.x & 31u;
-    const WaveSmem W = wave_carve(k1_smem + (size_t)(threadIdx.x >> 5) * wave_bytes_per_warp(stack_depth), stack_depth);
-    const int n_tri = M.n_tri;
-    const unsigned lt_mask = (1u << lane) - 1u;
-    const float F_INF = __int_as_float(0x7f800000);
-    W.meta[lane] = wave_meta(0, 0, WP_EMPTY, 0);
-    W.meta[lane + 32] = wave_meta(0, 0, WP_EMPTY, 0);
-    unsigned cur_unit = 0, cur_off = 32;          // warp-uniform: the brick being handed out and how many of its 32 nodes are already in slots
-    bool more = n_units > 0;
-    dg_syncwarp();
-    for (;;) {
-        const int ph0 = (W.meta[lane] >> 16) & 15, ph1 = (W.meta[lane + 32] >> 16) & 15;
-        // one warp-wide sum carries the four live-phase counts (8 bits each; empty slots add nothing)
-        const unsigned tally = __reduce_add_sync(0xffffffffu, ((ph0 < WP_EMPTY) ? (1u << (8 * ph0)) : 0u) + ((ph1 < WP_EMPTY) ? (1u << (8 * ph1)) : 0u));
-        const int c_node = (int)(tally & 0xffu), c_leaf = (int)((tally >> 8) & 0xffu), c_pop = (int)((tally >> 16) & 0xffu), c_fin = (int)(tally >> 24);
-#if K1_LEAF_FILTER
-        const int c_leafx = __popc(__ballot_sync(0xffffffffu, ph0 == WP_LEAFX)) + __popc(__ballot_sync(0xffffffffu, ph1 == WP_LEAFX));
-#else
-        const int c_leafx = 0;
-#endif
-        const int c_live = c_node + c_leaf + c_pop + c_fin + c_leafx, c_empty = WS - c_live;
-        DG_EMU_COUNT(0);
-        int chosen;
-        if (more && c_empty >= K1_WAVE_REFILL) chosen = WP_EMPTY;                       // refill
-        else if (c_live == 0) break;                                                    // nothing left and no more bricks
-        else {
-            // the fullest phase runs (ties: leaf > node > pop > finish); a finished query only needs its result written, which is cheap,
-            // so FIN waits until it fills most of a warp or nothing else is ready
-            chosen = WP_LEAF; int c_best = c_leaf;
-            if (c_node > c_best) { chosen = WP_NODE; c_best = c_node; }
-            if (c_pop > c_best) { chosen = WP_POP; c_best = c_pop; }
-            if (c_leafx > c_best) { chosen = WP_LEAFX; c_best = c_leafx; }
-            if (c_fin > c_best || c_best == 0) { chosen = WP_FIN; c_best = c_fin; }
-        }
-        // compaction: slots in the chosen phase -> lanes 0..n-1
-        const bool in0 = (ph0 == chosen), in1 = (ph1 == chosen);
-        const unsigned b0 = __ballot_sync(0xffffffffu, in0), b1 = __ballot_sync(0xffffffffu, in1);
-        const int r0 = __popc(b0 & lt_mask), r1 = __popc(b0) + __popc(b1 & lt_mask);
-        if (in0 && r0 < 32) W.wl[r0] = lane;
-        if (in1 && r1 < 32) W.wl[r1] = lane + 32u;
-        int n_work = __popc(b0) + __popc(b1); if (n_work > 32) n_work = 32;
-#if K1_WAVE_HOME
-        // home-slot assignment: lane i only ever touches slots i and i + 32 (bank == lane for every state array: no shared-memory bank
-        // conflicts, no work list); a lane is busy when either of its two slots is in the chosen phase
-        const int home_slot = in0 ? (int)lane : (in1 ? (int)lane + 32 : -1);
-        if (chosen != WP_EMPTY) n_work = __popc(b0 | b1);
-#endif
-        if (lane == 0) { DG_EMU_ADD(10 + chosen, 1); DG_EMU_ADD(16 + chosen, n_work); }     // emulation only: phase executions and lanes used
-        if (chosen == WP_EMPTY) {
-            // ---- REFILL: next nodes of the current brick into free slots
-            if (cur_off >= 32u) {
-                if (lane == 0) W.wl[32] = atomicAdd(unit_counter, 1u);
-                dg_syncwarp();
-                cur_unit = W.wl[32]; cur_off = 0;
-                if (cur_unit >= n_units) { more = false; dg_syncwarp(); continue; }
-            } else dg_syncwarp();
-            unsigned take = 32u - cur_off; if (take > (unsigned)n_work) take = (unsigned)n_work;
-            if (lane < take) {
-                const int slot = (int)W.wl[lane];
-                double px, py, pz; unsigned oi;
-                if (wave_brick_node(g, w, cur_unit, cur_off + lane, px, py, pz, oi)) {
-                    const float qx = (float)(px - M.cx), qy = (float)(py - M.cy), qz = (float)(pz - M.cz);
-                    const float Mq = fmaxf(fmaxf(M.half_extent, fabsf(qx)), fmaxf(fabsf(qy), fabsf(qz)));
-                    const float E = filter_slack(Mq);                                                 // 64 * 2^-24 * Mq, or inf
-                    W.px[slot] = px; W.py[slot] = py; W.pz[slot] = pz; W.out[slot] = oi;
-                    W.Q[slot] = make_float4(qx, qy, qz, E);
-                    W.best[slot] = DBL_MAX; W.s[slot] = 0.0; W.t[slot] = 0.0;
-                    W.B[slot] = make_float4(__double2float_rd(DBL_MAX), __double2float_ru(DBL_MAX), F_INF, F_INF);       // best_lo, best_hi, skip_sq, skip_lin
-                    W.BE[slot] = make_int2(0, n_tri); W.pos[slot] = -1;
-                    W.meta[slot] = wave_meta(0, 0, (n_tri == 1) ? WP_LEAF : WP_NODE, 0);
-                }
-            }
-            cur_off += take;
-            dg_syncwarp();
-            continue;
-        }
-        dg_syncwarp();
-#if K1_WAVE_HOME
-        const int slot = home_slot;
-#else
-        const int slot = ((int)lane < n_work) ? (int)W.wl[lane] : -1;
-#endif
-        if (slot >= 0) {
-            const int2 be = W.BE[slot];
-            const int mt = W.meta[slot];
-            int b = be.x, e = be.y, depth = mt & 255, sp = (mt >> 8) & 255, ent = (mt >> 20) & 7, phase = chosen;
-            if (chosen == WP_NODE) {
-                // ---- internal node (:537-561): identical decisions to the per-lane kernel
-                DG_EMU_COUNT(1);
-                const float4 q = W.Q[slot], bb = W.B[slot];
-                const float qx = q.x, qy = q.y, qz = q.z, E = q.w, E2 = E + E, best_lo = bb.x, best_hi = bb.y, skip_sq = bb.z;
-                const int m = (b + e) >> 1;
-                bool left_first, go_first, go_second = false, defer = true, decided;
-                {
-                    const float4* f4 = M.nodes_f + (size_t)m * K1_NODEF_STRIDE;
-                    const float4 l4 = __ldg(f4), r4 = __ldg(f4 + 1);
-                    const float4 b0f = __ldg(f4 + 2), b1f = __ldg(f4 + 3), b2f = __ldg(f4 + 4);
-                    const float lx = qx - l4.x, ly = qy - l4.y, lz = qz - l4.z;
-                    const float rx = qx - r4.x, ry = qy - r4.y, rz = qz - r4.z;
-                    const float dl = sqrt_approx(fmaf(lz, lz, fmaf(ly, ly, lx * lx))) - l4.w;
-                    const float dr = sqrt_approx(fmaf(rz, rz, fmaf(ry, ry, rx * rx))) - r4.w;
-                    left_first = dl < dr;
-                    const float d_first_f = left_first ? dl : dr, d_second_f = left_first ? dr : dl;
-                    const bool order_sure = (d_first_f + E2 < d_second_f);
-                    go_first = (d_first_f + E < best_lo);
-                    const bool skip_first = (d_first_f - E >= best_hi);
-                    decided = order_sure && (go_first || skip_first);
-                    defer = !(d_second_f - E >= best_hi);
-                    if (decided && go_first) {
-                        const float lgx = fmaxf(fmaxf(b0f.x - qx, qx - b0f.w), 0.f), lgy = fmaxf(fmaxf(b0f.y - qy, qy - b1f.x), 0.f), lgz = fmaxf(fmaxf(b0f.z - qz, qz - b1f.y), 0.f);
-                        const float rgx = fmaxf(fmaxf(b1f.z - qx, qx - b2f.y), 0.f), rgy = fmaxf(fmaxf(b1f.w - qy, qy - b2f.z), 0.f), rgz = fmaxf(fmaxf(b2f.x - qz, qz - b2f.w), 0.f);
-                        const float l2 = __fmaf_rd(lgz, lgz, __fmaf_rd(lgy, lgy, __fmul_rd(lgx, lgx)));
-                        const float r2 = __fmaf_rd(rgz, rgz, __fmaf_rd(rgy, rgy, __fmul_rd(rgx, rgx)));
-                        const bool hopeless_first = (left_first ? l2 : r2) > skip_sq, hopeless_second = (left_first ? r2 : l2) > skip_sq;
-                        if (hopeless_second) defer = false;
-                        if (hopeless_first) {
-                            const bool second_yes = (d_second_f + E < best_lo), second_no = (d_second_f - E >= best_hi);
-                            if (second_yes || second_no) { go_first = false; go_second = second_yes && !hopeless_second; }
-                        }
-                    }
-                }
-                if (!decided) {                                                 // fp64, exactly the reference
-                    DG_EMU_COUNT(2);
-                    const double px = W.px[slot], py = W.py[slot], pz = W.pz[slot], best = W.best[slot];
-                    const double* sp8 = reinterpret_cast<const double*>(M.spheres + m);
-                    const double2 a0 = ldg2(sp8), a1 = ldg2(sp8 + 2), a2 = ldg2(sp8 + 4), a3 = ldg2(sp8 + 6);
-                    const double d_left = sphere_dist(px, py, pz, a0.x, a0.y, a1.x, a1.y);      // :539
-                    const double d_right = sphere_dist(px, py, pz, a2.x, a2.y, a3.x, a3.y);     // :540
-                    left_first = d_left < d_right;                                            // :542
-                    const double d_first = left_first ? d_left : d_right, d_second = left_first ? d_right : d_left;
-                    go_first = d_first < best;                                                // :545 / :554
-                    go_second = !go_first && (d_second < best);
-                    defer = (d_second < best);
-                }
-                depth++;
-                if (go_first) {
-                    if (defer) {
-                        DG_EMU_COUNT(9);
-                        W.stack[sp * WS + slot] = left_first ? pack_range(m, e, depth, n_tri, false) : pack_range(b, m, depth, n_tri, true);
-                        sp++;
-                    }
-                    if (left_first) e = m; else b = m;
-                    phase = (e - b == 1) ? WP_LEAF : WP_NODE;
-                } else if (go_second) {
-                    if (left_first) b = m; else e = m;
-                    phase = (e - b == 1) ? WP_LEAF : WP_NODE;
-                } else phase = WP_POP;
-#if K1_LEAF_FILTER
-            } else if (chosen == WP_LEAF) {
-                // ---- leaf, fp32 filter: a certified lower bound of the point-triangle distance above best + slack means the reference's
-                // test would fail (nothing changes): straight to POP.  Everything else takes the exact test in the LEAFX phase.
-                const float4 q = W.Q[slot];
-                const float lb = leaf_lower_bound(M.leaves_f + b, q.x, q.y, q.z, q.w);
-                phase = (lb > W.B[slot].w) ? WP_POP : WP_LEAFX;
-            } else if (chosen == WP_LEAFX) {
-#else
-            } else if (chosen == WP_LEAF) {
-#endif
-                // ---- leaf (:517-534)
-                DG_EMU_COUNT(3);
-                const double px = W.px[slot], py = W.py[slot], pz = W.pz[slot], best = W.best[slot];
-                const double best_sq = best * best;                            // result.distance * result.distance (+inf initially), :528
-                double s, t; int en;
-                const double d2 = tri_dist2(M.leaves + b, px, py, pz, s, t, en);
-                if (d2 < best_sq) {
-                    DG_EMU_COUNT(4);
-                    const double nb = sqrt(d2);
-                    const float4 q = W.Q[slot];
-                    const float E2 = q.w + q.w;
-                    const float tiny_best = 1.0e-6f * fmaxf(fmaxf(M.half_extent, fabsf(q.x)), fmaxf(fabsf(q.y), fabsf(q.z)));
-                    const float best_lo = __double2float_rd(nb), best_hi = __double2float_ru(nb);
-                    const float th = __fadd_ru(best_hi, E2);
-                    const bool ok = best_lo >= tiny_best;                   // nothing is skipped for queries practically on the surface
-                    W.best[slot] = nb; W.s[slot] = s; W.t[slot] = t;
-                    W.B[slot] = make_float4(best_lo, best_hi, (K1_BOX_SKIP && ok) ? __fmul_ru(th, th) : F_INF, ok ? th : F_INF);
-                    W.pos[slot] = b; ent = en;
-                }
-                phase = WP_POP;
-            } else if (chosen == WP_POP) {
-                // ---- deferred siblings: the reference's second `if (d < result.distance)` (:549, :557) with the updated best
-                const float4 q = W.Q[slot], bb = W.B[slot];
-                const float qx = q.x, qy = q.y, qz = q.z, E = q.w, best_lo = bb.x, best_hi = bb.y, skip_sq = bb.z;
-#pragma unroll 1
-                for (int attempt = 0; attempt < K1_POP_TRIES; attempt++) {
-                    if (sp == 0) { phase = WP_FIN; break; }
-                    sp--;
-                    DG_EMU_COUNT(5);
-                    const unsigned r = W.stack[sp * WS + slot];
-                    const int rb = (int)(r & 0x01ffffffu), rd = (int)((r >> 25) & 31u);
-                    const int re = rb + (n_tri >> rd) + (int)((r >> 30) & 1u);
-                    const bool is_left = (r >> 31) != 0u;
-                    const int pm = is_left ? re : rb;                          // the parent's split position: its record holds this child's sphere and box
-                    const float4* f4 = M.nodes_f + (size_t)pm * K1_NODEF_STRIDE;
-                    const float4 c4 = __ldg(f4 + (is_left ? 0 : 1));
-                    const float cx = qx - c4.x, cy = qy - c4.y, cz = qz - c4.z;
-                    const float df = sqrt_approx(fmaf(cz, cz, fmaf(cy, cy, cx * cx))) - c4.w;
-                    bool visit = (df + E < best_lo);                           // certainly d < best
-                    const bool skip = (df - E >= best_hi);                     // certainly d >= best
-                    if (!(visit || skip)) {                                    // undecided in fp32: the reference's fp64 value
-                        DG_EMU_COUNT(6);
-                        const double* s8 = reinterpret_cast<const double*>(M.spheres + pm) + (is_left ? 0 : 4);
-                        const double2 c0 = ldg2(s8), c1 = ldg2(s8 + 2);
-                        visit = sphere_dist(W.px[slot], W.py[slot], W.pz[slot], c0.x, c0.y, c1.x, c1.y) < W.best[slot];
-                    }
-                    if (visit) {
-#if K1_BOX_SKIP
-                        const float4* bq = f4 + (is_left ? 2 : 3);            // the child's box: two of the record's three box quads
-                        const float4 u = __ldg(bq), v = __ldg(bq + 1);
-                        const float lox = is_left ? u.x : u.z, loy = is_left ? u.y : u.w, loz = is_left ? u.z : v.x;
-                        const float hix = is_left ? u.w : v.y, hiy = is_left ? v.x : v.z, hiz = is_left ? v.y : v.w;
-                        const float gx = fmaxf(fmaxf(lox - qx, qx - hix), 0.f), gy = fmaxf(fmaxf(loy - qy, qy - hiy), 0.f), gz = fmaxf(fmaxf(loz - qz, qz - hiz), 0.f);
-                        if (__fmaf_rd(gz, gz, __fmaf_rd(gy, gy, __fmul_rd(gx, gx))) > skip_sq) { DG_EMU_COUNT(7); continue; }   // visiting it could not change anything
-#endif
-                        b = rb; depth = rd; e = re;
-                        phase = (e - b == 1) ? WP_LEAF : WP_NODE;
-                        break;
-                    }
-                }
-            } else {
-                // ---- finished: nearest point + pseudonormal sign, coefficient out, slot free
-                QueryResult r;
-                r.dist = W.best[slot]; r.s = W.s[slot]; r.t = W.t[slot]; r.pos = W.pos[slot]; r.entity = ent;
-                const double px = W.px[slot], py = W.py[slot], pz = W.pz[slot];
-                double dist, qx, qy, qz; int tri;
-                finish_query(M.leaves, normals, r, px, py, pz, true, dist, qx, qy, qz, tri);
-                out[W.out[slot]] = (sign == 1.0) ? dist : sign * dist;           // cmd/generate_sdf/main.cpp:97 (-1.0 * d) / :101
-                phase = WP_EMPTY;
-            }
-            if (chosen == WP_NODE || chosen == WP_POP) W.BE[slot] = make_int2(b, e);
-            W.meta[slot] = wave_meta(depth, sp, phase, ent);
-        }
-        dg_syncwarp();
-    }
-}
-#endif  // K1_WAVE
 
 // =====================================================================================================================================
 // NARROW-BAND CLASSIFIER.  addFunction(func, pred) with pred(x) = |md.signed_distance(x).distance| <= band (cubic_lagrange_discrete_grid.cpp:
@@ -1306,7 +908,7 @@ __device__ bool band_box_near_mesh(const MeshDev M, const float* lo, const float
     }
 }
 
-// one thread per brick (unit = K1_BRICKS * block + warp, as wave_brick_node numbers them); keep[block] = any of its bricks may be in the band;
+// one thread per brick (unit = K1_BRICKS * block + warp, as brick_node numbers them); keep[block] = any of its bricks may be in the band;
 // the in-range nodes of a dropped block get DBL_MAX
 __global__ void __launch_bounds__(K1_BAND_THREADS)
 band_classify_kernel(MeshDev M, GridDev g, K1Work w, unsigned n_blocks, double band, double* __restrict__ out, unsigned char* __restrict__ keep)
@@ -1320,7 +922,7 @@ band_classify_kernel(MeshDev M, GridDev g, K1Work w, unsigned n_blocks, double b
     if (live) {
         for (unsigned ln = 0; ln < 32u; ln++) {
             double p[3]; unsigned oi;
-            if (!wave_brick_node(g, w, unit, ln, p[0], p[1], p[2], oi)) continue;
+            if (!brick_node(g, w, unit, ln, p[0], p[1], p[2], oi)) continue;
             any = true;
             for (int k = 0; k < 3; k++) {
                 if (!(fabs(p[k]) <= DBL_MAX)) finite = false;
@@ -1353,7 +955,7 @@ band_classify_kernel(MeshDev M, GridDev g, K1Work w, unsigned n_blocks, double b
     if (any && !block_kept) {
         for (unsigned ln = 0; ln < 32u; ln++) {
             double px, py, pz; unsigned oi;
-            if (wave_brick_node(g, w, unit, ln, px, py, pz, oi)) out[oi] = DBL_MAX;
+            if (brick_node(g, w, unit, ln, px, py, pz, oi)) out[oi] = DBL_MAX;
         }
     }
 }
@@ -1496,65 +1098,6 @@ cudaError_t k1_configure(int stack_depth)
 #endif
 }
 
-#if K1_WAVE
-// persistent launch of the wavefront kernel: one resident wave of blocks, bricks handed out by a global counter
-static cudaError_t launch_sampling_wave(const DeviceBvh& m, const GridDev& g, const K1Work& w, unsigned blocks, double sign, double* d_out, cudaStream_t stream)
-{
-    const unsigned n_units = blocks * (unsigned)(K1_THREADS / 32);
-    const size_t smem = (size_t)(K1_THREADS / 32) * wave_bytes_per_warp(m.stack_depth);
-#ifdef DG_EMU
-    static unsigned counter;
-    counter = 0;
-    const unsigned grid = blocks < 3u ? blocks : 3u;
-    DG_KERNEL_LAUNCH(sdf_sample_nodes_wave_kernel, grid, K1_THREADS, smem, stream, mesh_dev(m), m.normals, m.stack_depth, g, w, n_units, sign, d_out, &counter);
-    return cudaSuccess;
-#else
-    // per device: a ring of brick counters (a launch zeroes its own on its stream, so launches on different streams never share one)
-    // and the resident-block count of the kernel for this shared-memory size
-    struct PerDev { unsigned* counters = nullptr; unsigned next = 0; int sm = 0; int resident[64] = {0}; };
-    static std::mutex mu;
-    static PerDev per[64];
-    int dev = 0;
-    cudaError_t e = cudaGetDevice(&dev);
-    if (e != cudaSuccess) return e;
-    if (dev < 0 || dev >= 64) return cudaErrorInvalidDevice;
-    unsigned* counter; int resident, sm;
-    {
-        std::lock_guard<std::mutex> lock(mu);
-        PerDev& P = per[dev];
-        if (!P.counters) {
-            e = cudaMalloc(reinterpret_cast<void**>(&P.counters), 256 * sizeof(unsigned));
-            if (e != cudaSuccess) return e;
-            e = cudaDeviceGetAttribute(&P.sm, cudaDevAttrMultiProcessorCount, dev);
-            if (e != cudaSuccess) return e;
-        }
-        const int dkey = m.stack_depth < 64 ? m.stack_depth : 63;
-        if (!P.resident[dkey]) {
-            if (smem > 48 * 1024) { e = cudaFuncSetAttribute(sdf_sample_nodes_wave_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); if (e != cudaSuccess) return e; }
-            int nb = 0;
-            e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, sdf_sample_nodes_wave_kernel, K1_THREADS, smem);
-            if (e != cudaSuccess) return e;
-            P.resident[dkey] = nb > 0 ? nb : 1;
-        }
-        counter = P.counters + (P.next++ & 255u);
-        resident = P.resident[dkey]; sm = P.sm;
-    }
-    e = cudaMemsetAsync(counter, 0, sizeof(unsigned), stream);
-    if (e != cudaSuccess) return e;
-    const unsigned full = (unsigned)(resident * sm);
-    const unsigned grid = blocks < full ? blocks : full;
-    DG_KERNEL_LAUNCH(sdf_sample_nodes_wave_kernel, grid, K1_THREADS, smem, stream, mesh_dev(m), m.normals, m.stack_depth, g, w, n_units, sign, d_out, counter);
-    return DG_AFTER_LAUNCH();
-#endif
-}
-#define DG_LAUNCH_SAMPLING(m, g, w, blocks, sign, out, stream) return launch_sampling_wave((m), (g), (w), (blocks), (sign), (out), (stream))
-#else
-#define DG_LAUNCH_SAMPLING(m, g, w, blocks, sign, out, stream) \
-    DG_KERNEL_LAUNCH(sdf_sample_nodes_kernel, (blocks), K1_THREADS, k1_smem_bytes((m).stack_depth), (stream), mesh_dev(m), (m).normals, (m).stack_depth, (g), (w), (sign), (out)); \
-    return DG_AFTER_LAUNCH()
-#endif
-
-#if K1_BRICK_AUTO
 // brick shape of node array `kind`: (lf, lm, ls) with lf + lm + ls = 5 and lf >= 1 minimising the physical diagonal of the 32 nodes.
 // Node spacing along (f, m, s): vertices (cx, cy, cz); x-edge nodes (cx/2, cy, cz); y-edge (cy/2, cz, cx); z-edge (cz/2, cx, cy).
 static void choose_brick(const GridDev& g, int kind, unsigned& lf, unsigned& lm)
@@ -1571,10 +1114,6 @@ static void choose_brick(const GridDev& g, int kind, unsigned& lf, unsigned& lm)
             if (d < best * (1.0 - 1e-9)) { best = d; lf = a; lm = b; }
         }
 }
-#define SEG_SET_BRICK(S, g) choose_brick((g), (S).kind, (S).lf, (S).lm)
-#else
-#define SEG_SET_BRICK(S, g)
-#endif
 
 // Splits [l_begin, l_begin+count) into the (at most four) node arrays it touches and tiles whole slow-planes of each.
 static unsigned node_range_work(const GridDev& g, uint64_t l_begin, uint64_t count, K1Work& w)
@@ -1598,7 +1137,7 @@ static unsigned node_range_work(const GridDev& g, uint64_t l_begin, uint64_t cou
         S.pl_stride = 1u; S.out_base = 0u;
         S.s0 = (unsigned)((a - base[k]) / plane);
         S.s1 = (unsigned)((b - 1 - base[k]) / plane) + 1;
-        SEG_SET_BRICK(S, g);
+        choose_brick(g, S.kind, S.lf, S.lm);
         const unsigned bf = SEG_BF(S) * (K1_THREADS / 32);
         S.tiles_f = (S.Df + bf - 1) / bf; S.tiles_m = (S.Dm + SEG_BM(S) - 1) / SEG_BM(S);
         const unsigned tiles_s = (S.s1 - S.s0 + SEG_BS(S) - 1) / SEG_BS(S);
@@ -1615,7 +1154,8 @@ cudaError_t k1_launch_sample_nodes(const DeviceBvh& m, const GridDev& g, double 
     if (count == 0) return cudaSuccess;
     K1Work w;
     const unsigned blocks = node_range_work(g, l_begin, count, w);
-    DG_LAUNCH_SAMPLING(m, g, w, blocks, sign, d_out, stream);
+    DG_KERNEL_LAUNCH(sdf_sample_nodes_kernel, blocks, K1_THREADS, k1_smem_bytes(m.stack_depth), stream, mesh_dev(m), m.normals, m.stack_depth, g, w, sign, d_out);
+    return DG_AFTER_LAUNCH();
 }
 
 // scratch of the band form: keep flag per block (bytes), count per chunk, the list, its length
@@ -1676,7 +1216,7 @@ cudaError_t k1_launch_sample_slab(const DeviceBvh& m, const GridDev& g, double s
         S.kind = k; S.l_base = (unsigned)base[k];
         S.Ds = dims[k][0]; S.Dm = dims[k][1]; S.Df = dims[k][2];
         S.s0 = plane_begin[k]; S.s1 = plane_end[k]; S.pl_stride = 1u; S.out_base = 0u;
-        SEG_SET_BRICK(S, g);
+        choose_brick(g, S.kind, S.lf, S.lm);
         const unsigned bf = SEG_BF(S) * (K1_THREADS / 32);
         S.tiles_f = (S.Df + bf - 1) / bf; S.tiles_m = (S.Dm + SEG_BM(S) - 1) / SEG_BM(S);
         const unsigned tiles_s = (S.s1 - S.s0 + SEG_BS(S) - 1) / SEG_BS(S);
@@ -1685,7 +1225,8 @@ cudaError_t k1_launch_sample_slab(const DeviceBvh& m, const GridDev& g, double s
     }
     if (w.nseg == 0) return cudaSuccess;
     for (int k = w.nseg; k < 4; k++) { w.seg[k] = w.seg[0]; w.seg[k].block_begin = 0xffffffffu; }
-    DG_LAUNCH_SAMPLING(m, g, w, blocks, sign, d_full, stream);
+    DG_KERNEL_LAUNCH(sdf_sample_nodes_kernel, blocks, K1_THREADS, k1_smem_bytes(m.stack_depth), stream, mesh_dev(m), m.normals, m.stack_depth, g, w, sign, d_full);
+    return DG_AFTER_LAUNCH();
 }
 
 static void node_arrays(const GridDev& g, uint64_t base[4], unsigned dims[4][3])
@@ -1702,9 +1243,7 @@ bool k1_interleaved_layout(const GridDev& g, unsigned n_parts, InterleavedLayout
     uint64_t base[4]; unsigned dims[4][3];
     node_arrays(g, base, dims);
     L.n_parts = n_parts; L.slot_elems = 0;
-#if K1_BRICK_AUTO
     for (int a = 0; a < 4; a++) choose_brick(g, a, L.lf[a], L.lm[a]);
-#endif
     for (int a = 0; a < 4; a++) { L.pairs[a] = (dims[a][0] + LAY_BS(L, a) - 1) / LAY_BS(L, a); L.plane[a] = dims[a][1] * dims[a][2]; L.rot[a] = ((unsigned)a * (n_parts >= 4 ? n_parts / 4 : 1u)) % n_parts; }
     for (unsigned part = 0; part < n_parts; part++) {
         uint64_t off = 0;
@@ -1736,9 +1275,7 @@ cudaError_t k1_launch_sample_interleaved(const DeviceBvh& m, const GridDev& g, d
         K1Segment& S = w.seg[w.nseg++];
         S.kind = k; S.l_base = (unsigned)base[k];
         S.Ds = dims[k][0]; S.Dm = dims[k][1]; S.Df = dims[k][2];
-#if K1_BRICK_AUTO
         S.lf = L.lf[k]; S.lm = L.lm[k];
-#endif
         S.s0 = first * SEG_BS(S); S.s1 = S.Ds; S.pl_stride = L.n_parts; S.out_base = L.off[k][part];
         const unsigned bf = SEG_BF(S) * (K1_THREADS / 32);
         S.tiles_f = (S.Df + bf - 1) / bf; S.tiles_m = (S.Dm + SEG_BM(S) - 1) / SEG_BM(S);
@@ -1747,7 +1284,8 @@ cudaError_t k1_launch_sample_interleaved(const DeviceBvh& m, const GridDev& g, d
     }
     if (w.nseg == 0) return cudaSuccess;
     for (int k = w.nseg; k < 4; k++) { w.seg[k] = w.seg[0]; w.seg[k].block_begin = 0xffffffffu; }
-    DG_LAUNCH_SAMPLING(m, g, w, blocks, sign, d_slot, stream);
+    DG_KERNEL_LAUNCH(sdf_sample_nodes_kernel, blocks, K1_THREADS, k1_smem_bytes(m.stack_depth), stream, mesh_dev(m), m.normals, m.stack_depth, g, w, sign, d_slot);
+    return DG_AFTER_LAUNCH();
 }
 
 // node id -> (part, position inside that part's slot): the one statement of the exchange layout, shared by the unpack kernel and the host

@@ -25,51 +25,8 @@ constexpr int K1_THREADS = K1_THREADS_PER_BLOCK;
 #ifndef K1_POP_TRIES
 #define K1_POP_TRIES 4          // deferred siblings re-tested per POP phase and lane
 #endif
-#ifndef K1_POP_MERGED
-#define K1_POP_MERGED 0         // 1: POP lanes re-test siblings at the end of every iteration; 0: POP is a phase of its own
-#endif
-#ifndef K1_LEAF_MODE
-#define K1_LEAF_MODE 0          // leaf arithmetic: 0 compiler's branches, 1 fully straight-line, 2 one guarded division + one guarded quadratic form
-#endif
-#ifndef K1_FILTER
-#define K1_FILTER 1             // 1: fp32 interval filter for the sphere decisions (exact fp64 fallback); 0: all fp64
-#endif
-#ifndef K1_LEAF_FILTER
-#define K1_LEAF_FILTER 0         // 1: reject leaf tests whose certified fp32 lower bound exceeds the best, as a phase of its own.
-                                // Exact (all parity tests pass), but the extra phase costs more iterations than the fp64 tests it
-                                // saves.  Off.
-#endif
-#ifndef K1_LEAFF_WEIGHT
-#define K1_LEAFF_WEIGHT 2
-#endif
-// brick of nodes owned by one warp: fast x mid x slow = 32
-#ifndef K1_BRICK_F
-#define K1_BRICK_F 4
-#endif
-#ifndef K1_BRICK_M
-#define K1_BRICK_M 4
-#endif
-#ifndef K1_BRICK_S
-#define K1_BRICK_S 2
-#endif
-static_assert(K1_BRICK_F * K1_BRICK_M * K1_BRICK_S == 32, "a brick is one warp");
-#ifndef K1_NODE_REPEAT
-#define K1_NODE_REPEAT 0         // >0: up to this many consecutive node steps per phase vote (while >= half of the lanes stay at internal nodes)
-#endif
-#ifndef K1_PREFETCH
-#define K1_PREFETCH 0            // prefetch.global.L1 of both children's records during a node step
-#endif
 #ifndef K1_NODEF_STRIDE
 #define K1_NODEF_STRIDE 5         // float4s per fp32 node record: 5 = packed 80 B, 6 = padded to 96 B
-#endif
-#ifndef K1_EARLY_BOX
-#define K1_EARLY_BOX 1           // issue the box loads together with the sphere loads (latency) instead of after the sphere decision
-#endif
-#ifndef K1_BOX_SKIP
-#define K1_BOX_SKIP 1           // skip subtrees whose box is certainly farther than the best (they cannot change the result)
-#endif
-#ifndef K1_SKIP_HOPELESS
-#define K1_SKIP_HOPELESS 1      // do not stack a sibling whose sphere is already certainly farther than the best
 #endif
 #ifndef K1_MIN_BLOCKS
 #define K1_MIN_BLOCKS (1024 / K1_THREADS_PER_BLOCK)   // blocks per SM the register allocation must allow (32 warps)
@@ -88,41 +45,16 @@ static_assert(K1_BRICK_F * K1_BRICK_M * K1_BRICK_S == 32, "a brick is one warp")
 #ifndef K1_PKT_MIN_BLOCKS
 #define K1_PKT_MIN_BLOCKS 14
 #endif
-#define K1_NEEDS_LEAF_SHADOW (K1_LEAF_FILTER || K1_PACKET)     // the fp32 triangle shadows (LeafF) are built and uploaded
-// K1_WAVE 1: the node-loop kernel is the WAVEFRONT variant (k1_sdf.cu): persistent warps, a pool of K1_WAVE_SLOTS query slots per warp in
-// shared memory, per iteration the fullest phase is compacted onto the lanes by ballot.  0: the per-lane kernel (one query per lane).
-#ifndef K1_WAVE
-#define K1_WAVE 0
-#endif
-#ifndef K1_WAVE_SLOTS
-#define K1_WAVE_SLOTS 64           // query slots per warp (two home slots per lane)
-#endif
-#ifndef K1_WAVE_HOME
-#define K1_WAVE_HOME 0             // 1: no compaction across lanes -- a lane serves only its two home slots (conflict-free shared memory)
-#endif
-#ifndef K1_WAVE_REFILL
-#define K1_WAVE_REFILL 16          // refill from the next brick as soon as this many slots are free
-#endif
-#ifndef K1_WAVE_MIN_BLOCKS
-#define K1_WAVE_MIN_BLOCKS 10      // blocks of K1_THREADS per SM the register allocation must allow (shared memory allows about as many)
-#endif
 
 // One of the four row-major 3-D node arrays of the grid (vertex nodes, x-/y-/z-edge nodes), restricted to the
 // slow-planes [s0, s1) that a node range touches.  l = l_base + (s*Dm + m)*Df + f.
-// K1_BRICK_AUTO 1: the warp's brick is chosen per node array at launch time -- the power-of-two shape (f x m x s, 32 nodes) whose PHYSICAL
-// diagonal is shortest -- instead of the fixed K1_BRICK_F x K1_BRICK_M x K1_BRICK_S.  On cubic cells that is the default 4 x 4 x 2
-// (x-edge arrays: their node spacing along f is half a cell); on strongly anisotropic cells (a flat bounding box sampled with a cubic
-// resolution) a flatter brick keeps the 32 queries closer together (CPU schedule model: -6 % issued instructions on the bench torus).
-// Checked against the oracle by the emulated test builds (on and off).
-#ifndef K1_BRICK_AUTO
-#define K1_BRICK_AUTO 1
-#endif
-
+// The warp's brick is chosen per node array at launch time: the power-of-two shape (f x m x s, 32 nodes) whose PHYSICAL diagonal is
+// shortest.  On cubic cells that is 4 x 4 x 2 (x-edge arrays: their node spacing along f is half a cell); on strongly anisotropic cells
+// (a flat bounding box sampled with a cubic resolution) a flatter brick keeps the 32 queries closer together than a fixed 4 x 4 x 2
+// (CPU schedule model: -6 % issued instructions on the bench torus).
 struct K1Segment {
     unsigned l_base, Ds, Dm, Df, s0, s1, tiles_f, tiles_m, tiles_s, block_begin;
-#if K1_BRICK_AUTO
     unsigned lf, lm;               // log2 of the brick's extents along f and m (s extent = 32 >> (lf + lm))
-#endif
     unsigned pl_stride;            // plane groups between consecutive brick layers (1 = contiguous slab, n_parts = interleaved deal)
     unsigned out_base;             // interleaved mode: element offset of this array inside the part's exchange slot
     int kind;                      // 0 vertex (s,m,f)=(k,j,i); 1 x-edge (k,j,2i+b); 2 y-edge (i,k,2j+b); 3 z-edge (j,i,2k+b)
@@ -134,17 +66,11 @@ struct K1Work {
     int compact;                   // 0: out[l - l_begin]; 1: interleaved exchange slot (see k1_launch_sample_interleaved)
 };
 
-// K1_VOTE_REDUX 1: the phase vote reads the three lane counts from ONE warp-wide integer sum (redux.sync) instead of two ballots +
-// three popcounts (the loop head is ~19 % of the issued instructions).
-#ifndef K1_VOTE_REDUX
-#define K1_VOTE_REDUX 1
-#endif
-
 struct DeviceBvh {                 // device mirrors of HostBvh, uploaded once by dg_mesh_create
     const SpherePair* spheres = nullptr;
     const LeafRecord* leaves = nullptr;
     const PseudoNormals* normals = nullptr;
-    const LeafF* leaves_f = nullptr;            // fp32 triangle shadows (leaf filter)
+    const LeafF* leaves_f = nullptr;            // fp32 triangle shadows (the packet walk's leaf bound)
     const float4* nodes_f = nullptr;          // fp32 record per internal node, K1_NODEF_STRIDE float4s: SpherePairF (2) + BoxPairF (3) [+ pad]
     double ctr[3] = {0, 0, 0};
     float half_extent = 0.f;
@@ -176,9 +102,7 @@ struct InterleavedLayout {
     unsigned pairs[4];             // plane pairs of array a
     unsigned plane[4];             // elements per plane of array a
     uint64_t slot_elems = 0;       // elements per slot (max over parts)
-#if K1_BRICK_AUTO
     unsigned lf[4], lm[4];         // brick shape of array a (its plane groups are 32 >> (lf + lm) planes thick)
-#endif
 };
 bool k1_interleaved_layout(const GridDev& g, unsigned n_parts, InterleavedLayout& L);
 cudaError_t k1_launch_sample_interleaved(const DeviceBvh& m, const GridDev& g, double sign, const InterleavedLayout& L, unsigned part,

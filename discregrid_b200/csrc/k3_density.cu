@@ -37,12 +37,6 @@
 #include "fast_div.h"
 #include "dg_launch.h"
 
-// K3_FAST_DIV 1: gamma's d / h (one fp64 division per quadrature point, ~33 of ~400 instructions) through the reciprocal of h.
-// Bit-identical output either way (fast_div.h); 0 keeps the IEEE division.
-#ifndef K3_FAST_DIV
-#define K3_FAST_DIV 1
-#endif
-
 #include <algorithm>
 #include <cfloat>
 #include <climits>
@@ -74,9 +68,7 @@ struct QuadParams {
     double off[16];      // c0*xi + c1 per axis point (identical on the three axes: the domain is a cube)
     double w[16];
     double h, two_h, six_h_neg, rho0, c0prod, cell_diag;
-#if K3_FAST_DIV
     double inv_h;        // RN(1/h)
-#endif
 };
 
 // value-only interpolate (cubic_lagrange_discrete_grid.cpp:977-1023) reading the packed block through L1
@@ -156,9 +148,7 @@ density_map_kernel(FieldDev f, QuadParams qp, const double* __restrict__ Wtab, i
     const double dist = interp_value(f, x, y, z);                   // main.cpp:98
     if (dist > qp.two_h) { out[idx] = 0.0; return; }
     double res = 0.0;
-#if K3_FAST_DIV
     const bool fast_h = in_fast_div_range(qp.h);
-#endif
     for (int i = 0; i < 16; i++) {
         const double wi = qp.w[i], sx = x + qp.off[i];
         for (int j = 0; j < 16; j++) {
@@ -170,15 +160,12 @@ density_map_kernel(FieldDev f, QuadParams qp, const double* __restrict__ Wtab, i
                 if (SKIP_ZERO_W && W == 0.0) continue;               // contributes exactly +0 (see header)
                 const double wijk = wij * qp.w[k];
                 const double d = interp_value(f, sx, sy, z + qp.off[k]);
-#if K3_FAST_DIV
                 // d / h with h a launch constant: the same IEEE quotient from RN(1/h) and four FMAs (fast_div.h); plain division
-                // when d is zero or outside the range where nothing can over- or underflow
+                // when d is zero or outside the range where nothing can over- or underflow.  The division is ~33 of the ~400
+                // instructions per quadrature point, and this form was measured faster than it.
                 double dq = div_by_known_reciprocal(d, qp.h, qp.inv_h);
                 if (!(fast_h && in_fast_div_range(d))) dq = d / qp.h;
                 const double gam = (d > qp.h) ? 0.0 : 1.0 - dq;         // main.cpp:86-93
-#else
-                const double gam = (d > qp.h) ? 0.0 : 1.0 - d / qp.h;   // main.cpp:86-93
-#endif
                 res = res + wijk * (gam * W);                        // gauss_quadrature.cpp:5954
             }
         }
@@ -254,9 +241,7 @@ cudaError_t k3_launch_density(const FieldDev& f, double coeff_max, double h, dou
     const double c0 = 0.5 * (hi - lo), c1 = 0.5 * (lo + hi);
     for (int i = 0; i < 16; i++) { qp.off[i] = c0 * GA16[i] + c1; qp.w[i] = GW16[i]; }
     qp.h = h; qp.two_h = 2.0 * h; qp.six_h_neg = -6.0 * h; qp.rho0 = rho0;
-#if K3_FAST_DIV
     qp.inv_h = 1.0 / h;
-#endif
     qp.c0prod = c0 * c0 * c0;                                        // Eigen prod(): (c0*c0)*c0
     qp.cell_diag = k3_cell_diag(f.g);
     // W at the 4096 points (sph_kernel.hpp:10-42): k = 8/(pi h^3)

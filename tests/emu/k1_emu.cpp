@@ -36,13 +36,13 @@ void* emu_mesh_create(const double* V, uint64_t nV, const uint32_t* F, uint64_t 
 {
     auto* m = new EmuMesh();
     const char* err = "";
-    if (!build_host_bvh(V, nV, F, nT, m->host, &err, K1_NEEDS_LEAF_SHADOW != 0)) { std::fprintf(stderr, "emu_mesh_create: %s\n", err); delete m; return nullptr; }
+    if (!build_host_bvh(V, nV, F, nT, m->host, &err, true)) { std::fprintf(stderr, "emu_mesh_create: %s\n", err); delete m; return nullptr; }
     // the interleaved fp32 node record, as dg_mesh_create lays it out
     m->nodes_f.assign((size_t)nT * K1_NODEF_STRIDE, make_float4(0.f, 0.f, 0.f, 0.f));
     pack_node_records(m->host, K1_NODEF_STRIDE, reinterpret_cast<float*>(m->nodes_f.data()));
     DeviceBvh& d = m->dev;
     d.spheres = m->host.spheres.data(); d.leaves = m->host.leaves.data(); d.normals = m->host.normals.data();
-    d.leaves_f = m->host.leaves_f.empty() ? nullptr : m->host.leaves_f.data();
+    d.leaves_f = m->host.leaves_f.data();
     d.nodes_f = m->nodes_f.data();
     for (int k = 0; k < 3; k++) d.ctr[k] = m->host.center[k];
     d.half_extent = (float)m->host.half_extent * 1.0000002f;
@@ -93,6 +93,5 @@ int emu_build_cells(const double* gd, const uint32_t* res, uint64_t c_begin, uin
 void emu_counters(unsigned long long* out /*32*/, int reset) { for (int i = 0; i < 32; i++) { out[i] = dg_emu::g_counters[i]; if (reset) dg_emu::g_counters[i] = 0; } }
 // block ids in the order the last sampling launches ran them (cleared by reading)
 uint64_t emu_block_trace(uint32_t* out, uint64_t cap) { const uint64_t n = dg_emu::g_block_trace.size(); for (uint64_t i = 0; i < n && i < cap; i++) out[i] = dg_emu::g_block_trace[i]; dg_emu::g_block_trace.clear(); return n; }
-int emu_knobs(int* fast_div, int* vote_redux) { *fast_div = 0; *vote_redux = K1_VOTE_REDUX; return 0; }
 
 }  // extern "C"

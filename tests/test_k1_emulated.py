@@ -18,8 +18,8 @@ from test_oracle_golden import read_cdf, read_obj
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 import k1_fuzz  # noqa: E402  (tools/k1_fuzz.py: mesh generators, backends and checks shared with the fuzzer and the GPU tests)
 
-# default knobs, the knob variants (K1_VOTE_REDUX + K1_BRICK_AUTO), the wavefront kernel, the per-lane kernel and the packet walk (K1_PACKET); DG_K1_EMU_LIB adds any other build of tests/emu/k1_emu.cpp
-LIBS = [os.path.join(ROOT, "build", "bin", n) for n in ("libk1emu.so", "libk1emu_knobs.so", "libk1emu_wave.so", "libk1emu_perlane.so", "libk1emu_packet.so")] + \
+# the product's build (packet walk) and the per-lane node loop (K1_PACKET=0); DG_K1_EMU_LIB adds any other build of tests/emu/k1_emu.cpp
+LIBS = [os.path.join(ROOT, "build", "bin", n) for n in ("libk1emu.so", "libk1emu_perlane.so")] + \
        ([os.environ["DG_K1_EMU_LIB"]] if os.environ.get("DG_K1_EMU_LIB") else [])
 _dp, _u32p, _i32p, _u64p = C.POINTER(C.c_double), C.POINTER(C.c_uint32), C.POINTER(C.c_int32), C.POINTER(C.c_uint64)
 
@@ -185,7 +185,7 @@ def test_scale_sweep_vs_reference_header(so, mode):
     assert bad == 0, f"{bad} mismatches: " + "\n".join(msgs[:8])
 
 
-@pytest.mark.parametrize("name", ["libk1emu.so", "libk1emu_packet.so"])
+@pytest.mark.parametrize("name", ["libk1emu.so"])
 def test_small_meshes_leaf_bound_vs_reference_header(name):
     """the packet walk's leaf_lower_bound on meshes of size 1e-12 .. 1e-7, where its filter is on but the degree-4 products of its
     inside / outside test go subnormal and lose their relative error bound (the absolute floor of its tolerance covers them): sweep seeds
@@ -212,10 +212,10 @@ def test_tie_rich_fuzz_against_reference_header():
     assert r.returncode == 0 and "0 mismatches" in r.stdout, r.stdout[-2000:] + r.stderr[-2000:]
 
 
-@pytest.mark.parametrize("name", ["libk1emu.so", "libk1emu_packet.so"])
+@pytest.mark.parametrize("name", ["libk1emu.so"])
 def test_tie_rich_grid_fuzz_node_loop_against_reference_header(name):
-    """tools/k1_fuzz.py in grid mode: the addFunction node loop (bricks of lattice nodes; for libk1emu_packet.so the packet walk with its
-    tie replay, certificates and per-lane fallback) on half-integer lattices through coplanar grids, cubes, octahedra, duplicated triangles,
+    """tools/k1_fuzz.py in grid mode: the addFunction node loop (bricks of lattice nodes; the packet walk with its tie replay,
+    certificates and per-lane fallback) on half-integer lattices through coplanar grids, cubes, octahedra, duplicated triangles,
     slivers and random soups == sign * the reference header's signed distance at the node positions, bit for bit"""
     import subprocess
     import sys
@@ -247,11 +247,8 @@ def test_node_loop_on_a_mesh_with_non_finite_vertices(emu, orc):
 
 
 def test_emulated_launch_order(emu, orc):
-    """the per-lane sampling kernel takes its blocks in launch order, every block exactly once (the wavefront kernel hands out bricks
-    through a counter instead and has no block order)"""
+    """the sampling kernel takes its blocks in launch order, every block exactly once"""
     import discregrid_b200 as dg
-    if "wave" in emu.lib._name:
-        pytest.skip("the wavefront kernel hands out bricks through a counter: there is no block order")
     emu.lib.emu_block_trace.restype = C.c_uint64
     emu.lib.emu_block_trace.argtypes = [_u32p, C.c_uint64]
     t = dg.bumpy_torus(24, 20, 1.0, 0.4, 0.05, 7, 5)

@@ -12,7 +12,7 @@ from conftest import GOLDEN, ROOT, bits_equal
 from test_oracle_golden import read_cdf
 from test_oracle_reference_tools import split_inputs
 
-LIBS = [os.path.join(ROOT, "build", "bin", "libk23emu.so"), os.path.join(ROOT, "build", "bin", "libk23emu_knobs.so")]      # default; K3_FAST_DIV
+LIBS = [os.path.join(ROOT, "build", "bin", "libk23emu.so")]
 _dp, _u32p = C.POINTER(C.c_double), C.POINTER(C.c_uint32)
 DBL_MAX = np.finfo(np.float64).max
 
@@ -120,11 +120,10 @@ def test_interpolate_fuzz_against_reference_class():
 
 
 def test_density_map_fuzz_against_oracle(emu):
-    """a short run of tools/k3_fuzz.py on each emulated build (default, K3_FAST_DIV): random grids / fields / support radii / node ranges,
+    """a short run of tools/k3_fuzz.py on the emulated build: random grids / fields / support radii / node ranges,
     reduced inputs, -DBL_MAX / +-1e308 / NaN / +-inf / subnormal coefficients (where the reference's density is NaN), h either side of
     2^+-300, h = +inf, rho0 of 0 / -1 / NaN / +inf, both predicate modes"""
     import subprocess
     import sys
-    so = LIBS[0] if "knobs" not in emu.lib._name else LIBS[1]
-    r = subprocess.run([sys.executable, os.path.join(ROOT, "tools", "k3_fuzz.py"), "10", "3", so], capture_output=True, text=True, timeout=900)
+    r = subprocess.run([sys.executable, os.path.join(ROOT, "tools", "k3_fuzz.py"), "10", "3", emu.lib._name], capture_output=True, text=True, timeout=900)
     assert r.returncode == 0 and "0 mismatches" in r.stdout, r.stdout[-2000:] + r.stderr[-2000:]

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Event counts of the PACKET walk (nearest_triangle_packet) as tests/emu runs it (build/bin/libk1emu_packet.so; `make cpp`), per brick of 32
+"""Event counts of the PACKET walk (nearest_triangle_packet) as tests/emu runs it (build/bin/libk1emu.so; `make cpp`), per brick of 32
 queries: node steps, leaf visits, exact fp64 blocks, re-tests of deferred children, how the reference's choice was replayed (no order needed /
 tie shortcut / sort), comparator calls, and which check sent lanes to the per-lane fallback -- plus a bit-for-bit comparison of the output with
 the per-lane emulated build (libk1emu_perlane.so) over the same node range.  The event figures quoted in DESIGN.md section 4 come from here.
@@ -15,7 +15,7 @@ import bench
 from oracle_api import Oracle
 res = int(sys.argv[1]); 
 mesh = dg.TriangleMesh(sys.argv[2]) if len(sys.argv) > 2 and sys.argv[2] != "torus" else dg.bumpy_torus(*bench.WORKLOAD["torus"])
-lib = C.CDLL(os.path.join(ROOT, "build", "bin", "libk1emu_packet.so"))
+lib = C.CDLL(os.path.join(ROOT, "build", "bin", "libk1emu.so"))
 ref = C.CDLL(os.path.join(ROOT, "build", "bin", "libk1emu_perlane.so"))       # the per-lane walk: an independent implementation
 dp, u32p = C.POINTER(C.c_double), C.POINTER(C.c_uint32)
 orc = Oracle()
