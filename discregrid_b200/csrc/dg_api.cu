@@ -3,6 +3,7 @@
 #include "../../include/discregrid_b200.h"
 
 #include <atomic>
+#include <cassert>
 #include <condition_variable>
 #include <cfloat>
 #include <chrono>
@@ -76,15 +77,18 @@ int guarded(const char* who, F&& body)
     catch (const std::exception& ex) { return fail(DG_ERR_INVALID, "%s: %s", who, ex.what()); }
 }
 
-#define DG_CUDA(call)                                                                                    \
-    do {                                                                                                 \
-        cudaError_t e_ = (call);                                                                         \
-        if (e_ != cudaSuccess) {                                                                         \
-            const int code_ = (e_ == cudaErrorMemoryAllocation) ? DG_ERR_NOMEM                           \
-                              : (e_ == cudaErrorNoDevice || e_ == cudaErrorInsufficientDriver) ? DG_ERR_NO_DEVICE \
-                                                                                                : DG_ERR_CUDA; \
-            return fail(code_, "%s failed: %s", #call, cudaGetErrorString(e_));                         \
-        }                                                                                                \
+// the status code of a failed CUDA call
+int cuda_code(cudaError_t e)
+{
+    if (e == cudaErrorMemoryAllocation) return DG_ERR_NOMEM;
+    if (e == cudaErrorNoDevice || e == cudaErrorInsufficientDriver) return DG_ERR_NO_DEVICE;
+    return DG_ERR_CUDA;
+}
+
+#define DG_CUDA(call)                                                                                          \
+    do {                                                                                                       \
+        const cudaError_t e_ = (call);                                                                         \
+        if (e_ != cudaSuccess) return fail(cuda_code(e_), "%s failed: %s", #call, cudaGetErrorString(e_));     \
     } while (0)
 
 #define DG_LAUNCH(call)          \
@@ -146,23 +150,67 @@ struct DevBuf {
     size_t bytes() const { return n * sizeof(T); }
 };
 
-bool grid_to_dev(const dg_grid_desc* d, GridDev& g, const char** why)
+// the device copy of a grid descriptor; refuses the grids dg_grid_num_nodes refuses (2^31 nodes or more among them)
+int grid_checked(const dg_grid_desc* d, GridDev& g, const char* who)
 {
-    if (!d) { *why = "grid descriptor is NULL"; return false; }
+    if (!d) return fail(DG_ERR_INVALID, "%s: grid descriptor is NULL", who);
     for (int k = 0; k < 3; k++) {
-        if (d->resolution[k] == 0) { *why = "resolution must be >= 1 in every dimension"; return false; }
+        if (d->resolution[k] == 0) return fail(DG_ERR_INVALID, "%s: resolution must be >= 1 in every dimension", who);
         g.mn[k] = d->domain_min[k]; g.mx[k] = d->domain_max[k];
         g.cell[k] = d->cell_size[k]; g.inv[k] = d->inv_cell_size[k];
         g.n[k] = d->resolution[k];
     }
     uint64_t nn = 0;
-    if (dg_grid_num_nodes(d->resolution, &nn) != DG_OK) { *why = "grid too large: node ids must fit uint32 (reference file format)"; return false; }
+    if (dg_grid_num_nodes(d->resolution, &nn) != DG_OK)
+        return fail(DG_ERR_INVALID, "%s: grid too large: node ids must fit uint32 (reference file format)", who);
     const unsigned nx = g.n[0], ny = g.n[1], nz = g.n[2];
     g.nv = (nx + 1) * (ny + 1) * (nz + 1);
     g.ne_x = nx * (ny + 1) * (nz + 1);
     g.ne_y = (nx + 1) * ny * (nz + 1);
     g.ne_z = (nx + 1) * (ny + 1) * nz;
-    return true;
+    return DG_OK;
+}
+
+uint64_t grid_nodes(const GridDev& g) { return (uint64_t)g.nv + 2ull * ((uint64_t)g.ne_x + g.ne_y + g.ne_z); }
+uint64_t grid_cells(const GridDev& g) { return (uint64_t)g.n[0] * g.n[1] * g.n[2]; }
+
+int check_reduce_flags(uint32_t flags, const char* who)
+{
+    if (flags & ~DG_REDUCE_REFERENCE_SORT) return fail(DG_ERR_INVALID, "%s: unknown flags 0x%x (only DG_REDUCE_REFERENCE_SORT)", who, flags);
+    return DG_OK;
+}
+
+// The host-array form of a query: device buffers for `chunk` points of every input and of every non-NULL output (bytes: per point), then
+// upload -> launch -> download chunk by chunk on the legacy default stream, and a device synchronise.  launch(d_in, d_out, b, c) runs the
+// query on points [b, b + c) in the buffers (NULL for a NULL output); n == 0 makes one launch of no points.
+struct HostIn { const void* p; size_t bytes; };
+struct HostOut { void* p; size_t bytes; };
+
+template <class Launch>
+int stage_on_device(uint64_t n, uint64_t chunk, std::initializer_list<HostIn> in, std::initializer_list<HostOut> out, Launch&& launch)
+{
+    constexpr size_t kMax = 4;
+    assert(in.size() <= kMax && out.size() <= kMax);
+    const HostIn* ins = in.begin();
+    const HostOut* outs = out.begin();
+    DevBuf<char> d_in[kMax], d_out[kMax];
+    void* p_in[kMax] = {};
+    void* p_out[kMax] = {};
+    for (size_t k = 0; k < in.size(); k++) { DG_CUDA(d_in[k].alloc(chunk * ins[k].bytes)); p_in[k] = d_in[k].p; }
+    for (size_t k = 0; k < out.size(); k++)
+        if (outs[k].p) { DG_CUDA(d_out[k].alloc(chunk * outs[k].bytes)); p_out[k] = d_out[k].p; }
+    uint64_t b = 0;
+    do {
+        const uint64_t c = std::min(chunk, n - b);
+        for (size_t k = 0; k < in.size() && c; k++)
+            DG_CUDA(cudaMemcpy(p_in[k], static_cast<const char*>(ins[k].p) + b * ins[k].bytes, c * ins[k].bytes, cudaMemcpyHostToDevice));
+        if (int rc = launch(p_in, p_out, b, c)) return rc;
+        for (size_t k = 0; k < out.size() && c; k++)
+            if (p_out[k]) DG_CUDA(cudaMemcpy(static_cast<char*>(outs[k].p) + b * outs[k].bytes, p_out[k], c * outs[k].bytes, cudaMemcpyDeviceToHost));
+        b += c;
+    } while (b < n);
+    DG_CUDA(cudaDeviceSynchronize());
+    return DG_OK;
 }
 
 std::atomic<int> g_selftest_state{0};   // 0 = not run, 1 = ok, -1 = failed
@@ -208,10 +256,11 @@ struct dg_mesh {
     }
 };
 
-// every call on a mesh whose refit failed half way refuses it (its records are a mix of two vertex sets); NULL is left to the caller's check
+// every call on a mesh refuses NULL, and a mesh whose refit failed half way (its records are a mix of two vertex sets)
 static int mesh_usable(const dg_mesh* m, const char* who)
 {
-    if (m && m->failed)
+    if (!m) return fail(DG_ERR_INVALID, "%s: mesh is NULL (not constructed)", who);
+    if (m->failed)
         return fail(DG_ERR_INVALID, "%s: a refit of this mesh failed after it had started to write the records; the mesh is unusable "
                     "(dg_mesh_destroy it and create it again)", who);
     return DG_OK;
@@ -362,34 +411,32 @@ int dg_mesh_create(const double* V, uint64_t nV, const uint32_t* F, uint64_t nT,
     if (!V || !F || nT == 0 || nV == 0) return fail(DG_ERR_INVALID, "dg_mesh_create: empty triangle list");   // ref: exit(-1)
     if (int rc = require_device()) return rc;
     if (int rc = ensure_selftest()) return rc;
-    dg_mesh* m = new (std::nothrow) dg_mesh();
+    std::unique_ptr<dg_mesh> m(new (std::nothrow) dg_mesh());
     if (!m) return fail(DG_ERR_NOMEM, "dg_mesh_create: out of host memory");
     const auto t0 = std::chrono::steady_clock::now();
     const char* why = "";
     try {
-        if (!build_host_bvh(V, nV, F, nT, m->host, &why, true)) { delete m; return fail(DG_ERR_INVALID, "dg_mesh_create: %s", why); }
-    } catch (const std::bad_alloc&) { delete m; return fail(DG_ERR_NOMEM, "dg_mesh_create: out of host memory"); }
+        if (!build_host_bvh(V, nV, F, nT, m->host, &why, true)) return fail(DG_ERR_INVALID, "dg_mesh_create: %s", why);
+    } catch (const std::bad_alloc&) { return fail(DG_ERR_NOMEM, "dg_mesh_create: out of host memory"); }
     const auto t1 = std::chrono::steady_clock::now();
     m->build_us = (uint64_t)std::chrono::duration_cast<std::chrono::microseconds>(t1 - t0).count();
 
-    auto cleanup = [&](int rc) { delete m; return rc; };
-#define DG_CUDA_M(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return cleanup(fail(e_ == cudaErrorMemoryAllocation ? DG_ERR_NOMEM : DG_ERR_CUDA, "%s failed: %s", #call, cudaGetErrorString(e_))); } while (0)
-    DG_CUDA_M(cudaGetDevice(&m->device));
-    DG_CUDA_M(m->d_spheres.alloc(nT));
-    DG_CUDA_M(m->d_leaves.alloc(nT));
-    DG_CUDA_M(m->d_normals.alloc(nT));
-    DG_CUDA_M(m->d_nodes_f.alloc(nT * K1_NODEF_STRIDE));
-    DG_CUDA_M(m->d_leaves_f.alloc(nT));
-    DG_CUDA_M(cudaMemcpy(m->d_leaves_f.p, m->host.leaves_f.data(), nT * sizeof(LeafF), cudaMemcpyHostToDevice));
+    DG_CUDA(cudaGetDevice(&m->device));
+    DG_CUDA(m->d_spheres.alloc(nT));
+    DG_CUDA(m->d_leaves.alloc(nT));
+    DG_CUDA(m->d_normals.alloc(nT));
+    DG_CUDA(m->d_nodes_f.alloc(nT * K1_NODEF_STRIDE));
+    DG_CUDA(m->d_leaves_f.alloc(nT));
+    DG_CUDA(cudaMemcpy(m->d_leaves_f.p, m->host.leaves_f.data(), nT * sizeof(LeafF), cudaMemcpyHostToDevice));
     m->dev.leaves_f = m->d_leaves_f.p;
-    DG_CUDA_M(cudaMemcpy(m->d_spheres.p, m->host.spheres.data(), nT * sizeof(SpherePair), cudaMemcpyHostToDevice));
-    DG_CUDA_M(cudaMemcpy(m->d_leaves.p, m->host.leaves.data(), nT * sizeof(LeafRecord), cudaMemcpyHostToDevice));
-    DG_CUDA_M(cudaMemcpy(m->d_normals.p, m->host.normals.data(), nT * sizeof(PseudoNormals), cudaMemcpyHostToDevice));
+    DG_CUDA(cudaMemcpy(m->d_spheres.p, m->host.spheres.data(), nT * sizeof(SpherePair), cudaMemcpyHostToDevice));
+    DG_CUDA(cudaMemcpy(m->d_leaves.p, m->host.leaves.data(), nT * sizeof(LeafRecord), cudaMemcpyHostToDevice));
+    DG_CUDA(cudaMemcpy(m->d_normals.p, m->host.normals.data(), nT * sizeof(PseudoNormals), cudaMemcpyHostToDevice));
     {   // the fp32 record of every internal node: sphere pair + child boxes, bvh_build.h
         static_assert(K1_NODEF_STRIDE * sizeof(float4) >= sizeof(SpherePairF) + sizeof(BoxPairF), "node record too small");
         RawVec<float4> rec(nT * K1_NODEF_STRIDE);
         pack_node_records(m->host, K1_NODEF_STRIDE, reinterpret_cast<float*>(rec.data()));
-        DG_CUDA_M(cudaMemcpy(m->d_nodes_f.p, rec.data(), rec.size() * sizeof(float4), cudaMemcpyHostToDevice));
+        DG_CUDA(cudaMemcpy(m->d_nodes_f.p, rec.data(), rec.size() * sizeof(float4), cudaMemcpyHostToDevice));
     }
     m->dev.nodes_f = m->d_nodes_f.p;
     for (int d = 0; d < 3; d++) m->dev.ctr[d] = m->host.center[d];
@@ -397,8 +444,7 @@ int dg_mesh_create(const double* V, uint64_t nV, const uint32_t* F, uint64_t nT,
     m->dev.spheres = m->d_spheres.p; m->dev.leaves = m->d_leaves.p; m->dev.normals = m->d_normals.p;
     m->dev.n_tri = (int)nT;
     m->dev.stack_depth = m->host.max_depth > 1 ? m->host.max_depth - 1 : 1;
-    DG_CUDA_M(k1_configure(m->dev.stack_depth));
-#undef DG_CUDA_M
+    DG_CUDA(k1_configure(m->dev.stack_depth));
     const auto t2 = std::chrono::steady_clock::now();
     m->upload_us = (uint64_t)std::chrono::duration_cast<std::chrono::microseconds>(t2 - t1).count();
     // the device records are the product; the host copies of the big arrays are no longer needed
@@ -408,7 +454,7 @@ int dg_mesh_create(const double* V, uint64_t nV, const uint32_t* F, uint64_t nT,
     RawVec<LeafF>().swap(m->host.leaves_f);        // keep `order`, V, F, pseudonormals for diagnostics
     RawVec<LeafRecord>().swap(m->host.leaves);
     RawVec<PseudoNormals>().swap(m->host.normals);
-    *out = m;
+    *out = m.release();
     return DG_OK;
 }
 
@@ -422,7 +468,7 @@ int dg_mesh_destroy(dg_mesh* m)
 int dg_mesh_info(const dg_mesh* m, uint64_t info[8])
 {
     if (int rc = mesh_usable(m, "dg_mesh_info")) return rc;
-    if (!m || !info) return fail(DG_ERR_INVALID, "dg_mesh_info: NULL argument");
+    if (!info) return fail(DG_ERR_INVALID, "dg_mesh_info: NULL argument");
     info[0] = m->host.n_vertices; info[1] = m->host.n_triangles; info[2] = (uint64_t)m->dev.stack_depth;
     info[3] = (uint64_t)m->host.flags;
     info[4] = m->d_spheres.bytes() + m->d_leaves.bytes() + m->d_normals.bytes() + m->d_nodes_f.bytes() + m->d_leaves_f.bytes();
@@ -438,7 +484,6 @@ int dg_mesh_info(const dg_mesh* m, uint64_t info[8])
 int dg_mesh_tree(const dg_mesh* m, double* spheres, int32_t* kids)
 {
     if (int rc = mesh_usable(m, "dg_mesh_tree")) return rc;
-    if (!m) return fail(DG_ERR_INVALID, "dg_mesh_tree: mesh is NULL");
     // the sphere pairs were released after upload: read them back from the device
     HostBvh tmp;
     tmp.n_triangles = m->host.n_triangles;
@@ -451,7 +496,6 @@ int dg_mesh_tree(const dg_mesh* m, double* spheres, int32_t* kids)
 
 int dg_mesh_pseudonormals(const dg_mesh* m, double* tri, double* edge, double* vert)
 {
-    if (!m) return fail(DG_ERR_INVALID, "dg_mesh_pseudonormals: mesh is NULL");
     if (int rc = mesh_usable(m, "dg_mesh_pseudonormals")) return rc;
     if (m->refit_done) {        // the reference's arrays rebuilt from the device's per-leaf blocks (V0 V1 V2 E01 E12 E02 F)
         const uint64_t nT = m->host.n_triangles;
@@ -469,7 +513,6 @@ int dg_mesh_pseudonormals(const dg_mesh* m, double* tri, double* edge, double* v
         }
         return DG_OK;
     }
-    if (!m) return fail(DG_ERR_INVALID, "dg_mesh_pseudonormals: mesh is NULL");
     if (tri) std::memcpy(tri, m->host.pn_tri.data(), m->host.pn_tri.size() * sizeof(double));
     if (edge) std::memcpy(edge, m->host.pn_edge.data(), m->host.pn_edge.size() * sizeof(double));
     if (vert) std::memcpy(vert, m->host.pn_vert.data(), m->host.pn_vert.size() * sizeof(double));
@@ -553,7 +596,6 @@ static int refuse_winding(const dg_mesh* m, const char* who)
 int dg_mesh_set_sign_mode(dg_mesh* m, int mode, double beta)
 {
     if (int rc = mesh_usable(m, "dg_mesh_set_sign_mode")) return rc;
-    if (!m) return fail(DG_ERR_INVALID, "dg_mesh_set_sign_mode: mesh is NULL (not constructed)");
     if (mode != DG_SIGN_PSEUDONORMAL && mode != DG_SIGN_WINDING) return fail(DG_ERR_INVALID, "dg_mesh_set_sign_mode: unknown mode %d", mode);
     if (int rc = check_beta(beta, "dg_mesh_set_sign_mode")) return rc;
     m->sign_mode = mode;
@@ -587,7 +629,6 @@ static int refit_prepare(dg_mesh* m)
 
 static int refit_checks(dg_mesh* m, const void* v, uint64_t nV, const char* who)
 {
-    if (!m) return fail(DG_ERR_INVALID, "%s: mesh is NULL (not constructed)", who);
     if (int rc = mesh_usable(m, who)) return rc;
     if (nV && !v) return fail(DG_ERR_INVALID, "%s: vertices is NULL", who);
     if (nV != m->host.n_vertices)
@@ -617,7 +658,7 @@ int dg_mesh_refit_device(dg_mesh* m, const double* d_vertices, uint64_t n_vertic
     // from here on records are written: a CUDA error leaves the mesh failed
     auto broken = [&](cudaError_t e, const char* what) {
         m->failed = true;
-        return fail(e == cudaErrorMemoryAllocation ? DG_ERR_NOMEM : DG_ERR_CUDA, "dg_mesh_refit_device: %s failed: %s; the mesh is left unusable "
+        return fail(cuda_code(e), "dg_mesh_refit_device: %s failed: %s; the mesh is left unusable "
                     "(dg_mesh_destroy it)", what, cudaGetErrorString(e));
     };
     cudaError_t e;
@@ -646,92 +687,100 @@ int dg_mesh_refit(dg_mesh* m, const double* vertices, uint64_t n_vertices)
     const cudaError_t e = cudaMemcpy(m->d_V.p, vertices, 3 * n_vertices * sizeof(double), cudaMemcpyHostToDevice);
     if (e != cudaSuccess) {                   // d_V may now hold part of the new positions: out of step with the records
         m->failed = true;
-        return fail(e == cudaErrorMemoryAllocation ? DG_ERR_NOMEM : DG_ERR_CUDA, "dg_mesh_refit: upload of the vertices failed: %s; the mesh "
+        return fail(cuda_code(e), "dg_mesh_refit: upload of the vertices failed: %s; the mesh "
                     "is left unusable (dg_mesh_destroy it)", cudaGetErrorString(e));
     }
     return dg_mesh_refit_device(m, m->d_V.p, n_vertices, nullptr);
 }
 
+// the argument checks of the winding-number and distance queries; the device check is the caller's, since the host forms return at n == 0
+// before it
+static int winding_check(const dg_mesh* m, const void* x, uint64_t n, double beta, const void* w, const char* who)
+{
+    if (int rc = mesh_usable(m, who)) return rc;
+    if (int rc = check_beta(beta, who)) return rc;
+    if (n && (!x || !w)) return fail(DG_ERR_INVALID, "%s: points or output is NULL", who);
+    return DG_OK;
+}
+
+static int winding_launch(const dg_mesh* m, const double* d_x, uint64_t n, double beta, double* d_w, cudaStream_t st, const char* who)
+{
+    const WindDev* wd = nullptr;
+    if (int rc = winding_dev(m, wd, who)) return rc;
+    DG_LAUNCH(k5_launch_winding(*wd, d_x, n, beta, d_w, st));
+    return DG_OK;
+}
+
 int dg_mesh_winding_number_device(const dg_mesh* m, const double* d_x, uint64_t n, double beta, double* d_w, void* stream)
 {
-    if (int rc = mesh_usable(m, "dg_mesh_winding_number_device")) return rc;
-    if (!m) return fail(DG_ERR_INVALID, "dg_mesh_winding_number: mesh is NULL (not constructed)");
-    if (int rc = check_beta(beta, "dg_mesh_winding_number")) return rc;
-    if (n && (!d_x || !d_w)) return fail(DG_ERR_INVALID, "dg_mesh_winding_number: points or output is NULL");
-    if (int rc = check_handle_device(m->device, "dg_mesh_winding_number")) return rc;
+    static const char* who = "dg_mesh_winding_number_device";
+    if (int rc = winding_check(m, d_x, n, beta, d_w, who)) return rc;
+    if (int rc = check_handle_device(m->device, who)) return rc;
     if (n == 0) return DG_OK;
-    const WindDev* wd = nullptr;
-    if (int rc = winding_dev(m, wd, "dg_mesh_winding_number")) return rc;
-    DG_LAUNCH(k5_launch_winding(*wd, d_x, n, beta, d_w, (cudaStream_t)stream));
-    return DG_OK;
+    return winding_launch(m, d_x, n, beta, d_w, (cudaStream_t)stream, who);
 }
 
 int dg_mesh_winding_number(const dg_mesh* m, const double* x, uint64_t n, double beta, double* w)
 {
-    if (int rc = mesh_usable(m, "dg_mesh_winding_number")) return rc;
-    if (!m) return fail(DG_ERR_INVALID, "dg_mesh_winding_number: mesh is NULL (not constructed)");
-    if (int rc = check_beta(beta, "dg_mesh_winding_number")) return rc;
+    static const char* who = "dg_mesh_winding_number";
+    if (int rc = winding_check(m, x, n, beta, w, who)) return rc;
     if (n == 0) return DG_OK;
-    if (!x || !w) return fail(DG_ERR_INVALID, "dg_mesh_winding_number: points or output is NULL");
-    DevBuf<double> d_x, d_w;
-    DG_CUDA(d_x.alloc(3 * n));
-    DG_CUDA(d_w.alloc(n));
-    DG_CUDA(cudaMemcpy(d_x.p, x, 3 * n * sizeof(double), cudaMemcpyHostToDevice));
-    if (int rc = dg_mesh_winding_number_device(m, d_x.p, n, beta, d_w.p, nullptr)) return rc;
-    DG_CUDA(cudaMemcpy(w, d_w.p, n * sizeof(double), cudaMemcpyDeviceToHost));
-    DG_CUDA(cudaDeviceSynchronize());
+    if (int rc = check_handle_device(m->device, who)) return rc;
+    return stage_on_device(n, n, {{x, 3 * sizeof(double)}}, {{w, sizeof(double)}}, [&](void* const* in, void* const* out, uint64_t, uint64_t c) {
+        return winding_launch(m, (const double*)in[0], c, beta, (double*)out[0], nullptr, who);
+    });
+}
+
+static int distance_check(const dg_mesh* m, const void* pts, uint64_t n, const char* who)
+{
+    if (int rc = mesh_usable(m, who)) return rc;
+    if (n && !pts) return fail(DG_ERR_INVALID, "%s: points is NULL", who);
+    return DG_OK;
+}
+
+static int distance_launch(const dg_mesh* m, const double* d_pts, uint64_t n, int is_signed, double* d_dist, double* d_near, int32_t* d_ent,
+                           int32_t* d_tri, cudaStream_t st, const char* who)
+{
+    if (is_signed && m->sign_mode == DG_SIGN_WINDING) {       // the unsigned query, then the sign from w (k5_winding.cu)
+        const WindDev* wd = nullptr;
+        if (int rc = winding_dev(m, wd, who)) return rc;
+        DG_LAUNCH(k1_launch_distance(m->dev, d_pts, n, 0, d_dist, d_near, d_ent, d_tri, st));
+        if (d_dist) DG_LAUNCH(k5_launch_sign_points(*wd, d_pts, n, m->beta, d_dist, st));
+        return DG_OK;
+    }
+    DG_LAUNCH(k1_launch_distance(m->dev, d_pts, n, is_signed, d_dist, d_near, d_ent, d_tri, st));
     return DG_OK;
 }
 
 int dg_mesh_distance_device(const dg_mesh* m, const double* d_pts, uint64_t n, int is_signed, double* d_dist, double* d_near,
                             int32_t* d_ent, int32_t* d_tri, void* stream)
 {
-    if (int rc = mesh_usable(m, "dg_mesh_distance_device")) return rc;
-    if (!m) return fail(DG_ERR_INVALID, "dg_mesh_distance: mesh is NULL (not constructed)");
-    if (n && !d_pts) return fail(DG_ERR_INVALID, "dg_mesh_distance: points is NULL");
-    if (int rc = check_handle_device(m->device, "dg_mesh_distance")) return rc;
-    if (is_signed && m->sign_mode == DG_SIGN_WINDING) {       // the unsigned query, then the sign from w (k5_winding.cu)
-        const WindDev* wd = nullptr;
-        if (int rc = winding_dev(m, wd, "dg_mesh_distance")) return rc;
-        DG_LAUNCH(k1_launch_distance(m->dev, d_pts, n, 0, d_dist, d_near, d_ent, d_tri, (cudaStream_t)stream));
-        if (d_dist) DG_LAUNCH(k5_launch_sign_points(*wd, d_pts, n, m->beta, d_dist, (cudaStream_t)stream));
-        return DG_OK;
-    }
-    DG_LAUNCH(k1_launch_distance(m->dev, d_pts, n, is_signed, d_dist, d_near, d_ent, d_tri, (cudaStream_t)stream));
-    return DG_OK;
+    static const char* who = "dg_mesh_distance_device";
+    if (int rc = distance_check(m, d_pts, n, who)) return rc;
+    if (int rc = check_handle_device(m->device, who)) return rc;
+    return distance_launch(m, d_pts, n, is_signed, d_dist, d_near, d_ent, d_tri, (cudaStream_t)stream, who);
 }
 
 int dg_mesh_distance(const dg_mesh* m, const double* pts, uint64_t n, int is_signed, double* dist, double* nearp, int32_t* ent,
                      int32_t* tri)
 {
-    if (int rc = mesh_usable(m, "dg_mesh_distance")) return rc;
-    if (!m) return fail(DG_ERR_INVALID, "dg_mesh_distance: mesh is NULL (not constructed)");
+    static const char* who = "dg_mesh_distance";
+    if (int rc = distance_check(m, pts, n, who)) return rc;
     if (n == 0) return DG_OK;
-    if (!pts) return fail(DG_ERR_INVALID, "dg_mesh_distance: points is NULL");
-    DevBuf<double> d_pts, d_dist, d_near;
-    DevBuf<int> d_ent, d_tri;
-    DG_CUDA(d_pts.alloc(3 * n));
-    DG_CUDA(cudaMemcpy(d_pts.p, pts, 3 * n * sizeof(double), cudaMemcpyHostToDevice));
-    if (dist) DG_CUDA(d_dist.alloc(n));
-    if (nearp) DG_CUDA(d_near.alloc(3 * n));
-    if (ent) DG_CUDA(d_ent.alloc(n));
-    if (tri) DG_CUDA(d_tri.alloc(n));
-    if (int rc = dg_mesh_distance_device(m, d_pts.p, n, is_signed, d_dist.p, d_near.p, d_ent.p, d_tri.p, nullptr)) return rc;
-    if (dist) DG_CUDA(cudaMemcpy(dist, d_dist.p, n * sizeof(double), cudaMemcpyDeviceToHost));
-    if (nearp) DG_CUDA(cudaMemcpy(nearp, d_near.p, 3 * n * sizeof(double), cudaMemcpyDeviceToHost));
-    if (ent) DG_CUDA(cudaMemcpy(ent, d_ent.p, n * sizeof(int), cudaMemcpyDeviceToHost));
-    if (tri) DG_CUDA(cudaMemcpy(tri, d_tri.p, n * sizeof(int), cudaMemcpyDeviceToHost));
-    DG_CUDA(cudaDeviceSynchronize());
-    return DG_OK;
+    if (int rc = check_handle_device(m->device, who)) return rc;
+    return stage_on_device(n, n, {{pts, 3 * sizeof(double)}},
+                           {{dist, sizeof(double)}, {nearp, 3 * sizeof(double)}, {ent, sizeof(int32_t)}, {tri, sizeof(int32_t)}},
+                           [&](void* const* in, void* const* out, uint64_t, uint64_t c) {
+                               return distance_launch(m, (const double*)in[0], c, is_signed, (double*)out[0], (double*)out[1], (int32_t*)out[2],
+                                                      (int32_t*)out[3], nullptr, who);
+                           });
 }
 
 // ------------------------------------------------------------------------------------------------ K1
 static int check_range(const dg_grid_desc* grid, uint64_t b, uint64_t e, GridDev& g, const char* who)
 {
-    const char* why = "";
-    if (!grid_to_dev(grid, g, &why)) return fail(DG_ERR_INVALID, "%s: %s", who, why);
-    uint64_t nn = 0;
-    if (int rc = dg_grid_num_nodes(grid->resolution, &nn)) return rc;
+    if (int rc = grid_checked(grid, g, who)) return rc;
+    const uint64_t nn = grid_nodes(g);
     if (b > e || e > nn) return fail(DG_ERR_INVALID, "%s: node range [%llu, %llu) outside [0, %llu]", who, (unsigned long long)b,
                                       (unsigned long long)e, (unsigned long long)nn);
     return DG_OK;
@@ -740,15 +789,15 @@ static int check_range(const dg_grid_desc* grid, uint64_t b, uint64_t e, GridDev
 int dg_sample_sdf_device(const dg_mesh* m, const dg_grid_desc* grid, double sign, uint64_t l_begin, uint64_t l_end, double* d_out,
                          void* stream)
 {
-    if (int rc = mesh_usable(m, "dg_sample_sdf_device")) return rc;
-    if (!m) return fail(DG_ERR_INVALID, "dg_sample_sdf: mesh is NULL (not constructed)");
+    static const char* who = "dg_sample_sdf_device";
+    if (int rc = mesh_usable(m, who)) return rc;
     GridDev g;
-    if (int rc = check_range(grid, l_begin, l_end, g, "dg_sample_sdf")) return rc;
-    if (l_end > l_begin && !d_out) return fail(DG_ERR_INVALID, "dg_sample_sdf: output is NULL");
-    if (int rc = check_handle_device(m->device, "dg_sample_sdf")) return rc;
+    if (int rc = check_range(grid, l_begin, l_end, g, who)) return rc;
+    if (l_end > l_begin && !d_out) return fail(DG_ERR_INVALID, "%s: output is NULL", who);
+    if (int rc = check_handle_device(m->device, who)) return rc;
     if (m->sign_mode == DG_SIGN_WINDING) {      // K1 with sign = +1, then the node pass of k5_winding.cu
         const WindDev* wd = nullptr;
-        if (int rc = winding_dev(m, wd, "dg_sample_sdf")) return rc;
+        if (int rc = winding_dev(m, wd, who)) return rc;
         DG_LAUNCH(k1_launch_sample_nodes(m->dev, g, 1.0, l_begin, l_end - l_begin, d_out, (cudaStream_t)stream));
         DG_LAUNCH(k5_launch_sign_nodes(*wd, g, sign, INFINITY, m->beta, l_begin, l_end - l_begin, d_out, (cudaStream_t)stream));
         return DG_OK;
@@ -768,17 +817,17 @@ static int check_band(double band, const char* who)
 int dg_sample_sdf_band_device(const dg_mesh* m, const dg_grid_desc* grid, double sign, double band, uint64_t l_begin, uint64_t l_end, double* d_out,
                               void* stream)
 {
-    if (int rc = mesh_usable(m, "dg_sample_sdf_band_device")) return rc;
-    if (!m) return fail(DG_ERR_INVALID, "dg_sample_sdf_band: mesh is NULL (not constructed)");
+    static const char* who = "dg_sample_sdf_band_device";
+    if (int rc = mesh_usable(m, who)) return rc;
     GridDev g;
-    if (int rc = check_range(grid, l_begin, l_end, g, "dg_sample_sdf_band")) return rc;
-    if (int rc = check_band(band, "dg_sample_sdf_band")) return rc;
-    if (l_end > l_begin && !d_out) return fail(DG_ERR_INVALID, "dg_sample_sdf_band: output is NULL");
-    if (int rc = check_handle_device(m->device, "dg_sample_sdf_band")) return rc;
+    if (int rc = check_range(grid, l_begin, l_end, g, who)) return rc;
+    if (int rc = check_band(band, who)) return rc;
+    if (l_end > l_begin && !d_out) return fail(DG_ERR_INVALID, "%s: output is NULL", who);
+    if (int rc = check_handle_device(m->device, who)) return rc;
     if (l_end == l_begin) return DG_OK;
     const cudaStream_t st = (cudaStream_t)stream;
     const WindDev* wd = nullptr;
-    if (m->sign_mode == DG_SIGN_WINDING) { if (int rc = winding_dev(m, wd, "dg_sample_sdf_band")) return rc; }
+    if (m->sign_mode == DG_SIGN_WINDING) { if (int rc = winding_dev(m, wd, who)) return rc; }
     const double k1_sign = wd ? 1.0 : sign;     // winding mode: K1 with sign = +1, then the node pass
     const size_t bytes = k1_band_scratch_bytes(g, l_begin, l_end - l_begin);
     void* scratch = nullptr;
@@ -1068,7 +1117,6 @@ static void tables_job_copy(HostTablesJob* job, void* dst, const void* src, size
 int dg_sample_sdf(const dg_mesh* m, const dg_grid_desc* grid, double sign, uint64_t l_begin, uint64_t l_end, double* out_host)
 {
     if (int rc = mesh_usable(m, "dg_sample_sdf")) return rc;
-    if (!m) return fail(DG_ERR_INVALID, "dg_sample_sdf: mesh is NULL (not constructed)");
     GridDev g;
     if (int rc = check_range(grid, l_begin, l_end, g, "dg_sample_sdf")) return rc;
     const uint64_t n = l_end - l_begin;
@@ -1106,15 +1154,14 @@ int dg_sample_sdf(const dg_mesh* m, const dg_grid_desc* grid, double sign, uint6
 static int dg_add_function_sdf_impl(const dg_mesh* m, const dg_grid_desc* grid, double sign, double* nodes_host, uint32_t* cells_host, uint32_t* cell_map_host,
                         double* timings_ms, const double* band = nullptr)
 {
-    if (int rc = mesh_usable(m, "dg_add_function_sdf")) return rc;
-    if (!m) return fail(DG_ERR_INVALID, "dg_add_function_sdf: mesh is NULL (not constructed)");
-    if (band) { if (int rc = check_band(*band, "dg_add_function_sdf_band")) return rc; }
+    const char* who = band ? "dg_add_function_sdf_band" : "dg_add_function_sdf";
+    if (int rc = mesh_usable(m, who)) return rc;
+    if (band) { if (int rc = check_band(*band, who)) return rc; }
     GridDev g;
-    uint64_t n_nodes = 0;
-    if (grid && dg_grid_num_nodes(grid->resolution, &n_nodes)) return DG_ERR_INVALID;
-    if (int rc = check_range(grid, 0, n_nodes, g, "dg_add_function_sdf")) return rc;
-    if (!nodes_host) return fail(DG_ERR_INVALID, "dg_add_function_sdf: nodes output is NULL");
-    if (int rc = check_handle_device(m->device, "dg_add_function_sdf")) return rc;
+    if (int rc = grid_checked(grid, g, who)) return rc;
+    const uint64_t n_nodes = grid_nodes(g);
+    if (!nodes_host) return fail(DG_ERR_INVALID, "%s: nodes output is NULL", who);
+    if (int rc = check_handle_device(m->device, who)) return rc;
     const auto t0 = std::chrono::steady_clock::now();
     auto ms_since = [&](std::chrono::steady_clock::time_point t) { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t).count(); };
     HostTablesJob job;
@@ -1128,6 +1175,20 @@ static int dg_add_function_sdf_impl(const dg_mesh* m, const dg_grid_desc* grid, 
     job.finish();
     if (timings_ms) { timings_ms[0] = ms_since(t0); timings_ms[1] = ms_nodes; timings_ms[2] = timings_ms[0]; timings_ms[3] = job.ms_prefault; timings_ms[4] = (double)job.n_workers; timings_ms[5] = 1.0; }
     return rc;
+}
+
+int dg_add_function_sdf(const dg_mesh* m, const dg_grid_desc* grid, double sign, double* nodes_host, uint32_t* cells_host, uint32_t* cell_map_host,
+                        double* timings_ms)
+{
+    return guarded("dg_add_function_sdf", [&]() { return dg_add_function_sdf_impl(m, grid, sign, nodes_host, cells_host, cell_map_host, timings_ms); });
+}
+
+// addFunction(func, verbose, pred) with pred(x) = |md.signed_distance(x).distance| <= band (cubic_lagrange_discrete_grid.cpp:780-899, node
+// loop :806-817): the same pipeline as dg_add_function_sdf, every kernel chunk in its narrow-band form
+int dg_add_function_sdf_band(const dg_mesh* m, const dg_grid_desc* grid, double sign, double band, double* nodes_host, uint32_t* cells_host,
+                             uint32_t* cell_map_host, double* timings_ms)
+{
+    return guarded("dg_add_function_sdf_band", [&]() { return dg_add_function_sdf_impl(m, grid, sign, nodes_host, cells_host, cell_map_host, timings_ms, &band); });
 }
 
 // ------------------------------------------------------------------------------------------------ multi-GPU from ONE process
@@ -1227,10 +1288,9 @@ int dg_mesh_group_destroy(dg_mesh_group* grp)
 
 int dg_mesh_group_create(const dg_mesh* mesh, int n_gpus, const int* devices, dg_mesh_group** out)
 {
-    if (int rc = mesh_usable(mesh, "dg_mesh_group_create")) return rc;
     if (!out) return fail(DG_ERR_INVALID, "dg_mesh_group_create: out is NULL");
     *out = nullptr;
-    if (!mesh) return fail(DG_ERR_INVALID, "dg_mesh_group_create: mesh is NULL (not constructed)");
+    if (int rc = mesh_usable(mesh, "dg_mesh_group_create")) return rc;
     if (int rc = refuse_winding(mesh, "dg_mesh_group_create")) return rc;
     if (int rc = require_device()) return rc;
     const int have = dg_device_count();
@@ -1289,78 +1349,79 @@ int dg_mesh_group_size(const dg_mesh_group* grp) { return grp ? grp->n : 0; }
 // GPU's first part runs under its second launch); each GPU is driven by its own host thread and DMAs the contiguous plane-pair runs
 // of its parts to their final positions (directly when nodes_host is page-locked, else through pinned staging).  No collective is
 // needed: the exchange target is host memory.  cells_host / cell_map_host as in dg_add_function_sdf (nullable).
-static int dg_add_function_sdf_multi_impl(dg_mesh_group* grp, const dg_grid_desc* grid, double sign, double* nodes_host, uint32_t* cells_host,
+int dg_add_function_sdf_multi(dg_mesh_group* grp, const dg_grid_desc* grid, double sign, double* nodes_host, uint32_t* cells_host,
                               uint32_t* cell_map_host, double* timings_ms)
 {
-    if (!grp) return fail(DG_ERR_INVALID, "dg_add_function_sdf_multi: group is NULL");
-    if (int rc = refuse_winding(grp->parts[0], "dg_add_function_sdf_multi")) return rc;
-    GridDev g;
-    uint64_t n_nodes = 0;
-    if (grid && dg_grid_num_nodes(grid->resolution, &n_nodes)) return DG_ERR_INVALID;
-    if (int rc = check_range(grid, 0, n_nodes, g, "dg_add_function_sdf_multi")) return rc;
-    if (!nodes_host) return fail(DG_ERR_INVALID, "dg_add_function_sdf_multi: nodes output is NULL");
-    std::lock_guard<std::mutex> lock(grp->mu);
-    const int n = grp->n;
-    // parts per GPU: at least two (the D2H and the host copy of one part run under the next launch), more when the grid is large -- what
-    // stays exposed at the end is the copy of ONE part into the caller's memory -- but never below ~4 M
-    // nodes per launch (every launch ends with a tail of long-running warps) and never more than 16 parts in all
-    unsigned splits = (2 * n <= 16) ? 2u : 1u;
-    {
-        const uint64_t by_size = n_nodes / (4000000ull * (uint64_t)n);
-        const unsigned cap = 16u / (unsigned)n;
-        if (by_size > splits) splits = (unsigned)std::min<uint64_t>(by_size, cap);
-    }
-    InterleavedLayout L;
-    if (!k1_interleaved_layout(g, (unsigned)n * splits, L)) return fail(DG_ERR_INVALID, "dg_add_function_sdf_multi: grid too large for the exchange layout");
-    const auto t0 = std::chrono::steady_clock::now();
-    auto ms_since = [&](std::chrono::steady_clock::time_point t) { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t).count(); };
-    const bool direct = is_pinned_host(nodes_host);
-    HostTablesJob job;
-    job.start(g, n_nodes, nodes_host, cells_host, cell_map_host);
-    std::vector<int> rcs(n, DG_OK);
-    std::vector<std::string> errs(n);
-    std::vector<uint64_t> launches(n, 0);
-    auto drive = [&](int i) -> int {
-        DG_CUDA(cudaSetDevice(grp->devices[i]));
-        auto& d = grp->dev[i];
-        if (int rc = group_grow(d, (size_t)splits * L.slot_elems, direct ? 0 : (size_t)splits * L.slot_elems)) return rc;
-        std::vector<K1Run> runs[16];
-        for (unsigned sp = 0; sp < splits; sp++) {
-            const unsigned part = (unsigned)i + sp * (unsigned)n;
-            double* d_slot = d.d_buf + (size_t)sp * L.slot_elems;
-            cudaStream_t stream = d.st[sp & 1u];
-            DG_CUDA(k1_launch_sample_interleaved(grp->parts[i]->dev, g, sign, L, part, d_slot, stream));
-            launches[i]++;
-            k1_interleaved_runs(g, L, part, runs[sp]);
-            uint64_t used = 0;
-            for (const auto& r : runs[sp]) used = std::max<uint64_t>(used, r.slot_pos + r.count);
-            if (direct) { for (const auto& r : runs[sp]) DG_CUDA(cudaMemcpyAsync(nodes_host + r.node_begin, d_slot + r.slot_pos, r.count * sizeof(double), cudaMemcpyDeviceToHost, stream)); }
-            else if (used) DG_CUDA(cudaMemcpyAsync(d.h_stage + (size_t)sp * L.slot_elems, d_slot, used * sizeof(double), cudaMemcpyDeviceToHost, stream));
-            DG_CUDA(cudaEventRecord(d.ev[sp], stream));
+    return guarded("dg_add_function_sdf_multi", [&]() -> int {
+        if (!grp) return fail(DG_ERR_INVALID, "dg_add_function_sdf_multi: group is NULL");
+        if (int rc = refuse_winding(grp->parts[0], "dg_add_function_sdf_multi")) return rc;
+        GridDev g;
+        if (int rc = grid_checked(grid, g, "dg_add_function_sdf_multi")) return rc;
+        const uint64_t n_nodes = grid_nodes(g);
+        if (!nodes_host) return fail(DG_ERR_INVALID, "dg_add_function_sdf_multi: nodes output is NULL");
+        std::lock_guard<std::mutex> lock(grp->mu);
+        const int n = grp->n;
+        // parts per GPU: at least two (the D2H and the host copy of one part run under the next launch), more when the grid is large -- what
+        // stays exposed at the end is the copy of ONE part into the caller's memory -- but never below ~4 M
+        // nodes per launch (every launch ends with a tail of long-running warps) and never more than 16 parts in all
+        unsigned splits = (2 * n <= 16) ? 2u : 1u;
+        {
+            const uint64_t by_size = n_nodes / (4000000ull * (uint64_t)n);
+            const unsigned cap = 16u / (unsigned)n;
+            if (by_size > splits) splits = (unsigned)std::min<uint64_t>(by_size, cap);
         }
-        for (unsigned sp = 0; sp < splits; sp++) {
-            DG_CUDA(cudaEventSynchronize(d.ev[sp]));
-            if (!direct) for (const auto& r : runs[sp]) std::memcpy(nodes_host + r.node_begin, d.h_stage + (size_t)sp * L.slot_elems + r.slot_pos, r.count * sizeof(double));
-        }
-        return DG_OK;
-    };
-    {
-        DeviceGuard guard;
-        std::vector<std::thread> th;
-        auto guarded = [&](int i) {
-            try { rcs[i] = drive(i); if (rcs[i] != DG_OK) errs[i] = g_err; }
-            catch (const std::exception& ex) { rcs[i] = DG_ERR_NOMEM; errs[i] = ex.what(); }
+        InterleavedLayout L;
+        if (!k1_interleaved_layout(g, (unsigned)n * splits, L)) return fail(DG_ERR_INVALID, "dg_add_function_sdf_multi: grid too large for the exchange layout");
+        const auto t0 = std::chrono::steady_clock::now();
+        auto ms_since = [&](std::chrono::steady_clock::time_point t) { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t).count(); };
+        const bool direct = is_pinned_host(nodes_host);
+        HostTablesJob job;
+        job.start(g, n_nodes, nodes_host, cells_host, cell_map_host);
+        std::vector<int> rcs(n, DG_OK);
+        std::vector<std::string> errs(n);
+        std::vector<uint64_t> launches(n, 0);
+        auto drive = [&](int i) -> int {
+            DG_CUDA(cudaSetDevice(grp->devices[i]));
+            auto& d = grp->dev[i];
+            if (int rc = group_grow(d, (size_t)splits * L.slot_elems, direct ? 0 : (size_t)splits * L.slot_elems)) return rc;
+            std::vector<K1Run> runs[16];
+            for (unsigned sp = 0; sp < splits; sp++) {
+                const unsigned part = (unsigned)i + sp * (unsigned)n;
+                double* d_slot = d.d_buf + (size_t)sp * L.slot_elems;
+                cudaStream_t stream = d.st[sp & 1u];
+                DG_CUDA(k1_launch_sample_interleaved(grp->parts[i]->dev, g, sign, L, part, d_slot, stream));
+                launches[i]++;
+                k1_interleaved_runs(g, L, part, runs[sp]);
+                uint64_t used = 0;
+                for (const auto& r : runs[sp]) used = std::max<uint64_t>(used, r.slot_pos + r.count);
+                if (direct) { for (const auto& r : runs[sp]) DG_CUDA(cudaMemcpyAsync(nodes_host + r.node_begin, d_slot + r.slot_pos, r.count * sizeof(double), cudaMemcpyDeviceToHost, stream)); }
+                else if (used) DG_CUDA(cudaMemcpyAsync(d.h_stage + (size_t)sp * L.slot_elems, d_slot, used * sizeof(double), cudaMemcpyDeviceToHost, stream));
+                DG_CUDA(cudaEventRecord(d.ev[sp], stream));
+            }
+            for (unsigned sp = 0; sp < splits; sp++) {
+                DG_CUDA(cudaEventSynchronize(d.ev[sp]));
+                if (!direct) for (const auto& r : runs[sp]) std::memcpy(nodes_host + r.node_begin, d.h_stage + (size_t)sp * L.slot_elems + r.slot_pos, r.count * sizeof(double));
+            }
+            return DG_OK;
         };
-        for (int i = 1; i < n; i++) th.emplace_back([&, i]() { DeviceGuard tg; guarded(i); });
-        guarded(0);
-        for (auto& t : th) t.join();
-    }
-    const double ms_nodes = ms_since(t0);
-    job.finish();
-    for (int i = 0; i < n; i++) g_launches.fetch_add(launches[i]);
-    if (timings_ms) { timings_ms[0] = ms_since(t0); timings_ms[1] = ms_nodes; timings_ms[2] = timings_ms[0]; timings_ms[3] = job.ms_prefault; timings_ms[4] = (double)job.n_workers; timings_ms[5] = (double)n; }
-    for (int i = 0; i < n; i++) if (rcs[i] != DG_OK) return fail(rcs[i], "dg_add_function_sdf_multi (device %d): %s", grp->devices[i], errs[i].c_str());
-    return DG_OK;
+        {
+            DeviceGuard guard;
+            std::vector<std::thread> th;
+            auto guarded = [&](int i) {
+                try { rcs[i] = drive(i); if (rcs[i] != DG_OK) errs[i] = g_err; }
+                catch (const std::exception& ex) { rcs[i] = DG_ERR_NOMEM; errs[i] = ex.what(); }
+            };
+            for (int i = 1; i < n; i++) th.emplace_back([&, i]() { DeviceGuard tg; guarded(i); });
+            guarded(0);
+            for (auto& t : th) t.join();
+        }
+        const double ms_nodes = ms_since(t0);
+        job.finish();
+        for (int i = 0; i < n; i++) g_launches.fetch_add(launches[i]);
+        if (timings_ms) { timings_ms[0] = ms_since(t0); timings_ms[1] = ms_nodes; timings_ms[2] = timings_ms[0]; timings_ms[3] = job.ms_prefault; timings_ms[4] = (double)job.n_workers; timings_ms[5] = (double)n; }
+        for (int i = 0; i < n; i++) if (rcs[i] != DG_OK) return fail(rcs[i], "dg_add_function_sdf_multi (device %d): %s", grp->devices[i], errs[i].c_str());
+        return DG_OK;
+    });
 }
 
 // Device-resident form (the coefficient array is needed on every GPU, e.g. for K2/K3 replicas): GPU i samples part i of n into its
@@ -1371,9 +1432,7 @@ int dg_sample_sdf_multi_device(dg_mesh_group* grp, const dg_grid_desc* grid, dou
     if (!grp || !d_out) return fail(DG_ERR_INVALID, "dg_sample_sdf_multi_device: NULL argument");
     if (int rc = refuse_winding(grp->parts[0], "dg_sample_sdf_multi_device")) return rc;
     GridDev g;
-    uint64_t n_nodes = 0;
-    if (grid && dg_grid_num_nodes(grid->resolution, &n_nodes)) return DG_ERR_INVALID;
-    if (int rc = check_range(grid, 0, n_nodes, g, "dg_sample_sdf_multi_device")) return rc;
+    if (int rc = grid_checked(grid, g, "dg_sample_sdf_multi_device")) return rc;
     std::lock_guard<std::mutex> lock(grp->mu);
     const int n = grp->n;
     for (int i = 0; i < n; i++) if (!d_out[i]) return fail(DG_ERR_INVALID, "dg_sample_sdf_multi_device: d_out[%d] is NULL", i);
@@ -1431,8 +1490,8 @@ static void slab_planes(const GridDev& g, uint32_t part, uint32_t n_parts, unsig
 
 int dg_slab_ranges(const dg_grid_desc* grid, uint32_t part, uint32_t n_parts, uint64_t ranges[8])
 {
-    GridDev g; const char* why = "";
-    if (!grid_to_dev(grid, g, &why)) return fail(DG_ERR_INVALID, "dg_slab_ranges: %s", why);
+    GridDev g;
+    if (int rc = grid_checked(grid, g, "dg_slab_ranges")) return rc;
     if (!ranges || n_parts == 0 || part >= n_parts) return fail(DG_ERR_INVALID, "dg_slab_ranges: bad part / n_parts");
     unsigned pb[4], pe[4];
     slab_planes(g, part, n_parts, pb, pe);
@@ -1445,13 +1504,13 @@ int dg_slab_ranges(const dg_grid_desc* grid, uint32_t part, uint32_t n_parts, ui
 
 int dg_sample_sdf_slab_device(const dg_mesh* m, const dg_grid_desc* grid, double sign, uint32_t part, uint32_t n_parts, double* d_full, void* stream)
 {
-    if (int rc = mesh_usable(m, "dg_sample_sdf_slab_device")) return rc;
-    if (!m) return fail(DG_ERR_INVALID, "dg_sample_sdf_slab: mesh is NULL (not constructed)");
-    if (int rc = refuse_winding(m, "dg_sample_sdf_slab")) return rc;
-    GridDev g; const char* why = "";
-    if (!grid_to_dev(grid, g, &why)) return fail(DG_ERR_INVALID, "dg_sample_sdf_slab: %s", why);
-    if (n_parts == 0 || part >= n_parts || !d_full) return fail(DG_ERR_INVALID, "dg_sample_sdf_slab: bad part / n_parts / output");
-    if (int rc = check_handle_device(m->device, "dg_sample_sdf_slab")) return rc;
+    static const char* who = "dg_sample_sdf_slab_device";
+    if (int rc = mesh_usable(m, who)) return rc;
+    if (int rc = refuse_winding(m, who)) return rc;
+    GridDev g;
+    if (int rc = grid_checked(grid, g, who)) return rc;
+    if (n_parts == 0 || part >= n_parts || !d_full) return fail(DG_ERR_INVALID, "%s: bad part / n_parts / output", who);
+    if (int rc = check_handle_device(m->device, who)) return rc;
     unsigned pb[4], pe[4];
     slab_planes(g, part, n_parts, pb, pe);
     DG_LAUNCH(k1_launch_sample_slab(m->dev, g, sign, pb, pe, d_full, (cudaStream_t)stream));
@@ -1460,8 +1519,8 @@ int dg_sample_sdf_slab_device(const dg_mesh* m, const dg_grid_desc* grid, double
 
 int dg_interleaved_slot_elems(const dg_grid_desc* grid, uint32_t n_parts, uint64_t* slot_elems)
 {
-    GridDev g; const char* why = "";
-    if (!grid_to_dev(grid, g, &why)) return fail(DG_ERR_INVALID, "dg_interleaved_slot_elems: %s", why);
+    GridDev g;
+    if (int rc = grid_checked(grid, g, "dg_interleaved_slot_elems")) return rc;
     InterleavedLayout L;
     if (!slot_elems || !k1_interleaved_layout(g, n_parts, L)) return fail(DG_ERR_INVALID, "dg_interleaved_slot_elems: n_parts must be 1..16");
     *slot_elems = L.slot_elems;
@@ -1470,11 +1529,11 @@ int dg_interleaved_slot_elems(const dg_grid_desc* grid, uint32_t n_parts, uint64
 
 int dg_interleaved_node_slots(const dg_grid_desc* grid, uint32_t n_parts, uint64_t l_begin, uint64_t l_end, uint32_t* part_out, uint64_t* pos_out)
 {
-    GridDev g; const char* why = "";
-    if (!grid_to_dev(grid, g, &why)) return fail(DG_ERR_INVALID, "dg_interleaved_node_slots: %s", why);
+    GridDev g;
+    if (int rc = grid_checked(grid, g, "dg_interleaved_node_slots")) return rc;
     InterleavedLayout L;
     if (!k1_interleaved_layout(g, n_parts, L)) return fail(DG_ERR_INVALID, "dg_interleaved_node_slots: n_parts must be 1..16");
-    const uint64_t n = (uint64_t)g.nv + 2ull * ((uint64_t)g.ne_x + g.ne_y + g.ne_z);
+    const uint64_t n = grid_nodes(g);
     if (l_begin > l_end || l_end > n) return fail(DG_ERR_INVALID, "dg_interleaved_node_slots: node range outside [0, %llu]", (unsigned long long)n);
     k1_interleaved_node_slots(g, L, l_begin, l_end - l_begin, part_out, pos_out);
     return DG_OK;
@@ -1482,14 +1541,14 @@ int dg_interleaved_node_slots(const dg_grid_desc* grid, uint32_t n_parts, uint64
 
 int dg_sample_sdf_interleaved_device(const dg_mesh* m, const dg_grid_desc* grid, double sign, uint32_t part, uint32_t n_parts, double* d_slot, void* stream)
 {
-    if (int rc = mesh_usable(m, "dg_sample_sdf_interleaved_device")) return rc;
-    if (!m) return fail(DG_ERR_INVALID, "dg_sample_sdf_interleaved: mesh is NULL (not constructed)");
-    if (int rc = refuse_winding(m, "dg_sample_sdf_interleaved")) return rc;
-    GridDev g; const char* why = "";
-    if (!grid_to_dev(grid, g, &why)) return fail(DG_ERR_INVALID, "dg_sample_sdf_interleaved: %s", why);
+    static const char* who = "dg_sample_sdf_interleaved_device";
+    if (int rc = mesh_usable(m, who)) return rc;
+    if (int rc = refuse_winding(m, who)) return rc;
+    GridDev g;
+    if (int rc = grid_checked(grid, g, who)) return rc;
     InterleavedLayout L;
-    if (!k1_interleaved_layout(g, n_parts, L) || part >= n_parts || !d_slot) return fail(DG_ERR_INVALID, "dg_sample_sdf_interleaved: bad part / n_parts (1..16) / output");
-    if (int rc = check_handle_device(m->device, "dg_sample_sdf_interleaved")) return rc;
+    if (!k1_interleaved_layout(g, n_parts, L) || part >= n_parts || !d_slot) return fail(DG_ERR_INVALID, "%s: bad part / n_parts (1..16) / output", who);
+    if (int rc = check_handle_device(m->device, who)) return rc;
     DG_LAUNCH(k1_launch_sample_interleaved(m->dev, g, sign, L, part, d_slot, (cudaStream_t)stream));
     return DG_OK;
 }
@@ -1497,10 +1556,10 @@ int dg_sample_sdf_interleaved_device(const dg_mesh* m, const dg_grid_desc* grid,
 int dg_interleaved_unpack_device(const dg_grid_desc* grid, uint32_t n_parts, const double* d_slots, double* d_nodes, void* stream)
 {
     if (int rc = require_device()) return rc;
-    GridDev g; const char* why = "";
-    if (!grid_to_dev(grid, g, &why)) return fail(DG_ERR_INVALID, "dg_interleaved_unpack: %s", why);
+    GridDev g;
+    if (int rc = grid_checked(grid, g, "dg_interleaved_unpack_device")) return rc;
     InterleavedLayout L;
-    if (!k1_interleaved_layout(g, n_parts, L) || !d_slots || !d_nodes) return fail(DG_ERR_INVALID, "dg_interleaved_unpack: bad n_parts (1..16) / NULL buffer");
+    if (!k1_interleaved_layout(g, n_parts, L) || !d_slots || !d_nodes) return fail(DG_ERR_INVALID, "dg_interleaved_unpack_device: bad n_parts (1..16) / NULL buffer");
     DG_LAUNCH(k1_launch_unpack_interleaved(g, L, d_slots, d_nodes, (cudaStream_t)stream));
     return DG_OK;
 }
@@ -1528,9 +1587,9 @@ int dg_build_cells(const uint32_t res[3], uint64_t c_begin, uint64_t c_end, uint
     dg_grid_desc d;
     const double mn[3] = {0, 0, 0}, mx[3] = {1, 1, 1};
     if (int rc = dg_grid_init(mn, mx, res, &d)) return rc;
-    GridDev g; const char* why = "";
-    if (!grid_to_dev(&d, g, &why)) return fail(DG_ERR_INVALID, "dg_build_cells: %s", why);
-    const uint64_t nc = (uint64_t)res[0] * res[1] * res[2];
+    GridDev g;
+    if (int rc = grid_checked(&d, g, "dg_build_cells")) return rc;
+    const uint64_t nc = grid_cells(g);
     if (c_begin > c_end || c_end > nc) return fail(DG_ERR_INVALID, "dg_build_cells: cell range out of bounds");
     const uint64_t n = c_end - c_begin;
     if (n == 0) return DG_OK;
@@ -1561,17 +1620,14 @@ int dg_build_cells(const uint32_t res[3], uint64_t c_begin, uint64_t c_end, uint
 }
 
 // ------------------------------------------------------------------------------------------------ fields / K2
-static int field_common(const dg_grid_desc* grid, uint64_t n_nodes, dg_field** out, dg_field*& f)
+static int field_common(const dg_grid_desc* grid, dg_field** out, dg_field*& f)
 {
     if (!out) return fail(DG_ERR_INVALID, "dg_field_create: out is NULL");
     *out = nullptr;
     if (int rc = require_device()) return rc;
     if (int rc = ensure_selftest()) return rc;
-    GridDev g; const char* why = "";
-    if (!grid_to_dev(grid, g, &why)) return fail(DG_ERR_INVALID, "dg_field_create: %s", why);
-    uint64_t nn = 0;
-    if (int rc = dg_grid_num_nodes(grid->resolution, &nn)) return rc;
-    (void)n_nodes;
+    GridDev g;
+    if (int rc = grid_checked(grid, g, "dg_field_create")) return rc;
     f = new (std::nothrow) dg_field();
     if (!f) return fail(DG_ERR_NOMEM, "dg_field_create: out of host memory");
     f->desc = *grid; f->dev.g = g;
@@ -1587,7 +1643,7 @@ static int field_finish(dg_field* f, const double* d_nodes, const unsigned* d_ce
     if (e == cudaSuccess) { e = k2_launch_pack(f->dev.g, d_nodes, d_cells, f->n_cells_kept, f->d_packed.p, stream); g_launches.fetch_add(1); }
     if (e == cudaSuccess) { e = k2_launch_axis_tables(f->dev.g, f->d_tab.p, stream); g_launches.fetch_add(1); }
     if (e == cudaSuccess) { e = k3_coeff_max(f->d_packed.p, 32 * f->n_cells_kept, &f->coeff_max, stream); g_launches.fetch_add(1); }
-    if (e != cudaSuccess) return fail(e == cudaErrorMemoryAllocation ? DG_ERR_NOMEM : DG_ERR_CUDA, "dg_field_create: %s", cudaGetErrorString(e));
+    if (e != cudaSuccess) return fail(cuda_code(e), "dg_field_create: %s", cudaGetErrorString(e));
     f->dev.packed = f->d_packed.p;
     f->dev.cell_map = f->d_cell_map.p;
     f->dev.tab = f->d_tab.p;
@@ -1598,15 +1654,15 @@ int dg_field_create(const dg_grid_desc* grid, const double* nodes, uint64_t n_no
                     const uint32_t* cell_map, dg_field** out)
 {
     dg_field* f = nullptr;
-    if (int rc = field_common(grid, n_nodes, out, f)) return rc;
+    if (int rc = field_common(grid, out, f)) return rc;
     auto bail = [&](int rc) { delete f; return rc; };
-    const uint64_t n_cells = (uint64_t)grid->resolution[0] * grid->resolution[1] * grid->resolution[2];
+    const uint64_t n_cells = grid_cells(f->dev.g);
     if (!nodes && n_nodes) return bail(fail(DG_ERR_INVALID, "dg_field_create: nodes is NULL"));
     if (!cells && n_cells_kept != n_cells) return bail(fail(DG_ERR_INVALID, "dg_field_create: cells == NULL requires n_cells_kept == nx*ny*nz"));
     if (!cell_map && n_cells_kept != n_cells)      // K2/K3 read a NULL cell map as the identity: it must then cover every grid cell
         return bail(fail(DG_ERR_INVALID, "dg_field_create: cell_map == NULL requires n_cells_kept == nx*ny*nz (pass the reduced field's cell map)"));
     if (!cells) {
-        uint64_t nn = 0; dg_grid_num_nodes(grid->resolution, &nn);
+        const uint64_t nn = grid_nodes(f->dev.g);
         if (n_nodes != nn) return bail(fail(DG_ERR_INVALID, "dg_field_create: closed-form cells need all %llu nodes (got %llu)",
                                             (unsigned long long)nn, (unsigned long long)n_nodes));
     } else {
@@ -1630,7 +1686,7 @@ int dg_field_create(const dg_grid_desc* grid, const double* nodes, uint64_t n_no
         e = f->d_cell_map.alloc(n_cells);
         if (e == cudaSuccess) e = cudaMemcpy(f->d_cell_map.p, cell_map, n_cells * sizeof(unsigned), cudaMemcpyHostToDevice);
     }
-    if (e != cudaSuccess) return bail(fail(e == cudaErrorMemoryAllocation ? DG_ERR_NOMEM : DG_ERR_CUDA, "dg_field_create: %s", cudaGetErrorString(e)));
+    if (e != cudaSuccess) return bail(fail(cuda_code(e), "dg_field_create: %s", cudaGetErrorString(e)));
     if (int rc = field_finish(f, d_nodes.p, cells ? d_cells.p : nullptr, nullptr)) return bail(rc);
     e = cudaDeviceSynchronize();
     if (e != cudaSuccess) return bail(fail(DG_ERR_CUDA, "dg_field_create: %s", cudaGetErrorString(e)));
@@ -1641,11 +1697,11 @@ int dg_field_create(const dg_grid_desc* grid, const double* nodes, uint64_t n_no
 int dg_field_create_device(const dg_grid_desc* grid, const double* d_nodes, uint64_t n_nodes, void* stream, dg_field** out)
 {
     dg_field* f = nullptr;
-    if (int rc = field_common(grid, n_nodes, out, f)) return rc;
-    uint64_t nn = 0; dg_grid_num_nodes(grid->resolution, &nn);
+    if (int rc = field_common(grid, out, f)) return rc;
+    const uint64_t nn = grid_nodes(f->dev.g);
     if (!d_nodes || n_nodes != nn) { delete f; return fail(DG_ERR_INVALID, "dg_field_create_device: need all %llu node coefficients", (unsigned long long)nn); }
     f->n_nodes = n_nodes;
-    f->n_cells_kept = (uint64_t)grid->resolution[0] * grid->resolution[1] * grid->resolution[2];
+    f->n_cells_kept = grid_cells(f->dev.g);
     if (int rc = field_finish(f, d_nodes, nullptr, (cudaStream_t)stream)) { delete f; return rc; }
     *out = f;
     return DG_OK;
@@ -1667,18 +1723,18 @@ int dg_field_info(const dg_field* f, uint64_t info[4])
 
 int dg_interpolate_batch_device(const dg_field* f, const double* d_x, uint64_t n, double* d_phi, double* d_grad, void* stream)
 {
-    if (!f) return fail(DG_ERR_INVALID, "dg_interpolate_batch: field is NULL");
-    if (n && (!d_x || !d_phi)) return fail(DG_ERR_INVALID, "dg_interpolate_batch: x / phi is NULL");
-    if (int rc = check_handle_device(f->device, "dg_interpolate_batch")) return rc;
+    if (!f) return fail(DG_ERR_INVALID, "dg_interpolate_batch_device: field is NULL");
+    if (n && (!d_x || !d_phi)) return fail(DG_ERR_INVALID, "dg_interpolate_batch_device: x / phi is NULL");
+    if (int rc = check_handle_device(f->device, "dg_interpolate_batch_device")) return rc;
     DG_LAUNCH(k2_launch_interpolate(f->dev, d_x, n, d_phi, d_grad, (cudaStream_t)stream));
     return DG_OK;
 }
 
 int dg_interpolate_hessian_batch_device(const dg_field* f, const double* d_x, uint64_t n, double* d_phi, double* d_grad, double* d_hess, void* stream)
 {
-    if (!f) return fail(DG_ERR_INVALID, "dg_interpolate_hessian_batch: field is NULL");
-    if (n && (!d_x || !d_phi || !d_grad || !d_hess)) return fail(DG_ERR_INVALID, "dg_interpolate_hessian_batch: x / phi / grad / hess is NULL");
-    if (int rc = check_handle_device(f->device, "dg_interpolate_hessian_batch")) return rc;
+    if (!f) return fail(DG_ERR_INVALID, "dg_interpolate_hessian_batch_device: field is NULL");
+    if (n && (!d_x || !d_phi || !d_grad || !d_hess)) return fail(DG_ERR_INVALID, "dg_interpolate_hessian_batch_device: x / phi / grad / hess is NULL");
+    if (int rc = check_handle_device(f->device, "dg_interpolate_hessian_batch_device")) return rc;
     DG_LAUNCH(k2_launch_interpolate(f->dev, d_x, n, d_phi, d_grad, (cudaStream_t)stream, d_hess));
     return DG_OK;
 }
@@ -1755,12 +1811,12 @@ void threaded_copy(void* dst, const void* src, size_t bytes, unsigned nt)
 }  // namespace
 
 // hess (nullable; grad must then be given too) selects K2's Hessian mode; its buffers join the pool at the first call that passes it
-static int dg_interpolate_batch_impl(const dg_field* f, const double* x, uint64_t n, double* phi, double* grad, double* hess = nullptr)
+static int dg_interpolate_batch_impl(const dg_field* f, const double* x, uint64_t n, double* phi, double* grad, double* hess, const char* who)
 {
-    if (!f) return fail(DG_ERR_INVALID, "dg_interpolate_batch: field is NULL");
+    if (!f) return fail(DG_ERR_INVALID, "%s: field is NULL", who);
     if (n == 0) return DG_OK;
-    if (!x || !phi) return fail(DG_ERR_INVALID, "dg_interpolate_batch: x / phi is NULL");
-    if (int rc = check_handle_device(f->device, "dg_interpolate_batch")) return rc;
+    if (!x || !phi) return fail(DG_ERR_INVALID, "%s: x / phi is NULL", who);
+    if (int rc = check_handle_device(f->device, who)) return rc;
     std::lock_guard<std::mutex> lock(g_ipool.mu);
     constexpr int S = InterpPool::kSlots;
     const uint64_t chunk = std::min<uint64_t>(InterpPool::kChunk, n);
@@ -1802,49 +1858,45 @@ static int dg_interpolate_batch_impl(const dg_field* f, const double* x, uint64_
     return DG_OK;
 }
 
+int dg_interpolate_batch(const dg_field* f, const double* x, uint64_t n, double* phi, double* grad)
+{
+    static const char* who = "dg_interpolate_batch";
+    return guarded(who, [&]() { return dg_interpolate_batch_impl(f, x, n, phi, grad, nullptr, who); });
+}
+
+int dg_interpolate_hessian_batch(const dg_field* f, const double* x, uint64_t n, double* phi, double* grad, double* hess)
+{
+    static const char* who = "dg_interpolate_hessian_batch";
+    if (n && (!phi || !grad || !hess)) return fail(DG_ERR_INVALID, "%s: phi / grad / hess is NULL", who);
+    return guarded(who, [&]() { return dg_interpolate_batch_impl(f, x, n, phi, grad, hess, who); });
+}
+
 int dg_shape_functions(const double* xi, uint64_t n, double* N, double* dN)
 {
     if (int rc = require_device()) return rc;
     if (int rc = ensure_selftest()) return rc;
     if (n == 0) return DG_OK;
     if (!xi || !N) return fail(DG_ERR_INVALID, "dg_shape_functions: NULL argument");
-    DevBuf<double> d_xi, d_N, d_dN;
-    DG_CUDA(d_xi.alloc(3 * n));
-    DG_CUDA(d_N.alloc(32 * n));
-    if (dN) DG_CUDA(d_dN.alloc(96 * n));
-    DG_CUDA(cudaMemcpy(d_xi.p, xi, 3 * n * sizeof(double), cudaMemcpyHostToDevice));
-    DG_LAUNCH(k2_launch_shape_functions(d_xi.p, n, d_N.p, dN ? d_dN.p : nullptr, nullptr));
-    DG_CUDA(cudaMemcpy(N, d_N.p, 32 * n * sizeof(double), cudaMemcpyDeviceToHost));
-    if (dN) DG_CUDA(cudaMemcpy(dN, d_dN.p, 96 * n * sizeof(double), cudaMemcpyDeviceToHost));
-    return DG_OK;
+    return stage_on_device(n, n, {{xi, 3 * sizeof(double)}}, {{N, 32 * sizeof(double)}, {dN, 96 * sizeof(double)}},
+                           [](void* const* in, void* const* out, uint64_t, uint64_t c) -> int {
+                               DG_LAUNCH(k2_launch_shape_functions((const double*)in[0], c, (double*)out[0], (double*)out[1], nullptr));
+                               return DG_OK;
+                           });
 }
 
 // ------------------------------------------------------------------------------------------------ K3
-int dg_density_map_device(const dg_field* f, double h, double rho0, int no_reduction, uint64_t l_begin, uint64_t l_end, double* d_out,
-                          void* stream)
+// the argument checks of the density and the volume map over nodes [b, e) of f; why: the map's own check of its scalars (nullptr: valid)
+static int node_map_check(const dg_field* f, uint64_t b, uint64_t e, const char* why, const void* out, const char* who)
 {
-    if (!f) return fail(DG_ERR_INVALID, "dg_density_map: field is NULL");
+    if (!f) return fail(DG_ERR_INVALID, "%s: field is NULL", who);
     GridDev g;
-    if (int rc = check_range(&f->desc, l_begin, l_end, g, "dg_density_map")) return rc;
-    if (!(h > 0.0)) return fail(DG_ERR_INVALID, "dg_density_map: smoothing length must be > 0");
-    if (l_end > l_begin && !d_out) return fail(DG_ERR_INVALID, "dg_density_map: output is NULL");
-    if (int rc = check_handle_device(f->device, "dg_density_map")) return rc;
-    DG_LAUNCH(k3_launch_density(f->dev, f->coeff_max, h, rho0, no_reduction, l_begin, l_end - l_begin, d_out, (cudaStream_t)stream));
-    return DG_OK;
+    if (int rc = check_range(&f->desc, b, e, g, who)) return rc;
+    if (why) return fail(DG_ERR_INVALID, "%s: %s", who, why);
+    if (e > b && !out) return fail(DG_ERR_INVALID, "%s: output is NULL", who);
+    return check_handle_device(f->device, who);
 }
 
-int dg_density_map(const dg_field* f, double h, double rho0, int no_reduction, uint64_t l_begin, uint64_t l_end, double* out_host)
-{
-    if (!f) return fail(DG_ERR_INVALID, "dg_density_map: field is NULL");
-    if (l_end < l_begin) return fail(DG_ERR_INVALID, "dg_density_map: bad range");
-    const uint64_t n = l_end - l_begin;
-    if (n && !out_host) return fail(DG_ERR_INVALID, "dg_density_map: output is NULL");
-    DevBuf<double> d_out;
-    DG_CUDA(d_out.alloc(n));
-    if (int rc = dg_density_map_device(f, h, rho0, no_reduction, l_begin, l_end, d_out.p, nullptr)) return rc;
-    if (n) DG_CUDA(cudaMemcpy(out_host, d_out.p, n * sizeof(double), cudaMemcpyDeviceToHost));
-    return DG_OK;
-}
+static const char* density_args_invalid(double h, double) { return (h > 0.0) ? nullptr : "smoothing length must be > 0"; }
 
 // the volume map's arguments: h finite and > 0 (c1 = 0.5 * (-inf + inf) would make every offset NaN), scale finite
 static const char* volume_args_invalid(double h, double scale)
@@ -1854,30 +1906,48 @@ static const char* volume_args_invalid(double h, double scale)
     return nullptr;
 }
 
+static int density_launch(const dg_field* f, double h, double rho0, int no_reduction, uint64_t l_begin, uint64_t n, double* d_out, cudaStream_t st)
+{
+    DG_LAUNCH(k3_launch_density(f->dev, f->coeff_max, h, rho0, no_reduction, l_begin, n, d_out, st));
+    return DG_OK;
+}
+
+static int volume_launch(const dg_field* f, double h, double scale, int no_reduction, uint64_t l_begin, uint64_t n, double* d_out, cudaStream_t st)
+{
+    DG_LAUNCH(k3_launch_volume(f->dev, h, scale, no_reduction, l_begin, n, d_out, st));
+    return DG_OK;
+}
+
+int dg_density_map_device(const dg_field* f, double h, double rho0, int no_reduction, uint64_t l_begin, uint64_t l_end, double* d_out,
+                          void* stream)
+{
+    if (int rc = node_map_check(f, l_begin, l_end, density_args_invalid(h, rho0), d_out, "dg_density_map_device")) return rc;
+    return density_launch(f, h, rho0, no_reduction, l_begin, l_end - l_begin, d_out, (cudaStream_t)stream);
+}
+
+int dg_density_map(const dg_field* f, double h, double rho0, int no_reduction, uint64_t l_begin, uint64_t l_end, double* out_host)
+{
+    if (int rc = node_map_check(f, l_begin, l_end, density_args_invalid(h, rho0), out_host, "dg_density_map")) return rc;
+    const uint64_t n = l_end - l_begin;
+    return stage_on_device(n, n, {}, {{out_host, sizeof(double)}}, [&](void* const*, void* const* out, uint64_t b, uint64_t c) {
+        return density_launch(f, h, rho0, no_reduction, l_begin + b, c, (double*)out[0], nullptr);
+    });
+}
+
 int dg_volume_map_device(const dg_field* f, double h, double scale, int no_reduction, uint64_t l_begin, uint64_t l_end, double* d_out,
                          void* stream)
 {
-    if (!f) return fail(DG_ERR_INVALID, "dg_volume_map: field is NULL");
-    GridDev g;
-    if (int rc = check_range(&f->desc, l_begin, l_end, g, "dg_volume_map")) return rc;
-    if (const char* why = volume_args_invalid(h, scale)) return fail(DG_ERR_INVALID, "dg_volume_map: %s", why);
-    if (l_end > l_begin && !d_out) return fail(DG_ERR_INVALID, "dg_volume_map: output is NULL");
-    if (int rc = check_handle_device(f->device, "dg_volume_map")) return rc;
-    DG_LAUNCH(k3_launch_volume(f->dev, h, scale, no_reduction, l_begin, l_end - l_begin, d_out, (cudaStream_t)stream));
-    return DG_OK;
+    if (int rc = node_map_check(f, l_begin, l_end, volume_args_invalid(h, scale), d_out, "dg_volume_map_device")) return rc;
+    return volume_launch(f, h, scale, no_reduction, l_begin, l_end - l_begin, d_out, (cudaStream_t)stream);
 }
 
 int dg_volume_map(const dg_field* f, double h, double scale, int no_reduction, uint64_t l_begin, uint64_t l_end, double* out_host)
 {
-    if (!f) return fail(DG_ERR_INVALID, "dg_volume_map: field is NULL");
-    if (l_end < l_begin) return fail(DG_ERR_INVALID, "dg_volume_map: bad range");
+    if (int rc = node_map_check(f, l_begin, l_end, volume_args_invalid(h, scale), out_host, "dg_volume_map")) return rc;
     const uint64_t n = l_end - l_begin;
-    if (n && !out_host) return fail(DG_ERR_INVALID, "dg_volume_map: output is NULL");
-    DevBuf<double> d_out;
-    DG_CUDA(d_out.alloc(n));
-    if (int rc = dg_volume_map_device(f, h, scale, no_reduction, l_begin, l_end, d_out.p, nullptr)) return rc;
-    if (n) DG_CUDA(cudaMemcpy(out_host, d_out.p, n * sizeof(double), cudaMemcpyDeviceToHost));
-    return DG_OK;
+    return stage_on_device(n, n, {}, {{out_host, sizeof(double)}}, [&](void* const*, void* const* out, uint64_t b, uint64_t c) {
+        return volume_launch(f, h, scale, no_reduction, l_begin + b, c, (double*)out[0], nullptr);
+    });
 }
 
 // reduceField with its index passes on the GPU (k4_reduce.cu); the swap-walk compaction and the tie-order-preserving sort stay on the host
@@ -1943,32 +2013,33 @@ static int reduce_field_gpu(const GridDev& g, double* nodes, uint64_t n_nodes, c
     return DG_OK;
 }
 
-static int dg_reduce_field_impl(const dg_grid_desc* grid, double* nodes, uint64_t n_nodes, const uint8_t* keep_node, uint32_t* cells, uint64_t n_cells_in,
+int dg_reduce_field(const dg_grid_desc* grid, double* nodes, uint64_t n_nodes, const uint8_t* keep_node, uint32_t* cells, uint64_t n_cells_in,
                     uint32_t* cell_map, uint32_t flags, uint64_t* n_nodes_out, uint64_t* n_cells_out, double* timings_ms)
 {
-    GridDev g; const char* why = "";
-    if (!grid_to_dev(grid, g, &why)) return fail(DG_ERR_INVALID, "dg_reduce_field: %s", why);
-    const uint64_t n_grid_nodes = (uint64_t)g.nv + 2ull * ((uint64_t)g.ne_x + g.ne_y + g.ne_z);
-    const uint64_t n_grid_cells = (uint64_t)g.n[0] * g.n[1] * g.n[2];
-    if (!nodes || !keep_node || !cell_map || (n_cells_in && !cells) || !n_nodes_out || !n_cells_out)
-        return fail(DG_ERR_INVALID, "dg_reduce_field: NULL argument");
-    if (n_nodes != n_grid_nodes)          // node ids must be the grid's own numbering: their positions feed the Z-curve key (:1113)
-        return fail(DG_ERR_INVALID, "dg_reduce_field: the field has %llu nodes, the grid %llu (already reduced?)", (unsigned long long)n_nodes,
-                    (unsigned long long)n_grid_nodes);
-    if (n_cells_in > n_grid_cells) return fail(DG_ERR_INVALID, "dg_reduce_field: more cells than the grid has");
-    ReduceStats st; const char* err = "";
-    const char* env = std::getenv("DG_REDUCE_FIELD_HOST");
-    const bool host_passes = (flags & DG_REDUCE_HOST_PASSES) != 0 || (env && env[0] == '1');
-    if (host_passes) {
-        if (!reduce_field_host(g, nodes, n_nodes, keep_node, cells, n_cells_in, cell_map, n_grid_cells, (flags & DG_REDUCE_REFERENCE_SORT) != 0, st, &err))
-            return fail(DG_ERR_INVALID, "dg_reduce_field: %s", err);
-    } else {
-        if (int rc = require_device()) return rc;
-        if (int rc = reduce_field_gpu(g, nodes, n_nodes, keep_node, cells, n_cells_in, cell_map, n_grid_cells, (flags & DG_REDUCE_REFERENCE_SORT) != 0, st)) return rc;
-    }
-    *n_nodes_out = st.nodes_out; *n_cells_out = st.cells_out;
-    if (timings_ms) { timings_ms[0] = st.ms_cells; timings_ms[1] = st.ms_nodes; timings_ms[2] = st.ms_sort; timings_ms[3] = st.ms_write; timings_ms[4] = (double)st.tie_path; }
-    return DG_OK;
+    return guarded("dg_reduce_field", [&]() -> int {
+        GridDev g;
+        if (int rc = grid_checked(grid, g, "dg_reduce_field")) return rc;
+        const uint64_t n_grid_nodes = grid_nodes(g), n_grid_cells = grid_cells(g);
+        if (!nodes || !keep_node || !cell_map || (n_cells_in && !cells) || !n_nodes_out || !n_cells_out)
+            return fail(DG_ERR_INVALID, "dg_reduce_field: NULL argument");
+        if (n_nodes != n_grid_nodes)          // node ids must be the grid's own numbering: their positions feed the Z-curve key (:1113)
+            return fail(DG_ERR_INVALID, "dg_reduce_field: the field has %llu nodes, the grid %llu (already reduced?)", (unsigned long long)n_nodes,
+                        (unsigned long long)n_grid_nodes);
+        if (n_cells_in > n_grid_cells) return fail(DG_ERR_INVALID, "dg_reduce_field: more cells than the grid has");
+        ReduceStats st; const char* err = "";
+        const char* env = std::getenv("DG_REDUCE_FIELD_HOST");
+        const bool host_passes = (flags & DG_REDUCE_HOST_PASSES) != 0 || (env && env[0] == '1');
+        if (host_passes) {
+            if (!reduce_field_host(g, nodes, n_nodes, keep_node, cells, n_cells_in, cell_map, n_grid_cells, (flags & DG_REDUCE_REFERENCE_SORT) != 0, st, &err))
+                return fail(DG_ERR_INVALID, "dg_reduce_field: %s", err);
+        } else {
+            if (int rc = require_device()) return rc;
+            if (int rc = reduce_field_gpu(g, nodes, n_nodes, keep_node, cells, n_cells_in, cell_map, n_grid_cells, (flags & DG_REDUCE_REFERENCE_SORT) != 0, st)) return rc;
+        }
+        *n_nodes_out = st.nodes_out; *n_cells_out = st.cells_out;
+        if (timings_ms) { timings_ms[0] = st.ms_cells; timings_ms[1] = st.ms_nodes; timings_ms[2] = st.ms_sort; timings_ms[3] = st.ms_write; timings_ms[4] = (double)st.tie_path; }
+        return DG_OK;
+    });
 }
 
 // ------------------------------------------------------------------------------------------------ reduced fields on the device
@@ -2101,52 +2172,62 @@ static int device_reduce(const GridDev& g, const double* d_dense, uint64_t n, co
     return DG_OK;
 }
 
-// addFunction(func, verbose, band predicate) + reduceField(id, always true) on one GPU
-static int reduced_band_create_impl(const dg_mesh* m, const dg_grid_desc* grid, double sign, double band, uint32_t flags, dg_reduced_band** out,
-                                    double* timings_ms)
+// the reduction of a field made on the device (band, function, uploaded field): rows from `rows`, keep flags from d_mask (NULL: v != DBL_MAX
+// alone), the device_reduce stages
+static int reduce_device_field(const GridDev& g, const double* d_values, uint64_t n, const DenseRows& rows, const unsigned char* d_mask,
+                               uint32_t flags, dg_reduced_band& out, double ms[5], int& tie_path, StageClock& clock, const char* who, cudaStream_t st)
 {
-    if (int rc = mesh_usable(m, "dg_reduced_band_create")) return rc;
+    DevBuf<unsigned char> d_cell_keep;
+    if (int rc = device_cell_flags(g, d_values, n, rows, K4ValuePred{K4_KEEP_ANY, 0.0, 0.0, 0.0}, d_cell_keep, who, st, d_mask)) return rc;
+    return device_reduce(g, d_values, n, rows, d_cell_keep.p, grid_cells(g), (flags & DG_REDUCE_REFERENCE_SORT) != 0, out, ms + 1, tie_path, clock, st);
+}
+
+// timings_ms[0..7) of the reduced forms made by reduce_device_field: ms[0..5), the tie path, the total ms
+static void reduced_timings(double* timings_ms, const double ms[5], int tie_path, std::chrono::steady_clock::time_point t_start)
+{
+    if (!timings_ms) return;
+    for (int k = 0; k < 5; k++) timings_ms[k] = ms[k];
+    timings_ms[5] = (double)tie_path;
+    timings_ms[6] = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_start).count();
+}
+
+
+// addFunction(func, verbose, band predicate) + reduceField(id, always true) on one GPU
+int dg_reduced_band_create(const dg_mesh* m, const dg_grid_desc* grid, double sign, double band, uint32_t flags, dg_reduced_band** out,
+                           double* timings_ms)
+{
     static const char* who = "dg_reduced_band_create";
-    if (!out) return fail(DG_ERR_INVALID, "%s: out is NULL", who);
-    *out = nullptr;
-    if (!m) return fail(DG_ERR_INVALID, "%s: mesh is NULL (not constructed)", who);
-    GridDev g; const char* why = "";
-    if (!grid_to_dev(grid, g, &why)) return fail(DG_ERR_INVALID, "%s: %s", who, why);
-    if (int rc = check_band(band, who)) return rc;
-    if (flags & ~DG_REDUCE_REFERENCE_SORT) return fail(DG_ERR_INVALID, "%s: unknown flags 0x%x (only DG_REDUCE_REFERENCE_SORT)", who, flags);
-    const uint64_t n = (uint64_t)g.nv + 2ull * ((uint64_t)g.ne_x + g.ne_y + g.ne_z);
-    const uint64_t n_cells = (uint64_t)g.n[0] * g.n[1] * g.n[2];       // grid_to_dev has refused grids of 2^31 nodes or more
-    if (int rc = require_device()) return rc;
-    if (int rc = check_handle_device(m->device, who)) return rc;
-    StageClock clock;
-    const auto t_start = clock.t0;
-    const cudaStream_t st = nullptr;
-    double ms[5] = {0, 0, 0, 0, 0};
-    std::unique_ptr<dg_reduced_band> h(new dg_reduced_band());
-    h->desc = *grid;
-    DG_CUDA(cudaGetDevice(&h->device));
-    // ---- 1. the dense band coefficients (addFunction(func, pred), :806-817), on the device only
-    DevBuf<double> d_dense;
-    DG_CUDA(d_dense.alloc(n));
-    if (int rc = dg_sample_sdf_band_device(m, grid, sign, band, 0, n, d_dense.p, st)) return rc;
-    DG_CUDA(cudaStreamSynchronize(st));
-    ms[0] = clock.lap();
-    // ---- 2.-5. reduceField(id, always true): a node is kept iff its coefficient is not DBL_MAX; rows from the closed form
-    const DenseRows rows{nullptr, n_cells};
-    int tie_path = 0;
-    {
-        DevBuf<unsigned char> d_cell_keep;
-        if (int rc = device_cell_flags(g, d_dense.p, n, rows, K4ValuePred{K4_KEEP_ANY, 0.0, 0.0, 0.0}, d_cell_keep, who, st)) return rc;
-        if (int rc = device_reduce(g, d_dense.p, n, rows, d_cell_keep.p, n_cells, (flags & DG_REDUCE_REFERENCE_SORT) != 0, *h, ms + 1, tie_path, clock, st))
-            return rc;
-    }
-    if (timings_ms) {
-        for (int k = 0; k < 5; k++) timings_ms[k] = ms[k];
-        timings_ms[5] = (double)tie_path;
-        timings_ms[6] = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_start).count();
-    }
-    *out = h.release();
-    return DG_OK;
+    return guarded(who, [&]() -> int {
+        if (!out) return fail(DG_ERR_INVALID, "%s: out is NULL", who);
+        *out = nullptr;
+        if (int rc = mesh_usable(m, who)) return rc;
+        GridDev g;
+        if (int rc = grid_checked(grid, g, who)) return rc;
+        if (int rc = check_band(band, who)) return rc;
+        if (int rc = check_reduce_flags(flags, who)) return rc;
+        const uint64_t n = grid_nodes(g);
+        if (int rc = require_device()) return rc;
+        if (int rc = check_handle_device(m->device, who)) return rc;
+        StageClock clock;
+        const auto t_start = clock.t0;
+        const cudaStream_t st = nullptr;
+        double ms[5] = {0, 0, 0, 0, 0};
+        std::unique_ptr<dg_reduced_band> h(new dg_reduced_band());
+        h->desc = *grid;
+        DG_CUDA(cudaGetDevice(&h->device));
+        // ---- 1. the dense band coefficients (addFunction(func, pred), :806-817), on the device only
+        DevBuf<double> d_dense;
+        DG_CUDA(d_dense.alloc(n));
+        if (int rc = dg_sample_sdf_band_device(m, grid, sign, band, 0, n, d_dense.p, st)) return rc;
+        DG_CUDA(cudaStreamSynchronize(st));
+        ms[0] = clock.lap();
+        // ---- 2.-5. reduceField(id, always true): a node is kept iff its coefficient is not DBL_MAX; rows from the closed form
+        int tie_path = 0;
+        if (int rc = reduce_device_field(g, d_dense.p, n, DenseRows{nullptr, grid_cells(g)}, nullptr, flags, *h, ms, tie_path, clock, who, st)) return rc;
+        reduced_timings(timings_ms, ms, tie_path, t_start);
+        *out = h.release();
+        return DG_OK;
+    });
 }
 
 // What a reduced node map (GenerateDensityMap's pattern) takes from its node function: the entry point's name, the check of its
@@ -2168,17 +2249,16 @@ static int reduced_node_map_create_impl(const ReducedNodeMap& m, const dg_grid_d
     const char* who = m.who;
     if (!sdf_out || !density_out) return fail(DG_ERR_INVALID, "%s: out is NULL", who);
     *sdf_out = nullptr; *density_out = nullptr;
-    GridDev g; const char* why = "";
-    if (!grid_to_dev(grid, g, &why)) return fail(DG_ERR_INVALID, "%s: %s", who, why);     // refuses grids of 2^31 nodes or more
-    const uint64_t n = (uint64_t)g.nv + 2ull * ((uint64_t)g.ne_x + g.ne_y + g.ne_z);
-    const uint64_t n_grid_cells = (uint64_t)g.n[0] * g.n[1] * g.n[2];
+    GridDev g;
+    if (int rc = grid_checked(grid, g, who)) return rc;
+    const uint64_t n = grid_nodes(g), n_grid_cells = grid_cells(g);
     if (!sdf_nodes || !sdf_cell_map || (n_cells && !sdf_cells)) return fail(DG_ERR_INVALID, "%s: NULL argument", who);
     if (n_nodes != n)                     // node ids must be the grid's own numbering: their positions feed the Z-curve key (:1113)
         return fail(DG_ERR_INVALID, "%s: the SDF field has %llu nodes, the grid %llu (already reduced?)", who, (unsigned long long)n_nodes,
                     (unsigned long long)n);
     if (n_cells > n_grid_cells) return fail(DG_ERR_INVALID, "%s: more cells than the grid has", who);
     if (const char* why = m.args_invalid(h, param)) return fail(DG_ERR_INVALID, "%s: %s", who, why);
-    if (flags & ~DG_REDUCE_REFERENCE_SORT) return fail(DG_ERR_INVALID, "%s: unknown flags 0x%x (only DG_REDUCE_REFERENCE_SORT)", who, flags);
+    if (int rc = check_reduce_flags(flags, who)) return rc;
     if (int rc = require_device()) return rc;
     if (int rc = ensure_selftest()) return rc;
     // the tool's SDF predicate (main.cpp:139) with its bounds computed as its lambda computes them
@@ -2248,6 +2328,37 @@ static int reduced_node_map_create_impl(const ReducedNodeMap& m, const dg_grid_d
     }
     *sdf_out = r0.release(); *density_out = r1.release();
     return DG_OK;
+}
+
+int dg_reduced_density_map_create(const dg_grid_desc* grid, const double* sdf_nodes, uint64_t n_nodes, const uint32_t* sdf_cells, uint64_t n_cells,
+                                  const uint32_t* sdf_cell_map, double h, double rho0, uint32_t flags, dg_reduced_band** sdf_out,
+                                  dg_reduced_band** density_out, double* timings_ms)
+{
+    // GenerateDensityMap's second predicate, 0 <= v && v <= 3 rho0 (main.cpp:140)
+    const ReducedNodeMap m{"dg_reduced_density_map_create",
+                           density_args_invalid,
+                           [](const dg_field& f, double h_, double rho0_, uint64_t n, double* d_out, cudaStream_t st) {
+                               return k3_launch_density(f.dev, f.coeff_max, h_, rho0_, 0, 0, n, d_out, st);
+                           },
+                           K4ValuePred{K4_KEEP_RANGE, 0.0, 3.0 * rho0, 0.0}};
+    return guarded("dg_reduced_density_map_create", [&]() {
+        return reduced_node_map_create_impl(m, grid, sdf_nodes, n_nodes, sdf_cells, n_cells, sdf_cell_map, h, rho0, flags, sdf_out, density_out, timings_ms);
+    });
+}
+
+int dg_reduced_volume_map_create(const dg_grid_desc* grid, const double* sdf_nodes, uint64_t n_nodes, const uint32_t* sdf_cells, uint64_t n_cells,
+                                 const uint32_t* sdf_cell_map, double h, double scale, uint32_t flags, dg_reduced_band** sdf_out,
+                                 dg_reduced_band** volume_out, double* timings_ms)
+{
+    // the volume field keeps 0 <= v (and != DBL_MAX, as every reduceField): K4_KEEP_RANGE with b = +inf
+    const ReducedNodeMap m{"dg_reduced_volume_map_create", volume_args_invalid,
+                           [](const dg_field& f, double h_, double scale_, uint64_t n, double* d_out, cudaStream_t st) {
+                               return k3_launch_volume(f.dev, h_, scale_, 0, 0, n, d_out, st);
+                           },
+                           K4ValuePred{K4_KEEP_RANGE, 0.0, INFINITY, 0.0}};
+    return guarded("dg_reduced_volume_map_create", [&]() {
+        return reduced_node_map_create_impl(m, grid, sdf_nodes, n_nodes, sdf_cells, n_cells, sdf_cell_map, h, scale, flags, sdf_out, volume_out, timings_ms);
+    });
 }
 
 // ------------------------------------------------------------------------------------------------ user functions on the GPU (device callbacks)
@@ -2328,153 +2439,139 @@ static int run_device_callbacks(const GridDev& g, uint64_t n, uint64_t chunk_nod
     return DG_OK;
 }
 
-// checks shared by the three entry points: the grid (grid_to_dev refuses grids of 2^31 nodes or more), then a device
+// checks shared by the three entry points: the grid (grids of 2^31 nodes or more are refused), then a device
 static int device_callback_setup(const dg_grid_desc* grid, GridDev& g, uint64_t& n, const char* who)
 {
-    const char* why = "";
-    if (!grid_to_dev(grid, g, &why)) return fail(DG_ERR_INVALID, "%s: %s", who, why);
-    n = (uint64_t)g.nv + 2ull * ((uint64_t)g.ne_x + g.ne_y + g.ne_z);
+    if (int rc = grid_checked(grid, g, who)) return rc;
+    n = grid_nodes(g);
     if (int rc = require_device()) return rc;
     return ensure_selftest();
 }
 
-static int add_function_device_impl(const dg_grid_desc* grid, dg_device_function func, void* fu, dg_device_sample_predicate pred, void* pu,
-                                    uint64_t chunk_nodes, double* nodes_host, uint32_t* cells_host, uint32_t* cell_map_host, double* timings_ms)
+int dg_add_function_device(const dg_grid_desc* grid, dg_device_function func, void* fu, dg_device_sample_predicate pred, void* pu,
+                           uint64_t chunk_nodes, double* nodes_host, uint32_t* cells_host, uint32_t* cell_map_host, double* timings_ms)
 {
     static const char* who = "dg_add_function_device";
-    if (!func) return fail(DG_ERR_INVALID, "%s: the function callback is NULL", who);
-    if (!nodes_host) return fail(DG_ERR_INVALID, "%s: nodes output is NULL", who);
-    GridDev g; uint64_t n = 0;
-    if (int rc = device_callback_setup(grid, g, n, who)) return rc;
-    const auto t0 = std::chrono::steady_clock::now();
-    auto ms_since = [&](std::chrono::steady_clock::time_point t) { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t).count(); };
-    // host threads pre-fault nodes_host and write the connectivity + cell map (dg_add_function_sdf's HostTablesJob) while the callbacks run
-    HostTablesJob job;
-    job.start(g, n, nodes_host, cells_host, cell_map_host);
-    double ms_callbacks = 0.0;
-    int rc = DG_OK;
-    {
-        CallStreamSync st;
-        DevBuf<double> d_values;
-        if (int e = call_stream(st.s)) return e;
-        DG_CUDA(d_values.alloc(n));
-        DeviceCallbacks cb;
-        cb.func = func; cb.fu = fu; cb.sample = pred; cb.su = pu;
-        rc = run_device_callbacks(g, n, chunk_nodes, cb, d_values.p, nullptr, ms_callbacks, who, st.s);
-        if (rc == DG_OK) {
-            // the values -> nodes_host through dg_add_function_sdf's pinned double buffer, the table workers sharing the copies
-            std::lock_guard<std::mutex> lock(g_pool.mu);
-            DG_CUDA(g_pool.prepare(0, 1));
-            DG_CUDA(cudaEventRecord(g_pool.chunk_ev[0], st.s));
-            rc = drain_to_host_locked(d_values.p, n, n, nodes_host, &job);
+    return guarded(who, [&]() -> int {
+        if (!func) return fail(DG_ERR_INVALID, "%s: the function callback is NULL", who);
+        if (!nodes_host) return fail(DG_ERR_INVALID, "%s: nodes output is NULL", who);
+        GridDev g; uint64_t n = 0;
+        if (int rc = device_callback_setup(grid, g, n, who)) return rc;
+        const auto t0 = std::chrono::steady_clock::now();
+        auto ms_since = [&](std::chrono::steady_clock::time_point t) { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t).count(); };
+        // host threads pre-fault nodes_host and write the connectivity + cell map (dg_add_function_sdf's HostTablesJob) while the callbacks run
+        HostTablesJob job;
+        job.start(g, n, nodes_host, cells_host, cell_map_host);
+        double ms_callbacks = 0.0;
+        int rc = DG_OK;
+        {
+            CallStreamSync st;
+            DevBuf<double> d_values;
+            if (int e = call_stream(st.s)) return e;
+            DG_CUDA(d_values.alloc(n));
+            DeviceCallbacks cb;
+            cb.func = func; cb.fu = fu; cb.sample = pred; cb.su = pu;
+            rc = run_device_callbacks(g, n, chunk_nodes, cb, d_values.p, nullptr, ms_callbacks, who, st.s);
+            if (rc == DG_OK) {
+                // the values -> nodes_host through dg_add_function_sdf's pinned double buffer, the table workers sharing the copies
+                std::lock_guard<std::mutex> lock(g_pool.mu);
+                DG_CUDA(g_pool.prepare(0, 1));
+                DG_CUDA(cudaEventRecord(g_pool.chunk_ev[0], st.s));
+                rc = drain_to_host_locked(d_values.p, n, n, nodes_host, &job);
+            }
         }
-    }
-    const double ms_nodes = ms_since(t0);
-    job.finish();
-    if (rc == DG_OK && timings_ms) {
-        timings_ms[0] = ms_since(t0); timings_ms[1] = ms_nodes; timings_ms[2] = timings_ms[0]; timings_ms[3] = job.ms_prefault;
-        timings_ms[4] = (double)job.n_workers; timings_ms[5] = ms_callbacks;
-    }
-    return rc;
+        const double ms_nodes = ms_since(t0);
+        job.finish();
+        if (rc == DG_OK && timings_ms) {
+            timings_ms[0] = ms_since(t0); timings_ms[1] = ms_nodes; timings_ms[2] = timings_ms[0]; timings_ms[3] = job.ms_prefault;
+            timings_ms[4] = (double)job.n_workers; timings_ms[5] = ms_callbacks;
+        }
+        return rc;
+    });
 }
 
-// the reduction shared by both reduced forms: rows from `rows`, keep flags from d_mask (NULL: v != DBL_MAX alone), the device_reduce stages
-static int reduce_device_field(const GridDev& g, const double* d_values, uint64_t n, const DenseRows& rows, const unsigned char* d_mask,
-                               uint32_t flags, dg_reduced_band& out, double ms[5], int& tie_path, StageClock& clock, const char* who, cudaStream_t st)
-{
-    const uint64_t n_grid_cells = (uint64_t)g.n[0] * g.n[1] * g.n[2];
-    DevBuf<unsigned char> d_cell_keep;
-    if (int rc = device_cell_flags(g, d_values, n, rows, K4ValuePred{K4_KEEP_ANY, 0.0, 0.0, 0.0}, d_cell_keep, who, st, d_mask)) return rc;
-    return device_reduce(g, d_values, n, rows, d_cell_keep.p, n_grid_cells, (flags & DG_REDUCE_REFERENCE_SORT) != 0, out, ms + 1, tie_path, clock, st);
-}
-
-static void reduced_timings(double* timings_ms, const double ms[5], int tie_path, std::chrono::steady_clock::time_point t_start, double ms_callbacks)
-{
-    if (!timings_ms) return;
-    for (int k = 0; k < 5; k++) timings_ms[k] = ms[k];
-    timings_ms[5] = (double)tie_path;
-    timings_ms[6] = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_start).count();
-    timings_ms[7] = ms_callbacks;
-}
-
-static int reduced_function_create_impl(const dg_grid_desc* grid, dg_device_function func, void* fu, dg_device_sample_predicate sample_pred, void* su,
-                                        dg_device_node_predicate reduce_pred, void* ru, uint64_t chunk_nodes, uint32_t flags, dg_reduced_band** out,
-                                        double* timings_ms)
+int dg_reduced_function_create(const dg_grid_desc* grid, dg_device_function func, void* fu, dg_device_sample_predicate sample_pred, void* su,
+                               dg_device_node_predicate reduce_pred, void* ru, uint64_t chunk_nodes, uint32_t flags, dg_reduced_band** out,
+                               double* timings_ms)
 {
     static const char* who = "dg_reduced_function_create";
-    if (!out) return fail(DG_ERR_INVALID, "%s: out is NULL", who);
-    *out = nullptr;
-    if (!func) return fail(DG_ERR_INVALID, "%s: the function callback is NULL", who);
-    if (flags & ~DG_REDUCE_REFERENCE_SORT) return fail(DG_ERR_INVALID, "%s: unknown flags 0x%x (only DG_REDUCE_REFERENCE_SORT)", who, flags);
-    GridDev g; uint64_t n = 0;
-    if (int rc = device_callback_setup(grid, g, n, who)) return rc;
-    StageClock clock;
-    const auto t_start = clock.t0;
-    double ms[5] = {0, 0, 0, 0, 0}, ms_callbacks = 0.0;
-    int tie_path = 0;
-    std::unique_ptr<dg_reduced_band> h(new dg_reduced_band());
-    h->desc = *grid;
-    DG_CUDA(cudaGetDevice(&h->device));
-    CallStreamSync st;
-    if (int rc = call_stream(st.s)) return rc;
-    // ---- 1. addFunction(func, verbose, sample_pred) into a dense array on the device; the reduce predicate's mask per chunk meanwhile
-    DevBuf<double> d_values;
-    DevBuf<unsigned char> d_keep;
-    DG_CUDA(d_values.alloc(n));
-    if (reduce_pred) DG_CUDA(d_keep.alloc(n));
-    DeviceCallbacks cb;
-    cb.func = func; cb.fu = fu; cb.sample = sample_pred; cb.su = su; cb.node = reduce_pred; cb.nu = ru;
-    if (int rc = run_device_callbacks(g, n, chunk_nodes, cb, d_values.p, d_keep.p, ms_callbacks, who, st.s)) return rc;
-    ms[0] = clock.lap();
-    // ---- 2.-5. reduceField(id, reduce_pred) over the closed-form rows of the new field (addFunction's cells, identity map)
-    if (int rc = reduce_device_field(g, d_values.p, n, DenseRows{nullptr, (uint64_t)g.n[0] * g.n[1] * g.n[2]}, d_keep.p, flags, *h, ms, tie_path, clock, who,
-                                     st.s))
-        return rc;
-    reduced_timings(timings_ms, ms, tie_path, t_start, ms_callbacks);
-    *out = h.release();
-    return DG_OK;
+    return guarded(who, [&]() -> int {
+        if (!out) return fail(DG_ERR_INVALID, "%s: out is NULL", who);
+        *out = nullptr;
+        if (!func) return fail(DG_ERR_INVALID, "%s: the function callback is NULL", who);
+        if (int rc = check_reduce_flags(flags, who)) return rc;
+        GridDev g; uint64_t n = 0;
+        if (int rc = device_callback_setup(grid, g, n, who)) return rc;
+        StageClock clock;
+        const auto t_start = clock.t0;
+        double ms[5] = {0, 0, 0, 0, 0}, ms_callbacks = 0.0;
+        int tie_path = 0;
+        std::unique_ptr<dg_reduced_band> h(new dg_reduced_band());
+        h->desc = *grid;
+        DG_CUDA(cudaGetDevice(&h->device));
+        CallStreamSync st;
+        if (int rc = call_stream(st.s)) return rc;
+        // ---- 1. addFunction(func, verbose, sample_pred) into a dense array on the device; the reduce predicate's mask per chunk meanwhile
+        DevBuf<double> d_values;
+        DevBuf<unsigned char> d_keep;
+        DG_CUDA(d_values.alloc(n));
+        if (reduce_pred) DG_CUDA(d_keep.alloc(n));
+        DeviceCallbacks cb;
+        cb.func = func; cb.fu = fu; cb.sample = sample_pred; cb.su = su; cb.node = reduce_pred; cb.nu = ru;
+        if (int rc = run_device_callbacks(g, n, chunk_nodes, cb, d_values.p, d_keep.p, ms_callbacks, who, st.s)) return rc;
+        ms[0] = clock.lap();
+        // ---- 2.-5. reduceField(id, reduce_pred) over the closed-form rows of the new field (addFunction's cells, identity map)
+        if (int rc = reduce_device_field(g, d_values.p, n, DenseRows{nullptr, grid_cells(g)}, d_keep.p, flags, *h, ms, tie_path, clock, who, st.s)) return rc;
+        reduced_timings(timings_ms, ms, tie_path, t_start);
+        if (timings_ms) timings_ms[7] = ms_callbacks;
+        *out = h.release();
+        return DG_OK;
+    });
 }
 
-static int reduce_field_device_impl(const dg_grid_desc* grid, const double* nodes, uint64_t n_nodes, const uint32_t* cells, uint64_t n_cells,
-                                    dg_device_node_predicate pred, void* pu, uint64_t chunk_nodes, uint32_t flags, dg_reduced_band** out,
-                                    double* timings_ms)
+int dg_reduce_field_device(const dg_grid_desc* grid, const double* nodes, uint64_t n_nodes, const uint32_t* cells, uint64_t n_cells,
+                           dg_device_node_predicate pred, void* pu, uint64_t chunk_nodes, uint32_t flags, dg_reduced_band** out,
+                           double* timings_ms)
 {
     static const char* who = "dg_reduce_field_device";
-    if (!out) return fail(DG_ERR_INVALID, "%s: out is NULL", who);
-    *out = nullptr;
-    if (!pred) return fail(DG_ERR_INVALID, "%s: the node predicate callback is NULL", who);
-    if (!nodes || (n_cells && !cells)) return fail(DG_ERR_INVALID, "%s: NULL argument", who);
-    if (flags & ~DG_REDUCE_REFERENCE_SORT) return fail(DG_ERR_INVALID, "%s: unknown flags 0x%x (only DG_REDUCE_REFERENCE_SORT)", who, flags);
-    GridDev g; uint64_t n = 0;
-    if (int rc = device_callback_setup(grid, g, n, who)) return rc;
-    if (n_nodes != n)                     // node ids must be the grid's own numbering: their positions feed the Z-curve key (:1113)
-        return fail(DG_ERR_INVALID, "%s: the field has %llu nodes, the grid %llu (already reduced?)", who, (unsigned long long)n_nodes, (unsigned long long)n);
-    if (n_cells > (uint64_t)g.n[0] * g.n[1] * g.n[2]) return fail(DG_ERR_INVALID, "%s: more cells than the grid has", who);
-    StageClock clock;
-    const auto t_start = clock.t0;
-    double ms[5] = {0, 0, 0, 0, 0}, ms_callbacks = 0.0;
-    int tie_path = 0;
-    std::unique_ptr<dg_reduced_band> h(new dg_reduced_band());
-    h->desc = *grid;
-    DG_CUDA(cudaGetDevice(&h->device));
-    CallStreamSync st;
-    if (int rc = call_stream(st.s)) return rc;
-    // ---- 1. upload the field and its rows; the predicate's mask per chunk, ANDed with v != DBL_MAX (the rows are checked by the cell flags)
-    DevBuf<double> d_values;
-    DevBuf<unsigned> d_cells;
-    DevBuf<unsigned char> d_keep;
-    DG_CUDA(d_values.alloc(n)); DG_CUDA(d_cells.alloc(32 * n_cells)); DG_CUDA(d_keep.alloc(n));
-    DG_CUDA(cudaMemcpyAsync(d_values.p, nodes, n * sizeof(double), cudaMemcpyHostToDevice, st.s));
-    if (n_cells) DG_CUDA(cudaMemcpyAsync(d_cells.p, cells, 32 * n_cells * sizeof(unsigned), cudaMemcpyHostToDevice, st.s));
-    DeviceCallbacks cb;
-    cb.node = pred; cb.nu = pu;
-    if (int rc = run_device_callbacks(g, n, chunk_nodes, cb, d_values.p, d_keep.p, ms_callbacks, who, st.s)) return rc;
-    ms[0] = clock.lap();
-    // ---- 2.-5. reduceField over the uploaded rows
-    if (int rc = reduce_device_field(g, d_values.p, n, DenseRows{d_cells.p, n_cells}, d_keep.p, flags, *h, ms, tie_path, clock, who, st.s)) return rc;
-    reduced_timings(timings_ms, ms, tie_path, t_start, ms_callbacks);
-    *out = h.release();
-    return DG_OK;
+    return guarded(who, [&]() -> int {
+        if (!out) return fail(DG_ERR_INVALID, "%s: out is NULL", who);
+        *out = nullptr;
+        if (!pred) return fail(DG_ERR_INVALID, "%s: the node predicate callback is NULL", who);
+        if (!nodes || (n_cells && !cells)) return fail(DG_ERR_INVALID, "%s: NULL argument", who);
+        if (int rc = check_reduce_flags(flags, who)) return rc;
+        GridDev g; uint64_t n = 0;
+        if (int rc = device_callback_setup(grid, g, n, who)) return rc;
+        if (n_nodes != n)                     // node ids must be the grid's own numbering: their positions feed the Z-curve key (:1113)
+            return fail(DG_ERR_INVALID, "%s: the field has %llu nodes, the grid %llu (already reduced?)", who, (unsigned long long)n_nodes, (unsigned long long)n);
+        if (n_cells > grid_cells(g)) return fail(DG_ERR_INVALID, "%s: more cells than the grid has", who);
+        StageClock clock;
+        const auto t_start = clock.t0;
+        double ms[5] = {0, 0, 0, 0, 0}, ms_callbacks = 0.0;
+        int tie_path = 0;
+        std::unique_ptr<dg_reduced_band> h(new dg_reduced_band());
+        h->desc = *grid;
+        DG_CUDA(cudaGetDevice(&h->device));
+        CallStreamSync st;
+        if (int rc = call_stream(st.s)) return rc;
+        // ---- 1. upload the field and its rows; the predicate's mask per chunk, ANDed with v != DBL_MAX (the rows are checked by the cell flags)
+        DevBuf<double> d_values;
+        DevBuf<unsigned> d_cells;
+        DevBuf<unsigned char> d_keep;
+        DG_CUDA(d_values.alloc(n)); DG_CUDA(d_cells.alloc(32 * n_cells)); DG_CUDA(d_keep.alloc(n));
+        DG_CUDA(cudaMemcpyAsync(d_values.p, nodes, n * sizeof(double), cudaMemcpyHostToDevice, st.s));
+        if (n_cells) DG_CUDA(cudaMemcpyAsync(d_cells.p, cells, 32 * n_cells * sizeof(unsigned), cudaMemcpyHostToDevice, st.s));
+        DeviceCallbacks cb;
+        cb.node = pred; cb.nu = pu;
+        if (int rc = run_device_callbacks(g, n, chunk_nodes, cb, d_values.p, d_keep.p, ms_callbacks, who, st.s)) return rc;
+        ms[0] = clock.lap();
+        // ---- 2.-5. reduceField over the uploaded rows
+        if (int rc = reduce_device_field(g, d_values.p, n, DenseRows{d_cells.p, n_cells}, d_keep.p, flags, *h, ms, tie_path, clock, who, st.s)) return rc;
+        reduced_timings(timings_ms, ms, tie_path, t_start);
+        if (timings_ms) timings_ms[7] = ms_callbacks;
+        *out = h.release();
+        return DG_OK;
+    });
 }
 
 int dg_reduced_band_sizes(const dg_reduced_band* h, uint64_t* n_nodes, uint64_t* n_cells)
@@ -2510,7 +2607,7 @@ int dg_field_create_reduced(const dg_reduced_band* h, dg_field** out)
     *out = nullptr;
     if (!h) return fail(DG_ERR_INVALID, "%s: handle is NULL", who);
     dg_field* f = nullptr;
-    if (int rc = field_common(&h->desc, h->n_nodes, out, f)) return rc;
+    if (int rc = field_common(&h->desc, out, f)) return rc;
     std::unique_ptr<dg_field> own(f);
     if (int rc = check_handle_device(h->device, who)) return rc;
     f->n_nodes = h->n_nodes; f->n_cells_kept = h->n_cells;
@@ -2534,84 +2631,81 @@ struct dg_isosurface {
 // values, classify, scans, emit (k6_isosurface.cu); each stage ends with a synchronise.  Device memory: 8 B per lattice point of values,
 // 7 B per point of edge flags, 1 B per lattice cell of counts, 1/8 B per point of chunk ranks, the tile arrays, one chunk of positions
 // (24 B x min(Np, 2^24)), then 24 B per vertex and 12 B per triangle of output.
-static int isosurface_create_impl(const dg_field* f, double iso, uint32_t s, dg_isosurface** out, double* timings_ms)
+int dg_isosurface_create(const dg_field* f, double iso, uint32_t s, dg_isosurface** out, double* timings_ms)
 {
     static const char* who = "dg_isosurface_create";
-    if (!out) return fail(DG_ERR_INVALID, "%s: out is NULL", who);
-    *out = nullptr;
-    if (!f) return fail(DG_ERR_INVALID, "%s: field is NULL", who);
-    if (!std::isfinite(iso)) return fail(DG_ERR_INVALID, "%s: iso must be finite (got %g)", who, iso);
-    if (s == 0 || s > K6_MAX_SUBDIVISIONS) return fail(DG_ERR_INVALID, "%s: subdivisions must be 1..%u (got %u)", who, K6_MAX_SUBDIVISIONS, s);
-    uint64_t np = 0;
-    const K6Lattice L = k6_lattice(f->dev.g, s, np);
-    if (np >= (1ull << 31))
-        return fail(DG_ERR_INVALID, "%s: the lattice of %llu points (%u x %u x %u) has 2^31 points or more; use fewer subdivisions", who,
-                    (unsigned long long)np, L.np[0], L.np[1], L.np[2]);
-    if (int rc = check_handle_device(f->device, who)) return rc;
-    const uint64_t n_cells = (uint64_t)(L.np[0] - 1) * (L.np[1] - 1) * (L.np[2] - 1);
-    const uint64_t n_edges = 7 * np, tile = k6_tile();
-    StageClock clock;
-    const auto t_start = clock.t0;
-    const cudaStream_t st = nullptr;
-    double ms[4] = {0, 0, 0, 0};
-    std::unique_ptr<dg_isosurface> h(new dg_isosurface());
-    h->device = f->device;
-    // ---- values: lattice positions per chunk, K2 value-only
-    DevBuf<double> d_values;
-    DG_CUDA(d_values.alloc(np));
-    {
-        DevBuf<double> d_x;
-        const uint64_t chunk = std::min<uint64_t>(np, K6_CHUNK);
-        DG_CUDA(d_x.alloc(3 * chunk));
-        for (uint64_t b = 0; b < np; b += chunk) {
-            const uint64_t n = std::min(chunk, np - b);
-            DG_LAUNCH(k6_launch_positions(L, b, n, d_x.p, st));
-            DG_LAUNCH(k2_launch_interpolate(f->dev, d_x.p, n, d_values.p + b, nullptr, st));
+    return guarded(who, [&]() -> int {
+        if (!out) return fail(DG_ERR_INVALID, "%s: out is NULL", who);
+        *out = nullptr;
+        if (!f) return fail(DG_ERR_INVALID, "%s: field is NULL", who);
+        if (!std::isfinite(iso)) return fail(DG_ERR_INVALID, "%s: iso must be finite (got %g)", who, iso);
+        if (s == 0 || s > K6_MAX_SUBDIVISIONS) return fail(DG_ERR_INVALID, "%s: subdivisions must be 1..%u (got %u)", who, K6_MAX_SUBDIVISIONS, s);
+        uint64_t np = 0;
+        const K6Lattice L = k6_lattice(f->dev.g, s, np);
+        if (np >= (1ull << 31))
+            return fail(DG_ERR_INVALID, "%s: the lattice of %llu points (%u x %u x %u) has 2^31 points or more; use fewer subdivisions", who,
+                        (unsigned long long)np, L.np[0], L.np[1], L.np[2]);
+        if (int rc = check_handle_device(f->device, who)) return rc;
+        const uint64_t n_cells = (uint64_t)(L.np[0] - 1) * (L.np[1] - 1) * (L.np[2] - 1);
+        const uint64_t n_edges = 7 * np, tile = k6_tile();
+        StageClock clock;
+        const auto t_start = clock.t0;
+        const cudaStream_t st = nullptr;
+        double ms[4] = {0, 0, 0, 0};
+        std::unique_ptr<dg_isosurface> h(new dg_isosurface());
+        h->device = f->device;
+        // ---- values: lattice positions per chunk, K2 value-only
+        DevBuf<double> d_values;
+        DG_CUDA(d_values.alloc(np));
+        {
+            DevBuf<double> d_x;
+            const uint64_t chunk = std::min<uint64_t>(np, K6_CHUNK);
+            DG_CUDA(d_x.alloc(3 * chunk));
+            for (uint64_t b = 0; b < np; b += chunk) {
+                const uint64_t n = std::min(chunk, np - b);
+                DG_LAUNCH(k6_launch_positions(L, b, n, d_x.p, st));
+                DG_LAUNCH(k2_launch_interpolate(f->dev, d_x.p, n, d_values.p + b, nullptr, st));
+            }
+            DG_CUDA(cudaStreamSynchronize(st));
         }
+        ms[0] = clock.lap();
+        // ---- classify: triangle count per lattice cell, flags of the crossing edges (rounded up to whole 32-edge chunks, which emit reads)
+        DevBuf<unsigned char> d_count, d_flags;
+        DG_CUDA(d_count.alloc(n_cells));
+        DG_CUDA(d_flags.alloc((n_edges + 31) / 32 * 32));
+        DG_CUDA(cudaMemsetAsync(d_flags.p, 0, d_flags.bytes(), st));
+        DG_LAUNCH(k6_launch_classify(L, d_values.p, iso, d_count.p, d_flags.p, st));
         DG_CUDA(cudaStreamSynchronize(st));
-    }
-    ms[0] = clock.lap();
-    // ---- classify: triangle count per lattice cell, flags of the crossing edges (rounded up to whole 32-edge chunks, which emit reads)
-    DevBuf<unsigned char> d_count, d_flags;
-    DG_CUDA(d_count.alloc(n_cells));
-    DG_CUDA(d_flags.alloc((n_edges + 31) / 32 * 32));
-    DG_CUDA(cudaMemsetAsync(d_flags.p, 0, d_flags.bytes(), st));
-    DG_LAUNCH(k6_launch_classify(L, d_values.p, iso, d_count.p, d_flags.p, st));
-    DG_CUDA(cudaStreamSynchronize(st));
-    ms[1] = clock.lap();
-    // ---- scans: triangles per tile of cells, vertices per tile of edges; both totals must fit the uint32 indices of the output
-    DevBuf<unsigned> d_tri_tile, d_edge_tile;
-    DG_CUDA(d_tri_tile.alloc((n_cells + tile - 1) / tile));
-    DG_CUDA(d_edge_tile.alloc((n_edges + tile - 1) / tile));
-    uint64_t n_tri = 0, n_vert = 0;
-    DG_LAUNCH(k6_scan_counts(d_count.p, n_cells, d_tri_tile.p, n_tri, st));
-    DG_LAUNCH(k4_scan_flags(d_flags.p, n_edges, d_edge_tile.p, n_vert, st));
-    if (n_vert >= (1ull << 32)) return fail(DG_ERR_INVALID, "%s: %llu vertices do not fit uint32 indices; use fewer subdivisions", who, (unsigned long long)n_vert);
-    if (n_tri >= (1ull << 32)) return fail(DG_ERR_INVALID, "%s: %llu triangles do not fit uint32 counts; use fewer subdivisions", who, (unsigned long long)n_tri);
-    ms[2] = clock.lap();
-    // ---- emit: vertices at their ranks (and the rank of every 32-edge chunk), then the triangles
-    if (n_vert) {
-        DevBuf<unsigned> d_chunk;
-        DG_CUDA(d_chunk.alloc((n_edges + 31) / 32));
-        DG_CUDA(h->d_vertices.alloc(3 * n_vert));
-        DG_CUDA(h->d_triangles.alloc(3 * n_tri));
-        DG_LAUNCH(k6_launch_vertices(L, d_values.p, iso, d_flags.p, n_edges, d_edge_tile.p, d_chunk.p, h->d_vertices.p, st));
-        DG_LAUNCH(k6_launch_triangles(L, d_values.p, iso, d_count.p, d_tri_tile.p, d_flags.p, d_chunk.p, h->d_triangles.p, st));
-        DG_CUDA(cudaStreamSynchronize(st));
-    }
-    h->n_vertices = n_vert; h->n_triangles = n_tri;
-    ms[3] = clock.lap();
-    if (timings_ms) {
-        for (int k = 0; k < 4; k++) timings_ms[k] = ms[k];
-        timings_ms[4] = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_start).count();
-    }
-    *out = h.release();
-    return DG_OK;
-}
-
-int dg_isosurface_create(const dg_field* field, double iso, uint32_t subdivisions, dg_isosurface** out, double* timings_ms)
-{
-    return guarded("dg_isosurface_create", [&]() { return isosurface_create_impl(field, iso, subdivisions, out, timings_ms); });
+        ms[1] = clock.lap();
+        // ---- scans: triangles per tile of cells, vertices per tile of edges; both totals must fit the uint32 indices of the output
+        DevBuf<unsigned> d_tri_tile, d_edge_tile;
+        DG_CUDA(d_tri_tile.alloc((n_cells + tile - 1) / tile));
+        DG_CUDA(d_edge_tile.alloc((n_edges + tile - 1) / tile));
+        uint64_t n_tri = 0, n_vert = 0;
+        DG_LAUNCH(k6_scan_counts(d_count.p, n_cells, d_tri_tile.p, n_tri, st));
+        DG_LAUNCH(k4_scan_flags(d_flags.p, n_edges, d_edge_tile.p, n_vert, st));
+        if (n_vert >= (1ull << 32)) return fail(DG_ERR_INVALID, "%s: %llu vertices do not fit uint32 indices; use fewer subdivisions", who, (unsigned long long)n_vert);
+        if (n_tri >= (1ull << 32)) return fail(DG_ERR_INVALID, "%s: %llu triangles do not fit uint32 counts; use fewer subdivisions", who, (unsigned long long)n_tri);
+        ms[2] = clock.lap();
+        // ---- emit: vertices at their ranks (and the rank of every 32-edge chunk), then the triangles
+        if (n_vert) {
+            DevBuf<unsigned> d_chunk;
+            DG_CUDA(d_chunk.alloc((n_edges + 31) / 32));
+            DG_CUDA(h->d_vertices.alloc(3 * n_vert));
+            DG_CUDA(h->d_triangles.alloc(3 * n_tri));
+            DG_LAUNCH(k6_launch_vertices(L, d_values.p, iso, d_flags.p, n_edges, d_edge_tile.p, d_chunk.p, h->d_vertices.p, st));
+            DG_LAUNCH(k6_launch_triangles(L, d_values.p, iso, d_count.p, d_tri_tile.p, d_flags.p, d_chunk.p, h->d_triangles.p, st));
+            DG_CUDA(cudaStreamSynchronize(st));
+        }
+        h->n_vertices = n_vert; h->n_triangles = n_tri;
+        ms[3] = clock.lap();
+        if (timings_ms) {
+            for (int k = 0; k < 4; k++) timings_ms[k] = ms[k];
+            timings_ms[4] = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_start).count();
+        }
+        *out = h.release();
+        return DG_OK;
+    });
 }
 
 int dg_isosurface_sizes(const dg_isosurface* s, uint64_t* n_vertices, uint64_t* n_triangles)
@@ -2668,44 +2762,28 @@ int dg_field_raycast_device(const dg_field* f, const double* d_o, const double* 
     return DG_OK;
 }
 
-// host arrays: chunks of 2^20 rays (64 MiB of device buffers) uploaded, cast and downloaded in turn on the legacy default stream
-static int raycast_host_impl(const dg_field* f, const double* o, const double* d, uint64_t n, double iso, double t_min, double t_max,
-                             double* t_lo, double* t_hi, int32_t* status)
-{
-    static const char* who = "dg_field_raycast";
-    if (int rc = raycast_check(f, o, d, n, iso, t_min, t_max, t_lo, t_hi, status, who)) return rc;
-    if (n == 0) return DG_OK;
-    const uint64_t chunk = std::min<uint64_t>(n, 1ull << 20);
-    DevBuf<double> d_o, d_d, d_lo, d_hi;
-    DevBuf<int32_t> d_st;
-    DG_CUDA(d_o.alloc(3 * chunk));
-    DG_CUDA(d_d.alloc(3 * chunk));
-    DG_CUDA(d_lo.alloc(chunk));
-    DG_CUDA(d_hi.alloc(chunk));
-    DG_CUDA(d_st.alloc(chunk));
-    for (uint64_t b = 0; b < n; b += chunk) {
-        const uint64_t c = std::min(chunk, n - b);
-        DG_CUDA(cudaMemcpy(d_o.p, o + 3 * b, 3 * c * sizeof(double), cudaMemcpyHostToDevice));
-        DG_CUDA(cudaMemcpy(d_d.p, d + 3 * b, 3 * c * sizeof(double), cudaMemcpyHostToDevice));
-        DG_LAUNCH(k7_launch_raycast(f->dev, d_o.p, d_d.p, c, iso, t_min, t_max, d_lo.p, d_hi.p, d_st.p, nullptr));
-        DG_CUDA(cudaMemcpy(t_lo + b, d_lo.p, c * sizeof(double), cudaMemcpyDeviceToHost));
-        DG_CUDA(cudaMemcpy(t_hi + b, d_hi.p, c * sizeof(double), cudaMemcpyDeviceToHost));
-        DG_CUDA(cudaMemcpy(status + b, d_st.p, c * sizeof(int32_t), cudaMemcpyDeviceToHost));
-    }
-    return DG_OK;
-}
-
+// host arrays: chunks of 2^20 rays (64 MiB of device buffers)
 int dg_field_raycast(const dg_field* f, const double* o, const double* d, uint64_t n, double iso, double t_min, double t_max, double* t_lo,
                      double* t_hi, int32_t* status)
 {
-    return guarded("dg_field_raycast", [&]() { return raycast_host_impl(f, o, d, n, iso, t_min, t_max, t_lo, t_hi, status); });
+    static const char* who = "dg_field_raycast";
+    return guarded(who, [&]() -> int {
+        if (int rc = raycast_check(f, o, d, n, iso, t_min, t_max, t_lo, t_hi, status, who)) return rc;
+        if (n == 0) return DG_OK;
+        return stage_on_device(n, std::min<uint64_t>(n, 1ull << 20), {{o, 3 * sizeof(double)}, {d, 3 * sizeof(double)}},
+                               {{t_lo, sizeof(double)}, {t_hi, sizeof(double)}, {status, sizeof(int32_t)}},
+                               [&](void* const* in, void* const* out, uint64_t, uint64_t c) -> int {
+                                   DG_LAUNCH(k7_launch_raycast(f->dev, (const double*)in[0], (const double*)in[1], c, iso, t_min, t_max, (double*)out[0],
+                                                               (double*)out[1], (int32_t*)out[2], nullptr));
+                                   return DG_OK;
+                               });
+    });
 }
 
 // ------------------------------------------------------------------------------------------------ K9: ray casts on a mesh
 static int mesh_raycast_check(const dg_mesh* m, const void* o, const void* d, uint64_t n, double t_min, double t_max, const void* t,
                               const void* id, const void* status, const char* who)
 {
-    if (!m) return fail(DG_ERR_INVALID, "%s: mesh is NULL (not constructed)", who);
     if (int rc = mesh_usable(m, who)) return rc;
     if (n && (!o || !d || !t || !id || !status)) return fail(DG_ERR_INVALID, "%s: origins / directions / t / triangle_id / status is NULL", who);
     if (std::isnan(t_min) || std::isnan(t_max)) return fail(DG_ERR_INVALID, "%s: t_min and t_max must not be NaN", who);
@@ -2714,53 +2792,39 @@ static int mesh_raycast_check(const dg_mesh* m, const void* o, const void* d, ui
     return check_handle_device(m->device, who);
 }
 
+static int mesh_raycast_launch(const dg_mesh* m, const double* d_o, const double* d_d, uint64_t n, double t_min, double t_max, double* d_t,
+                               int32_t* d_id, double* d_bary, int32_t* d_status, cudaStream_t st, const char* who)
+{
+    const WindDev* wd = nullptr;
+    if (int rc = winding_dev(m, wd, who)) return rc;
+    DG_LAUNCH(k9_launch_mesh_raycast(m->dev, *wd, d_o, d_d, n, t_min, t_max, d_t, d_id, d_bary, d_status, st));
+    return DG_OK;
+}
+
 int dg_mesh_raycast_device(const dg_mesh* m, const double* d_o, const double* d_d, uint64_t n, double t_min, double t_max, double* d_t,
                            int32_t* d_id, double* d_bary, int32_t* d_status, void* stream)
 {
     static const char* who = "dg_mesh_raycast_device";
     if (int rc = mesh_raycast_check(m, d_o, d_d, n, t_min, t_max, d_t, d_id, d_status, who)) return rc;
     if (n == 0) return DG_OK;
-    const WindDev* wd = nullptr;
-    if (int rc = winding_dev(m, wd, who)) return rc;
-    DG_LAUNCH(k9_launch_mesh_raycast(m->dev, *wd, d_o, d_d, n, t_min, t_max, d_t, d_id, d_bary, d_status, (cudaStream_t)stream));
-    return DG_OK;
+    return mesh_raycast_launch(m, d_o, d_d, n, t_min, t_max, d_t, d_id, d_bary, d_status, (cudaStream_t)stream, who);
 }
 
-// host arrays: chunks of 2^20 rays uploaded, cast and downloaded in turn on the legacy default stream
-static int mesh_raycast_host_impl(const dg_mesh* m, const double* o, const double* d, uint64_t n, double t_min, double t_max, double* t,
-                                  int32_t* id, double* bary, int32_t* status)
-{
-    static const char* who = "dg_mesh_raycast";
-    if (int rc = mesh_raycast_check(m, o, d, n, t_min, t_max, t, id, status, who)) return rc;
-    if (n == 0) return DG_OK;
-    const WindDev* wd = nullptr;
-    if (int rc = winding_dev(m, wd, who)) return rc;
-    const uint64_t chunk = std::min<uint64_t>(n, 1ull << 20);
-    DevBuf<double> d_o, d_d, d_t, d_b;
-    DevBuf<int32_t> d_id, d_st;
-    DG_CUDA(d_o.alloc(3 * chunk));
-    DG_CUDA(d_d.alloc(3 * chunk));
-    DG_CUDA(d_t.alloc(chunk));
-    DG_CUDA(d_id.alloc(chunk));
-    DG_CUDA(d_st.alloc(chunk));
-    if (bary) DG_CUDA(d_b.alloc(3 * chunk));
-    for (uint64_t b = 0; b < n; b += chunk) {
-        const uint64_t c = std::min(chunk, n - b);
-        DG_CUDA(cudaMemcpy(d_o.p, o + 3 * b, 3 * c * sizeof(double), cudaMemcpyHostToDevice));
-        DG_CUDA(cudaMemcpy(d_d.p, d + 3 * b, 3 * c * sizeof(double), cudaMemcpyHostToDevice));
-        DG_LAUNCH(k9_launch_mesh_raycast(m->dev, *wd, d_o.p, d_d.p, c, t_min, t_max, d_t.p, d_id.p, bary ? d_b.p : nullptr, d_st.p, nullptr));
-        DG_CUDA(cudaMemcpy(t + b, d_t.p, c * sizeof(double), cudaMemcpyDeviceToHost));
-        DG_CUDA(cudaMemcpy(id + b, d_id.p, c * sizeof(int32_t), cudaMemcpyDeviceToHost));
-        DG_CUDA(cudaMemcpy(status + b, d_st.p, c * sizeof(int32_t), cudaMemcpyDeviceToHost));
-        if (bary) DG_CUDA(cudaMemcpy(bary + 3 * b, d_b.p, 3 * c * sizeof(double), cudaMemcpyDeviceToHost));
-    }
-    return DG_OK;
-}
-
+// host arrays: chunks of 2^20 rays
 int dg_mesh_raycast(const dg_mesh* m, const double* o, const double* d, uint64_t n, double t_min, double t_max, double* t, int32_t* id,
                     double* bary, int32_t* status)
 {
-    return guarded("dg_mesh_raycast", [&]() { return mesh_raycast_host_impl(m, o, d, n, t_min, t_max, t, id, bary, status); });
+    static const char* who = "dg_mesh_raycast";
+    return guarded(who, [&]() -> int {
+        if (int rc = mesh_raycast_check(m, o, d, n, t_min, t_max, t, id, status, who)) return rc;
+        if (n == 0) return DG_OK;
+        return stage_on_device(n, std::min<uint64_t>(n, 1ull << 20), {{o, 3 * sizeof(double)}, {d, 3 * sizeof(double)}},
+                               {{t, sizeof(double)}, {id, sizeof(int32_t)}, {status, sizeof(int32_t)}, {bary, 3 * sizeof(double)}},
+                               [&](void* const* in, void* const* out, uint64_t, uint64_t c) {
+                                   return mesh_raycast_launch(m, (const double*)in[0], (const double*)in[1], c, t_min, t_max, (double*)out[0],
+                                                              (int32_t*)out[1], (double*)out[3], (int32_t*)out[2], nullptr, who);
+                               });
+    });
 }
 
 int dg_obj_read(const char* path, double** vertices, uint64_t* n_vertices, uint32_t** triangles, uint64_t* n_triangles)
@@ -2781,106 +2845,6 @@ int dg_obj_read(const char* path, double** vertices, uint64_t* n_vertices, uint3
 void dg_obj_free(double* vertices, uint32_t* triangles)
 {
     std::free(vertices); std::free(triangles);
-}
-
-
-// ---- entry points whose bodies use host containers / threads: exceptions are turned into status codes
-int dg_add_function_sdf(const dg_mesh* m, const dg_grid_desc* grid, double sign, double* nodes_host, uint32_t* cells_host, uint32_t* cell_map_host,
-                        double* timings_ms)
-{
-    return guarded("dg_add_function_sdf", [&]() { return dg_add_function_sdf_impl(m, grid, sign, nodes_host, cells_host, cell_map_host, timings_ms); });
-}
-
-// addFunction(func, verbose, pred) with pred(x) = |md.signed_distance(x).distance| <= band (cubic_lagrange_discrete_grid.cpp:780-899, node
-// loop :806-817): the same pipeline as dg_add_function_sdf, every kernel chunk in its narrow-band form
-int dg_add_function_sdf_band(const dg_mesh* m, const dg_grid_desc* grid, double sign, double band, double* nodes_host, uint32_t* cells_host,
-                             uint32_t* cell_map_host, double* timings_ms)
-{
-    return guarded("dg_add_function_sdf_band", [&]() { return dg_add_function_sdf_impl(m, grid, sign, nodes_host, cells_host, cell_map_host, timings_ms, &band); });
-}
-
-int dg_add_function_sdf_multi(dg_mesh_group* grp, const dg_grid_desc* grid, double sign, double* nodes_host, uint32_t* cells_host,
-                              uint32_t* cell_map_host, double* timings_ms)
-{
-    return guarded("dg_add_function_sdf_multi", [&]() { return dg_add_function_sdf_multi_impl(grp, grid, sign, nodes_host, cells_host, cell_map_host, timings_ms); });
-}
-
-int dg_interpolate_batch(const dg_field* f, const double* x, uint64_t n, double* phi, double* grad)
-{
-    return guarded("dg_interpolate_batch", [&]() { return dg_interpolate_batch_impl(f, x, n, phi, grad); });
-}
-
-int dg_interpolate_hessian_batch(const dg_field* f, const double* x, uint64_t n, double* phi, double* grad, double* hess)
-{
-    if (n && (!phi || !grad || !hess)) return fail(DG_ERR_INVALID, "dg_interpolate_hessian_batch: phi / grad / hess is NULL");
-    return guarded("dg_interpolate_hessian_batch", [&]() { return dg_interpolate_batch_impl(f, x, n, phi, grad, hess); });
-}
-
-int dg_reduce_field(const dg_grid_desc* grid, double* nodes, uint64_t n_nodes, const uint8_t* keep_node, uint32_t* cells, uint64_t n_cells_in,
-                    uint32_t* cell_map, uint32_t flags, uint64_t* n_nodes_out, uint64_t* n_cells_out, double* timings_ms)
-{
-    return guarded("dg_reduce_field", [&]() { return dg_reduce_field_impl(grid, nodes, n_nodes, keep_node, cells, n_cells_in, cell_map, flags, n_nodes_out, n_cells_out, timings_ms); });
-}
-
-int dg_reduced_band_create(const dg_mesh* m, const dg_grid_desc* grid, double sign, double band, uint32_t flags, dg_reduced_band** out, double* timings_ms)
-{
-    return guarded("dg_reduced_band_create", [&]() { return reduced_band_create_impl(m, grid, sign, band, flags, out, timings_ms); });
-}
-
-int dg_reduced_density_map_create(const dg_grid_desc* grid, const double* sdf_nodes, uint64_t n_nodes, const uint32_t* sdf_cells, uint64_t n_cells,
-                                  const uint32_t* sdf_cell_map, double h, double rho0, uint32_t flags, dg_reduced_band** sdf_out,
-                                  dg_reduced_band** density_out, double* timings_ms)
-{
-    // GenerateDensityMap's second predicate, 0 <= v && v <= 3 rho0 (main.cpp:140)
-    const ReducedNodeMap m{"dg_reduced_density_map_create",
-                           [](double h_, double) -> const char* { return (h_ > 0.0) ? nullptr : "smoothing length must be > 0"; },
-                           [](const dg_field& f, double h_, double rho0_, uint64_t n, double* d_out, cudaStream_t st) {
-                               return k3_launch_density(f.dev, f.coeff_max, h_, rho0_, 0, 0, n, d_out, st);
-                           },
-                           K4ValuePred{K4_KEEP_RANGE, 0.0, 3.0 * rho0, 0.0}};
-    return guarded("dg_reduced_density_map_create", [&]() {
-        return reduced_node_map_create_impl(m, grid, sdf_nodes, n_nodes, sdf_cells, n_cells, sdf_cell_map, h, rho0, flags, sdf_out, density_out, timings_ms);
-    });
-}
-
-int dg_reduced_volume_map_create(const dg_grid_desc* grid, const double* sdf_nodes, uint64_t n_nodes, const uint32_t* sdf_cells, uint64_t n_cells,
-                                 const uint32_t* sdf_cell_map, double h, double scale, uint32_t flags, dg_reduced_band** sdf_out,
-                                 dg_reduced_band** volume_out, double* timings_ms)
-{
-    // the volume field keeps 0 <= v (and != DBL_MAX, as every reduceField): K4_KEEP_RANGE with b = +inf
-    const ReducedNodeMap m{"dg_reduced_volume_map_create", volume_args_invalid,
-                           [](const dg_field& f, double h_, double scale_, uint64_t n, double* d_out, cudaStream_t st) {
-                               return k3_launch_volume(f.dev, h_, scale_, 0, 0, n, d_out, st);
-                           },
-                           K4ValuePred{K4_KEEP_RANGE, 0.0, INFINITY, 0.0}};
-    return guarded("dg_reduced_volume_map_create", [&]() {
-        return reduced_node_map_create_impl(m, grid, sdf_nodes, n_nodes, sdf_cells, n_cells, sdf_cell_map, h, scale, flags, sdf_out, volume_out, timings_ms);
-    });
-}
-
-int dg_add_function_device(const dg_grid_desc* grid, dg_device_function func, void* fu, dg_device_sample_predicate pred, void* pu, uint64_t chunk_nodes,
-                           double* nodes_host, uint32_t* cells_host, uint32_t* cell_map_host, double* timings_ms)
-{
-    return guarded("dg_add_function_device", [&]() {
-        return add_function_device_impl(grid, func, fu, pred, pu, chunk_nodes, nodes_host, cells_host, cell_map_host, timings_ms);
-    });
-}
-
-int dg_reduced_function_create(const dg_grid_desc* grid, dg_device_function func, void* fu, dg_device_sample_predicate sample_pred, void* su,
-                               dg_device_node_predicate reduce_pred, void* ru, uint64_t chunk_nodes, uint32_t flags, dg_reduced_band** out,
-                               double* timings_ms)
-{
-    return guarded("dg_reduced_function_create", [&]() {
-        return reduced_function_create_impl(grid, func, fu, sample_pred, su, reduce_pred, ru, chunk_nodes, flags, out, timings_ms);
-    });
-}
-
-int dg_reduce_field_device(const dg_grid_desc* grid, const double* nodes, uint64_t n_nodes, const uint32_t* cells, uint64_t n_cells,
-                           dg_device_node_predicate pred, void* pu, uint64_t chunk_nodes, uint32_t flags, dg_reduced_band** out, double* timings_ms)
-{
-    return guarded("dg_reduce_field_device", [&]() {
-        return reduce_field_device_impl(grid, nodes, n_nodes, cells, n_cells, pred, pu, chunk_nodes, flags, out, timings_ms);
-    });
 }
 
 }  // extern "C"
