@@ -148,6 +148,27 @@ public:
         if (dg_mesh_raycast_device(m_mesh, d_origins, d_directions, n, t_min, t_max, d_t, d_triangle_id, d_barycentric, d_status, stream) != DG_OK)
             throw std::runtime_error(std::string("TriangleMeshDistance: ") + dg_last_error());
     }
+    // new: the distance query on n points in the mesh's device memory with the barycentric weights (3 per point) of the nearest point on
+    // its triangle's vertices; every output may be NULL; asynchronous on `stream` (dg_mesh_distance_bary_device; contract in
+    // k10_distance_grad.cu).  Follows setSignMode when is_signed.
+    void nearest(size_t n, const double* d_points, bool is_signed, double* d_distance, double* d_nearest_point, int32_t* d_nearest_entity,
+                 int32_t* d_triangle_id, double* d_barycentric, void* stream) const
+    {
+        require();
+        if (dg_mesh_distance_bary_device(m_mesh, d_points, n, is_signed ? 1 : 0, d_distance, d_nearest_point, d_nearest_entity, d_triangle_id,
+                                         d_barycentric, stream) != DG_OK)
+            throw std::runtime_error(std::string("TriangleMeshDistance: ") + dg_last_error());
+    }
+    // new: the gradients of sum(grad_distance * distance) for the outputs of nearest(): d_grad_points (n x 3) and d_grad_vertices
+    // (n_vertices x 3, overwritten, summed in a fixed order), each may be NULL; on `stream` (dg_mesh_distance_vjp_device)
+    void distance_vjp(size_t n, const double* d_points, const double* d_distance, const double* d_nearest_point, const int32_t* d_triangle_id,
+                      const double* d_barycentric, const double* d_grad_distance, double* d_grad_points, double* d_grad_vertices, void* stream) const
+    {
+        require();
+        if (dg_mesh_distance_vjp_device(m_mesh, n, d_points, d_distance, d_nearest_point, d_triangle_id, d_barycentric, d_grad_distance,
+                                        d_grad_points, d_grad_vertices, stream) != DG_OK)
+            throw std::runtime_error(std::string("TriangleMeshDistance: ") + dg_last_error());
+    }
 
 private:
     dg_mesh* m_mesh = nullptr;

@@ -7,11 +7,11 @@ discregrid_b200/lib/libdiscregrid_b200.so and fails if it has not been built; th
 from . import _capi
 from ._capi import DiscregridError, DBL_MAX, LIB_PATH
 from .mesh import TriangleMesh, bumpy_torus, uv_sphere, box
-from .distance import TriangleMeshDistance, MeshSignedDistance, MeshDistanceBand, NearestEntity, Result
+from .distance import TriangleMeshDistance, MeshSignedDistance, MeshDistanceBand, NearestEntity, NearestResult, Result
 from .grid import (CubicLagrangeDiscreteGrid, DensityMapFunction, VolumeMapFunction, DeviceFunction, DeviceNodePredicate, DeviceSamplePredicate, grid_desc,
                    generate_sdf_domain)
 
-__all__ = ["TriangleMesh", "TriangleMeshDistance", "MeshSignedDistance", "MeshDistanceBand", "NearestEntity", "Result",
+__all__ = ["TriangleMesh", "TriangleMeshDistance", "MeshSignedDistance", "MeshDistanceBand", "NearestEntity", "NearestResult", "Result",
            "CubicLagrangeDiscreteGrid", "DensityMapFunction", "VolumeMapFunction", "DeviceFunction", "DeviceSamplePredicate", "DeviceNodePredicate", "grid_desc",
            "generate_sdf_domain", "DiscregridError",
            "DBL_MAX", "LIB_PATH", "bumpy_torus", "uv_sphere", "box"]

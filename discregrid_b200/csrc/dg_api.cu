@@ -46,6 +46,7 @@
 #include "k7_raycast.h"
 #include "k8_refit.h"
 #include "k9_mesh_raycast.h"
+#include "k10_distance_grad.h"
 #include "reduce_field.h"
 #include "obj_reader.h"
 
@@ -189,7 +190,7 @@ struct HostOut { void* p; size_t bytes; };
 template <class Launch>
 int stage_on_device(uint64_t n, uint64_t chunk, std::initializer_list<HostIn> in, std::initializer_list<HostOut> out, Launch&& launch)
 {
-    constexpr size_t kMax = 4;
+    constexpr size_t kMax = 5;
     assert(in.size() <= kMax && out.size() <= kMax);
     const HostIn* ins = in.begin();
     const HostOut* outs = out.begin();
@@ -239,7 +240,10 @@ struct dg_mesh {
     // dg_mesh_refit (k8_refit.cu): topology tables and scratch, allocated at the first refit and kept
     std::atomic<int> borrows{0};            // live dg_mesh_group's whose replicas copy this mesh's records
     bool failed = false;                    // a refit stopped after it had started to write records
-    bool refit_ready = false;               // the tables below are allocated and uploaded
+    bool refit_ready = false;               // the refit's scratch below is allocated
+    // the topology tables (d_F, d_f_leaf, d_order, d_inc_begin, d_inc, d_nodes, refit_levels): built at the first refit or distance gradient
+    mutable std::mutex topo_mu;
+    bool topo_ready = false;
     bool refit_done = false;                // the records are those of a refit: d_V holds the positions, host V and pseudonormals are stale
     std::vector<uint32_t> refit_levels;     // RefitTopoHost::level_begin
     DevBuf<double> d_V;                     // [nV][3] the positions of the last refit
@@ -472,7 +476,7 @@ int dg_mesh_info(const dg_mesh* m, uint64_t info[8])
     info[0] = m->host.n_vertices; info[1] = m->host.n_triangles; info[2] = (uint64_t)m->dev.stack_depth;
     info[3] = (uint64_t)m->host.flags;
     info[4] = m->d_spheres.bytes() + m->d_leaves.bytes() + m->d_normals.bytes() + m->d_nodes_f.bytes() + m->d_leaves_f.bytes();
-    info[4] += m->refit_bytes();                                            // 0 until the first dg_mesh_refit
+    info[4] += m->refit_bytes();                                            // 0 until the first dg_mesh_refit or vertex gradient
     {
         std::lock_guard<std::mutex> lock(m->wind_mu);
         info[4] += m->d_wind_leaves.bytes() + m->d_wind_clusters.bytes();      // 0 until the winding records are first used
@@ -603,19 +607,17 @@ int dg_mesh_set_sign_mode(dg_mesh* m, int mode, double beta)
     return DG_OK;
 }
 
-// topology tables (from F and the leaf order, once) and every scratch buffer: all allocated before any record is written
-static int refit_prepare(dg_mesh* m)
+// topology tables (from F and the leaf order, once): K8's refit and K10's vertex gradient share them, whichever runs first builds them
+static int topo_prepare(dg_mesh* m)
 {
-    if (m->refit_ready) return DG_OK;
+    std::lock_guard<std::mutex> lock(m->topo_mu);
+    if (m->topo_ready) return DG_OK;
     const uint64_t nT = m->host.n_triangles, nV = m->host.n_vertices;
     RefitTopoHost topo;
     k8_build_topology(m->host, topo);
-    DG_CUDA(m->d_V.alloc(3 * nV));
     DG_CUDA(m->d_F.alloc(3 * nT)); DG_CUDA(m->d_f_leaf.alloc(3 * nT)); DG_CUDA(m->d_order.alloc(nT));
     DG_CUDA(m->d_inc_begin.alloc(nV + 1)); DG_CUDA(m->d_inc.alloc(3 * nT));
     DG_CUDA(m->d_nodes.alloc(topo.nodes.size()));
-    DG_CUDA(m->d_sums.alloc(nT)); DG_CUDA(m->d_part.alloc(k8_bounds_entries(nV))); DG_CUDA(m->d_bounds.alloc(5));
-    DG_CUDA(m->d_pn_tri.alloc(3 * nT)); DG_CUDA(m->d_angle.alloc(3 * nT)); DG_CUDA(m->d_pn_vert.alloc(3 * nV)); DG_CUDA(m->d_pn_edge.alloc(9 * nT));
     DG_CUDA(cudaMemcpy(m->d_F.p, m->host.F.data(), 3 * nT * sizeof(uint32_t), cudaMemcpyHostToDevice));
     DG_CUDA(cudaMemcpy(m->d_f_leaf.p, topo.f_leaf.data(), 3 * nT * sizeof(uint32_t), cudaMemcpyHostToDevice));
     DG_CUDA(cudaMemcpy(m->d_order.p, m->host.order.data(), nT * sizeof(int32_t), cudaMemcpyHostToDevice));
@@ -623,6 +625,19 @@ static int refit_prepare(dg_mesh* m)
     DG_CUDA(cudaMemcpy(m->d_inc.p, topo.inc.data(), 3 * nT * sizeof(uint32_t), cudaMemcpyHostToDevice));
     if (!topo.nodes.empty()) DG_CUDA(cudaMemcpy(m->d_nodes.p, topo.nodes.data(), topo.nodes.size() * sizeof(RefitNodeRef), cudaMemcpyHostToDevice));
     m->refit_levels = topo.level_begin;
+    m->topo_ready = true;
+    return DG_OK;
+}
+
+// the topology tables and every scratch buffer of the refit: all allocated before any record is written
+static int refit_prepare(dg_mesh* m)
+{
+    if (m->refit_ready) return DG_OK;
+    if (int rc = topo_prepare(m)) return rc;
+    const uint64_t nT = m->host.n_triangles, nV = m->host.n_vertices;
+    DG_CUDA(m->d_V.alloc(3 * nV));
+    DG_CUDA(m->d_sums.alloc(nT)); DG_CUDA(m->d_part.alloc(k8_bounds_entries(nV))); DG_CUDA(m->d_bounds.alloc(5));
+    DG_CUDA(m->d_pn_tri.alloc(3 * nT)); DG_CUDA(m->d_angle.alloc(3 * nT)); DG_CUDA(m->d_pn_vert.alloc(3 * nV)); DG_CUDA(m->d_pn_edge.alloc(9 * nT));
     m->refit_ready = true;
     return DG_OK;
 }
@@ -738,17 +753,17 @@ static int distance_check(const dg_mesh* m, const void* pts, uint64_t n, const c
     return DG_OK;
 }
 
+// d_bary non-NULL: K1's kernel that also writes the weights (mesh_distance_bary_kernel), otherwise mesh_distance_kernel
 static int distance_launch(const dg_mesh* m, const double* d_pts, uint64_t n, int is_signed, double* d_dist, double* d_near, int32_t* d_ent,
-                           int32_t* d_tri, cudaStream_t st, const char* who)
+                           int32_t* d_tri, double* d_bary, cudaStream_t st, const char* who)
 {
-    if (is_signed && m->sign_mode == DG_SIGN_WINDING) {       // the unsigned query, then the sign from w (k5_winding.cu)
-        const WindDev* wd = nullptr;
-        if (int rc = winding_dev(m, wd, who)) return rc;
-        DG_LAUNCH(k1_launch_distance(m->dev, d_pts, n, 0, d_dist, d_near, d_ent, d_tri, st));
-        if (d_dist) DG_LAUNCH(k5_launch_sign_points(*wd, d_pts, n, m->beta, d_dist, st));
-        return DG_OK;
-    }
-    DG_LAUNCH(k1_launch_distance(m->dev, d_pts, n, is_signed, d_dist, d_near, d_ent, d_tri, st));
+    const bool winding = is_signed && m->sign_mode == DG_SIGN_WINDING;     // the unsigned query, then the sign from w (k5_winding.cu)
+    const WindDev* wd = nullptr;
+    if (winding) { if (int rc = winding_dev(m, wd, who)) return rc; }
+    const int k1_signed = winding ? 0 : is_signed;
+    if (d_bary) DG_LAUNCH(k1_launch_distance_bary(m->dev, d_pts, n, k1_signed, d_dist, d_near, d_ent, d_tri, d_bary, st));
+    else DG_LAUNCH(k1_launch_distance(m->dev, d_pts, n, k1_signed, d_dist, d_near, d_ent, d_tri, st));
+    if (winding && d_dist) DG_LAUNCH(k5_launch_sign_points(*wd, d_pts, n, m->beta, d_dist, st));
     return DG_OK;
 }
 
@@ -758,7 +773,7 @@ int dg_mesh_distance_device(const dg_mesh* m, const double* d_pts, uint64_t n, i
     static const char* who = "dg_mesh_distance_device";
     if (int rc = distance_check(m, d_pts, n, who)) return rc;
     if (int rc = check_handle_device(m->device, who)) return rc;
-    return distance_launch(m, d_pts, n, is_signed, d_dist, d_near, d_ent, d_tri, (cudaStream_t)stream, who);
+    return distance_launch(m, d_pts, n, is_signed, d_dist, d_near, d_ent, d_tri, nullptr, (cudaStream_t)stream, who);
 }
 
 int dg_mesh_distance(const dg_mesh* m, const double* pts, uint64_t n, int is_signed, double* dist, double* nearp, int32_t* ent,
@@ -772,8 +787,121 @@ int dg_mesh_distance(const dg_mesh* m, const double* pts, uint64_t n, int is_sig
                            {{dist, sizeof(double)}, {nearp, 3 * sizeof(double)}, {ent, sizeof(int32_t)}, {tri, sizeof(int32_t)}},
                            [&](void* const* in, void* const* out, uint64_t, uint64_t c) {
                                return distance_launch(m, (const double*)in[0], c, is_signed, (double*)out[0], (double*)out[1], (int32_t*)out[2],
-                                                      (int32_t*)out[3], nullptr, who);
+                                                      (int32_t*)out[3], nullptr, nullptr, who);
                            });
+}
+
+// ------------------------------------------------------------------------------------------------ K10: the distance with weights, its gradient
+int dg_mesh_distance_bary_device(const dg_mesh* m, const double* d_pts, uint64_t n, int is_signed, double* d_dist, double* d_near,
+                                 int32_t* d_ent, int32_t* d_tri, double* d_bary, void* stream)
+{
+    static const char* who = "dg_mesh_distance_bary_device";
+    if (int rc = distance_check(m, d_pts, n, who)) return rc;
+    if (int rc = check_handle_device(m->device, who)) return rc;
+    if (n == 0) return DG_OK;
+    return distance_launch(m, d_pts, n, is_signed, d_dist, d_near, d_ent, d_tri, d_bary, (cudaStream_t)stream, who);
+}
+
+int dg_mesh_distance_bary(const dg_mesh* m, const double* pts, uint64_t n, int is_signed, double* dist, double* nearp, int32_t* ent,
+                          int32_t* tri, double* bary)
+{
+    static const char* who = "dg_mesh_distance_bary";
+    if (int rc = distance_check(m, pts, n, who)) return rc;
+    if (n == 0) return DG_OK;
+    if (int rc = check_handle_device(m->device, who)) return rc;
+    return stage_on_device(n, n, {{pts, 3 * sizeof(double)}},
+                           {{dist, sizeof(double)}, {nearp, 3 * sizeof(double)}, {ent, sizeof(int32_t)}, {tri, sizeof(int32_t)},
+                            {bary, 3 * sizeof(double)}},
+                           [&](void* const* in, void* const* out, uint64_t, uint64_t c) {
+                               return distance_launch(m, (const double*)in[0], c, is_signed, (double*)out[0], (double*)out[1], (int32_t*)out[2],
+                                                      (int32_t*)out[3], (double*)out[4], nullptr, who);
+                           });
+}
+
+static int vjp_check(const dg_mesh* m, uint64_t n, const void* x, const void* d, const void* p, const void* t, const void* w, const void* g,
+                     const char* who)
+{
+    if (int rc = mesh_usable(m, who)) return rc;
+    if (n && (!x || !d || !p || !t || !w || !g))
+        return fail(DG_ERR_INVALID, "%s: points / distance / nearest_point / triangle_id / barycentric / grad_distance is NULL", who);
+    if (n >= (1ull << 32) - 1) return fail(DG_ERR_INVALID, "%s: %llu queries; at most 2^32 - 2 per call", who, (unsigned long long)n);
+    return DG_OK;
+}
+
+// the triangle ids are checked on the device first (one synchronise); nothing is written unless they are all in [-1, T)
+static int vjp_launch(const dg_mesh* m, uint64_t n, const double* d_x, const double* d_d, const double* d_p, const int32_t* d_t,
+                      const double* d_w, const double* d_g, double* d_gp, double* d_gv, cudaStream_t st, const char* who)
+{
+    const uint64_t nT = m->host.n_triangles, nV = m->host.n_vertices;
+    if (n) {
+        DevBuf<unsigned> bad;
+        DG_CUDA(bad.alloc(1));
+        DG_LAUNCH(k10_launch_check(d_t, n, (int)nT, bad.p, st));
+        unsigned h_bad = 0;
+        DG_CUDA(cudaMemcpyAsync(&h_bad, bad.p, sizeof h_bad, cudaMemcpyDeviceToHost, st));
+        DG_CUDA(cudaStreamSynchronize(st));
+        if (h_bad) return fail(DG_ERR_INVALID, "%s: %u triangle ids outside [-1, %llu)", who, h_bad, (unsigned long long)nT);
+    }
+    if (n && d_gv) { if (int rc = topo_prepare(const_cast<dg_mesh*>(m))) return rc; }
+    K10Topo topo;
+    topo.F = m->d_F.p; topo.inc_begin = m->d_inc_begin.p; topo.inc = m->d_inc.p; topo.n_vertices = nV; topo.n_tri = (int)nT;
+    K10Query q;
+    q.x = d_x; q.dist = d_d; q.near = d_p; q.tri = d_t; q.bary = d_w; q.g = d_g; q.n = n;
+    const size_t bytes = k10_scratch_bytes(n, (int)nT, d_gp != nullptr, d_gv != nullptr);
+    void* scratch = nullptr;
+#ifdef DG_EMU
+    if (bytes) DG_CUDA(cudaMalloc(&scratch, bytes));
+    const cudaError_t e = k10_launch_vjp(topo, q, d_gp, d_gv, scratch, st);
+    if (scratch) cudaFree(scratch);
+#else
+    if (bytes) DG_CUDA(cudaMallocAsync(&scratch, bytes, st));
+    const cudaError_t e = k10_launch_vjp(topo, q, d_gp, d_gv, scratch, st);
+    if (scratch) cudaFreeAsync(scratch, st);
+#endif
+    DG_LAUNCH(e);
+    return DG_OK;
+}
+
+int dg_mesh_distance_vjp_device(const dg_mesh* m, uint64_t n, const double* d_points, const double* d_distance, const double* d_nearest_point,
+                                const int32_t* d_triangle_id, const double* d_barycentric, const double* d_grad_distance, double* d_grad_points,
+                                double* d_grad_vertices, void* stream)
+{
+    static const char* who = "dg_mesh_distance_vjp_device";
+    if (int rc = vjp_check(m, n, d_points, d_distance, d_nearest_point, d_triangle_id, d_barycentric, d_grad_distance, who)) return rc;
+    if (int rc = check_handle_device(m->device, who)) return rc;
+    if (!d_grad_points && !d_grad_vertices) return DG_OK;
+    return vjp_launch(m, n, d_points, d_distance, d_nearest_point, d_triangle_id, d_barycentric, d_grad_distance, d_grad_points, d_grad_vertices,
+                      (cudaStream_t)stream, who);
+}
+
+// host arrays: every input uploaded in one piece (the vertex sums span all queries), then the device form on the legacy default stream
+int dg_mesh_distance_vjp(const dg_mesh* m, uint64_t n, const double* points, const double* distance, const double* nearest_point,
+                         const int32_t* triangle_id, const double* barycentric, const double* grad_distance, double* grad_points,
+                         double* grad_vertices)
+{
+    static const char* who = "dg_mesh_distance_vjp";
+    if (int rc = vjp_check(m, n, points, distance, nearest_point, triangle_id, barycentric, grad_distance, who)) return rc;
+    if (!grad_points && !grad_vertices) return DG_OK;
+    if (int rc = check_handle_device(m->device, who)) return rc;
+    const uint64_t nV = m->host.n_vertices;
+    DevBuf<double> x, d, p, w, g, gp, gv;
+    DevBuf<int32_t> t;
+    DG_CUDA(x.alloc(3 * n)); DG_CUDA(d.alloc(n)); DG_CUDA(p.alloc(3 * n)); DG_CUDA(t.alloc(n)); DG_CUDA(w.alloc(3 * n)); DG_CUDA(g.alloc(n));
+    if (grad_points) DG_CUDA(gp.alloc(3 * n));
+    if (grad_vertices) DG_CUDA(gv.alloc(3 * nV));
+    if (n) {
+        DG_CUDA(cudaMemcpy(x.p, points, 3 * n * sizeof(double), cudaMemcpyHostToDevice));
+        DG_CUDA(cudaMemcpy(d.p, distance, n * sizeof(double), cudaMemcpyHostToDevice));
+        DG_CUDA(cudaMemcpy(p.p, nearest_point, 3 * n * sizeof(double), cudaMemcpyHostToDevice));
+        DG_CUDA(cudaMemcpy(t.p, triangle_id, n * sizeof(int32_t), cudaMemcpyHostToDevice));
+        DG_CUDA(cudaMemcpy(w.p, barycentric, 3 * n * sizeof(double), cudaMemcpyHostToDevice));
+        DG_CUDA(cudaMemcpy(g.p, grad_distance, n * sizeof(double), cudaMemcpyHostToDevice));
+    }
+    if (int rc = vjp_launch(m, n, x.p, d.p, p.p, t.p, w.p, g.p, gp.p, gv.p, nullptr, who)) return rc;
+    if (grad_points && n) DG_CUDA(cudaMemcpy(grad_points, gp.p, 3 * n * sizeof(double), cudaMemcpyDeviceToHost));
+    if (grad_vertices && nV) DG_CUDA(cudaMemcpy(grad_vertices, gv.p, 3 * nV * sizeof(double), cudaMemcpyDeviceToHost));
+    DG_CUDA(cudaDeviceSynchronize());
+    return DG_OK;
 }
 
 // ------------------------------------------------------------------------------------------------ K1

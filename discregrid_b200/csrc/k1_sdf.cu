@@ -1018,6 +1018,37 @@ mesh_distance_kernel(MeshDev mesh, const PseudoNormals* __restrict__ normals, in
     if (tri_out) tri_out[idx] = tri;
 }
 
+// mesh_distance_kernel that also writes the barycentric weights (fl(fl(1 - s) - t), s, t) of the nearest point (dg_mesh_distance_bary, K10's
+// forward; NaN when nothing was accepted).  A separate kernel rather than a flag, so that mesh_distance_kernel's code stays as it is; the
+// walk and finish_query are the same inlined functions, hence the same distance, nearest point, entity and triangle id.
+__global__ void __launch_bounds__(K1_THREADS, K1_MIN_BLOCKS)
+mesh_distance_bary_kernel(MeshDev mesh, const PseudoNormals* __restrict__ normals, int stack_depth,
+                          const double* __restrict__ pts, unsigned long long count, int is_signed,
+                          double* __restrict__ dist_out, double* __restrict__ near_out, int* __restrict__ ent_out,
+                          int* __restrict__ tri_out, double* __restrict__ bary_out)
+{
+    float* stack_d = reinterpret_cast<float*>(k1_smem);
+    unsigned* stack_rng = reinterpret_cast<unsigned*>(k1_smem + (size_t)stack_depth * K1_THREADS * sizeof(float));
+    const unsigned long long idx = (unsigned long long)blockIdx.x * K1_THREADS + threadIdx.x;
+    const bool alive = idx < count;
+    const unsigned long long ix = alive ? idx : 0ull;
+    const double px = pts[3 * ix], py = pts[3 * ix + 1], pz = pts[3 * ix + 2];
+    const QueryResult r = nearest_triangle(mesh, alive, px, py, pz, stack_rng + threadIdx.x, stack_d + threadIdx.x, K1_THREADS);
+    if (!alive) return;
+    double dist, qx, qy, qz; int tri;
+    finish_query(mesh.leaves, normals, r, px, py, pz, is_signed != 0, dist, qx, qy, qz, tri);
+    if (dist_out) dist_out[idx] = dist;
+    if (near_out) { near_out[3 * idx] = qx; near_out[3 * idx + 1] = qy; near_out[3 * idx + 2] = qz; }
+    if (ent_out) ent_out[idx] = r.entity;
+    if (tri_out) tri_out[idx] = tri;
+    if (bary_out) {
+        const double nan = __longlong_as_double(0x7ff8000000000000ll);
+        bary_out[3 * idx] = r.pos < 0 ? nan : (1.0 - r.s) - r.t;
+        bary_out[3 * idx + 1] = r.pos < 0 ? nan : r.s;
+        bary_out[3 * idx + 2] = r.pos < 0 ? nan : r.t;
+    }
+}
+
 
 __global__ void node_positions_kernel(GridDev g, unsigned l_begin, unsigned long long count, double* __restrict__ x)
 {
@@ -1093,6 +1124,8 @@ cudaError_t k1_configure(int stack_depth)
     e = cudaFuncSetAttribute(sdf_sample_nodes_band_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
     if (e != cudaSuccess) return e;
     e = cudaFuncSetAttribute(mesh_distance_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    if (e != cudaSuccess) return e;
+    e = cudaFuncSetAttribute(mesh_distance_bary_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
     if (e == cudaSuccess && dev >= 0 && dev < 64) configured[dev] = stack_depth;
     return e;
 #endif
@@ -1358,6 +1391,16 @@ cudaError_t k1_launch_distance(const DeviceBvh& m, const double* d_pts, uint64_t
     if (count == 0) return cudaSuccess;
     const unsigned blocks = (unsigned)((count + K1_THREADS - 1) / K1_THREADS);
     DG_KERNEL_LAUNCH(mesh_distance_kernel, blocks, K1_THREADS, k1_smem_bytes(m.stack_depth), stream, mesh_dev(m), m.normals, m.stack_depth, d_pts, (unsigned long long)count, is_signed, d_dist, d_near, d_ent, d_tri);
+    return DG_AFTER_LAUNCH();
+}
+
+cudaError_t k1_launch_distance_bary(const DeviceBvh& m, const double* d_pts, uint64_t count, int is_signed, double* d_dist,
+                                    double* d_near, int* d_ent, int* d_tri, double* d_bary, cudaStream_t stream)
+{
+    if (count == 0) return cudaSuccess;
+    const unsigned blocks = (unsigned)((count + K1_THREADS - 1) / K1_THREADS);
+    DG_KERNEL_LAUNCH(mesh_distance_bary_kernel, blocks, K1_THREADS, k1_smem_bytes(m.stack_depth), stream, mesh_dev(m), m.normals, m.stack_depth,
+                     d_pts, (unsigned long long)count, is_signed, d_dist, d_near, d_ent, d_tri, d_bary);
     return DG_AFTER_LAUNCH();
 }
 

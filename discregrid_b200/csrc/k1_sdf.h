@@ -113,6 +113,9 @@ void k1_interleaved_runs(const GridDev& g, const InterleavedLayout& L, unsigned 
 cudaError_t k1_launch_unpack_interleaved(const GridDev& g, const InterleavedLayout& L, const double* d_slots, double* d_nodes, cudaStream_t stream);
 cudaError_t k1_launch_distance(const DeviceBvh& m, const double* d_pts, uint64_t count, int is_signed, double* d_dist,
                                double* d_near, int* d_ent, int* d_tri, cudaStream_t stream);
+// the same query that also writes the weights d_bary[count][3] of the nearest point (K10's forward; mesh_distance_bary_kernel)
+cudaError_t k1_launch_distance_bary(const DeviceBvh& m, const double* d_pts, uint64_t count, int is_signed, double* d_dist,
+                                    double* d_near, int* d_ent, int* d_tri, double* d_bary, cudaStream_t stream);
 cudaError_t k1_launch_node_positions(const GridDev& g, uint64_t l_begin, uint64_t count, double* d_x, cudaStream_t stream);
 cudaError_t k1_launch_build_cells(const GridDev& g, uint64_t c_begin, uint64_t count, unsigned* d_cells, cudaStream_t stream);
 cudaError_t k1_launch_fp64_rate_probe(int blocks, int iters, double* d_out, cudaStream_t stream);

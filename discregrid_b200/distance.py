@@ -29,6 +29,47 @@ class NearestEntity(IntEnum):          # TriangleMeshDistance.h:75
 
 
 Result = namedtuple("Result", ["distance", "nearest_point", "nearest_entity", "triangle_id"])   # :80-86
+# Result with the barycentric weights (n, 3) of the nearest point on its triangle's vertices (beyond the reference)
+NearestResult = namedtuple("NearestResult", ["distance", "nearest_point", "nearest_entity", "triangle_id", "barycentric"])
+
+_MESH_DISTANCE = None
+
+
+def _mesh_distance_function():
+    """the autograd Function of the mesh distance on CUDA tensors (K10): distance(x, V) with d/dx = (x - p) / d and d/dV[F[t][i]] = -w_i d/dx,
+    first order only.  The backward reads the saved forward outputs and the mesh's triangles, never its vertex positions.  Made at first
+    use: torch is only imported by callers that pass tensors."""
+    global _MESH_DISTANCE
+    if _MESH_DISTANCE is None:
+        import torch
+        from torch.autograd.function import once_differentiable
+
+        class MeshDistance(torch.autograd.Function):
+            @staticmethod
+            def forward(ctx, x, V, md, signed):
+                r = md._nearest_device(x, signed)
+                ctx.mark_non_differentiable(r.nearest_point, r.nearest_entity, r.triangle_id, r.barycentric)
+                ctx.save_for_backward(x, r.distance, r.nearest_point, r.triangle_id, r.barycentric)
+                ctx.md = md
+                return tuple(r)
+
+            @staticmethod
+            @once_differentiable
+            def backward(ctx, grad_distance, *_unused):
+                x, dist, near, tri, bary = ctx.saved_tensors
+                md = ctx.md
+                n = len(x)
+                if grad_distance is None:
+                    grad_distance = torch.zeros(n, dtype=torch.float64, device=x.device)
+                g = grad_distance.to(torch.float64).contiguous()
+                gx = torch.empty((n, 3), dtype=torch.float64, device=x.device) if ctx.needs_input_grad[0] else None
+                gv = torch.empty((md.n_vertices, 3), dtype=torch.float64, device=x.device) if ctx.needs_input_grad[1] else None
+                capi.check(capi.lib.dg_mesh_distance_vjp_device(md.handle, n, x.data_ptr(), dist.data_ptr(), near.data_ptr(), tri.data_ptr(),
+                                                                bary.data_ptr(), g.data_ptr(), None if gx is None else gx.data_ptr(),
+                                                                None if gv is None else gv.data_ptr(), _device.stream(x)))
+                return gx, gv, None, None
+        _MESH_DISTANCE = MeshDistance
+    return _MESH_DISTANCE
 
 
 class TriangleMeshDistance:
@@ -199,8 +240,64 @@ class TriangleMeshDistance:
                                                     tri.data_ptr(), _device.stream(x)))
         return Result(dist, near, ent, tri)
 
-    def _query(self, points, signed):
+    def _nearest_device(self, x, signed):
+        """dg_mesh_distance_bary_device on torch's current stream; x a contiguous float64 (n, 3) tensor on the mesh's device"""
+        import torch
+        n = len(x)
+        dist = torch.empty(n, dtype=torch.float64, device=x.device)
+        near = torch.empty((n, 3), dtype=torch.float64, device=x.device)
+        ent = torch.empty(n, dtype=torch.int32, device=x.device)
+        tri = torch.empty(n, dtype=torch.int32, device=x.device)
+        bary = torch.empty((n, 3), dtype=torch.float64, device=x.device)
+        capi.check(capi.lib.dg_mesh_distance_bary_device(self.handle, x.data_ptr(), n, int(signed), dist.data_ptr(), near.data_ptr(),
+                                                         ent.data_ptr(), tri.data_ptr(), bary.data_ptr(), _device.stream(x)))
+        return NearestResult(dist, near, ent, tri, bary)
+
+    def nearest(self, points, signed=True):
+        """The query of signed_distance (signed=True) or unsigned_distance with the barycentric weights of the nearest point (beyond the
+        reference; dg_mesh_distance_bary): NearestResult(distance, nearest_point, nearest_entity, triangle_id, barycentric).  barycentric
+        (n, 3) weighs the vertices F[t][0], F[t][1], F[t][2] of the nearest triangle t, so that nearest_point is their weighted sum as the
+        query computes it: one-hot at a vertex, on the edge for an edge, NaN where no triangle was found (NaN points).  The other four fields
+        are bit for bit those of signed_distance / unsigned_distance.  numpy in, numpy out; a float64 CUDA tensor on the mesh's device
+        returns CUDA tensors, computed on torch's current stream.  No autograd (see signed_distance)."""
         if _device.is_device_query(points):
+            x = _device.points(points, self.device, "nearest")
+            return self._nearest_device(x.detach(), signed)
+        x = np.ascontiguousarray(points, dtype=np.float64).reshape(-1, 3)
+        n = len(x)
+        dist = np.empty(n); near = np.empty((n, 3)); ent = np.empty(n, np.int32); tri = np.empty(n, np.int32); bary = np.empty((n, 3))
+        capi.check(capi.lib.dg_mesh_distance_bary(self.handle, capi.ptr(x, capi.F64P), n, int(signed), capi.ptr(dist, capi.F64P),
+                                                  capi.ptr(near, capi.F64P), capi.ptr(ent, capi.I32P), capi.ptr(tri, capi.I32P),
+                                                  capi.ptr(bary, capi.F64P)))
+        return NearestResult(dist, near, ent, tri, bary)
+
+    def _differentiable(self, points, vertices, signed):
+        """the autograd route of a CUDA-tensor query: None when nothing asks for a gradient"""
+        import torch
+        if not torch.is_grad_enabled():
+            return None
+        if not (points.requires_grad or (vertices is not None and vertices.requires_grad)):
+            return None
+        x = _device.points(points, self.device, "signed_distance" if signed else "unsigned_distance")
+        dist, near, ent, tri, _bary = _mesh_distance_function().apply(x, vertices, self, signed)
+        return Result(dist, near, ent, tri)
+
+    def _refit_to(self, vertices, who):
+        import torch
+        if not _device.is_device_query(vertices):
+            raise TypeError(f"{who}: vertices must be a float64 CUDA tensor of shape (n_vertices, 3) (got {type(vertices).__name__})")
+        if vertices.dtype != torch.float64 or vertices.dim() != 2 or tuple(vertices.shape) != (self.n_vertices, 3):
+            raise ValueError(f"{who}: vertices must be a float64 tensor of shape ({self.n_vertices}, 3) (got {vertices.dtype}, "
+                             f"{tuple(vertices.shape)})")
+        self.refit(vertices.detach())
+
+    def _query(self, points, signed, vertices=None):
+        if vertices is not None:
+            self._refit_to(vertices, "signed_distance" if signed else "unsigned_distance")
+        if _device.is_device_query(points):
+            r = self._differentiable(points, vertices, signed)
+            if r is not None:
+                return r
             return self._query_device(points, signed)
         x = np.ascontiguousarray(points, dtype=np.float64).reshape(-1, 3)
         n = len(x)
@@ -209,16 +306,24 @@ class TriangleMeshDistance:
                                              capi.ptr(near, capi.F64P), capi.ptr(ent, capi.I32P), capi.ptr(tri, capi.I32P)))
         return Result(dist, near, ent, tri)
 
-    def signed_distance(self, points):      # :269-314
+    def signed_distance(self, points, vertices=None):      # :269-314
         """points: (n, 3) or (3,).  A numpy array (or anything numpy converts, CPU tensors included) goes through the host pipeline and
         returns numpy arrays.  A float64 torch tensor on the mesh's CUDA device stays there: the query runs on torch's current stream,
         asynchronously, and the Result holds CUDA tensors (distance float64 (n,), nearest_point float64 (n, 3), nearest_entity and
-        triangle_id int32 (n,)) with the same bits as the host route."""
-        return self._query(points, True)
+        triangle_id int32 (n,)) with the same bits as the host route.
 
-    def unsigned_distance(self, points):    # :316-334
+        Gradients (beyond the reference): when the tensor requires grad, `distance` is differentiable in the points, d/dx = (x - p) / d
+        (0 where d = 0 or no triangle was found).  vertices=V, a float64 CUDA tensor (n_vertices, 3) on the mesh's device, first refits the
+        mesh to V.detach() -- a side effect that stays, as refit(V) -- and makes `distance` differentiable in V as well, through the nearest
+        point's barycentric weights (envelope theorem).  The vertex gradient is summed in a fixed order: the same bits on every run.  The
+        backward runs on torch's current stream and reads only the forward's outputs and the triangles, so refitting the mesh again before
+        backward() does not change it.  First order only: a double backward raises.  nearest_point, nearest_entity and triangle_id carry no
+        gradient."""
+        return self._query(points, True, vertices)
+
+    def unsigned_distance(self, points, vertices=None):    # :316-334
         """as signed_distance, unsigned"""
-        return self._query(points, False)
+        return self._query(points, False, vertices)
 
 
 class MeshSignedDistance:

@@ -423,6 +423,36 @@ DG_API int dg_mesh_raycast(const dg_mesh* mesh, const double* origins, const dou
 DG_API int dg_mesh_raycast_device(const dg_mesh* mesh, const double* d_origins, const double* d_directions, uint64_t n, double t_min,
                                   double t_max, double* d_t, int32_t* d_triangle_id, double* d_barycentric, int32_t* d_status, void* stream);
 
+/* ---- differentiable mesh distance (K10, k10_distance_grad.cu; beyond the reference) -------------------------------------------------
+ * dg_mesh_distance_bary[_device]: dg_mesh_distance[_device] that also writes barycentric[n x 3], the weights of the nearest point on the
+ *     vertices F[t][0], F[t][1], F[t][2] of its triangle t: (fl(fl(1 - s) - t'), s, t') with (s, t') the parameters of the leaf test, so that
+ *     nearest_point = v0 + s (v1 - v0) + t' (v2 - v0) as the query computes it; one-hot on a vertex, on the edge for an edge.  NaN when no
+ *     triangle was accepted (triangle_id -1, distance DBL_MAX).  Distance, nearest point, entity and triangle id are bit for bit those of
+ *     dg_mesh_distance[_device], in both sign modes.  Every output is nullable.  Refusals as dg_mesh_distance: NULL mesh, NULL points with
+ *     n > 0, a mesh on another device and a mesh left unusable by a failed refit (DG_ERR_INVALID).
+ * dg_mesh_distance_vjp[_device]: for the outputs of that call (points, distance, nearest_point, triangle_id, barycentric; either sign mode)
+ *     and an upstream gradient grad_distance[n], the gradient with respect to the points, grad_points[n x 3] = (g / d) (x - p) (0 where
+ *     d == 0 or triangle_id == -1), and with respect to the vertices, grad_vertices[n_vertices x 3] = the sum over queries of
+ *     -w_i * grad_points on vertex F[t][i] (envelope theorem).  Both nullable; grad_vertices is overwritten (0 where nothing arrives; n = 0
+ *     writes zeros).  The vertex sums are in a fixed order stated in k10_distance_grad.cu: the same bits on every run, stream and device.
+ *     Only the given outputs and the mesh's triangles are read, not its vertex positions, so the gradient stays right after a later refit.
+ *     First order only.  The _device form is queued on `stream` after one synchronise that checks the triangle ids; the host form uploads
+ *     every input in one piece and returns when done.  The first call with grad_vertices builds the topology tables dg_mesh_refit uses
+ *     (kept, counted in dg_mesh_info[4]); device scratch of about 130 B per query is taken and released in stream order.
+ *     DG_ERR_INVALID, before anything is written: NULL mesh; a NULL input with n > 0; n >= 2^32 - 1; a mesh on another device; a mesh left
+ *     unusable by a failed refit; a triangle id outside [-1, n_triangles) (checked on the device, reported by the call). */
+DG_API int dg_mesh_distance_bary(const dg_mesh* mesh, const double* points, uint64_t n, int is_signed, double* distance, double* nearest_point,
+                                 int32_t* nearest_entity, int32_t* triangle_id, double* barycentric);
+DG_API int dg_mesh_distance_bary_device(const dg_mesh* mesh, const double* d_points, uint64_t n, int is_signed, double* d_distance,
+                                        double* d_nearest_point, int32_t* d_nearest_entity, int32_t* d_triangle_id, double* d_barycentric,
+                                        void* stream);
+DG_API int dg_mesh_distance_vjp(const dg_mesh* mesh, uint64_t n, const double* points, const double* distance, const double* nearest_point,
+                                const int32_t* triangle_id, const double* barycentric, const double* grad_distance, double* grad_points,
+                                double* grad_vertices);
+DG_API int dg_mesh_distance_vjp_device(const dg_mesh* mesh, uint64_t n, const double* d_points, const double* d_distance,
+                                       const double* d_nearest_point, const int32_t* d_triangle_id, const double* d_barycentric,
+                                       const double* d_grad_distance, double* d_grad_points, double* d_grad_vertices, void* stream);
+
 /* ---- reduced density map: GenerateDensityMap with reduction in one call -----------------------------------------------------------
  * GenerateDensityMap with reduction (cmd/generate_density_map/main.cpp:117-147) in one call:
  *   id = addFunction(density_func, verbose, pred);  reduceField(0, p0);  reduceField(id, p1);
