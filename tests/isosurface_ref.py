@@ -74,7 +74,7 @@ def lattice_values(grid, field_id, L, chunk=1 << 22):
 
 
 def _cell_edges(L, valid, neg, c0, c1):
-    """edge ids of the triangles of lattice cells [c0, c1), (m, 3), in (cell, t, table position) order"""
+    """edge ids of the triangles of lattice cells [c0, c1), (m, 3), in (cell, t, table position) order, and the cell of each triangle"""
     m0, m1 = L.np[0] - 1, L.np[1] - 1
     c = np.arange(c0, c1, dtype=np.int64)
     l0 = L.lin(c % m0, (c // m0) % m1, c // (m0 * m1))
@@ -96,34 +96,91 @@ def _cell_edges(L, valid, neg, c0, c1):
     eid = 7 * (l0[cc][:, None, None] + L.corner_offset(lo)) + DIR_OF_MASK[lo ^ hi]
     odd = ODD[tt]
     eid[odd] = eid[odd][:, :, [0, 2, 1]]
-    return eid[keep]
+    return eid[keep], np.broadcast_to(c[cc][:, None], keep.shape)[keep]
 
 
-def extract(L, f, iso, chunk=1 << 21):
-    """(vertices (n, 3) float64, triangles (m, 3) uint32) of the contract, from the lattice values f[Np]"""
+def _classify(f, iso):
     f = np.asarray(f, np.float64)
-    iso = float(iso)
     with np.errstate(invalid="ignore", over="ignore"):
-        valid = (np.abs(f) <= DBL_MAX) & (f != DBL_MAX)
-        neg = f < iso
-    eid = np.concatenate([_cell_edges(L, valid, neg, b, min(L.n_cells, b + chunk)) for b in range(0, L.n_cells, chunk)] or
-                         [np.zeros((0, 3), np.int64)])
-    uniq, inv = np.unique(eid.reshape(-1), return_inverse=True)           # vertices by increasing edge id
-    T = inv.reshape(-1, 3).astype(np.uint32)
-    # vertex arithmetic: t = (iso - f_p) / (f_q - f_p), x = x_p + t * (x_q - x_p)
+        return (np.abs(f) <= DBL_MAX) & (f != DBL_MAX), f < float(iso)
+
+
+def _vertices(L, uniq, fp, fq, iso):
+    """vertex arithmetic on the edges uniq: t = (iso - f_p) / (f_q - f_p), x = x_p + t * (x_q - x_p)"""
     lp = uniq // 7
     dm = MASK_OF_DIR[uniq % 7]
-    lq = lp + L.corner_offset(dm)
-    fp, fq = f[lp], f[lq]
     with np.errstate(invalid="ignore", over="ignore", divide="ignore"):
-        t = (iso - fp) / (fq - fp)
+        t = (float(iso) - fp) / (fq - fp)
         ip = L.unlin(lp)
         V = np.empty((len(uniq), 3))
         for a in range(3):
             xp = L.coord(a, ip[a])
             xq = L.coord(a, ip[a] + ((dm >> a) & 1))
             V[:, a] = xp + t * (xq - xp)
-    return V, T
+    return V
+
+
+def extract(L, f, iso, chunk=1 << 21):
+    """(vertices (n, 3) float64, triangles (m, 3) uint32) of the contract, from the lattice values f[Np]"""
+    f = np.asarray(f, np.float64)
+    valid, neg = _classify(f, iso)
+    eid = np.concatenate([_cell_edges(L, valid, neg, b, min(L.n_cells, b + chunk))[0] for b in range(0, L.n_cells, chunk)] or
+                         [np.zeros((0, 3), np.int64)])
+    uniq, inv = np.unique(eid.reshape(-1), return_inverse=True)           # vertices by increasing edge id
+    T = inv.reshape(-1, 3).astype(np.uint32)
+    lp = uniq // 7
+    lq = lp + L.corner_offset(MASK_OF_DIR[uniq % 7])
+    return _vertices(L, uniq, f[lp], f[lq], iso), T
+
+
+def extract_windows(L, windows, iso):
+    """extract() restricted to the lattice cells inside index boxes: windows = [(lo, hi, f_box)], lo and hi the first and last lattice
+    point of the box per axis, f_box the values of the box's points (I fastest).  Lattice points, edge ids, cells and coordinates stay
+    those of L, so when no tetrahedron outside the boxes changes sign or is invalid next to a crossing (and the boxes share no lattice
+    cell), the result equals extract(L, f, iso) of the whole lattice, without its values.  -> (V, T, the edge id of every vertex)"""
+    eids, cells, lins, vals = [], [], [], []
+    for lo, hi, fb in windows:
+        lo, hi = np.asarray(lo, np.int64), np.asarray(hi, np.int64)
+        W = Lattice(np.zeros(3), np.zeros(3), np.zeros(3), hi - lo, 1)       # the box's own numbering
+        valid, neg = _classify(fb, iso)
+        e, c = _cell_edges(W, valid, neg, 0, W.n_cells)
+        I, J, K = W.unlin(e // 7)
+        eids.append(7 * L.lin(I + lo[0], J + lo[1], K + lo[2]) + e % 7)
+        m0, m1 = W.np[0] - 1, W.np[1] - 1
+        g0, g1 = L.np[0] - 1, L.np[1] - 1
+        cells.append(c % m0 + lo[0] + g0 * ((c // m0) % m1 + lo[1] + g1 * (c // (m0 * m1) + lo[2])))
+        I, J, K = W.unlin(np.arange(W.n_points))
+        lins.append(L.lin(I + lo[0], J + lo[1], K + lo[2]))
+        vals.append(np.asarray(fb, np.float64))
+    eid = np.concatenate(eids or [np.zeros((0, 3), np.int64)])
+    eid = eid[np.argsort(np.concatenate(cells or [np.zeros(0, np.int64)]), kind="stable")]   # triangles by cell, then t and table position
+    uniq, inv = np.unique(eid.reshape(-1), return_inverse=True)
+    lin, val = np.concatenate(lins or [np.zeros(0, np.int64)]), np.concatenate(vals or [np.zeros(0)])
+    order = np.argsort(lin)
+    lin, val = lin[order], val[order]
+    lp = uniq // 7
+    lq = lp + L.corner_offset(MASK_OF_DIR[uniq % 7])
+    fp, fq = val[np.searchsorted(lin, lp)], val[np.searchsorted(lin, lq)]
+    return _vertices(L, uniq, fp, fq, iso), inv.reshape(-1, 3).astype(np.uint32), uniq
+
+
+def case_counts(L, f, iso, chunk=1 << 21):
+    """how often each case (the 4-bit negative mask) occurs among the tetrahedra whose four vertices are valid: (16, 2) counts, column 0
+    the even permutations (t = 0, 3, 4), column 1 the odd ones"""
+    valid, neg = _classify(f, iso)
+    out = np.zeros((16, 2), np.int64)
+    m0, m1 = L.np[0] - 1, L.np[1] - 1
+    off = L.corner_offset(np.arange(8))
+    for b in range(0, L.n_cells, chunk):
+        c = np.arange(b, min(L.n_cells, b + chunk), dtype=np.int64)
+        l0 = L.lin(c % m0, (c // m0) % m1, c // (m0 * m1))
+        cv = valid[l0[:, None] + off[None, :]][:, TET].all(axis=2)
+        tn = neg[l0[:, None] + off[None, :]].astype(np.int64)[:, TET]
+        case = tn[..., 0] | (tn[..., 1] << 1) | (tn[..., 2] << 2) | (tn[..., 3] << 3)
+        for odd in (0, 1):
+            sel = cv & (ODD[None, :] == bool(odd))
+            out[:, odd] += np.bincount(case[sel], minlength=16)
+    return out
 
 
 # ---- mesh checks -------------------------------------------------------------------------------------------------------------------
