@@ -387,6 +387,35 @@ public:
         check(dg_field_raycast(deviceField(field_id), origins, directions, n, iso, t_min, t_max, t_lo, t_hi, status));
     }
 
+    // ---- trainable fields (new, beyond the reference; contract in k11_field_grad.cu).  One trainable device field per field id, made at first
+    // use from the members (dg_field_create_trainable, which synchronises) and dropped with the other device copies.  Device pointers, `stream`
+    // a cudaStream_t (NULL: the legacy default stream); neither call synchronises the host.
+    // setNodesDevice: the trainable field takes the n_nodes values at d_nodes (dg_field_set_nodes_device); n_nodes must be the field's count
+    void setNodesDevice(unsigned int field_id, const double* d_nodes, std::size_t n_nodes, void* stream = nullptr)
+    {
+        check(dg_field_set_nodes_device(trainableField(field_id), d_nodes, n_nodes, stream));
+    }
+    // interpolate_vjp: d_grad_nodes [nodes] = the gradient in the trainable field's node values of sum_q d_grad_phi[q] phi(x_q) +
+    // d_grad_grad[q] . grad(x_q) over the n points d_x [n x 3] (dg_interpolate_vjp_device; either upstream may be NULL, not both)
+    void interpolate_vjp(unsigned int field_id, std::size_t n, const double* d_x, const double* d_grad_phi, const double* d_grad_grad,
+                         double* d_grad_nodes, void* stream = nullptr)
+    {
+        check(dg_interpolate_vjp_device(trainableField(field_id), d_x, n, d_grad_phi, d_grad_grad, d_grad_nodes, stream));
+    }
+    // the trainable field itself, for the library's other calls on its current values (dg_interpolate_batch_device, ...)
+    dg_field* trainableField(unsigned int field_id)
+    {
+        auto it = m_trainable.find(field_id);
+        if (it != m_trainable.end()) return it->second;
+        const dg_grid_desc d = desc();
+        dg_field* f = nullptr;
+        check(dg_field_create_trainable(&d, m_nodes.at(field_id).data(), m_nodes[field_id].size(),
+                                        reinterpret_cast<const std::uint32_t*>(m_cells[field_id].data()), m_cells[field_id].size(),
+                                        m_cell_map[field_id].data(), &f));
+        m_trainable[field_id] = f;
+        return f;
+    }
+
     // ---- split API (:901-975): shape functions on the GPU (dg_shape_functions), index algebra on the host
     DG_NO_CONTRACT bool determineShapeFunctions(unsigned int field_id, Eigen::Vector3d const& x, std::array<unsigned int, 32>& cell, Eigen::Vector3d& c0,
                                                 Eigen::Matrix<double, 32, 1>& N, Eigen::Matrix<double, 32, 3>* dN = nullptr) const override
@@ -526,6 +555,7 @@ private:
     // the handles the reduced calls returned, kept until their field's first deviceField or the next invalidate(): a field made from a
     // handle needs no upload.  Owned like m_dev.
     mutable std::map<unsigned int, dg_reduced_band*> m_reduced;
+    std::map<unsigned int, dg_field*> m_trainable;          // trainableField's, owned like m_dev
 
     // owns a dg_reduced_band until keep_reduced takes it; destroys it on every other path
     struct ReducedHandle {
@@ -559,6 +589,8 @@ private:
         m_dev.clear();
         for (auto& kv : m_reduced) dg_reduced_band_destroy(kv.second);
         m_reduced.clear();
+        for (auto& kv : m_trainable) dg_field_destroy(kv.second);
+        m_trainable.clear();
     }
     bool in_kept_cell(unsigned int field_id, Eigen::Vector3d const& x) const
     {

@@ -107,6 +107,11 @@ SIGNATURES = {
     "dg_build_cells": (C.c_int, [_u32p, C.c_uint64, C.c_uint64, _u32p]),
     "dg_field_create": (C.c_int, [_gp, _dp, C.c_uint64, _u32p, C.c_uint64, _u32p, C.POINTER(_vp)]),
     "dg_field_create_device": (C.c_int, [_gp, _vp, C.c_uint64, _vp, C.POINTER(_vp)]),
+    "dg_field_create_trainable": (C.c_int, [_gp, _dp, C.c_uint64, _u32p, C.c_uint64, _u32p, C.POINTER(_vp)]),
+    "dg_field_set_nodes": (C.c_int, [_vp, _dp, C.c_uint64]),
+    "dg_field_set_nodes_device": (C.c_int, [_vp, _vp, C.c_uint64, _vp]),
+    "dg_interpolate_vjp": (C.c_int, [_vp, _dp, C.c_uint64, _dp, _dp, _dp]),
+    "dg_interpolate_vjp_device": (C.c_int, [_vp, _vp, C.c_uint64, _vp, _vp, _vp, _vp]),
     "dg_field_destroy": (C.c_int, [_vp]),
     "dg_field_info": (C.c_int, [_vp, _u64p]),
     "dg_interpolate_batch": (C.c_int, [_vp, _dp, C.c_uint64, _dp, _dp]),

@@ -47,6 +47,7 @@
 #include "k8_refit.h"
 #include "k9_mesh_raycast.h"
 #include "k10_distance_grad.h"
+#include "k11_field_grad.h"
 #include "reduce_field.h"
 #include "obj_reader.h"
 
@@ -279,6 +280,15 @@ struct dg_field {
     uint64_t n_nodes = 0, n_cells_kept = 0;
     double coeff_max = 0.0;      // k3_coeff_max of the packed coefficients: whether K3 may skip points outside the kernel support
     int device = 0;
+    // dg_field_create_trainable: what dg_field_set_nodes and dg_interpolate_vjp need (k11_field_grad.cu)
+    bool trainable = false;
+    DevBuf<unsigned> d_cells;                       // [n_cells_kept][32] node ids; not kept for the closed-form table (cells == NULL)
+    DevBuf<uint32_t> d_inc_begin, d_inc;            // node -> (cell, slot) incidences, CSR
+    DevBuf<unsigned char> d_has_max;                // [n_cells_kept]: the cell's block holds a DBL_MAX coefficient
+    size_t bytes() const
+    {
+        return d_packed.bytes() + d_cell_map.bytes() + d_tab.bytes() + d_cells.bytes() + d_inc_begin.bytes() + d_inc.bytes() + d_has_max.bytes();
+    }
 };
 
 // ------------------------------------------------------------------------------------------------ library
@@ -1748,21 +1758,21 @@ int dg_build_cells(const uint32_t res[3], uint64_t c_begin, uint64_t c_end, uint
 }
 
 // ------------------------------------------------------------------------------------------------ fields / K2
-static int field_common(const dg_grid_desc* grid, dg_field** out, dg_field*& f)
+static int field_common(const dg_grid_desc* grid, dg_field** out, dg_field*& f, const char* who)
 {
-    if (!out) return fail(DG_ERR_INVALID, "dg_field_create: out is NULL");
+    if (!out) return fail(DG_ERR_INVALID, "%s: out is NULL", who);
     *out = nullptr;
     if (int rc = require_device()) return rc;
     if (int rc = ensure_selftest()) return rc;
     GridDev g;
-    if (int rc = grid_checked(grid, g, "dg_field_create")) return rc;
+    if (int rc = grid_checked(grid, g, who)) return rc;
     f = new (std::nothrow) dg_field();
-    if (!f) return fail(DG_ERR_NOMEM, "dg_field_create: out of host memory");
+    if (!f) return fail(DG_ERR_NOMEM, "%s: out of host memory", who);
     f->desc = *grid; f->dev.g = g;
     return DG_OK;
 }
 
-static int field_finish(dg_field* f, const double* d_nodes, const unsigned* d_cells, cudaStream_t stream)
+static int field_finish(dg_field* f, const double* d_nodes, const unsigned* d_cells, cudaStream_t stream, const char* who)
 {
     cudaError_t e = cudaGetDevice(&f->device);
     if (e == cudaSuccess) e = f->d_packed.alloc(32 * (f->n_cells_kept ? f->n_cells_kept : 1));
@@ -1771,39 +1781,62 @@ static int field_finish(dg_field* f, const double* d_nodes, const unsigned* d_ce
     if (e == cudaSuccess) { e = k2_launch_pack(f->dev.g, d_nodes, d_cells, f->n_cells_kept, f->d_packed.p, stream); g_launches.fetch_add(1); }
     if (e == cudaSuccess) { e = k2_launch_axis_tables(f->dev.g, f->d_tab.p, stream); g_launches.fetch_add(1); }
     if (e == cudaSuccess) { e = k3_coeff_max(f->d_packed.p, 32 * f->n_cells_kept, &f->coeff_max, stream); g_launches.fetch_add(1); }
-    if (e != cudaSuccess) return fail(cuda_code(e), "dg_field_create: %s", cudaGetErrorString(e));
+    if (e != cudaSuccess) return fail(cuda_code(e), "%s: %s", who, cudaGetErrorString(e));
     f->dev.packed = f->d_packed.p;
     f->dev.cell_map = f->d_cell_map.p;
     f->dev.tab = f->d_tab.p;
     return DG_OK;
 }
 
-int dg_field_create(const dg_grid_desc* grid, const double* nodes, uint64_t n_nodes, const uint32_t* cells, uint64_t n_cells_kept,
-                    const uint32_t* cell_map, dg_field** out)
+// the DBL_MAX flags of the packed blocks and the node -> (cell, slot) incidence table of a trainable field, queued on the legacy stream
+static int trainable_tables(dg_field* f)
+{
+    static const char* who = "dg_field_create_trainable";
+    DG_CUDA(f->d_has_max.alloc(f->n_cells_kept));
+    DG_CUDA(f->d_inc_begin.alloc(f->n_nodes + 1));
+    DG_CUDA(f->d_inc.alloc(32 * f->n_cells_kept));
+    DG_LAUNCH(k11_launch_flags(f->d_packed.p, f->n_cells_kept, f->d_has_max.p, nullptr));
+    DevBuf<char> scratch;
+    DG_CUDA(scratch.alloc(k11_incidence_scratch_bytes(f->n_cells_kept)));
+    const cudaError_t e = k11_launch_incidence(f->dev.g, f->d_cells.p, f->n_cells_kept, f->n_nodes, f->d_inc_begin.p, f->d_inc.p, scratch.p, nullptr);
+    if (e != cudaSuccess) return fail(cuda_code(e), "%s: %s", who, cudaGetErrorString(e));
+    g_launches.fetch_add(1);
+    DG_CUDA(cudaDeviceSynchronize());                       // the scratch is released on return
+    f->trainable = true;
+    return DG_OK;
+}
+
+// dg_field_create and dg_field_create_trainable: the same checks and upload; a trainable field also keeps its cell table and builds the
+// tables of k11_field_grad.cu
+static int field_create_host(const dg_grid_desc* grid, const double* nodes, uint64_t n_nodes, const uint32_t* cells, uint64_t n_cells_kept,
+                             const uint32_t* cell_map, bool trainable, dg_field** out, const char* who)
 {
     dg_field* f = nullptr;
-    if (int rc = field_common(grid, out, f)) return rc;
+    if (int rc = field_common(grid, out, f, who)) return rc;
     auto bail = [&](int rc) { delete f; return rc; };
     const uint64_t n_cells = grid_cells(f->dev.g);
-    if (!nodes && n_nodes) return bail(fail(DG_ERR_INVALID, "dg_field_create: nodes is NULL"));
-    if (!cells && n_cells_kept != n_cells) return bail(fail(DG_ERR_INVALID, "dg_field_create: cells == NULL requires n_cells_kept == nx*ny*nz"));
+    if (!nodes && n_nodes) return bail(fail(DG_ERR_INVALID, "%s: nodes is NULL", who));
+    if (!cells && n_cells_kept != n_cells) return bail(fail(DG_ERR_INVALID, "%s: cells == NULL requires n_cells_kept == nx*ny*nz", who));
     if (!cell_map && n_cells_kept != n_cells)      // K2/K3 read a NULL cell map as the identity: it must then cover every grid cell
-        return bail(fail(DG_ERR_INVALID, "dg_field_create: cell_map == NULL requires n_cells_kept == nx*ny*nz (pass the reduced field's cell map)"));
+        return bail(fail(DG_ERR_INVALID, "%s: cell_map == NULL requires n_cells_kept == nx*ny*nz (pass the reduced field's cell map)", who));
+    if (trainable && 32 * n_cells_kept >= (1ull << 32))
+        return bail(fail(DG_ERR_INVALID, "%s: %llu kept cells; the incidence table needs 32 * n_cells_kept < 2^32",
+                         who, (unsigned long long)n_cells_kept));
     if (!cells) {
         const uint64_t nn = grid_nodes(f->dev.g);
-        if (n_nodes != nn) return bail(fail(DG_ERR_INVALID, "dg_field_create: closed-form cells need all %llu nodes (got %llu)",
+        if (n_nodes != nn) return bail(fail(DG_ERR_INVALID, "%s: closed-form cells need all %llu nodes (got %llu)", who,
                                             (unsigned long long)nn, (unsigned long long)n_nodes));
     } else {
         for (uint64_t i = 0; i < 32 * n_cells_kept; i++)
-            if (cells[i] >= n_nodes) return bail(fail(DG_ERR_INVALID, "dg_field_create: cell table references node %u >= n_nodes", cells[i]));
+            if (cells[i] >= n_nodes) return bail(fail(DG_ERR_INVALID, "%s: cell table references node %u >= n_nodes", who, cells[i]));
     }
     if (cell_map)
         for (uint64_t i = 0; i < n_cells; i++)
             if (cell_map[i] != UINT32_MAX && cell_map[i] >= n_cells_kept)
-                return bail(fail(DG_ERR_INVALID, "dg_field_create: cell_map entry %u >= n_cells_kept", cell_map[i]));
+                return bail(fail(DG_ERR_INVALID, "%s: cell_map entry %u >= n_cells_kept", who, cell_map[i]));
     f->n_nodes = n_nodes; f->n_cells_kept = n_cells_kept;
     DevBuf<double> d_nodes;
-    DevBuf<unsigned> d_cells;
+    DevBuf<unsigned>& d_cells = f->d_cells;
     cudaError_t e = d_nodes.alloc(n_nodes);
     if (e == cudaSuccess) e = cudaMemcpy(d_nodes.p, nodes, n_nodes * sizeof(double), cudaMemcpyHostToDevice);
     if (e == cudaSuccess && cells) {
@@ -1814,23 +1847,38 @@ int dg_field_create(const dg_grid_desc* grid, const double* nodes, uint64_t n_no
         e = f->d_cell_map.alloc(n_cells);
         if (e == cudaSuccess) e = cudaMemcpy(f->d_cell_map.p, cell_map, n_cells * sizeof(unsigned), cudaMemcpyHostToDevice);
     }
-    if (e != cudaSuccess) return bail(fail(cuda_code(e), "dg_field_create: %s", cudaGetErrorString(e)));
-    if (int rc = field_finish(f, d_nodes.p, cells ? d_cells.p : nullptr, nullptr)) return bail(rc);
+    if (e != cudaSuccess) return bail(fail(cuda_code(e), "%s: %s", who, cudaGetErrorString(e)));
+    if (int rc = field_finish(f, d_nodes.p, cells ? d_cells.p : nullptr, nullptr, who)) return bail(rc);
+    if (trainable) { if (int rc = trainable_tables(f)) return bail(rc); }
     e = cudaDeviceSynchronize();
-    if (e != cudaSuccess) return bail(fail(DG_ERR_CUDA, "dg_field_create: %s", cudaGetErrorString(e)));
+    if (e != cudaSuccess) return bail(fail(DG_ERR_CUDA, "%s: %s", who, cudaGetErrorString(e)));
+    if (!trainable) d_cells.release();
     *out = f;
     return DG_OK;
+}
+
+int dg_field_create(const dg_grid_desc* grid, const double* nodes, uint64_t n_nodes, const uint32_t* cells, uint64_t n_cells_kept,
+                    const uint32_t* cell_map, dg_field** out)
+{
+    return field_create_host(grid, nodes, n_nodes, cells, n_cells_kept, cell_map, false, out, "dg_field_create");
+}
+
+int dg_field_create_trainable(const dg_grid_desc* grid, const double* nodes, uint64_t n_nodes, const uint32_t* cells, uint64_t n_cells_kept,
+                              const uint32_t* cell_map, dg_field** out)
+{
+    static const char* who = "dg_field_create_trainable";
+    return guarded(who, [&]() { return field_create_host(grid, nodes, n_nodes, cells, n_cells_kept, cell_map, true, out, who); });
 }
 
 int dg_field_create_device(const dg_grid_desc* grid, const double* d_nodes, uint64_t n_nodes, void* stream, dg_field** out)
 {
     dg_field* f = nullptr;
-    if (int rc = field_common(grid, out, f)) return rc;
+    if (int rc = field_common(grid, out, f, "dg_field_create")) return rc;
     const uint64_t nn = grid_nodes(f->dev.g);
     if (!d_nodes || n_nodes != nn) { delete f; return fail(DG_ERR_INVALID, "dg_field_create_device: need all %llu node coefficients", (unsigned long long)nn); }
     f->n_nodes = n_nodes;
     f->n_cells_kept = grid_cells(f->dev.g);
-    if (int rc = field_finish(f, d_nodes, nullptr, (cudaStream_t)stream)) { delete f; return rc; }
+    if (int rc = field_finish(f, d_nodes, nullptr, (cudaStream_t)stream, "dg_field_create")) { delete f; return rc; }
     *out = f;
     return DG_OK;
 }
@@ -1845,7 +1893,7 @@ int dg_field_info(const dg_field* f, uint64_t info[4])
 {
     if (!f || !info) return fail(DG_ERR_INVALID, "dg_field_info: NULL argument");
     info[0] = f->n_nodes; info[1] = f->n_cells_kept;
-    info[2] = f->d_packed.bytes() + f->d_cell_map.bytes() + f->d_tab.bytes(); info[3] = (uint64_t)f->device;
+    info[2] = f->bytes(); info[3] = (uint64_t)f->device;
     return DG_OK;
 }
 
@@ -2010,6 +2058,112 @@ int dg_shape_functions(const double* xi, uint64_t n, double* N, double* dN)
                                DG_LAUNCH(k2_launch_shape_functions((const double*)in[0], c, (double*)out[0], (double*)out[1], nullptr));
                                return DG_OK;
                            });
+}
+
+// ------------------------------------------------------------------------------------------------ K11: trainable fields
+static int trainable_check(const dg_field* f, const char* who)
+{
+    if (!f) return fail(DG_ERR_INVALID, "%s: field is NULL", who);
+    if (!f->trainable) return fail(DG_ERR_INVALID, "%s: the field was not made by dg_field_create_trainable", who);
+    return check_handle_device(f->device, who);
+}
+
+static int set_nodes_check(const dg_field* f, const void* nodes, uint64_t n_nodes, const char* who)
+{
+    if (int rc = trainable_check(f, who)) return rc;
+    if (n_nodes != f->n_nodes) return fail(DG_ERR_INVALID, "%s: the field has %llu nodes (got %llu)", who, (unsigned long long)f->n_nodes,
+                                           (unsigned long long)n_nodes);
+    if (n_nodes && !nodes) return fail(DG_ERR_INVALID, "%s: nodes is NULL", who);
+    return DG_OK;
+}
+
+// K2's pack of the new values, the DBL_MAX flags again, and coeff_max = +inf: K3 then samples all 4096 points, which gives the bits of the
+// skipping kernel wherever that one is exact (k3_density.cu), so nothing has to be read back
+static int set_nodes_launch(dg_field* f, const double* d_nodes, cudaStream_t st)
+{
+    DG_LAUNCH(k2_launch_pack(f->dev.g, d_nodes, f->d_cells.p, f->n_cells_kept, f->d_packed.p, st));
+    DG_LAUNCH(k11_launch_flags(f->d_packed.p, f->n_cells_kept, f->d_has_max.p, st));
+    f->coeff_max = std::numeric_limits<double>::infinity();
+    return DG_OK;
+}
+
+int dg_field_set_nodes_device(dg_field* f, const double* d_nodes, uint64_t n_nodes, void* stream)
+{
+    static const char* who = "dg_field_set_nodes_device";
+    if (int rc = set_nodes_check(f, d_nodes, n_nodes, who)) return rc;
+    return set_nodes_launch(f, d_nodes, (cudaStream_t)stream);
+}
+
+int dg_field_set_nodes(dg_field* f, const double* nodes, uint64_t n_nodes)
+{
+    static const char* who = "dg_field_set_nodes";
+    if (int rc = set_nodes_check(f, nodes, n_nodes, who)) return rc;
+    DevBuf<double> d;
+    DG_CUDA(d.alloc(n_nodes));
+    DG_CUDA(cudaMemcpy(d.p, nodes, n_nodes * sizeof(double), cudaMemcpyHostToDevice));
+    if (int rc = set_nodes_launch(f, d.p, nullptr)) return rc;
+    DG_CUDA(cudaDeviceSynchronize());
+    return DG_OK;
+}
+
+static int vjp_field_check(const dg_field* f, const void* x, uint64_t n, const void* gphi, const void* ggrad, const void* grad_nodes, const char* who)
+{
+    if (int rc = trainable_check(f, who)) return rc;
+    if (n >= (1ull << 32) - 1) return fail(DG_ERR_INVALID, "%s: %llu queries; at most 2^32 - 2 per call", who, (unsigned long long)n);
+    if (!gphi && !ggrad) return fail(DG_ERR_INVALID, "%s: give grad_phi, grad_grad or both", who);
+    if (n && !x) return fail(DG_ERR_INVALID, "%s: x is NULL", who);
+    if (f->n_nodes && !grad_nodes) return fail(DG_ERR_INVALID, "%s: grad_nodes is NULL", who);
+    return DG_OK;
+}
+
+// the scratch is stream-ordered: allocated and released on `st`, so the call queues everything and returns
+static int vjp_field_launch(const dg_field* f, const double* d_x, uint64_t n, const double* d_gphi, const double* d_ggrad, double* d_grad_nodes,
+                            cudaStream_t st)
+{
+    K11Field kf;
+    kf.f = f->dev; kf.inc_begin = f->d_inc_begin.p; kf.inc = f->d_inc.p; kf.has_max = f->d_has_max.p;
+    kf.n_nodes = f->n_nodes; kf.n_cells_kept = f->n_cells_kept;
+    const size_t bytes = k11_scratch_bytes(n, f->n_cells_kept);
+    void* scratch = nullptr;
+#ifdef DG_EMU
+    if (bytes) DG_CUDA(cudaMalloc(&scratch, bytes));
+    const cudaError_t e = k11_launch_vjp(kf, d_x, n, d_gphi, d_ggrad, d_grad_nodes, scratch, st);
+    if (scratch) cudaFree(scratch);
+#else
+    if (bytes) DG_CUDA(cudaMallocAsync(&scratch, bytes, st));
+    const cudaError_t e = k11_launch_vjp(kf, d_x, n, d_gphi, d_ggrad, d_grad_nodes, scratch, st);
+    if (scratch) cudaFreeAsync(scratch, st);
+#endif
+    DG_LAUNCH(e);
+    return DG_OK;
+}
+
+int dg_interpolate_vjp_device(const dg_field* f, const double* d_x, uint64_t n, const double* d_grad_phi, const double* d_grad_grad,
+                              double* d_grad_nodes, void* stream)
+{
+    static const char* who = "dg_interpolate_vjp_device";
+    if (int rc = vjp_field_check(f, d_x, n, d_grad_phi, d_grad_grad, d_grad_nodes, who)) return rc;
+    return vjp_field_launch(f, d_x, n, d_grad_phi, d_grad_grad, d_grad_nodes, (cudaStream_t)stream);
+}
+
+// host arrays: every input uploaded in one piece (the node sums span all queries), then the device form on the legacy default stream
+int dg_interpolate_vjp(const dg_field* f, const double* x, uint64_t n, const double* grad_phi, const double* grad_grad, double* grad_nodes)
+{
+    static const char* who = "dg_interpolate_vjp";
+    if (int rc = vjp_field_check(f, x, n, grad_phi, grad_grad, grad_nodes, who)) return rc;
+    DevBuf<double> d_x, d_gp, d_gg, d_out;
+    DG_CUDA(d_x.alloc(3 * n)); DG_CUDA(d_out.alloc(f->n_nodes));
+    if (grad_phi) DG_CUDA(d_gp.alloc(n));
+    if (grad_grad) DG_CUDA(d_gg.alloc(3 * n));
+    if (n) {
+        DG_CUDA(cudaMemcpy(d_x.p, x, 3 * n * sizeof(double), cudaMemcpyHostToDevice));
+        if (grad_phi) DG_CUDA(cudaMemcpy(d_gp.p, grad_phi, n * sizeof(double), cudaMemcpyHostToDevice));
+        if (grad_grad) DG_CUDA(cudaMemcpy(d_gg.p, grad_grad, 3 * n * sizeof(double), cudaMemcpyHostToDevice));
+    }
+    if (int rc = vjp_field_launch(f, d_x.p, n, grad_phi ? d_gp.p : nullptr, grad_grad ? d_gg.p : nullptr, d_out.p, nullptr)) return rc;
+    if (f->n_nodes) DG_CUDA(cudaMemcpy(grad_nodes, d_out.p, f->n_nodes * sizeof(double), cudaMemcpyDeviceToHost));
+    DG_CUDA(cudaDeviceSynchronize());
+    return DG_OK;
 }
 
 // ------------------------------------------------------------------------------------------------ K3
@@ -2428,7 +2582,7 @@ static int reduced_node_map_create_impl(const ReducedNodeMap& m, const dg_grid_d
         DG_CUDA(cudaStreamSynchronize(st));
         if (bad) return fail(DG_ERR_INVALID, "%s: a cell_map entry is >= n_cells", who);
     }
-    if (int rc = field_finish(f.get(), d_sdf.p, d_cells.p, st)) return rc;
+    if (int rc = field_finish(f.get(), d_sdf.p, d_cells.p, st, "dg_field_create")) return rc;
     DG_CUDA(cudaStreamSynchronize(st));
     ms[0] += clock.lap();
     // ---- 2. addFunction(node_func, verbose, pred) (main.cpp:96-133): K3 over every node, predicate on
@@ -2735,13 +2889,13 @@ int dg_field_create_reduced(const dg_reduced_band* h, dg_field** out)
     *out = nullptr;
     if (!h) return fail(DG_ERR_INVALID, "%s: handle is NULL", who);
     dg_field* f = nullptr;
-    if (int rc = field_common(&h->desc, out, f)) return rc;
+    if (int rc = field_common(&h->desc, out, f, "dg_field_create")) return rc;
     std::unique_ptr<dg_field> own(f);
     if (int rc = check_handle_device(h->device, who)) return rc;
     f->n_nodes = h->n_nodes; f->n_cells_kept = h->n_cells;
     DG_CUDA(f->d_cell_map.alloc(h->n_grid_cells));
     if (h->n_grid_cells) DG_CUDA(cudaMemcpyAsync(f->d_cell_map.p, h->d_cell_map.p, h->n_grid_cells * sizeof(unsigned), cudaMemcpyDeviceToDevice, nullptr));
-    if (int rc = field_finish(f, h->d_nodes.p, h->d_cells.p, nullptr)) return rc;
+    if (int rc = field_finish(f, h->d_nodes.p, h->d_cells.p, nullptr, "dg_field_create")) return rc;
     DG_CUDA(cudaDeviceSynchronize());
     *out = own.release();
     return DG_OK;

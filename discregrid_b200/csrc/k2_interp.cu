@@ -38,6 +38,7 @@
 #include "dg_device.cuh"
 #include "k2_interp.h"
 #include "dg_launch.h"
+#include "shape_rows.cuh"
 
 #include <cfloat>
 #include <climits>
@@ -360,79 +361,17 @@ interpolate_kernel(GridDev g, const double* __restrict__ packed, const unsigned*
     }
 }
 
-// shape_function_ alone (diagnostics / dg_shape_functions): evaluates through the same code path by
-// interpolating 32 unit fields would be wasteful; instead a direct restatement, one thread per point.
+// shape_function_ alone (diagnostics / dg_shape_functions): the rows of shape_rows.cuh, one thread per point.
 __global__ void shape_functions_kernel(const double* __restrict__ xi, unsigned long long n, double* __restrict__ N, double* __restrict__ dN)
 {
     const unsigned long long q = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (q >= n) return;
-    const double X = xi[3 * q], Y = xi[3 * q + 1], Z = xi[3 * q + 2];
-    const double x2 = X * X, y2 = Y * Y, z2 = Z * Z;
-    const double _1mx = 1.0 - X, _1my = 1.0 - Y, _1mz = 1.0 - Z;
-    const double _1px = 1.0 + X, _1py = 1.0 + Y, _1pz = 1.0 + Z;
-    const double _1m3x = 1.0 - 3.0 * X, _1m3y = 1.0 - 3.0 * Y, _1m3z = 1.0 - 3.0 * Z;
-    const double _1p3x = 1.0 + 3.0 * X, _1p3y = 1.0 + 3.0 * Y, _1p3z = 1.0 + 3.0 * Z;
-    const double mxmy = _1mx * _1my, mxpy = _1mx * _1py, pxmy = _1px * _1my, pxpy = _1px * _1py;
-    const double mxmz = _1mx * _1mz, mxpz = _1mx * _1pz, pxmz = _1px * _1mz, pxpz = _1px * _1pz;
-    const double mymz = _1my * _1mz, mypz = _1my * _1pz, pymz = _1py * _1mz, pypz = _1py * _1pz;
-    const double _1mx2 = 1.0 - x2, _1my2 = 1.0 - y2, _1mz2 = 1.0 - z2;
-    const double facc = 1.0 / 64.0 * (9.0 * (x2 + y2 + z2) - 19.0);
-    const double fx = 9.0 / 64.0 * _1mx2, fy = 9.0 / 64.0 * _1my2, fz = 9.0 / 64.0 * _1mz2;
-    const double fxm = fx * _1m3x, fxp = fx * _1p3x, fym = fy * _1m3y, fyp = fy * _1p3y, fzm = fz * _1m3z, fzp = fz * _1p3z;
-    const double A = 9.0 * (3.0 * x2 + y2 + z2) - 19.0, B = 9.0 * (x2 + 3.0 * y2 + z2) - 19.0, C = 9.0 * (x2 + y2 + 3.0 * z2) - 19.0;
-    const double _18x = 18.0 * X, _18y = 18.0 * Y, _18z = 18.0 * Z;
-    const double xmA = _18x - A, xpA = _18x + A, ymB = _18y - B, ypB = _18y + B, zmC = _18z - C, zpC = _18z + C;
-    const double _3m9x2 = 3.0 - 9.0 * x2, _3m9y2 = 3.0 - 9.0 * y2, _3m9z2 = 3.0 - 9.0 * z2;
-    const double _2x = 2.0 * X, _2y = 2.0 * Y, _2z = 2.0 * Z;
-    const double mX = -_3m9x2 - _2x, pX = _3m9x2 - _2x, Xm = _1mx2 * _1m3x, Xp = _1mx2 * _1p3x;
-    const double mY = -_3m9y2 - _2y, pY = _3m9y2 - _2y, Ym = _1my2 * _1m3y, Yp = _1my2 * _1p3y;
-    const double mZ = -_3m9z2 - _2z, pZ = _3m9z2 - _2z, Zm = _1mz2 * _1m3z, Zp = _1mz2 * _1p3z;
     double* Nq = N + 32 * q;
     double* Dq = dN ? dN + 96 * q : nullptr;
-    int j = 0;
-#define DG_ROW(n, dx, dy, dz, SC)                                                            \
-    {                                                                                        \
-        Nq[j] = (n);                                                                         \
-        if (Dq) { Dq[3 * j] = SC(dx); Dq[3 * j + 1] = SC(dy); Dq[3 * j + 2] = SC(dz); }      \
-        j++;                                                                                 \
-    }
-#define DG_SC_C(v) ((v) * 0.015625)   /* == /64.0 exactly */
-#define DG_SC_E(v) ((v) * (9.0 / 64.0))
-    DG_ROW(facc * mxmy * _1mz, xmA * mymz, mxmz * ymB, mxmy * zmC, DG_SC_C)
-    DG_ROW(facc * pxmy * _1mz, xpA * mymz, pxmz * ymB, pxmy * zmC, DG_SC_C)
-    DG_ROW(facc * mxpy * _1mz, xmA * pymz, mxmz * ypB, mxpy * zmC, DG_SC_C)
-    DG_ROW(facc * pxpy * _1mz, xpA * pymz, pxmz * ypB, pxpy * zmC, DG_SC_C)
-    DG_ROW(facc * mxmy * _1pz, xmA * mypz, mxpz * ymB, mxmy * zpC, DG_SC_C)
-    DG_ROW(facc * pxmy * _1pz, xpA * mypz, pxpz * ymB, pxmy * zpC, DG_SC_C)
-    DG_ROW(facc * mxpy * _1pz, xmA * pypz, mxpz * ypB, mxpy * zpC, DG_SC_C)
-    DG_ROW(facc * pxpy * _1pz, xpA * pypz, pxpz * ypB, pxpy * zpC, DG_SC_C)
-    DG_ROW(fxm * mymz, mX * mymz, -Xm * _1mz, -Xm * _1my, DG_SC_E)
-    DG_ROW(fxp * mymz, pX * mymz, -Xp * _1mz, -Xp * _1my, DG_SC_E)
-    DG_ROW(fxm * mypz, mX * mypz, -Xm * _1pz, Xm * _1my, DG_SC_E)
-    DG_ROW(fxp * mypz, pX * mypz, -Xp * _1pz, Xp * _1my, DG_SC_E)
-    DG_ROW(fxm * pymz, mX * pymz, Xm * _1mz, -Xm * _1py, DG_SC_E)
-    DG_ROW(fxp * pymz, pX * pymz, Xp * _1mz, -Xp * _1py, DG_SC_E)
-    DG_ROW(fxm * pypz, mX * pypz, Xm * _1pz, Xm * _1py, DG_SC_E)
-    DG_ROW(fxp * pypz, pX * pypz, Xp * _1pz, Xp * _1py, DG_SC_E)
-    DG_ROW(fym * mxmz, -Ym * _1mz, mY * mxmz, -Ym * _1mx, DG_SC_E)
-    DG_ROW(fyp * mxmz, -Yp * _1mz, pY * mxmz, -Yp * _1mx, DG_SC_E)
-    DG_ROW(fym * pxmz, Ym * _1mz, mY * pxmz, -Ym * _1px, DG_SC_E)
-    DG_ROW(fyp * pxmz, Yp * _1mz, pY * pxmz, -Yp * _1px, DG_SC_E)
-    DG_ROW(fym * mxpz, -Ym * _1pz, mY * mxpz, Ym * _1mx, DG_SC_E)
-    DG_ROW(fyp * mxpz, -Yp * _1pz, pY * mxpz, Yp * _1mx, DG_SC_E)
-    DG_ROW(fym * pxpz, Ym * _1pz, mY * pxpz, Ym * _1px, DG_SC_E)
-    DG_ROW(fyp * pxpz, Yp * _1pz, pY * pxpz, Yp * _1px, DG_SC_E)
-    DG_ROW(fzm * mxmy, -Zm * _1my, -Zm * _1mx, mZ * mxmy, DG_SC_E)
-    DG_ROW(fzp * mxmy, -Zp * _1my, -Zp * _1mx, pZ * mxmy, DG_SC_E)
-    DG_ROW(fzm * mxpy, -Zm * _1py, Zm * _1mx, mZ * mxpy, DG_SC_E)
-    DG_ROW(fzp * mxpy, -Zp * _1py, Zp * _1mx, pZ * mxpy, DG_SC_E)
-    DG_ROW(fzm * pxmy, Zm * _1my, -Zm * _1px, mZ * pxmy, DG_SC_E)
-    DG_ROW(fzp * pxmy, Zp * _1my, -Zp * _1px, pZ * pxmy, DG_SC_E)
-    DG_ROW(fzm * pxpy, Zm * _1py, Zm * _1px, mZ * pxpy, DG_SC_E)
-    DG_ROW(fzp * pxpy, Zp * _1py, Zp * _1px, pZ * pxpy, DG_SC_E)
-#undef DG_ROW
-#undef DG_SC_C
-#undef DG_SC_E
+    shape_rows(xi[3 * q], xi[3 * q + 1], xi[3 * q + 2], [&](int j, double nj, double d0, double d1, double d2) {
+        Nq[j] = nj;
+        if (Dq) { Dq[3 * j] = d0; Dq[3 * j + 1] = d1; Dq[3 * j + 2] = d2; }
+    });
 }
 
 }  // namespace

@@ -147,10 +147,28 @@ unsigned rs_blocks_for_warps(uint64_t warps) { return (unsigned)((warps * 32 + R
 
 int radix_sort_passes(int key_bits) { return key_bits <= RS_DIGIT_BITS ? 1 : (key_bits + RS_DIGIT_BITS - 1) / RS_DIGIT_BITS; }
 
+uint64_t exclusive_scan_scratch_bytes(uint64_t len) { return rs_align(4 * ((len + RS_SCAN_CHUNK - 1) / RS_SCAN_CHUNK)); }
+
 uint64_t radix_sort_scratch_bytes(uint64_t n)
 {
-    const uint64_t len = (uint64_t)RS_RADIX * rs_tiles(n), chunks = (len + RS_SCAN_CHUNK - 1) / RS_SCAN_CHUNK;
-    return 2 * rs_align(4 * n) + rs_align(4 * len) + rs_align(4 * chunks);
+    const uint64_t len = (uint64_t)RS_RADIX * rs_tiles(n);
+    return 2 * rs_align(4 * n) + rs_align(4 * len) + exclusive_scan_scratch_bytes(len);
+}
+
+cudaError_t exclusive_scan_u32(unsigned* a, uint64_t len, void* scratch, cudaStream_t stream)
+{
+    if (len == 0) return cudaSuccess;
+    const uint64_t chunks = (len + RS_SCAN_CHUNK - 1) / RS_SCAN_CHUNK;
+    unsigned* sums = static_cast<unsigned*>(scratch);
+    cudaError_t e;
+    DG_KERNEL_LAUNCH(rs_chunk_sum_kernel, rs_blocks_for_warps(chunks), RS_THREADS, 0, stream, a, (unsigned long long)len,
+                     (unsigned long long)chunks, sums);
+    if ((e = DG_AFTER_LAUNCH()) != cudaSuccess) return e;
+    DG_KERNEL_LAUNCH(rs_chunk_offsets_kernel, 1, 32, 0, stream, sums, (unsigned long long)chunks);
+    if ((e = DG_AFTER_LAUNCH()) != cudaSuccess) return e;
+    DG_KERNEL_LAUNCH(rs_scan_apply_kernel, rs_blocks_for_warps(chunks), RS_THREADS, 0, stream, a, (unsigned long long)len,
+                     (unsigned long long)chunks, sums);
+    return DG_AFTER_LAUNCH();
 }
 
 cudaError_t radix_sort_pairs(const uint32_t* keys_in, const uint32_t* vals_in, uint64_t n, int key_bits, uint32_t* keys_out,
@@ -158,7 +176,7 @@ cudaError_t radix_sort_pairs(const uint32_t* keys_in, const uint32_t* vals_in, u
 {
     if (key_bits < 1 || key_bits > 32 || n >= (1ull << 32)) return cudaErrorInvalidValue;
     if (n == 0) return cudaSuccess;
-    const uint64_t tiles = rs_tiles(n), len = (uint64_t)RS_RADIX * tiles, chunks = (len + RS_SCAN_CHUNK - 1) / RS_SCAN_CHUNK;
+    const uint64_t tiles = rs_tiles(n), len = (uint64_t)RS_RADIX * tiles;
     char* s = static_cast<char*>(scratch);
     uint32_t* alt_keys = reinterpret_cast<uint32_t*>(s); s += rs_align(4 * n);
     uint32_t* alt_vals = reinterpret_cast<uint32_t*>(s); s += rs_align(4 * n);
@@ -176,14 +194,7 @@ cudaError_t radix_sort_pairs(const uint32_t* keys_in, const uint32_t* vals_in, u
         DG_KERNEL_LAUNCH(rs_hist_kernel, rs_blocks_for_warps(tiles), RS_THREADS, 0, stream, src_k, (unsigned long long)n, shift,
                          (unsigned long long)tiles, hist);
         if ((e = DG_AFTER_LAUNCH()) != cudaSuccess) return e;
-        DG_KERNEL_LAUNCH(rs_chunk_sum_kernel, rs_blocks_for_warps(chunks), RS_THREADS, 0, stream, hist, (unsigned long long)len,
-                         (unsigned long long)chunks, sums);
-        if ((e = DG_AFTER_LAUNCH()) != cudaSuccess) return e;
-        DG_KERNEL_LAUNCH(rs_chunk_offsets_kernel, 1, 32, 0, stream, sums, (unsigned long long)chunks);
-        if ((e = DG_AFTER_LAUNCH()) != cudaSuccess) return e;
-        DG_KERNEL_LAUNCH(rs_scan_apply_kernel, rs_blocks_for_warps(chunks), RS_THREADS, 0, stream, hist, (unsigned long long)len,
-                         (unsigned long long)chunks, sums);
-        if ((e = DG_AFTER_LAUNCH()) != cudaSuccess) return e;
+        if ((e = exclusive_scan_u32(hist, len, sums, stream)) != cudaSuccess) return e;
         DG_KERNEL_LAUNCH(rs_scatter_kernel, rs_blocks_for_warps(tiles), RS_THREADS, 0, stream, src_k, src_v, (unsigned long long)n, shift,
                          (unsigned long long)tiles, hist, dk, dv);
         if ((e = DG_AFTER_LAUNCH()) != cudaSuccess) return e;

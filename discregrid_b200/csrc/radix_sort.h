@@ -1,5 +1,5 @@
 // Launch interface of the device radix sort (radix_sort.cu): a stable LSD sort of (uint32 key, uint32 value) pairs.  Host-callable, no
-// kernel code here.  Used by K10 (k10_distance_grad.cu) to group queries by triangle; written to be reused (DESIGN §7: reduceField).
+// kernel code here.  Used by K10 (k10_distance_grad.cu) to group queries by triangle and by K11 (k11_field_grad.cu) to group them by cell; written to be reused (DESIGN §7: reduceField).
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -23,5 +23,10 @@ uint64_t radix_sort_scratch_bytes(uint64_t n);
 // `stream`; no host synchronisation.  n < 2^32; n == 0 launches nothing.
 cudaError_t radix_sort_pairs(const uint32_t* keys_in, const uint32_t* vals_in, uint64_t n, int key_bits, uint32_t* keys_out,
                              uint32_t* vals_out, void* scratch, cudaStream_t stream);
+
+// bytes of device scratch exclusive_scan_u32 needs for len entries
+uint64_t exclusive_scan_scratch_bytes(uint64_t len);
+// In place: a[i] = a[0] + ... + a[i - 1] (a[0] = 0), the sort's own scan.  The total must be below 2^32.  Queued on `stream`.
+cudaError_t exclusive_scan_u32(unsigned* a, uint64_t len, void* scratch, cudaStream_t stream);
 
 }  // namespace dgb

@@ -25,6 +25,8 @@ that save()/load() stay byte-compatible with the reference's .cdf/.cdm files
                                             -> dg_interpolate_batch_device on torch's current stream (CUDA tensors out, autograd in x)
   interpolate(field_id, x, hessian=True) -> dg_interpolate_hessian_batch[_device] (K2's Hessian mode; second-order autograd in x)
   raycast(field_id, origins, directions) -> dg_field_raycast[_device] (K7: first crossings of a level set along rays and segments)
+  interpolate(field_id, x, coefficients=c) -> dg_field_set_nodes_device + K2 on a trainable field, differentiable in c through
+                                            dg_interpolate_vjp_device (K11, csrc/k11_field_grad.cu)
 
 The reduced calls keep the handle they get from the library until the field's first device use, which builds the interpolation
 field from it on the device (dg_field_create_reduced) instead of uploading the host copy again.
@@ -279,6 +281,68 @@ def _interpolate_hessian_function():
     return _INTERPOLATE_HESSIAN
 
 
+class _TrainableField:
+    """A trainable device field (dg_field_create_trainable) and the token of the interpolate(coefficients=) call whose values it holds.
+    The grid keeps one per field id until its device copies are dropped; the autograd graph of every call made on it keeps it too, so a
+    backward runs on the field its forward used (same topology, still allocated) even after setNodes, addFunction, reduceField or load
+    dropped it from the grid, or after the grid itself was collected.  The handle is destroyed with the last reference."""
+
+    def __init__(self, handle):
+        self.handle, self.holds = handle, None
+        info = (C.c_uint64 * 4)()
+        capi.check(capi.lib.dg_field_info(handle, info))
+        self.n_nodes, self.device = int(info[0]), int(info[3])
+
+    def __del__(self):
+        try:
+            capi.lib.dg_field_destroy(self.handle)
+        except Exception:
+            pass
+
+
+_INTERPOLATE_TRAINABLE = None
+
+
+def _interpolate_trainable_function():
+    """the autograd Function of interpolate(field_id, x, gradient, coefficients=c): phi and grad differentiable in c through K11's VJP, phi in
+    x through K2's gradient and, when the forward ran K2's Hessian mode, grad in x through einsum('na,nab->nb', v, hess).  First order
+    only: a double backward raises."""
+    global _INTERPOLATE_TRAINABLE
+    if _INTERPOLATE_TRAINABLE is None:
+        import torch
+        from torch.autograd.function import once_differentiable
+
+        class InterpolateTrainable(torch.autograd.Function):
+            @staticmethod
+            def forward(ctx, x, c, run, vjp):
+                phi, grad, hess = run(x, c)
+                ctx.set_materialize_grads(False)
+                ctx.vjp = vjp
+                ctx.save_for_backward(x, c, grad, hess)
+                return phi, grad
+
+            @staticmethod
+            @once_differentiable
+            def backward(ctx, grad_phi, grad_grad):
+                x, c, grad, hess = ctx.saved_tensors
+                dx = dc = None
+                if ctx.needs_input_grad[0]:
+                    if grad_phi is not None:
+                        dx = grad_phi[:, None] * grad
+                    if grad_grad is not None:
+                        if hess is None:
+                            raise RuntimeError("interpolate: grad is differentiable in x only when x requires grad at the forward")
+                        v = torch.einsum("na,nab->nb", grad_grad, hess)
+                        dx = v if dx is None else dx + v
+                    if dx is None:
+                        dx = torch.zeros_like(x)
+                if ctx.needs_input_grad[1]:
+                    dc = ctx.vjp(x, c, grad_phi, grad_grad)
+                return dx, dc, None, None
+        _INTERPOLATE_TRAINABLE = InterpolateTrainable
+    return _INTERPOLATE_TRAINABLE
+
+
 def grid_desc(domain_min, domain_max, resolution, cell_size=None, inv_cell_size=None):
     """dg_grid_desc; cell sizes computed like the DiscreteGrid ctor (discrete_grid.hpp:22-29) unless given verbatim."""
     d = capi.GridDesc()
@@ -307,6 +371,7 @@ class CubicLagrangeDiscreteGrid:
         self.m_n_fields = 0
         self._fields = {}          # field_id -> device handle (cache; invalidated by addFunction/load/reduceField)
         self._reduced = {}         # field_id -> the dg_reduced_band its reduced call returned, until its first _device_field (or invalidation)
+        self._trainable = {}       # field_id -> _TrainableField (interpolate(coefficients=))
         self._desc = None
         if isinstance(domain_or_filename, str):
             self.load(domain_or_filename)
@@ -586,7 +651,38 @@ class CubicLagrangeDiscreteGrid:
             capi.lib.dg_field_destroy(h)
         for h in self._reduced.values():
             capi.lib.dg_reduced_band_destroy(h)
-        self._fields, self._reduced = {}, {}
+        self._fields, self._reduced, self._trainable = {}, {}, {}
+
+    def _trainable_field(self, field_id):
+        """the trainable device field of field_id (dg_field_create_trainable of the host members), made at first use; it synchronises"""
+        if field_id not in self._trainable:
+            h = C.c_void_p()
+            nodes, cells, cmap = self.m_nodes[field_id], self.m_cells[field_id], self.m_cell_map[field_id]
+            nodes = np.ascontiguousarray(nodes, np.float64)
+            cells = np.ascontiguousarray(cells, np.uint32)
+            cmap = np.ascontiguousarray(cmap, np.uint32)
+            capi.check(capi.lib.dg_field_create_trainable(C.byref(self._desc), capi.ptr(nodes, capi.F64P), len(nodes), capi.ptr(cells, capi.U32P),
+                                                          len(cells), capi.ptr(cmap, capi.U32P), C.byref(h)))
+            self._trainable[field_id] = _TrainableField(h)
+        return self._trainable[field_id]
+
+    def setNodes(self, field_id, values):
+        """Replaces the node values of field field_id (beyond the reference): values, a numpy array or a tensor of len(m_nodes[field_id])
+        values, is copied to m_nodes[field_id], and the field's device copies are dropped, so that save() and every other method see it.
+        The way to keep a field trained through interpolate(..., coefficients=c): grid.setNodes(field_id, c.detach())."""
+        if hasattr(values, "detach"):
+            values = values.detach().cpu().numpy()
+        values = np.array(values, np.float64, copy=True).reshape(-1)
+        if len(values) != len(self.m_nodes[field_id]):
+            raise ValueError(f"setNodes: field {field_id} has {len(self.m_nodes[field_id])} nodes (got {len(values)})")
+        h = self._fields.pop(field_id, None)
+        if h is not None:
+            capi.lib.dg_field_destroy(h)
+        r = self._reduced.pop(field_id, None)
+        if r is not None:
+            capi.lib.dg_reduced_band_destroy(r)
+        self._trainable.pop(field_id, None)          # destroyed with the last graph that still uses it
+        self.m_nodes[field_id] = values
 
     def __del__(self):
         try:
@@ -595,7 +691,7 @@ class CubicLagrangeDiscreteGrid:
             pass
 
     # ------------------------------------------------------------------ interpolate (cubic_lagrange_discrete_grid.cpp:977-1063)
-    def interpolate(self, field_id_or_x, x=None, gradient=False, hessian=False):
+    def interpolate(self, field_id_or_x, x=None, gradient=False, hessian=False, coefficients=None):
         """interpolate(x) == interpolate(0, x) (discrete_grid.hpp:38-41).  x: (n, 3).  Returns phi[n], or
         (phi[n], grad[n,3]) when gradient=True.  Out-of-domain / removed cell / missing coefficient -> DBL_MAX, grad 0.
         A numpy array (or a CPU tensor) goes through the host pipeline and gives numpy arrays.  A float64 torch tensor (n, 3) or (3,) on
@@ -608,11 +704,25 @@ class CubicLagrangeDiscreteGrid:
         The interpolant is only C0 across cell faces, so on a face hess is that of the cell the point is assigned to.  On CUDA tensors
         that require grad, phi is differentiable to second order and grad to first order (its vector-Jacobian product is
         einsum('na,nab->nb', v, hess)), so torch.autograd.grad(..., create_graph=True) works on phi; hess has no derivative, and a
-        gradient that reaches it (a third derivative of phi) raises RuntimeError."""
+        gradient that reaches it (a third derivative of phi) raises RuntimeError.
+
+        coefficients=c (beyond the reference) interpolates the field with the node values c instead of its own: c is a float64 CUDA tensor
+        of len(m_nodes[field_id]) values on the field's device, and x must be a CUDA tensor.  The grid keeps one trainable device field
+        per field id (dg_field_create_trainable, made at first use from the field's cells and cell map); each call writes c into it and runs
+        K2 on torch's current stream, so phi and grad have the bits interpolate() gives on a field whose m_nodes are c.  phi and grad are
+        differentiable in c (dg_interpolate_vjp_device: the transpose of K2's map, summed in a fixed order, see csrc/k11_field_grad.cu) and
+        phi in x; with gradient=True and x requiring grad the forward runs K2's Hessian mode, so that grad is differentiable in x too.
+        First order only (a double backward raises); hessian=True is refused.  setNodes(field_id, c.detach()) keeps the result."""
         if x is None:
             field_id, x = 0, field_id_or_x
         else:
             field_id = field_id_or_x
+        if coefficients is not None:
+            if hessian:
+                raise ValueError("interpolate: hessian=True is not differentiable in the coefficients; drop one of the two")
+            if not _device.is_device_query(x):
+                raise TypeError("interpolate: coefficients= needs x as a float64 CUDA tensor")
+            return self._interpolate_trainable(field_id, x, gradient, coefficients)
         if _device.is_device_query(x):
             if hessian:
                 return self._interpolate_hessian_device(field_id, x)
@@ -647,6 +757,61 @@ class CubicLagrangeDiscreteGrid:
             phi, grad = _interpolate_function().apply(x, run)
         else:
             phi, grad = run(x, gradient)
+        return (phi, grad) if gradient else phi
+
+    def _interpolate_trainable(self, field_id, x, gradient, c):
+        """interpolate(..., coefficients=c): dg_field_set_nodes_device, then K2, on torch's current stream"""
+        import torch
+        tf = self._trainable_field(field_id)        # the closures below keep it (not the grid) alive for the backward
+        h, n_nodes = tf.handle, tf.n_nodes
+        x = _device.points(x, tf.device, "interpolate")
+        if not isinstance(c, torch.Tensor) or c.dtype != torch.float64:
+            raise TypeError(f"interpolate: coefficients must be a float64 tensor (got {type(c).__name__ if not isinstance(c, torch.Tensor) else c.dtype})")
+        if tuple(c.shape) != (n_nodes,):
+            raise ValueError(f"interpolate: coefficients must have shape ({n_nodes},), got {tuple(c.shape)}")
+        if not capi.EMULATED and (not c.is_cuda or c.device.index != tf.device):
+            raise ValueError(f"interpolate: coefficients are on {c.device} but the field lives on cuda:{tf.device}")
+        c = c.contiguous()
+
+        token = object()                   # this call's pack: the backward repacks c unless the field still holds it
+
+        def hold(cc, again):
+            if again and tf.holds is token:
+                return
+            capi.check(capi.lib.dg_field_set_nodes_device(h, cc.data_ptr(), n_nodes, _device.stream(cc)))
+            tf.holds = token
+
+        x_grad = x.requires_grad and torch.is_grad_enabled()
+        with_hess = gradient and x_grad
+
+        def run(xc, cc):
+            hold(cc, False)
+            n = len(xc)
+            phi = torch.empty(n, dtype=torch.float64, device=xc.device)
+            grad = torch.empty((n, 3), dtype=torch.float64, device=xc.device) if (gradient or x_grad) else None
+            hess = torch.empty((n, 3, 3), dtype=torch.float64, device=xc.device) if with_hess else None
+            if with_hess:
+                capi.check(capi.lib.dg_interpolate_hessian_batch_device(h, xc.data_ptr(), n, phi.data_ptr(), grad.data_ptr(), hess.data_ptr(),
+                                                                        _device.stream(xc)))
+            else:
+                capi.check(capi.lib.dg_interpolate_batch_device(h, xc.data_ptr(), n, phi.data_ptr(), None if grad is None else grad.data_ptr(),
+                                                                _device.stream(xc)))
+            return phi, grad, hess
+
+        def vjp(xc, cc, grad_phi, grad_grad):
+            hold(cc, True)
+            gp = None if grad_phi is None else grad_phi.contiguous()
+            gg = None if grad_grad is None else grad_grad.contiguous()
+            out = torch.empty(n_nodes, dtype=torch.float64, device=cc.device)
+            if gp is None and gg is None:
+                return out.zero_()
+            capi.check(capi.lib.dg_interpolate_vjp_device(h, xc.data_ptr(), len(xc), None if gp is None else gp.data_ptr(),
+                                                          None if gg is None else gg.data_ptr(), out.data_ptr(), _device.stream(xc)))
+            return out
+        if torch.is_grad_enabled() and (x.requires_grad or c.requires_grad):
+            phi, grad = _interpolate_trainable_function().apply(x, c, run, vjp)
+        else:
+            phi, grad, _ = run(x, c)
         return (phi, grad) if gradient else phi
 
     def _interpolate_hessian_device(self, field_id, x):

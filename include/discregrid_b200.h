@@ -289,6 +289,29 @@ DG_API int dg_interpolate_hessian_batch_device(const dg_field* field, const doub
  * N[n x 32], dN[n x 32 x 3] (nullable). */
 DG_API int dg_shape_functions(const double* xi, uint64_t n, double* N, double* dN);
 
+/* ---- K11: trainable fields (beyond the reference) -----------------------------------------------------
+ * dg_field_create_trainable takes dg_field_create's arguments and checks, and makes an ordinary dg_field (interpolate, Hessian, isosurface,
+ * raycast, density and volume maps all take it) that also keeps what it needs to replace its node values and to sum their gradient: its
+ * cell table (when cells is given), the node -> (cell, slot) incidence table and a per-cell DBL_MAX flag (counted in dg_field_info[2]).
+ * Refused when 32 * n_cells_kept >= 2^32.  Synchronises the device.
+ * dg_field_set_nodes[_device] replaces the field's n_nodes node values (n_nodes must be the field's count) and repacks its blocks; the
+ * _device form takes a device pointer and queues the work on `stream` with no host synchronisation.  Refused for a field not made by
+ * dg_field_create_trainable.
+ * dg_interpolate_vjp[_device]: for n points x[n x 3] and the upstream gradients grad_phi[n] of phi and grad_grad[n x 3] of grad (either
+ * may be NULL, not both), grad_nodes[n_nodes] = the gradient with respect to the node values of sum_q grad_phi[q] phi(x_q) +
+ * grad_grad[q] . grad(x_q), with K2's phi and grad on the field's current values.  Queries where K2 returns its sentinel contribute
+ * nothing.  grad_nodes is always overwritten (zeros for n = 0); its bits depend only on the field's topology, x and the upstream gradients
+ * (the summation order is in k11_field_grad.cu).  n must be below 2^32 - 1.  The _device form runs on `stream` with stream-ordered
+ * scratch and no host synchronisation; the host form uploads every input in one piece and returns when grad_nodes is written. */
+DG_API int dg_field_create_trainable(const dg_grid_desc* grid, const double* nodes, uint64_t n_nodes, const uint32_t* cells,
+                                     uint64_t n_cells_kept, const uint32_t* cell_map, dg_field** out);
+DG_API int dg_field_set_nodes(dg_field* field, const double* nodes, uint64_t n_nodes);
+DG_API int dg_field_set_nodes_device(dg_field* field, const double* d_nodes, uint64_t n_nodes, void* stream);
+DG_API int dg_interpolate_vjp(const dg_field* field, const double* x, uint64_t n, const double* grad_phi, const double* grad_grad,
+                              double* grad_nodes);
+DG_API int dg_interpolate_vjp_device(const dg_field* field, const double* d_x, uint64_t n, const double* d_grad_phi, const double* d_grad_grad,
+                                     double* d_grad_nodes, void* stream);
+
 /* ---- K3: GenerateDensityMap node function ---------------------------------------------------------
  * replaces addFunction(density_func, verbose, pred) of cmd/generate_density_map/main.cpp:96-133 with
  * GaussQuadrature::integrate(p=30 -> 16^3 points, gauss_quadrature.cpp:5927-5960) and CubicKernel::W
