@@ -402,6 +402,18 @@ public:
     {
         check(dg_interpolate_vjp_device(trainableField(field_id), d_x, n, d_grad_phi, d_grad_grad, d_grad_nodes, stream));
     }
+    // raycast_vjp: the gradients of the first crossings (t_lo, t_hi from raycast on device arrays) in the origins, the directions and, when
+    // d_grad_nodes is given, the trainable field's node values, for the upstream gradients d_grad_t_lo and d_grad_t_hi [n] (either may be
+    // NULL, not both); every output [n x 3], [n x 3], [nodes] may be NULL (dg_field_raycast_vjp_device; contract in k12_raycast_grad.cu).
+    // With d_grad_nodes the rays must have been cast on trainableField(field_id) holding the same values; without it on deviceField(field_id).
+    void raycast_vjp(unsigned int field_id, std::size_t n, const double* d_origins, const double* d_directions, const double* d_t_lo,
+                     const std::int32_t* d_status, const double* d_grad_t_lo, const double* d_grad_t_hi, double* d_grad_origins,
+                     double* d_grad_directions, double* d_grad_nodes, void* stream = nullptr)
+    {
+        const dg_field* f = d_grad_nodes ? trainableField(field_id) : deviceField(field_id);
+        check(dg_field_raycast_vjp_device(f, n, d_origins, d_directions, d_t_lo, d_status, d_grad_t_lo, d_grad_t_hi, d_grad_origins,
+                                          d_grad_directions, d_grad_nodes, stream));
+    }
     // the trainable field itself, for the library's other calls on its current values (dg_interpolate_batch_device, ...)
     dg_field* trainableField(unsigned int field_id)
     {

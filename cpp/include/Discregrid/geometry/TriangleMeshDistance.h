@@ -169,6 +169,19 @@ public:
                                         d_grad_points, d_grad_vertices, stream) != DG_OK)
             throw std::runtime_error(std::string("TriangleMeshDistance: ") + dg_last_error());
     }
+    // new: the gradients of the first hits (t, barycentric from raycast on device arrays) in the origins, the directions and the vertices,
+    // for the upstream gradients d_grad_t [n] and d_grad_barycentric [n x 3] (either may be NULL, not both), taken at the positions
+    // d_vertices [n_vertices x 3] the rays were cast against; every output [n x 3], [n x 3], [n_vertices x 3] may be NULL, the vertex
+    // gradient is overwritten and summed in a fixed order; on `stream` (dg_mesh_raycast_vjp_device; contract in k12_raycast_grad.cu)
+    void raycast_vjp(size_t n, const double* d_directions, const double* d_t, const int32_t* d_triangle_id, const double* d_barycentric,
+                     const double* d_vertices, const double* d_grad_t, const double* d_grad_barycentric, double* d_grad_origins,
+                     double* d_grad_directions, double* d_grad_vertices, void* stream) const
+    {
+        require();
+        if (dg_mesh_raycast_vjp_device(m_mesh, n, d_directions, d_t, d_triangle_id, d_barycentric, d_vertices, d_grad_t, d_grad_barycentric,
+                                       d_grad_origins, d_grad_directions, d_grad_vertices, stream) != DG_OK)
+            throw std::runtime_error(std::string("TriangleMeshDistance: ") + dg_last_error());
+    }
 
 private:
     dg_mesh* m_mesh = nullptr;

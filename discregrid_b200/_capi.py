@@ -87,6 +87,10 @@ SIGNATURES = {
     "dg_mesh_distance_bary_device": (C.c_int, [_vp, _vp, C.c_uint64, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp]),
     "dg_mesh_distance_vjp": (C.c_int, [_vp, C.c_uint64, _dp, _dp, _dp, _i32p, _dp, _dp, _dp, _dp]),
     "dg_mesh_distance_vjp_device": (C.c_int, [_vp, C.c_uint64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "dg_mesh_raycast_vjp": (C.c_int, [_vp, C.c_uint64, _dp, _dp, _i32p, _dp, _dp, _dp, _dp, _dp, _dp, _dp]),
+    "dg_mesh_raycast_vjp_device": (C.c_int, [_vp, C.c_uint64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "dg_field_raycast_vjp": (C.c_int, [_vp, C.c_uint64, _dp, _dp, _dp, _i32p, _dp, _dp, _dp, _dp, _dp]),
+    "dg_field_raycast_vjp_device": (C.c_int, [_vp, C.c_uint64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "dg_sample_sdf": (C.c_int, [_vp, _gp, C.c_double, C.c_uint64, C.c_uint64, _dp]),
     "dg_add_function_sdf": (C.c_int, [_vp, _gp, C.c_double, _dp, _u32p, _u32p, _dp]),
     "dg_mesh_group_create": (C.c_int, [_vp, C.c_int, C.POINTER(C.c_int), C.POINTER(_vp)]),

@@ -48,6 +48,7 @@
 #include "k9_mesh_raycast.h"
 #include "k10_distance_grad.h"
 #include "k11_field_grad.h"
+#include "k12_raycast_grad.h"
 #include "reduce_field.h"
 #include "obj_reader.h"
 
@@ -3107,6 +3108,181 @@ int dg_mesh_raycast(const dg_mesh* m, const double* o, const double* d, uint64_t
                                                               (int32_t*)out[1], (double*)out[3], (int32_t*)out[2], nullptr, who);
                                });
     });
+}
+
+// ------------------------------------------------------------------------------------------------ K12: ray-cast gradients
+static int mesh_raycast_vjp_check(const dg_mesh* m, uint64_t n, const void* d, const void* t, const void* id, const void* w, const void* V,
+                                  const void* gt, const void* gw, const char* who)
+{
+    if (int rc = mesh_usable(m, who)) return rc;
+    if (n && (!d || !t || !id || !w || !V))
+        return fail(DG_ERR_INVALID, "%s: directions / t / triangle_id / barycentric / vertices is NULL", who);
+    if (!gt && !gw) return fail(DG_ERR_INVALID, "%s: give grad_t, grad_barycentric or both", who);
+    if (n >= (1ull << 32) - 1) return fail(DG_ERR_INVALID, "%s: %llu rays; at most 2^32 - 2 per call", who, (unsigned long long)n);
+    return check_handle_device(m->device, who);
+}
+
+// the triangle ids are checked on the device first (one synchronise); nothing is written unless they are all in [-1, T)
+static int mesh_raycast_vjp_launch(const dg_mesh* m, const K12MeshRays& r, double* d_go, double* d_gd, double* d_gv, cudaStream_t st,
+                                   const char* who)
+{
+    const uint64_t n = r.n, nT = m->host.n_triangles;
+    if (n) {
+        DevBuf<unsigned> bad;
+        DG_CUDA(bad.alloc(1));
+        DG_LAUNCH(k10_launch_check(r.id, n, (int)nT, bad.p, st));
+        unsigned h_bad = 0;
+        DG_CUDA(cudaMemcpyAsync(&h_bad, bad.p, sizeof h_bad, cudaMemcpyDeviceToHost, st));
+        DG_CUDA(cudaStreamSynchronize(st));
+        if (h_bad) return fail(DG_ERR_INVALID, "%s: %u triangle ids outside [-1, %llu)", who, h_bad, (unsigned long long)nT);
+        if (int rc = topo_prepare(const_cast<dg_mesh*>(m))) return rc;      // F, and the incidences of the vertex sums
+    }
+    K10Topo topo;
+    topo.F = m->d_F.p; topo.inc_begin = m->d_inc_begin.p; topo.inc = m->d_inc.p; topo.n_vertices = m->host.n_vertices; topo.n_tri = (int)nT;
+    const size_t bytes = k12_mesh_scratch_bytes(n, (int)nT, d_go != nullptr, d_gv != nullptr);
+    void* scratch = nullptr;
+#ifdef DG_EMU
+    if (bytes) DG_CUDA(cudaMalloc(&scratch, bytes));
+    const cudaError_t e = k12_launch_mesh_vjp(topo, r, d_go, d_gd, d_gv, scratch, st);
+    if (scratch) cudaFree(scratch);
+#else
+    if (bytes) DG_CUDA(cudaMallocAsync(&scratch, bytes, st));
+    const cudaError_t e = k12_launch_mesh_vjp(topo, r, d_go, d_gd, d_gv, scratch, st);
+    if (scratch) cudaFreeAsync(scratch, st);
+#endif
+    DG_LAUNCH(e);
+    return DG_OK;
+}
+
+int dg_mesh_raycast_vjp_device(const dg_mesh* m, uint64_t n, const double* d_directions, const double* d_t, const int32_t* d_triangle_id,
+                               const double* d_barycentric, const double* d_vertices, const double* d_grad_t, const double* d_grad_barycentric,
+                               double* d_grad_origins, double* d_grad_directions, double* d_grad_vertices, void* stream)
+{
+    static const char* who = "dg_mesh_raycast_vjp_device";
+    if (int rc = mesh_raycast_vjp_check(m, n, d_directions, d_t, d_triangle_id, d_barycentric, d_vertices, d_grad_t, d_grad_barycentric, who))
+        return rc;
+    if (!d_grad_origins && !d_grad_directions && !d_grad_vertices) return DG_OK;
+    K12MeshRays r;
+    r.d = d_directions; r.t = d_t; r.id = d_triangle_id; r.bary = d_barycentric; r.V = d_vertices; r.grad_t = d_grad_t;
+    r.grad_bary = d_grad_barycentric; r.n = n;
+    return mesh_raycast_vjp_launch(m, r, d_grad_origins, d_grad_directions, d_grad_vertices, (cudaStream_t)stream, who);
+}
+
+// host arrays: every input uploaded in one piece (the vertex sums span all rays), then the device form on the legacy default stream
+int dg_mesh_raycast_vjp(const dg_mesh* m, uint64_t n, const double* directions, const double* t, const int32_t* triangle_id,
+                        const double* barycentric, const double* vertices, const double* grad_t, const double* grad_barycentric,
+                        double* grad_origins, double* grad_directions, double* grad_vertices)
+{
+    static const char* who = "dg_mesh_raycast_vjp";
+    if (int rc = mesh_raycast_vjp_check(m, n, directions, t, triangle_id, barycentric, vertices, grad_t, grad_barycentric, who)) return rc;
+    if (!grad_origins && !grad_directions && !grad_vertices) return DG_OK;
+    const uint64_t nV = m->host.n_vertices;
+    DevBuf<double> d, tt, w, V, gt, gw, go, gd, gv;
+    DevBuf<int32_t> id;
+    DG_CUDA(d.alloc(3 * n)); DG_CUDA(tt.alloc(n)); DG_CUDA(id.alloc(n)); DG_CUDA(w.alloc(3 * n)); DG_CUDA(V.alloc(n ? 3 * nV : 0));
+    if (grad_t) DG_CUDA(gt.alloc(n));
+    if (grad_barycentric) DG_CUDA(gw.alloc(3 * n));
+    if (grad_origins) DG_CUDA(go.alloc(3 * n));
+    if (grad_directions) DG_CUDA(gd.alloc(3 * n));
+    if (grad_vertices) DG_CUDA(gv.alloc(3 * nV));
+    if (n) {
+        DG_CUDA(cudaMemcpy(d.p, directions, 3 * n * sizeof(double), cudaMemcpyHostToDevice));
+        DG_CUDA(cudaMemcpy(tt.p, t, n * sizeof(double), cudaMemcpyHostToDevice));
+        DG_CUDA(cudaMemcpy(id.p, triangle_id, n * sizeof(int32_t), cudaMemcpyHostToDevice));
+        DG_CUDA(cudaMemcpy(w.p, barycentric, 3 * n * sizeof(double), cudaMemcpyHostToDevice));
+        DG_CUDA(cudaMemcpy(V.p, vertices, 3 * nV * sizeof(double), cudaMemcpyHostToDevice));
+        if (grad_t) DG_CUDA(cudaMemcpy(gt.p, grad_t, n * sizeof(double), cudaMemcpyHostToDevice));
+        if (grad_barycentric) DG_CUDA(cudaMemcpy(gw.p, grad_barycentric, 3 * n * sizeof(double), cudaMemcpyHostToDevice));
+    }
+    K12MeshRays r;
+    r.d = d.p; r.t = tt.p; r.id = id.p; r.bary = w.p; r.V = V.p; r.grad_t = grad_t ? gt.p : nullptr;
+    r.grad_bary = grad_barycentric ? gw.p : nullptr; r.n = n;
+    if (int rc = mesh_raycast_vjp_launch(m, r, go.p, gd.p, gv.p, nullptr, who)) return rc;
+    if (grad_origins && n) DG_CUDA(cudaMemcpy(grad_origins, go.p, 3 * n * sizeof(double), cudaMemcpyDeviceToHost));
+    if (grad_directions && n) DG_CUDA(cudaMemcpy(grad_directions, gd.p, 3 * n * sizeof(double), cudaMemcpyDeviceToHost));
+    if (grad_vertices && nV) DG_CUDA(cudaMemcpy(grad_vertices, gv.p, 3 * nV * sizeof(double), cudaMemcpyDeviceToHost));
+    DG_CUDA(cudaDeviceSynchronize());
+    return DG_OK;
+}
+
+static int field_raycast_vjp_check(const dg_field* f, uint64_t n, const void* o, const void* d, const void* t_lo, const void* status,
+                                   const void* glo, const void* ghi, const void* grad_nodes, const char* who)
+{
+    if (!f) return fail(DG_ERR_INVALID, "%s: field is NULL", who);
+    if (n && (!o || !d || !t_lo || !status)) return fail(DG_ERR_INVALID, "%s: origins / directions / t_lo / status is NULL", who);
+    if (!glo && !ghi) return fail(DG_ERR_INVALID, "%s: give grad_t_lo, grad_t_hi or both", who);
+    if (grad_nodes && !f->trainable)
+        return fail(DG_ERR_INVALID, "%s: grad_nodes needs a field made by dg_field_create_trainable", who);
+    if (n >= (1ull << 32) - 1) return fail(DG_ERR_INVALID, "%s: %llu rays; at most 2^32 - 2 per call", who, (unsigned long long)n);
+    return check_handle_device(f->device, who);
+}
+
+// the scratch is stream-ordered: allocated and released on `st`, so the call queues everything and returns
+static int field_raycast_vjp_launch(const dg_field* f, const K12FieldRays& r, double* d_go, double* d_gd, double* d_gn, cudaStream_t st)
+{
+    K11Field kf;
+    kf.f = f->dev; kf.inc_begin = f->d_inc_begin.p; kf.inc = f->d_inc.p; kf.has_max = f->d_has_max.p;
+    kf.n_nodes = f->n_nodes; kf.n_cells_kept = f->n_cells_kept;
+    const size_t bytes = k12_field_scratch_bytes(r.n, f->n_cells_kept, d_gn != nullptr);
+    void* scratch = nullptr;
+#ifdef DG_EMU
+    if (bytes) DG_CUDA(cudaMalloc(&scratch, bytes));
+    const cudaError_t e = k12_launch_field_vjp(f->dev, f->trainable ? &kf : nullptr, r, d_go, d_gd, d_gn, scratch, st);
+    if (scratch) cudaFree(scratch);
+#else
+    if (bytes) DG_CUDA(cudaMallocAsync(&scratch, bytes, st));
+    const cudaError_t e = k12_launch_field_vjp(f->dev, f->trainable ? &kf : nullptr, r, d_go, d_gd, d_gn, scratch, st);
+    if (scratch) cudaFreeAsync(scratch, st);
+#endif
+    DG_LAUNCH(e);
+    return DG_OK;
+}
+
+int dg_field_raycast_vjp_device(const dg_field* f, uint64_t n, const double* d_origins, const double* d_directions, const double* d_t_lo,
+                                const int32_t* d_status, const double* d_grad_t_lo, const double* d_grad_t_hi, double* d_grad_origins,
+                                double* d_grad_directions, double* d_grad_nodes, void* stream)
+{
+    static const char* who = "dg_field_raycast_vjp_device";
+    if (int rc = field_raycast_vjp_check(f, n, d_origins, d_directions, d_t_lo, d_status, d_grad_t_lo, d_grad_t_hi, d_grad_nodes, who)) return rc;
+    if (!d_grad_origins && !d_grad_directions && !d_grad_nodes) return DG_OK;
+    K12FieldRays r;
+    r.o = d_origins; r.d = d_directions; r.t_lo = d_t_lo; r.status = d_status; r.grad_t_lo = d_grad_t_lo; r.grad_t_hi = d_grad_t_hi; r.n = n;
+    return field_raycast_vjp_launch(f, r, d_grad_origins, d_grad_directions, d_grad_nodes, (cudaStream_t)stream);
+}
+
+// host arrays: every input uploaded in one piece (the node sums span all rays), then the device form on the legacy default stream
+int dg_field_raycast_vjp(const dg_field* f, uint64_t n, const double* origins, const double* directions, const double* t_lo,
+                         const int32_t* status, const double* grad_t_lo, const double* grad_t_hi, double* grad_origins,
+                         double* grad_directions, double* grad_nodes)
+{
+    static const char* who = "dg_field_raycast_vjp";
+    if (int rc = field_raycast_vjp_check(f, n, origins, directions, t_lo, status, grad_t_lo, grad_t_hi, grad_nodes, who)) return rc;
+    if (!grad_origins && !grad_directions && !grad_nodes) return DG_OK;
+    DevBuf<double> o, d, tl, glo, ghi, go, gd, gn;
+    DevBuf<int32_t> st;
+    DG_CUDA(o.alloc(3 * n)); DG_CUDA(d.alloc(3 * n)); DG_CUDA(tl.alloc(n)); DG_CUDA(st.alloc(n));
+    if (grad_t_lo) DG_CUDA(glo.alloc(n));
+    if (grad_t_hi) DG_CUDA(ghi.alloc(n));
+    if (grad_origins) DG_CUDA(go.alloc(3 * n));
+    if (grad_directions) DG_CUDA(gd.alloc(3 * n));
+    if (grad_nodes) DG_CUDA(gn.alloc(f->n_nodes));
+    if (n) {
+        DG_CUDA(cudaMemcpy(o.p, origins, 3 * n * sizeof(double), cudaMemcpyHostToDevice));
+        DG_CUDA(cudaMemcpy(d.p, directions, 3 * n * sizeof(double), cudaMemcpyHostToDevice));
+        DG_CUDA(cudaMemcpy(tl.p, t_lo, n * sizeof(double), cudaMemcpyHostToDevice));
+        DG_CUDA(cudaMemcpy(st.p, status, n * sizeof(int32_t), cudaMemcpyHostToDevice));
+        if (grad_t_lo) DG_CUDA(cudaMemcpy(glo.p, grad_t_lo, n * sizeof(double), cudaMemcpyHostToDevice));
+        if (grad_t_hi) DG_CUDA(cudaMemcpy(ghi.p, grad_t_hi, n * sizeof(double), cudaMemcpyHostToDevice));
+    }
+    K12FieldRays r;
+    r.o = o.p; r.d = d.p; r.t_lo = tl.p; r.status = st.p; r.grad_t_lo = grad_t_lo ? glo.p : nullptr; r.grad_t_hi = grad_t_hi ? ghi.p : nullptr;
+    r.n = n;
+    if (int rc = field_raycast_vjp_launch(f, r, go.p, gd.p, gn.p, nullptr)) return rc;
+    if (grad_origins && n) DG_CUDA(cudaMemcpy(grad_origins, go.p, 3 * n * sizeof(double), cudaMemcpyDeviceToHost));
+    if (grad_directions && n) DG_CUDA(cudaMemcpy(grad_directions, gd.p, 3 * n * sizeof(double), cudaMemcpyDeviceToHost));
+    if (grad_nodes && f->n_nodes) DG_CUDA(cudaMemcpy(grad_nodes, gn.p, f->n_nodes * sizeof(double), cudaMemcpyDeviceToHost));
+    DG_CUDA(cudaDeviceSynchronize());
+    return DG_OK;
 }
 
 int dg_obj_read(const char* path, double** vertices, uint64_t* n_vertices, uint32_t** triangles, uint64_t* n_triangles)

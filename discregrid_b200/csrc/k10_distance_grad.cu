@@ -30,6 +30,7 @@
 //   levels   : for S = 1, 32, 1024, ... < n, one thread per sorted position whose offset in its segment is a multiple of 32 S sums the
 //              <= 32 entries S apart in place with the tree.  After the last level a segment's sum sits at its first position.
 //   vertices : one thread per vertex over its incidences.
+// The passes after the point pass are k10_launch_scatter, which K12 (k12_raycast_grad.cu) calls with its own per-ray gradients and keys.
 #include "k10_distance_grad.h"
 #include "radix_sort.h"
 #include "dg_launch.h"
@@ -146,13 +147,19 @@ cudaError_t k10_launch_check(const int32_t* d_tri, uint64_t n, int n_tri, unsign
     return DG_AFTER_LAUNCH();
 }
 
+uint64_t k10_scatter_scratch_bytes(uint64_t n, int n_tri)
+{
+    if (n == 0) return 0;
+    uint64_t b = 2 * k10_align(4 * n) + radix_sort_scratch_bytes(n);  // sorted keys, sorted query ids, the sort's own
+    b += k10_align(72 * n) + 2 * k10_align(4 * ((uint64_t)n_tri + 1));
+    return b;
+}
+
 uint64_t k10_scratch_bytes(uint64_t n, int n_tri, bool grad_points, bool grad_vertices)
 {
     if (!grad_vertices || n == 0) return 0;
     uint64_t b = grad_points ? 0 : k10_align(24 * n);                 // gx when grad_points is not wanted
-    b += 3 * k10_align(4 * n) + radix_sort_scratch_bytes(n);          // keys, sorted keys, sorted query ids, the sort's own
-    b += k10_align(72 * n) + 2 * k10_align(4 * ((uint64_t)n_tri + 1));
-    return b;
+    return b + k10_align(4 * n) + k10_scatter_scratch_bytes(n, n_tri); // keys, then the scatter's
 }
 
 cudaError_t k10_launch_vjp(const K10Topo& topo, const K10Query& q, double* d_grad_points, double* d_grad_vertices, void* scratch,
@@ -171,6 +178,18 @@ cudaError_t k10_launch_vjp(const K10Topo& topo, const K10Query& q, double* d_gra
     double* gx = d_grad_points;
     if (!gx) { gx = reinterpret_cast<double*>(s); s += k10_align(24 * n); }
     uint32_t* key = reinterpret_cast<uint32_t*>(s); s += k10_align(4 * n);
+    DG_KERNEL_LAUNCH(k10_point_kernel, k10_blocks(n), K10_THREADS, 0, stream, q, gx, key);
+    if ((e = DG_AFTER_LAUNCH()) != cudaSuccess) return e;
+    return k10_launch_scatter(topo, n, gx, key, q.bary, d_grad_vertices, s, stream);
+}
+
+cudaError_t k10_launch_scatter(const K10Topo& topo, uint64_t n, const double* gx, const uint32_t* key, const double* bary,
+                               double* d_grad_vertices, void* scratch, cudaStream_t stream)
+{
+    cudaError_t e;
+    if (n == 0) return cudaMemsetAsync(d_grad_vertices, 0, 3 * topo.n_vertices * sizeof(double), stream);
+    if (n >= (1ull << 32) - 1) return cudaErrorInvalidValue;           // sorted positions are uint32, 0xffffffff marks an empty segment
+    char* s = static_cast<char*>(scratch);
     uint32_t* skey = reinterpret_cast<uint32_t*>(s); s += k10_align(4 * n);
     uint32_t* sval = reinterpret_cast<uint32_t*>(s); s += k10_align(4 * n);
     void* sort_scratch = s; s += radix_sort_scratch_bytes(n);
@@ -178,10 +197,8 @@ cudaError_t k10_launch_vjp(const K10Topo& topo, const K10Query& q, double* d_gra
     uint32_t* seg_begin = reinterpret_cast<uint32_t*>(s); s += k10_align(4 * ((uint64_t)topo.n_tri + 1));
     uint32_t* seg_end = reinterpret_cast<uint32_t*>(s);
     const unsigned long long nn = n;
-    DG_KERNEL_LAUNCH(k10_point_kernel, k10_blocks(n), K10_THREADS, 0, stream, q, gx, key);
-    if ((e = DG_AFTER_LAUNCH()) != cudaSuccess) return e;
     if ((e = radix_sort_pairs(key, nullptr, n, k10_key_bits(topo.n_tri), skey, sval, sort_scratch, stream)) != cudaSuccess) return e;
-    DG_KERNEL_LAUNCH(k10_contrib_kernel, k10_blocks(n), K10_THREADS, 0, stream, nn, skey, sval, gx, q.bary, c);
+    DG_KERNEL_LAUNCH(k10_contrib_kernel, k10_blocks(n), K10_THREADS, 0, stream, nn, skey, sval, gx, bary, c);
     if ((e = DG_AFTER_LAUNCH()) != cudaSuccess) return e;
     if ((e = cudaMemsetAsync(seg_begin, 0xff, 4 * ((size_t)topo.n_tri + 1), stream)) != cudaSuccess) return e;
     DG_KERNEL_LAUNCH(k10_segment_kernel, k10_blocks(n), K10_THREADS, 0, stream, nn, skey, seg_begin, seg_end);

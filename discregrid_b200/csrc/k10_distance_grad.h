@@ -38,4 +38,11 @@ uint64_t k10_scratch_bytes(uint64_t n, int n_tri, bool grad_points, bool grad_ve
 cudaError_t k10_launch_vjp(const K10Topo& topo, const K10Query& q, double* d_grad_points, double* d_grad_vertices, void* scratch,
                            cudaStream_t stream);
 
+// The vertex passes of k10_launch_vjp on their own (sort, contributions, segments, levels, vertices), for a caller that computed the
+// per-query gradient itself (K12's ray casts): query q with key[q] = t + 1 (0: takes no part) gives -(bary[q][i] * g[q][k]) to slot i of
+// triangle t, summed as K10's contract states.  grad_vertices [nV][3] is overwritten; n < 2^32 - 1.  Queued on `stream`.
+uint64_t k10_scatter_scratch_bytes(uint64_t n, int n_tri);
+cudaError_t k10_launch_scatter(const K10Topo& topo, uint64_t n, const double* d_g, const uint32_t* d_key, const double* d_bary,
+                               double* d_grad_vertices, void* scratch, cudaStream_t stream);
+
 }  // namespace dgb

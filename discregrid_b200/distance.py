@@ -72,6 +72,51 @@ def _mesh_distance_function():
     return _MESH_DISTANCE
 
 
+_MESH_RAYCAST = None
+
+
+def _mesh_raycast_function():
+    """the autograd Function of the mesh ray cast on CUDA tensors (K12): t and barycentric differentiable in the origins, the directions and
+    the vertex positions, first order only.  The backward differentiates at the positions the forward cast against: V when it was given,
+    otherwise the positions the mesh last took from construct or refit (uploaded at the first backward that needs them)."""
+    global _MESH_RAYCAST
+    if _MESH_RAYCAST is None:
+        import torch
+        from torch.autograd.function import once_differentiable
+
+        class MeshRaycast(torch.autograd.Function):
+            @staticmethod
+            def forward(ctx, o, d, V, md, t_min, t_max):
+                t, tid, bary, st = md._raycast_device(o, d, t_min, t_max)
+                ctx.mark_non_differentiable(tid, st)
+                ctx.set_materialize_grads(False)
+                ctx.save_for_backward(d, t, tid, bary, V)
+                ctx.md, ctx.positions = md, (None if V is not None else md._positions)
+                return t, tid, bary, st
+
+            @staticmethod
+            @once_differentiable
+            def backward(ctx, grad_t, _grad_tid, grad_bary, _grad_status):
+                d, t, tid, bary, V = ctx.saved_tensors
+                md = ctx.md
+                need_o, need_d, need_v = ctx.needs_input_grad[0], ctx.needs_input_grad[1], ctx.needs_input_grad[2]
+                if grad_t is None and grad_bary is None:
+                    return None, None, None, None, None, None
+                n = len(d)
+                pos = V.detach().contiguous() if V is not None else md._positions_on(ctx.positions, d.device)
+                go = torch.empty((n, 3), dtype=torch.float64, device=d.device) if need_o else None
+                gd = torch.empty((n, 3), dtype=torch.float64, device=d.device) if need_d else None
+                gv = torch.empty((md.n_vertices, 3), dtype=torch.float64, device=d.device) if need_v else None
+                gt = None if grad_t is None else grad_t.to(torch.float64).contiguous()
+                gb = None if grad_bary is None else grad_bary.to(torch.float64).contiguous()
+                ptr = lambda a: None if a is None else a.data_ptr()
+                capi.check(capi.lib.dg_mesh_raycast_vjp_device(md.handle, n, d.data_ptr(), t.data_ptr(), tid.data_ptr(), bary.data_ptr(),
+                                                               pos.data_ptr(), ptr(gt), ptr(gb), ptr(go), ptr(gd), ptr(gv), _device.stream(d)))
+                return go, gd, gv, None, None, None
+        _MESH_RAYCAST = MeshRaycast
+    return _MESH_RAYCAST
+
+
 class TriangleMeshDistance:
     def __init__(self, mesh_or_vertices=None, triangles=None):
         self._h = None
@@ -93,6 +138,7 @@ class TriangleMeshDistance:
         self._h = h
         self._sign_mode = "pseudonormal"
         self.n_vertices, self.n_triangles = len(V), len(F)
+        self._positions, self._positions_dev = V, None        # what raycast's backward differentiates at when it is not given V
         return self
 
     @property
@@ -166,11 +212,13 @@ class TriangleMeshDistance:
         if _device.is_device_query(vertices):
             x = _device.points(vertices, self.device, "refit")
             capi.check(capi.lib.dg_mesh_refit_device(self.handle, x.data_ptr(), len(x), _device.stream(x)))
+            self._positions, self._positions_dev = x.detach(), None
             return self
         V = np.ascontiguousarray(vertices, dtype=np.float64)
         if V.ndim != 2 or V.shape[1] != 3:
             raise ValueError(f"refit: vertices must have shape (n_vertices, 3) (got {V.shape})")
         capi.check(capi.lib.dg_mesh_refit(self.handle, capi.ptr(V, capi.F64P), len(V)))
+        self._positions, self._positions_dev = V, None
         return self
 
     @property
@@ -194,29 +242,34 @@ class TriangleMeshDistance:
         capi.check(capi.lib.dg_mesh_winding_number(self.handle, capi.ptr(x, capi.F64P), len(x), beta, capi.ptr(w, capi.F64P)))
         return w
 
-    def raycast(self, origins, directions, t_min=0.0, t_max=math.inf):
+    def raycast(self, origins, directions, t_min=0.0, t_max=math.inf, vertices=None):
         """The first hit of each ray on the mesh's triangles (beyond the reference; dg_mesh_raycast, contract in csrc/k9_mesh_raycast.cu and
         DESIGN §3).  origins and directions (n, 3) or (3,); t in [t_min, t_max].  A segment x0 -> x1 (continuous collision detection of a
         step against a deforming mesh: refit, then cast) is raycast(x0, x1 - x0, 0.0, 1.0).  The test is watertight: a ray through a shared
         edge or vertex is not lost.  Returns (t, triangle_id, barycentric, status): the least t (the lower id wins a tie), the original
         triangle index, the weights (n, 3) of that triangle's vertices 0, 1, 2, and DG_RAY_ENTER (1: crossing from the outside of an
         outward-oriented mesh) or DG_RAY_LEAVE (2); a miss gives DG_RAY_MISS (0), t = inf, id -1 and NaN weights.  numpy inputs return numpy
-        arrays; float64 CUDA tensors on the mesh's device stay there and the cast runs on torch's current stream.  No autograd."""
+        arrays; float64 CUDA tensors on the mesh's device stay there and the cast runs on torch's current stream.
+
+        Gradients (K12, contract in csrc/k12_raycast_grad.cu): on CUDA tensors under grad mode, t and barycentric are differentiable in the
+        origins and the directions, and in the vertex positions: vertices=V, a float64 CUDA tensor (n_vertices, 3) on the mesh's device,
+        first refits the mesh to V.detach() -- a side effect that stays, as refit(V) -- and makes the hit differentiable in V.  The backward
+        differentiates at the positions the forward cast against (V, or else those the mesh last took from construct or refit), so a refit
+        between forward and backward does not change it.  A miss, or a ray parallel to its triangle, gets 0; the vertex gradient is summed
+        in a fixed order, the same bits on every run.  triangle_id and status carry no gradient.  First order only: a double backward
+        raises.  A depth loss is loss(t); the time of impact of a step x0 -> x1 is raycast(x0, x1 - x0, 0, 1)[0]."""
         t_min, t_max = float(t_min), float(t_max)
+        if vertices is not None:
+            self._refit_to(vertices, "raycast")
         if _device.is_device_query(origins) or _device.is_device_query(directions):
             import torch
             o = _device.points(origins, self.device, "raycast")
             d = _device.points(directions, self.device, "raycast")
             if o.shape != d.shape:
                 raise ValueError(f"raycast: origins {tuple(o.shape)} and directions {tuple(d.shape)} differ in shape")
-            n = len(o)
-            t = torch.empty(n, dtype=torch.float64, device=o.device)
-            tid = torch.empty(n, dtype=torch.int32, device=o.device)
-            bary = torch.empty((n, 3), dtype=torch.float64, device=o.device)
-            st = torch.empty(n, dtype=torch.int32, device=o.device)
-            capi.check(capi.lib.dg_mesh_raycast_device(self.handle, o.data_ptr(), d.data_ptr(), n, t_min, t_max, t.data_ptr(), tid.data_ptr(),
-                                                       bary.data_ptr(), st.data_ptr(), _device.stream(o)))
-            return t, tid, bary, st
+            if torch.is_grad_enabled() and (o.requires_grad or d.requires_grad or (vertices is not None and vertices.requires_grad)):
+                return _mesh_raycast_function().apply(o, d, vertices, self, t_min, t_max)
+            return self._raycast_device(o, d, t_min, t_max)
         o = np.ascontiguousarray(origins, dtype=np.float64).reshape(-1, 3)
         d = np.ascontiguousarray(directions, dtype=np.float64).reshape(-1, 3)
         if o.shape != d.shape:
@@ -226,6 +279,32 @@ class TriangleMeshDistance:
         capi.check(capi.lib.dg_mesh_raycast(self.handle, capi.ptr(o, capi.F64P), capi.ptr(d, capi.F64P), n, t_min, t_max, capi.ptr(t, capi.F64P),
                                             capi.ptr(tid, capi.I32P), capi.ptr(bary, capi.F64P), capi.ptr(st, capi.I32P)))
         return t, tid, bary, st
+
+    def _raycast_device(self, o, d, t_min, t_max):
+        """dg_mesh_raycast_device on torch's current stream; o, d contiguous float64 (n, 3) tensors on the mesh's device"""
+        import torch
+        n = len(o)
+        t = torch.empty(n, dtype=torch.float64, device=o.device)
+        tid = torch.empty(n, dtype=torch.int32, device=o.device)
+        bary = torch.empty((n, 3), dtype=torch.float64, device=o.device)
+        st = torch.empty(n, dtype=torch.int32, device=o.device)
+        capi.check(capi.lib.dg_mesh_raycast_device(self.handle, o.data_ptr(), d.data_ptr(), n, t_min, t_max, t.data_ptr(), tid.data_ptr(),
+                                                   bary.data_ptr(), st.data_ptr(), _device.stream(o)))
+        return t, tid, bary, st
+
+    def _positions_on(self, positions, device):
+        """positions (what construct or refit last took) as a contiguous float64 tensor on `device`; a host array is uploaded once, at the
+        first backward that needs it, and kept while it stays the mesh's positions"""
+        import torch
+        if isinstance(positions, torch.Tensor):
+            return positions.to(device=device, dtype=torch.float64).contiguous()
+        cached = self._positions_dev
+        if cached is not None and cached[0] is positions:
+            return cached[1]
+        dev = torch.from_numpy(np.ascontiguousarray(positions, np.float64).reshape(-1, 3)).to(device)
+        if positions is self._positions:
+            self._positions_dev = (positions, dev)
+        return dev
 
     def _query_device(self, points, signed):
         """the CUDA-tensor route: dg_mesh_distance_device on torch's current stream, asynchronous like a torch op"""

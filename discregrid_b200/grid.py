@@ -343,6 +343,54 @@ def _interpolate_trainable_function():
     return _INTERPOLATE_TRAINABLE
 
 
+_FIELD_RAYCAST = None
+
+
+def _field_raycast_function():
+    """the autograd Function of the level-set ray cast on CUDA tensors (K12): t_lo and t_hi differentiable in the origins, the directions
+    and, with coefficients=c, in c, through the implicit function theorem at the crossing.  First order only: a double backward raises."""
+    global _FIELD_RAYCAST
+    if _FIELD_RAYCAST is None:
+        import torch
+        from torch.autograd.function import once_differentiable
+
+        class FieldRaycast(torch.autograd.Function):
+            @staticmethod
+            def forward(ctx, o, d, c, run, vjp):
+                t_lo, t_hi, status = run(o, d, c)
+                ctx.mark_non_differentiable(status)
+                ctx.set_materialize_grads(False)
+                ctx.vjp = vjp
+                ctx.save_for_backward(o, d, c, t_lo, status)
+                return t_lo, t_hi, status
+
+            @staticmethod
+            @once_differentiable
+            def backward(ctx, grad_t_lo, grad_t_hi, _grad_status):
+                o, d, c, t_lo, status = ctx.saved_tensors
+                if grad_t_lo is None and grad_t_hi is None:
+                    return None, None, None, None, None
+                go, gd, gc = ctx.vjp(o, d, c, t_lo, status, grad_t_lo, grad_t_hi, ctx.needs_input_grad[:3])
+                return go, gd, gc, None, None
+        _FIELD_RAYCAST = FieldRaycast
+    return _FIELD_RAYCAST
+
+
+def _raycast_vjp(h, o, d, t_lo, status, g_lo, g_hi, want_o, want_d, n_nodes):
+    """dg_field_raycast_vjp_device on torch's current stream: (grad_origins, grad_directions, grad_nodes), each None unless wanted"""
+    import torch
+    n = len(o)
+    go = torch.empty((n, 3), dtype=torch.float64, device=o.device) if want_o else None
+    gd = torch.empty((n, 3), dtype=torch.float64, device=o.device) if want_d else None
+    gn = torch.empty(n_nodes, dtype=torch.float64, device=o.device) if n_nodes is not None else None
+    glo = None if g_lo is None else g_lo.to(torch.float64).contiguous()
+    ghi = None if g_hi is None else g_hi.to(torch.float64).contiguous()
+    ptr = lambda a: None if a is None else a.data_ptr()
+    capi.check(capi.lib.dg_field_raycast_vjp_device(h, n, o.data_ptr(), d.data_ptr(), t_lo.data_ptr(), status.data_ptr(), ptr(glo), ptr(ghi),
+                                                    ptr(go), ptr(gd), ptr(gn), _device.stream(o)))
+    return go, gd, gn
+
+
 def grid_desc(domain_min, domain_max, resolution, cell_size=None, inv_cell_size=None):
     """dg_grid_desc; cell sizes computed like the DiscreteGrid ctor (discrete_grid.hpp:22-29) unless given verbatim."""
     d = capi.GridDesc()
@@ -872,7 +920,7 @@ class CubicLagrangeDiscreteGrid:
         finally:
             capi.lib.dg_isosurface_destroy(s)
 
-    def raycast(self, field_id, origins, directions, iso=0.0, t_min=0.0, t_max=math.inf):
+    def raycast(self, field_id, origins, directions, iso=0.0, t_min=0.0, t_max=math.inf, coefficients=None):
         """The first crossing of {phi = iso} along rays x(t) = origin + t * direction, t in [t_min, t_max] clipped to the domain, on the
         field's GPU (dg_field_raycast; the contract is in csrc/k7_raycast.cu and DESIGN §3).  The crossing is isolated cell by cell with
         Bernstein bounds of the interpolant along the line, so features thinner than any step are not missed, on any field (SDF, density
@@ -882,9 +930,21 @@ class CubicLagrangeDiscreteGrid:
         Returns (t_lo, t_hi, status): the final bisection bracket and DG_RAY_ENTER (1: phi(x(t_lo)) >= iso > phi(x(t_hi))), DG_RAY_LEAVE (2:
         the reverse; a ray that starts inside reports its first LEAVE) or DG_RAY_MISS (0, with t_lo = t_hi = inf).  numpy inputs (n, 3)
         give numpy arrays (float64, float64, int32).  float64 CUDA tensors (n, 3) on the field's device stay there: the cast runs on
-        torch's current stream and returns CUDA tensors.  Not differentiable.  A reduced field's kept device handle is used directly."""
-        h = self._device_field(field_id)
+        torch's current stream and returns CUDA tensors.  A reduced field's kept device handle is used directly.
+
+        Gradients (K12, contract in csrc/k12_raycast_grad.cu): on CUDA tensors under grad mode, t_lo and t_hi are differentiable in the
+        origins and the directions, by the implicit function theorem at x_c = x(t_lo): dt = -(grad phi . dx) / (grad phi . d), with both
+        ends of the bracket following the crossing.  coefficients=c casts against the field with the node values c instead of its own, on
+        the trainable device field interpolate(coefficients=) uses (same rules: c a float64 CUDA tensor of len(m_nodes[field_id]) values),
+        and makes t_lo and t_hi differentiable in c as well, summed in a fixed order (K11).  A miss, a crossing at DBL_MAX or a ray tangent
+        to the level set gets 0.  status carries no gradient.  First order only: a double backward raises.  Not differentiable in iso,
+        t_min or t_max."""
         iso, t_min, t_max = float(iso), float(t_min), float(t_max)
+        if coefficients is not None:
+            if not (_device.is_device_query(origins) and _device.is_device_query(directions)):
+                raise TypeError("raycast: coefficients= needs origins and directions as float64 CUDA tensors")
+            return self._raycast_trainable(field_id, origins, directions, iso, t_min, t_max, coefficients)
+        h = self._device_field(field_id)
         if _device.is_device_query(origins) or _device.is_device_query(directions):
             import torch
             info = (C.c_uint64 * 4)()
@@ -893,13 +953,19 @@ class CubicLagrangeDiscreteGrid:
             d = _device.points(directions, int(info[3]), "raycast")
             if o.shape != d.shape:
                 raise ValueError(f"raycast: origins {tuple(o.shape)} and directions {tuple(d.shape)} differ in shape")
-            n = len(o)
-            t_lo = torch.empty(n, dtype=torch.float64, device=o.device)
-            t_hi = torch.empty(n, dtype=torch.float64, device=o.device)
-            status = torch.empty(n, dtype=torch.int32, device=o.device)
-            capi.check(capi.lib.dg_field_raycast_device(h, o.data_ptr(), d.data_ptr(), n, iso, t_min, t_max, t_lo.data_ptr(), t_hi.data_ptr(),
-                                                        status.data_ptr(), _device.stream(o)))
-            return t_lo, t_hi, status
+
+            def run(oc, dc, _c):
+                return self._raycast_device(h, oc, dc, iso, t_min, t_max)
+
+            def vjp(oc, dc, _c, t_lo, status, g_lo, g_hi, needs):
+                if self._fields.get(field_id) is not h:
+                    raise RuntimeError(f"raycast: field {field_id} was replaced since the forward (setNodes, addFunction, reduceField or load); "
+                                       "cast with coefficients= to keep a differentiable field")
+                go, gd, _ = _raycast_vjp(h, oc, dc, t_lo, status, g_lo, g_hi, needs[0], needs[1], None)
+                return go, gd, None
+            if torch.is_grad_enabled() and (o.requires_grad or d.requires_grad):
+                return _field_raycast_function().apply(o, d, None, run, vjp)
+            return run(o, d, None)
         o = np.ascontiguousarray(origins, np.float64).reshape(-1, 3)
         d = np.ascontiguousarray(directions, np.float64).reshape(-1, 3)
         if o.shape != d.shape:
@@ -908,6 +974,54 @@ class CubicLagrangeDiscreteGrid:
         capi.check(capi.lib.dg_field_raycast(h, capi.ptr(o, capi.F64P), capi.ptr(d, capi.F64P), len(o), iso, t_min, t_max,
                                              capi.ptr(t_lo, capi.F64P), capi.ptr(t_hi, capi.F64P), capi.ptr(status, capi.I32P)))
         return t_lo, t_hi, status
+
+    @staticmethod
+    def _raycast_device(h, o, d, iso, t_min, t_max):
+        """dg_field_raycast_device on torch's current stream; o, d contiguous float64 (n, 3) tensors on the field's device"""
+        import torch
+        n = len(o)
+        t_lo = torch.empty(n, dtype=torch.float64, device=o.device)
+        t_hi = torch.empty(n, dtype=torch.float64, device=o.device)
+        status = torch.empty(n, dtype=torch.int32, device=o.device)
+        capi.check(capi.lib.dg_field_raycast_device(h, o.data_ptr(), d.data_ptr(), n, iso, t_min, t_max, t_lo.data_ptr(), t_hi.data_ptr(),
+                                                    status.data_ptr(), _device.stream(o)))
+        return t_lo, t_hi, status
+
+    def _raycast_trainable(self, field_id, origins, directions, iso, t_min, t_max, c):
+        """raycast(..., coefficients=c): dg_field_set_nodes_device, then K7, on torch's current stream (the route of interpolate(coefficients=))"""
+        import torch
+        tf = self._trainable_field(field_id)        # the closures below keep it (not the grid) alive for the backward
+        h, n_nodes = tf.handle, tf.n_nodes
+        o = _device.points(origins, tf.device, "raycast")
+        d = _device.points(directions, tf.device, "raycast")
+        if o.shape != d.shape:
+            raise ValueError(f"raycast: origins {tuple(o.shape)} and directions {tuple(d.shape)} differ in shape")
+        if not isinstance(c, torch.Tensor) or c.dtype != torch.float64:
+            raise TypeError(f"raycast: coefficients must be a float64 tensor (got {type(c).__name__ if not isinstance(c, torch.Tensor) else c.dtype})")
+        if tuple(c.shape) != (n_nodes,):
+            raise ValueError(f"raycast: coefficients must have shape ({n_nodes},), got {tuple(c.shape)}")
+        if not capi.EMULATED and (not c.is_cuda or c.device.index != tf.device):
+            raise ValueError(f"raycast: coefficients are on {c.device} but the field lives on cuda:{tf.device}")
+        c = c.contiguous()
+
+        token = object()                   # this call's pack: the backward repacks c unless the field still holds it
+
+        def hold(cc, again):
+            if again and tf.holds is token:
+                return
+            capi.check(capi.lib.dg_field_set_nodes_device(h, cc.data_ptr(), n_nodes, _device.stream(cc)))
+            tf.holds = token
+
+        def run(oc, dc, cc):
+            hold(cc, False)
+            return self._raycast_device(h, oc, dc, iso, t_min, t_max)
+
+        def vjp(oc, dc, cc, t_lo, status, g_lo, g_hi, needs):
+            hold(cc, True)
+            return _raycast_vjp(h, oc, dc, t_lo, status, g_lo, g_hi, needs[0], needs[1], n_nodes if needs[2] else None)
+        if torch.is_grad_enabled() and (o.requires_grad or d.requires_grad or c.requires_grad):
+            return _field_raycast_function().apply(o, d, c, run, vjp)
+        return run(o, d, c)
 
     # ------------------------------------------------------------------ save / load (cubic_lagrange_discrete_grid.cpp:678-778)
     def save(self, filename):

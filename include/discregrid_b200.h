@@ -476,6 +476,39 @@ DG_API int dg_mesh_distance_vjp_device(const dg_mesh* mesh, uint64_t n, const do
                                        const double* d_nearest_point, const int32_t* d_triangle_id, const double* d_barycentric,
                                        const double* d_grad_distance, double* d_grad_points, double* d_grad_vertices, void* stream);
 
+/* ---- differentiable ray casts (K12, k12_raycast_grad.cu; beyond the reference) ------------------------------------------------------
+ * The vector-Jacobian products of the two ray casts above.  The contract (operation order, validity, summation order) is stated in
+ * discregrid_b200/csrc/k12_raycast_grad.cu and DESIGN.md section 3; the results depend only on the inputs, the same bits on every run and
+ * stream.  First order only.  Every output is nullable and asking for none is a no-op.  n < 2^32 - 1.  Arrays may be NULL only when n is 0
+ * (the upstream gradients as stated below).  Device scratch is taken and released in stream order.  The _device forms are queued on
+ * `stream`; the host forms upload every input in one piece, run the device form and return when done.
+ * dg_mesh_raycast_vjp[_device]: for the outputs of dg_mesh_raycast (directions, t, triangle_id, barycentric) and the upstream gradients
+ *     grad_t[n] and grad_barycentric[n x 3] (either may be NULL for zeros, not both): grad_origins[n x 3], grad_directions[n x 3] and
+ *     grad_vertices[n_vertices x 3].  vertices[n_vertices x 3] are the positions the forward cast against (the mesh may have been refit
+ *     since): the gradient is taken there.  A ray with triangle id -1, or whose triangle is degenerate or parallel to it (n . d == 0), gets 0.
+ *     grad_vertices is overwritten (0 where nothing arrives) and is summed as K10 sums the distance gradient.  The triangle ids are checked
+ *     on the device first (one synchronise); DG_ERR_INVALID, before anything is written: NULL mesh, a NULL input, both upstreams NULL, a mesh
+ *     on another device or left unusable by a failed refit, n too large, a triangle id outside [-1, n_triangles).
+ * dg_field_raycast_vjp[_device]: for the rays (origins, directions) and the outputs t_lo and status of dg_field_raycast, and the upstream
+ *     gradients grad_t_lo[n] and grad_t_hi[n] (either may be NULL for zeros, not both; both ends of the bracket follow the crossing, so they
+ *     are added): grad_origins[n x 3], grad_directions[n x 3] on any field (dense, reduced, a kept reduced handle), and grad_nodes[n_nodes],
+ *     overwritten, only on a field made by dg_field_create_trainable (DG_ERR_INVALID on any other).  The field must hold the node values of
+ *     the forward.  A miss, a crossing where the field is DBL_MAX or not finite, or a ray tangent to the level set (grad phi . d == 0) gets 0.
+ *     DG_ERR_INVALID, before anything is written: NULL field, a NULL input, both upstreams NULL, a field on another device, n too large. */
+DG_API int dg_mesh_raycast_vjp(const dg_mesh* mesh, uint64_t n, const double* directions, const double* t, const int32_t* triangle_id,
+                               const double* barycentric, const double* vertices, const double* grad_t, const double* grad_barycentric,
+                               double* grad_origins, double* grad_directions, double* grad_vertices);
+DG_API int dg_mesh_raycast_vjp_device(const dg_mesh* mesh, uint64_t n, const double* d_directions, const double* d_t,
+                                      const int32_t* d_triangle_id, const double* d_barycentric, const double* d_vertices,
+                                      const double* d_grad_t, const double* d_grad_barycentric, double* d_grad_origins,
+                                      double* d_grad_directions, double* d_grad_vertices, void* stream);
+DG_API int dg_field_raycast_vjp(const dg_field* field, uint64_t n, const double* origins, const double* directions, const double* t_lo,
+                                const int32_t* status, const double* grad_t_lo, const double* grad_t_hi, double* grad_origins,
+                                double* grad_directions, double* grad_nodes);
+DG_API int dg_field_raycast_vjp_device(const dg_field* field, uint64_t n, const double* d_origins, const double* d_directions,
+                                       const double* d_t_lo, const int32_t* d_status, const double* d_grad_t_lo, const double* d_grad_t_hi,
+                                       double* d_grad_origins, double* d_grad_directions, double* d_grad_nodes, void* stream);
+
 /* ---- reduced density map: GenerateDensityMap with reduction in one call -----------------------------------------------------------
  * GenerateDensityMap with reduction (cmd/generate_density_map/main.cpp:117-147) in one call:
  *   id = addFunction(density_func, verbose, pred);  reduceField(0, p0);  reduceField(id, p1);
