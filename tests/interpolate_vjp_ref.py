@@ -123,6 +123,80 @@ def interpolate_vjp(mn, mx, cell, inv, res, nodes, cells, cmap, x, gphi=None, gg
     return out
 
 
+def closed_form_cells(res, c):
+    """the closed-form cell table (cell_node_id, csrc/dg_device.cuh) for the unreduced cells c of a grid of resolution res: [len(c), 32]
+    node ids, int64.  Cell c is (i, j, k) with c = i + nx (j + ny k); slots 0-7 are the corners (di, dj, dk) = bits of the slot, slots 8-31
+    the two inner nodes of each x, y and z edge"""
+    nx, ny, nz = (int(r) for r in res)
+    c = np.asarray(c, np.int64)
+    k = c // (nx * ny); t = c - k * (nx * ny); j = t // nx; i = t - j * nx
+    nv = (nx + 1) * (ny + 1) * (nz + 1)
+    ne_x, ne_y = nx * (ny + 1) * (nz + 1), (nx + 1) * ny * (nz + 1)
+    cols = []
+    for jn in range(8):
+        di, dj, dk = jn & 1, (jn >> 1) & 1, (jn >> 2) & 1
+        cols.append((nx + 1) * (ny + 1) * (k + dk) + (nx + 1) * (j + dj) + i + di)
+    for jn in range(8, 32):
+        par, q = jn & 1, (jn - 8) >> 1
+        grp, w = q >> 2, q & 3
+        if grp == 0:                                                 # x edges at (j, k), (j, k + 1), (j + 1, k), (j + 1, k + 1)
+            cols.append(nv + 2 * (nx * (ny + 1) * (k + (w & 1)) + nx * (j + (w >> 1)) + i) + par)
+        elif grp == 1:                                               # y edges at (i, k), (i + 1, k), (i, k + 1), (i + 1, k + 1)
+            cols.append(nv + 2 * ne_x + 2 * (ny * (nz + 1) * (i + (w & 1)) + ny * (k + (w >> 1)) + j) + par)
+        else:                                                        # z edges at (i, j), (i, j + 1), (i + 1, j), (i + 1, j + 1)
+            cols.append(nv + 2 * (ne_x + ne_y) + 2 * (nz * (nx + 1) * (j + (w & 1)) + nz * (i + (w >> 1)) + k) + par)
+    return np.stack(cols, 1) if len(c) else np.zeros((0, 32), np.int64)
+
+
+def _fold(out, node, flat, vals):
+    """out[node] = ((out[node] + vals_1) + vals_2) + ... over each node's entries in ascending flat order"""
+    order = np.lexsort((flat, node))
+    node, vals = node[order], vals[order]
+    first = np.ones(len(node), bool); first[1:] = node[1:] != node[:-1]
+    rank = np.arange(len(node)) - np.flatnonzero(first)[np.cumsum(first) - 1]
+    by_rank = np.argsort(rank, kind="stable")                       # step r adds every node's r-th entry: each node once per step
+    bounds = np.concatenate([[0], np.cumsum(np.bincount(rank))]) if len(rank) else [0]
+    for r in range(len(bounds) - 1):
+        sel = by_rank[bounds[r]:bounds[r + 1]]
+        out[node[sel]] = out[node[sel]] + vals[sel]
+
+
+def interpolate_vjp_touched(mn, mx, cell, inv, res, nodes, cells, cmap, x, gphi=None, ggrad=None, chunk=1 << 17):
+    """interpolate_vjp read from the rows of the cells that queries touch: cells is the [n_cells_kept, 32] table or a callable that returns
+    the rows of an array of kept cell indices (closed_form_cells for a field made without a table); cmap None is the identity.  The node
+    fold visits only the incidences of touched cells.  Skipping an empty segment gives the bits of adding +0.0 for it (the fold starts at
+    +0.0 and a sum with a +0.0 operand is never -0.0), so this equals interpolate_vjp; it needs memory in the queries, not in the field."""
+    rows_of = cells if callable(cells) else (lambda c, t=np.asarray(cells, np.int64).reshape(-1, 32): t[c])
+    nodes = np.asarray(nodes, np.float64)
+    x = np.ascontiguousarray(x, np.float64).reshape(-1, 3)
+    out = np.zeros(len(nodes))
+    valid, c, c0, c1 = locate(mn, mx, cell, inv, res, cmap, x)
+    touched = np.unique(c[valid])
+    if len(touched):
+        has_max = (nodes[rows_of(touched)] == DBL_MAX).any(axis=1)
+        valid &= ~has_max[np.minimum(np.searchsorted(touched, c), len(touched) - 1)]
+    key = np.where(valid, c + 1, 0)
+    perm = np.argsort(key, kind="stable")
+    perm = perm[key[perm] > 0]
+    if len(perm) == 0:
+        return out
+    gphi = None if gphi is None else np.asarray(gphi, np.float64)
+    ggrad = None if ggrad is None else np.asarray(ggrad, np.float64).reshape(-1, 3)
+    t = np.empty((len(perm), 32))
+    for b in range(0, len(perm), chunk):
+        p = perm[b:b + chunk]
+        with np.errstate(all="ignore"):
+            xi = c0[p] * x[p] - c1[p]
+        N, D = rows(xi[:, 0], xi[:, 1], xi[:, 2])
+        t[b:b + chunk] = contributions(N, D, c0[p], None if gphi is None else gphi[p], None if ggrad is None else ggrad[p])
+    ids, R = segment_sums(key[perm], t)
+    cc = ids.astype(np.int64) - 1
+    node = rows_of(cc).astype(np.int64).reshape(-1)
+    flat = (32 * cc[:, None] + np.arange(32)).reshape(-1)
+    _fold(out, node, flat, R.reshape(-1))
+    return out
+
+
 def grid_vjp(grid, field_id, x, gphi=None, ggrad=None, nodes=None):
     """interpolate_vjp on a CubicLagrangeDiscreteGrid's field (its own node values unless `nodes` is given)"""
     d = grid._desc
