@@ -11,7 +11,7 @@ CXXFLAGS := -std=c++17 -O3 -fPIC -ffp-contract=off -fvisibility=hidden
 SRC      := discregrid_b200/csrc
 OBJ      := build/obj
 LIB      := discregrid_b200/lib/libdiscregrid_b200.so
-CU       := k1_sdf k2_interp k3_density k4_reduce k5_winding k6_isosurface k7_raycast k8_refit k9_mesh_raycast k10_distance_grad k11_field_grad k12_raycast_grad radix_sort dg_api
+CU       := k1_sdf k2_interp k3_density k4_reduce k5_winding k6_isosurface k7_raycast k8_refit k9_mesh_raycast k10_distance_grad k11_field_grad k12_raycast_grad k13_isosurface_grad radix_sort dg_api
 HDRS     := $(wildcard $(SRC)/*.h $(SRC)/*.cuh) include/discregrid_b200.h
 
 all: lib cpp oracle
@@ -24,7 +24,7 @@ CPPBIN   := build/bin
 CPPFLAGS := -std=c++11 -O2 -ffp-contract=off -I$(EIGEN3_INCLUDE_DIR) -Icpp/include -Iinclude
 CPPLINK  := -Ldiscregrid_b200/lib -ldiscregrid_b200 -Wl,-rpath,'$$ORIGIN/../../discregrid_b200/lib'
 CPPHDRS  := $(wildcard cpp/include/Discregrid/* cpp/include/Discregrid/*/*) include/discregrid_b200.h
-cpp: $(CPPBIN)/GenerateSDF $(CPPBIN)/GenerateDensityMap $(CPPBIN)/GenerateVolumeMap $(CPPBIN)/liborcvolume.so ref_volume $(CPPBIN)/DiscreteFieldToBitmap $(CPPBIN)/DiscreteFieldToMesh $(CPPBIN)/facade_check $(CPPBIN)/bvh_host_check $(CPPBIN)/reduce_facade_check $(CPPBIN)/sort_replay_check $(CPPBIN)/fast_div_check $(CPPBIN)/libk1emu.so $(CPPBIN)/libk1emu_perlane.so $(CPPBIN)/libk1emu_band.so $(CPPBIN)/libk1emu_band_perlane.so $(CPPBIN)/libk23emu.so $(CPPBIN)/libk3vemu.so $(CPPBIN)/libk2hemu.so $(CPPBIN)/libk5emu.so $(CPPBIN)/libk8emu.so $(CPPBIN)/libk9emu.so $(CPPBIN)/libk9emu_nocull.so $(CPPBIN)/libk10emu.so $(CPPBIN)/libdgemu.so $(CPPBIN)/libk4emu.so $(CPPBIN)/device_function_check $(CPPBIN)/device_query_check $(CPPBIN)/hessian_check $(CPPBIN)/winding_check $(CPPBIN)/raycast_check $(CPPBIN)/refit_check $(CPPBIN)/mesh_raycast_check $(CPPBIN)/field_grad_check $(CPPBIN)/raycast_grad_check $(CPPBIN)/liborctree.so
+cpp: $(CPPBIN)/GenerateSDF $(CPPBIN)/GenerateDensityMap $(CPPBIN)/GenerateVolumeMap $(CPPBIN)/liborcvolume.so ref_volume $(CPPBIN)/DiscreteFieldToBitmap $(CPPBIN)/DiscreteFieldToMesh $(CPPBIN)/facade_check $(CPPBIN)/bvh_host_check $(CPPBIN)/reduce_facade_check $(CPPBIN)/sort_replay_check $(CPPBIN)/fast_div_check $(CPPBIN)/libk1emu.so $(CPPBIN)/libk1emu_perlane.so $(CPPBIN)/libk1emu_band.so $(CPPBIN)/libk1emu_band_perlane.so $(CPPBIN)/libk23emu.so $(CPPBIN)/libk3vemu.so $(CPPBIN)/libk2hemu.so $(CPPBIN)/libk5emu.so $(CPPBIN)/libk8emu.so $(CPPBIN)/libk9emu.so $(CPPBIN)/libk9emu_nocull.so $(CPPBIN)/libk10emu.so $(CPPBIN)/libdgemu.so $(CPPBIN)/libk4emu.so $(CPPBIN)/device_function_check $(CPPBIN)/device_query_check $(CPPBIN)/hessian_check $(CPPBIN)/winding_check $(CPPBIN)/raycast_check $(CPPBIN)/refit_check $(CPPBIN)/mesh_raycast_check $(CPPBIN)/field_grad_check $(CPPBIN)/raycast_grad_check $(CPPBIN)/isosurface_grad_check $(CPPBIN)/liborctree.so
 $(CPPBIN)/DiscreteFieldToBitmap: cpp/cmd/discrete_field_to_bitmap.cpp $(CPPHDRS) $(LIB)
 	@mkdir -p $(CPPBIN)
 	$(HOSTCXX) $(CPPFLAGS) $< -o $@ $(CPPLINK)
@@ -93,7 +93,7 @@ $(CPPBIN)/libk10emu.so: tests/emu/k10_emu.cpp tests/emu/cudart_stub.cpp tests/em
 	$(HOSTCXX) -std=c++17 -O2 -ffp-contract=off -fPIC -shared -Wl,-Bsymbolic -DK10_EMU_SURFACE=1 -I$(CUDA_INC) -Itests/emu -I$(SRC) tests/emu/k10_emu.cpp tests/emu/cudart_stub.cpp -o $@ -lpthread
 # test library: the WHOLE product library with every kernel emulated and the CUDA runtime stubbed on host memory -- lets the Python-level
 # and tool-level `-m gpu` tests be rehearsed on the CPU (tests/test_gpu_rehearsal.py); never loaded by the product
-DGEMU_SRC := tests/emu/dgapi_emu.cpp tests/emu/k1_emu.cpp tests/emu/k2_emu.cpp tests/emu/k3_emu.cpp tests/emu/k4_emu.cpp tests/emu/k5_emu.cpp tests/emu/k6_emu.cpp tests/emu/k7_emu.cpp tests/emu/k8_emu.cpp tests/emu/k9_emu.cpp tests/emu/k10_emu.cpp tests/emu/k11_emu.cpp tests/emu/k12_emu.cpp tests/emu/cudart_stub.cpp \
+DGEMU_SRC := tests/emu/dgapi_emu.cpp tests/emu/k1_emu.cpp tests/emu/k2_emu.cpp tests/emu/k3_emu.cpp tests/emu/k4_emu.cpp tests/emu/k5_emu.cpp tests/emu/k6_emu.cpp tests/emu/k7_emu.cpp tests/emu/k8_emu.cpp tests/emu/k9_emu.cpp tests/emu/k10_emu.cpp tests/emu/k11_emu.cpp tests/emu/k12_emu.cpp tests/emu/k13_emu.cpp tests/emu/cudart_stub.cpp \
              $(SRC)/bvh_build.cpp $(SRC)/host_threads.cpp $(SRC)/reduce_field.cpp $(SRC)/obj_reader.cpp $(SRC)/sort_replay.cpp
 $(CPPBIN)/libdgemu.so: $(DGEMU_SRC) tests/emu/cuda_emu.h $(wildcard $(SRC)/*.cu) $(HDRS)
 	@mkdir -p $(CPPBIN)
@@ -150,6 +150,10 @@ $(CPPBIN)/field_grad_check: tests/cpp/field_grad_check.cpp $(CPPHDRS) $(LIB)
 	$(HOSTCXX) $(CPPFLAGS) -I$(CUDA_INC) $< -o $@ $(CPPLINK) -L$(CUDA_LIB) -lcudart_static -ldl -lrt -lpthread
 # test binary: the facade's ray-cast gradients (raycast_vjp of the mesh and of the grid on device pointers), for comparison with the Python route
 $(CPPBIN)/raycast_grad_check: tests/cpp/raycast_grad_check.cpp $(CPPHDRS) $(LIB)
+	@mkdir -p $(CPPBIN)
+	$(HOSTCXX) $(CPPFLAGS) -I$(CUDA_INC) $< -o $@ $(CPPLINK) -L$(CUDA_LIB) -lcudart_static -ldl -lrt -lpthread
+# test binary: the facade's level-set gradient (isosurface with edge ids, isosurface_vjp on device pointers), for comparison with the Python route
+$(CPPBIN)/isosurface_grad_check: tests/cpp/isosurface_grad_check.cpp $(CPPHDRS) $(LIB)
 	@mkdir -p $(CPPBIN)
 	$(HOSTCXX) $(CPPFLAGS) -I$(CUDA_INC) $< -o $@ $(CPPLINK) -L$(CUDA_LIB) -lcudart_static -ldl -lrt -lpthread
 # test library: the oracle with a given tree and given pseudonormals (the reference's query rule over a refit mesh's records)

@@ -18,6 +18,7 @@
 //   interpolate(field, x, grad*)             -> dg_interpolate_batch (K2), also batched: interpolate(field, n, x, phi, grad)
 //   interpolate(field, n, x, phi, grad, hess) -> dg_interpolate_hessian_batch (K2's Hessian mode; not in the reference)
 //   isosurface(field, iso, subdivisions)     -> dg_isosurface_create (K6: the level set as a TriangleMesh; not in the reference)
+//   isosurface_vjp(field, iso, s, n, ...)    -> dg_isosurface_vjp_device (K13: its vertices' gradient in the trainable field's node values)
 //   raycast(field, n, o, d, iso, t0, t1, ...) -> dg_field_raycast (K7: first crossings along rays and segments; not in the reference)
 //   connectivity table of addFunction        -> dg_build_cells  (GPU)  replaces the serial loop :833-886
 //
@@ -364,8 +365,9 @@ public:
         check(dg_interpolate_hessian_batch(deviceField(field_id), x, n, phi, grad, hess));
     }
     // the level set {phi = iso} of a field by marching tetrahedra on a lattice that subdivides every cell `subdivisions` times (new, beyond
-    // the reference; contract in k6_isosurface.cu): outward-oriented triangles for an SDF, coincident vertices not welded
-    TriangleMesh isosurface(unsigned int field_id, double iso = 0.0, unsigned int subdivisions = 1) const
+    // the reference; contract in k6_isosurface.cu): outward-oriented triangles for an SDF, coincident vertices not welded.  edge_ids, when
+    // given, receives the lattice edge of every vertex (dg_isosurface_copy_edges), what isosurface_vjp takes
+    TriangleMesh isosurface(unsigned int field_id, double iso = 0.0, unsigned int subdivisions = 1, std::vector<std::uint64_t>* edge_ids = nullptr) const
     {
         dg_isosurface* s = nullptr;
         check(dg_isosurface_create(deviceField(field_id), iso, subdivisions, &s, nullptr));
@@ -373,7 +375,11 @@ public:
         dg_isosurface_sizes(s, &nv, &nt);
         std::vector<double> v(3 * nv);
         std::vector<std::uint32_t> t(3 * nt);
-        const int rc = dg_isosurface_copy(s, v.data(), t.data());
+        int rc = dg_isosurface_copy(s, v.data(), t.data());
+        if (rc == DG_OK && edge_ids) {
+            edge_ids->resize((std::size_t)nv);
+            rc = dg_isosurface_copy_edges(s, edge_ids->data());
+        }
         dg_isosurface_destroy(s);
         check(rc);
         return TriangleMesh(v.data(), t.data(), (std::size_t)nv, (std::size_t)nt);
@@ -413,6 +419,14 @@ public:
         const dg_field* f = d_grad_nodes ? trainableField(field_id) : deviceField(field_id);
         check(dg_field_raycast_vjp_device(f, n, d_origins, d_directions, d_t_lo, d_status, d_grad_t_lo, d_grad_t_hi, d_grad_origins,
                                           d_grad_directions, d_grad_nodes, stream));
+    }
+    // isosurface_vjp: d_grad_nodes [nodes] = the gradient in the trainable field's node values of sum_v d_grad_vertices[v] . V_v over the n
+    // vertices on the lattice edges d_edge_ids [n] of isosurface(field_id, iso, subdivisions) extracted on trainableField(field_id) holding
+    // the same values (dg_isosurface_vjp_device; contract in k13_isosurface_grad.cu)
+    void isosurface_vjp(unsigned int field_id, double iso, unsigned int subdivisions, std::size_t n, const std::uint64_t* d_edge_ids,
+                        const double* d_grad_vertices, double* d_grad_nodes, void* stream = nullptr)
+    {
+        check(dg_isosurface_vjp_device(trainableField(field_id), iso, subdivisions, n, d_edge_ids, d_grad_vertices, d_grad_nodes, stream));
     }
     // the trainable field itself, for the library's other calls on its current values (dg_interpolate_batch_device, ...)
     dg_field* trainableField(unsigned int field_id)

@@ -138,6 +138,10 @@ SIGNATURES = {
     "dg_isosurface_copy": (C.c_int, [_vp, _dp, _u32p]),
     "dg_isosurface_copy_device": (C.c_int, [_vp, _vp, _vp, _vp]),
     "dg_isosurface_destroy": (C.c_int, [_vp]),
+    "dg_isosurface_copy_edges": (C.c_int, [_vp, _u64p]),
+    "dg_isosurface_copy_edges_device": (C.c_int, [_vp, _vp, _vp]),
+    "dg_isosurface_vjp": (C.c_int, [_vp, C.c_double, C.c_uint32, C.c_uint64, _u64p, _dp, _dp]),
+    "dg_isosurface_vjp_device": (C.c_int, [_vp, C.c_double, C.c_uint32, C.c_uint64, _vp, _vp, _vp, _vp]),
     "dg_field_raycast": (C.c_int, [_vp, _dp, _dp, C.c_uint64, C.c_double, C.c_double, C.c_double, _dp, _dp, _i32p]),
     "dg_field_raycast_device": (C.c_int, [_vp, _vp, _vp, C.c_uint64, C.c_double, C.c_double, C.c_double, _vp, _vp, _vp, _vp]),
     "dg_reduced_density_map_create": (C.c_int, [_gp, _dp, C.c_uint64, _u32p, C.c_uint64, _u32p, C.c_double, C.c_double, C.c_uint32,

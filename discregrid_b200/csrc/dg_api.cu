@@ -49,6 +49,7 @@
 #include "k10_distance_grad.h"
 #include "k11_field_grad.h"
 #include "k12_raycast_grad.h"
+#include "k13_isosurface_grad.h"
 #include "reduce_field.h"
 #include "obj_reader.h"
 
@@ -2906,6 +2907,7 @@ int dg_field_create_reduced(const dg_reduced_band* h, dg_field** out)
 // The mesh stays on the field's device in the handle until dg_isosurface_copy[_device].
 struct dg_isosurface {
     DevBuf<double> d_vertices;
+    DevBuf<uint64_t> d_edge_ids;                      // the lattice edge of every vertex (K13 differentiates through it)
     DevBuf<unsigned> d_triangles;
     uint64_t n_vertices = 0, n_triangles = 0;
     int device = 0;
@@ -2913,7 +2915,7 @@ struct dg_isosurface {
 
 // values, classify, scans, emit (k6_isosurface.cu); each stage ends with a synchronise.  Device memory: 8 B per lattice point of values,
 // 7 B per point of edge flags, 1 B per lattice cell of counts, 1/8 B per point of chunk ranks, the tile arrays, one chunk of positions
-// (24 B x min(Np, 2^24)), then 24 B per vertex and 12 B per triangle of output.
+// (24 B x min(Np, 2^24)), then 24 B per vertex, 8 B per vertex of edge ids and 12 B per triangle of output.
 int dg_isosurface_create(const dg_field* f, double iso, uint32_t s, dg_isosurface** out, double* timings_ms)
 {
     static const char* who = "dg_isosurface_create";
@@ -2975,8 +2977,9 @@ int dg_isosurface_create(const dg_field* f, double iso, uint32_t s, dg_isosurfac
             DevBuf<unsigned> d_chunk;
             DG_CUDA(d_chunk.alloc((n_edges + 31) / 32));
             DG_CUDA(h->d_vertices.alloc(3 * n_vert));
+            DG_CUDA(h->d_edge_ids.alloc(n_vert));
             DG_CUDA(h->d_triangles.alloc(3 * n_tri));
-            DG_LAUNCH(k6_launch_vertices(L, d_values.p, iso, d_flags.p, n_edges, d_edge_tile.p, d_chunk.p, h->d_vertices.p, st));
+            DG_LAUNCH(k6_launch_vertices(L, d_values.p, iso, d_flags.p, n_edges, d_edge_tile.p, d_chunk.p, h->d_vertices.p, h->d_edge_ids.p, st));
             DG_LAUNCH(k6_launch_triangles(L, d_values.p, iso, d_count.p, d_tri_tile.p, d_flags.p, d_chunk.p, h->d_triangles.p, st));
             DG_CUDA(cudaStreamSynchronize(st));
         }
@@ -3016,6 +3019,25 @@ int dg_isosurface_copy_device(const dg_isosurface* s, double* d_vertices, uint32
     const cudaStream_t st = (cudaStream_t)stream;
     if (s->n_vertices) DG_CUDA(cudaMemcpyAsync(d_vertices, s->d_vertices.p, 3 * s->n_vertices * sizeof(double), cudaMemcpyDeviceToDevice, st));
     if (s->n_triangles) DG_CUDA(cudaMemcpyAsync(d_triangles, s->d_triangles.p, 3 * s->n_triangles * sizeof(unsigned), cudaMemcpyDeviceToDevice, st));
+    return DG_OK;
+}
+
+int dg_isosurface_copy_edges(const dg_isosurface* s, uint64_t* edge_ids)
+{
+    if (!s) return fail(DG_ERR_INVALID, "dg_isosurface_copy_edges: handle is NULL");
+    if (!edge_ids && s->n_vertices) return fail(DG_ERR_INVALID, "dg_isosurface_copy_edges: NULL output");
+    if (int rc = check_handle_device(s->device, "dg_isosurface_copy_edges")) return rc;
+    if (s->n_vertices) DG_CUDA(cudaMemcpy(edge_ids, s->d_edge_ids.p, s->n_vertices * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+    return DG_OK;
+}
+
+int dg_isosurface_copy_edges_device(const dg_isosurface* s, uint64_t* d_edge_ids, void* stream)
+{
+    if (!s) return fail(DG_ERR_INVALID, "dg_isosurface_copy_edges_device: handle is NULL");
+    if (!d_edge_ids && s->n_vertices) return fail(DG_ERR_INVALID, "dg_isosurface_copy_edges_device: NULL output");
+    if (int rc = check_handle_device(s->device, "dg_isosurface_copy_edges_device")) return rc;
+    if (s->n_vertices)
+        DG_CUDA(cudaMemcpyAsync(d_edge_ids, s->d_edge_ids.p, s->n_vertices * sizeof(uint64_t), cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
     return DG_OK;
 }
 
@@ -3283,6 +3305,87 @@ int dg_field_raycast_vjp(const dg_field* f, uint64_t n, const double* origins, c
     if (grad_nodes && f->n_nodes) DG_CUDA(cudaMemcpy(grad_nodes, gn.p, f->n_nodes * sizeof(double), cudaMemcpyDeviceToHost));
     DG_CUDA(cudaDeviceSynchronize());
     return DG_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ K13: level-set gradients
+static int isosurface_vjp_check(const dg_field* f, double iso, uint32_t s, uint64_t n, const void* edge_ids, const void* gV,
+                                const void* grad_nodes, K6Lattice& L, const char* who)
+{
+    if (int rc = trainable_check(f, who)) return rc;
+    if (n && (!edge_ids || !gV)) return fail(DG_ERR_INVALID, "%s: edge_ids / grad_vertices is NULL", who);
+    if (f->n_nodes && !grad_nodes) return fail(DG_ERR_INVALID, "%s: grad_nodes is NULL", who);
+    if (!std::isfinite(iso)) return fail(DG_ERR_INVALID, "%s: iso must be finite (got %g)", who, iso);
+    if (s == 0 || s > K6_MAX_SUBDIVISIONS) return fail(DG_ERR_INVALID, "%s: subdivisions must be 1..%u (got %u)", who, K6_MAX_SUBDIVISIONS, s);
+    uint64_t np = 0;
+    L = k6_lattice(f->dev.g, s, np);
+    if (np >= (1ull << 31))
+        return fail(DG_ERR_INVALID, "%s: the lattice of %llu points (%u x %u x %u) has 2^31 points or more", who, (unsigned long long)np,
+                    L.np[0], L.np[1], L.np[2]);
+    if (n >= (1ull << 31)) return fail(DG_ERR_INVALID, "%s: %llu vertices; at most 2^31 - 1 per call", who, (unsigned long long)n);
+    return DG_OK;
+}
+
+// the edge ids are checked on the device first (one synchronise); nothing is written unless every one is an edge of the lattice.  The
+// scratch is stream-ordered: allocated and released on `st`
+static int isosurface_vjp_launch(const dg_field* f, const K6Lattice& L, double iso, uint64_t n, const uint64_t* d_e, const double* d_gV,
+                                 double* d_gn, cudaStream_t st, const char* who)
+{
+    if (n) {
+        DevBuf<unsigned> bad;
+        DG_CUDA(bad.alloc(1));
+        DG_LAUNCH(k13_launch_check(L, d_e, n, bad.p, st));
+        unsigned h_bad = 0;
+        DG_CUDA(cudaMemcpyAsync(&h_bad, bad.p, sizeof h_bad, cudaMemcpyDeviceToHost, st));
+        DG_CUDA(cudaStreamSynchronize(st));
+        if (h_bad) return fail(DG_ERR_INVALID, "%s: %u edge ids are not edges of the %u x %u x %u lattice", who, h_bad, L.np[0], L.np[1], L.np[2]);
+    }
+    K11Field kf;
+    kf.f = f->dev; kf.inc_begin = f->d_inc_begin.p; kf.inc = f->d_inc.p; kf.has_max = f->d_has_max.p;
+    kf.n_nodes = f->n_nodes; kf.n_cells_kept = f->n_cells_kept;
+    const size_t bytes = k13_scratch_bytes(n, f->n_cells_kept);
+    void* scratch = nullptr;
+#ifdef DG_EMU
+    if (bytes) DG_CUDA(cudaMalloc(&scratch, bytes));
+    const cudaError_t e = k13_launch_vjp(kf, L, iso, d_e, n, d_gV, d_gn, scratch, st);
+    if (scratch) cudaFree(scratch);
+#else
+    if (bytes) DG_CUDA(cudaMallocAsync(&scratch, bytes, st));
+    const cudaError_t e = k13_launch_vjp(kf, L, iso, d_e, n, d_gV, d_gn, scratch, st);
+    if (scratch) cudaFreeAsync(scratch, st);
+#endif
+    DG_LAUNCH(e);
+    return DG_OK;
+}
+
+int dg_isosurface_vjp_device(const dg_field* f, double iso, uint32_t subdivisions, uint64_t n, const uint64_t* d_edge_ids,
+                             const double* d_grad_vertices, double* d_grad_nodes, void* stream)
+{
+    static const char* who = "dg_isosurface_vjp_device";
+    K6Lattice L;
+    if (int rc = isosurface_vjp_check(f, iso, subdivisions, n, d_edge_ids, d_grad_vertices, d_grad_nodes, L, who)) return rc;
+    return isosurface_vjp_launch(f, L, iso, n, d_edge_ids, d_grad_vertices, d_grad_nodes, (cudaStream_t)stream, who);
+}
+
+// host arrays: every input uploaded in one piece (the node sums span all vertices), then the device form on the legacy default stream
+int dg_isosurface_vjp(const dg_field* f, double iso, uint32_t subdivisions, uint64_t n, const uint64_t* edge_ids, const double* grad_vertices,
+                      double* grad_nodes)
+{
+    static const char* who = "dg_isosurface_vjp";
+    return guarded(who, [&]() -> int {
+        K6Lattice L;
+        if (int rc = isosurface_vjp_check(f, iso, subdivisions, n, edge_ids, grad_vertices, grad_nodes, L, who)) return rc;
+        DevBuf<uint64_t> e;
+        DevBuf<double> gV, gn;
+        DG_CUDA(e.alloc(n)); DG_CUDA(gV.alloc(3 * n)); DG_CUDA(gn.alloc(f->n_nodes));
+        if (n) {
+            DG_CUDA(cudaMemcpy(e.p, edge_ids, n * sizeof(uint64_t), cudaMemcpyHostToDevice));
+            DG_CUDA(cudaMemcpy(gV.p, grad_vertices, 3 * n * sizeof(double), cudaMemcpyHostToDevice));
+        }
+        if (int rc = isosurface_vjp_launch(f, L, iso, n, e.p, gV.p, gn.p, nullptr, who)) return rc;
+        if (f->n_nodes) DG_CUDA(cudaMemcpy(grad_nodes, gn.p, f->n_nodes * sizeof(double), cudaMemcpyDeviceToHost));
+        DG_CUDA(cudaDeviceSynchronize());
+        return DG_OK;
+    });
 }
 
 int dg_obj_read(const char* path, double** vertices, uint64_t* n_vertices, uint32_t** triangles, uint64_t* n_triangles)

@@ -16,7 +16,8 @@
 //   shared faces match.  A tetrahedron emits only if its four vertices are valid.
 // Edges and vertices.  Every tetrahedron edge is (p, p + delta) with delta one of 7 directions, d = 0..6 <-> (1,0,0), (0,1,0), (0,0,1),
 //   (1,1,0), (1,0,1), (0,1,1), (1,1,1); edge id 7 * lin(p) + d.  An edge crosses iff exactly one endpoint is negative.  A vertex is emitted
-//   for a crossing edge iff an emitting tetrahedron contains the edge (no vertex is unreferenced); vertices are ordered by edge id.  With p
+//   for a crossing edge iff an emitting tetrahedron contains the edge (no vertex is unreferenced); vertices are ordered by edge id, and the
+//   edge id of every vertex is written beside it (ascending; K13 differentiates the vertex through it, k13_isosurface_grad.cu).  With p
 //   the lower endpoint and q = p + delta: t = (iso - f_p) / (f_q - f_p), then x_a = x_p,a + t * (x_q,a - x_p,a), in that order, no FMA.
 //   Monotone rounding keeps t in [0, 1] while both differences are finite; near +-DBL_MAX they can overflow and t can become 0 or NaN -- the
 //   contract keeps whatever that arithmetic gives.
@@ -47,7 +48,7 @@
 // Passes (the host side is dg_isosurface_create in dg_api.cu): lattice positions per chunk of K6_CHUNK points, evaluated by K2's value-only
 // kernel; classify (one thread per lattice cell: triangle count byte, idempotent byte flags of the crossing edges); scans (K4's flag scan over
 // the 7 * Np edge flags, a warp-synchronous scan of the counts over the four bit planes of 0..12); emit (one warp per tile of edges writes the
-// vertices at their ranks and the rank of every 32-edge chunk; one warp per tile of cells writes the triangles).  Integer work apart from the
+// vertices and their edge ids at their ranks and the rank of every 32-edge chunk; one warp per tile of cells writes the triangles).  Integer work apart from the
 // positions and the vertex arithmetic above; nothing depends on block or chunk size.  Warp-synchronous (ballot / popc only), so tests/emu
 // runs it unchanged.
 #include "k6_isosurface.h"
@@ -97,19 +98,9 @@ DG_HD unsigned tet_corner(unsigned t, unsigned i)
     return i == 0 ? 0u : i == 1 ? (1u << pi0) : i == 2 ? ((1u << pi0) | (1u << pi1)) : 7u;
 }
 DG_HD bool tet_odd(unsigned t) { return (0x26u >> t) & 1u; }               // t = 1, 2, 5
-// direction d of an edge whose endpoints differ by the corner mask m (1..7), and back
+// direction d of an edge whose endpoints differ by the corner mask m (1..7); mask_of_dir (k6_isosurface.h) is its inverse
 DG_HD unsigned dir_of_mask(unsigned m) { return (((0u << 3) | (1u << 6) | (3u << 9) | (2u << 12) | (4u << 15) | (5u << 18) | (6u << 21)) >> (3 * m)) & 7u; }
-DG_HD unsigned mask_of_dir(unsigned d) { return ((1u | (2u << 3) | (4u << 6) | (3u << 9) | (5u << 12) | (6u << 15) | (7u << 18)) >> (3 * d)) & 7u; }
 
-DG_HD double lat_coord(const K6Lattice& L, int a, unsigned i)
-{
-    const double x = L.mn[a] + L.cell[a] * ((double)i / (double)L.s);
-    return x > L.mx[a] ? L.mx[a] : x;
-}
-DG_HD unsigned corner_offset(const K6Lattice& L, unsigned m)
-{
-    return (m & 1u) + L.np[0] * (((m >> 1) & 1u) + L.np[1] * (m >> 2));
-}
 // finite and not the sentinel
 DG_HD bool value_valid(double v) { return fabs(v) <= DBL_MAX && v != DBL_MAX; }
 
@@ -212,7 +203,7 @@ DG_HD unsigned flags_before(const unsigned char* __restrict__ flags, unsigned lo
 
 __global__ void vertices_kernel(K6Lattice L, const double* __restrict__ values, double iso, const unsigned char* __restrict__ flags,
                                 unsigned long long n_edges, const unsigned* __restrict__ edge_tile, unsigned* __restrict__ chunk,
-                                double* __restrict__ vout)
+                                double* __restrict__ vout, unsigned long long* __restrict__ eout)
 {
     const unsigned long long tile = ((unsigned long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const unsigned lane = threadIdx.x & 31u;
@@ -232,7 +223,9 @@ __global__ void vertices_kernel(K6Lattice L, const double* __restrict__ values, 
             const unsigned ip[3] = {I, J, K};
             const double fp = values[lp], fq = values[lq];
             const double t = (iso - fp) / (fq - fp);
-            double* v = vout + 3ull * (run + (unsigned)__popc(m & lt));
+            const unsigned rank = run + (unsigned)__popc(m & lt);
+            double* v = vout + 3ull * rank;
+            eout[rank] = e;
             for (int a = 0; a < 3; a++) {
                 const double xp = lat_coord(L, a, ip[a]), xq = lat_coord(L, a, ip[a] + ((dm >> a) & 1u));
                 v[a] = xp + t * (xq - xp);
@@ -339,12 +332,12 @@ cudaError_t k6_scan_counts(const unsigned char* d_count, uint64_t n, unsigned* d
 }
 
 cudaError_t k6_launch_vertices(const K6Lattice& L, const double* d_values, double iso, const unsigned char* d_flags, uint64_t n_edges,
-                               const unsigned* d_edge_tile, unsigned* d_chunk, double* d_vertices, cudaStream_t stream)
+                               const unsigned* d_edge_tile, unsigned* d_chunk, double* d_vertices, uint64_t* d_edge_ids, cudaStream_t stream)
 {
     if (n_edges == 0) return cudaSuccess;
     const uint64_t tiles = (n_edges + TILE - 1) / TILE;
     DG_KERNEL_LAUNCH(vertices_kernel, blocks_for(tiles * 32ull, 128), 128, 0, stream, L, d_values, iso, d_flags, (unsigned long long)n_edges,
-                     d_edge_tile, d_chunk, d_vertices);
+                     d_edge_tile, d_chunk, d_vertices, reinterpret_cast<unsigned long long*>(d_edge_ids));
     return DG_AFTER_LAUNCH();
 }
 

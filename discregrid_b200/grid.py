@@ -27,6 +27,9 @@ that save()/load() stay byte-compatible with the reference's .cdf/.cdm files
   raycast(field_id, origins, directions) -> dg_field_raycast[_device] (K7: first crossings of a level set along rays and segments)
   interpolate(field_id, x, coefficients=c) -> dg_field_set_nodes_device + K2 on a trainable field, differentiable in c through
                                             dg_interpolate_vjp_device (K11, csrc/k11_field_grad.cu)
+  isosurface(field_id, iso, s, device=True, coefficients=c)
+                                         -> dg_field_set_nodes_device + K6 on the trainable field, the vertices differentiable in c through
+                                            dg_isosurface_vjp_device (K13, csrc/k13_isosurface_grad.cu)
 
 The reduced calls keep the handle they get from the library until the field's first device use, which builds the interpolation
 field from it on the device (dg_field_create_reduced) instead of uploading the host copy again.
@@ -389,6 +392,39 @@ def _raycast_vjp(h, o, d, t_lo, status, g_lo, g_hi, want_o, want_d, n_nodes):
     capi.check(capi.lib.dg_field_raycast_vjp_device(h, n, o.data_ptr(), d.data_ptr(), t_lo.data_ptr(), status.data_ptr(), ptr(glo), ptr(ghi),
                                                     ptr(go), ptr(gd), ptr(gn), _device.stream(o)))
     return go, gd, gn
+
+
+_ISOSURFACE = None
+
+
+def _isosurface_function():
+    """the autograd Function of isosurface(..., coefficients=c) (K13): the vertices differentiable in c, each moving along its lattice edge as
+    its crossing parameter t = (iso - f_p) / (f_q - f_p) follows the edge's two lattice values.  The triangles and the edge ids carry no
+    gradient.  First order only: a double backward raises."""
+    global _ISOSURFACE
+    if _ISOSURFACE is None:
+        import torch
+        from torch.autograd.function import once_differentiable
+
+        class Isosurface(torch.autograd.Function):
+            @staticmethod
+            def forward(ctx, c, run, vjp):
+                V, T, E = run(c)
+                ctx.mark_non_differentiable(T, E)
+                ctx.set_materialize_grads(False)
+                ctx.vjp = vjp
+                ctx.save_for_backward(c, E)
+                return V, T, E
+
+            @staticmethod
+            @once_differentiable
+            def backward(ctx, grad_V, _grad_T, _grad_E):
+                if grad_V is None:
+                    return None, None, None
+                c, E = ctx.saved_tensors
+                return ctx.vjp(c, E, grad_V), None, None
+        _ISOSURFACE = Isosurface
+    return _ISOSURFACE
 
 
 def grid_desc(domain_min, domain_max, resolution, cell_size=None, inv_cell_size=None):
@@ -882,7 +918,7 @@ class CubicLagrangeDiscreteGrid:
         return run(x)
 
     # ------------------------------------------------------------------ level sets (beyond the reference)
-    def isosurface(self, field_id=0, iso=0.0, subdivisions=1, device=False):
+    def isosurface(self, field_id=0, iso=0.0, subdivisions=1, device=False, coefficients=None, edges=False):
         """The level set {phi = iso} of a field as a triangle mesh: marching tetrahedra on a lattice that subdivides every grid cell
         `subdivisions` times (1..16), on the field's GPU (dg_isosurface_create; the contract is in csrc/k6_isosurface.cu and DESIGN §3).
         The lattice values are the bits interpolate() returns there; points where it returns DBL_MAX or a non-finite value (outside the
@@ -891,11 +927,31 @@ class CubicLagrangeDiscreteGrid:
         Returns (vertices float64 (n, 3), triangles uint32 (m, 3)) as numpy arrays -- the layout TriangleMeshDistance takes.  With
         device=True they are CUDA tensors on the field's device, filled on torch's current stream, with triangles as torch.int32 (same
         values; 2^31 vertices or more are refused on this route).  A reduced field's kept device handle is used without a host round trip.
-        Stage times (values, classify, scans, emit, total; ms) are left in last_isosurface_ms."""
-        h = self._device_field(field_id)
+        Stage times (values, classify, scans, emit, total; ms) are left in last_isosurface_ms.
+
+        edges=True adds a third output: the lattice edge 7 * lin(p) + d of every vertex, ascending (uint64 numpy, or torch.int64 with
+        device=True; the contract's numbering).
+
+        coefficients=c (beyond the reference) extracts the level set of the field with the node values c instead of its own, on the trainable
+        device field interpolate(coefficients=) uses (same rules: c a float64 CUDA tensor of len(m_nodes[field_id]) values); it needs
+        device=True (ValueError otherwise), so that the result type never changes silently.  The vertices have the bits isosurface() gives on
+        a field whose m_nodes are c, and are differentiable in c (K13, csrc/k13_isosurface_grad.cu): each vertex moves along its lattice edge
+        as t = (iso - f_p) / (f_q - f_p) follows the edge's lattice values, summed into the nodes in a fixed order (K11).  A vertex at a
+        DBL_MAX or non-finite value, or on an edge whose two values are equal, gets 0.  The triangles and the edge ids carry no gradient; not
+        differentiable in iso; first order only (a double backward raises)."""
+        if coefficients is not None:
+            if not device:
+                raise ValueError("isosurface: coefficients= needs device=True (the vertices are then CUDA tensors differentiable in c)")
+            return self._isosurface_trainable(field_id, float(iso), int(subdivisions), coefficients, edges)
+        V, T, E = self._isosurface(self._device_field(field_id), float(iso), int(subdivisions), device, edges)
+        return (V, T, E) if edges else (V, T)
+
+    def _isosurface(self, h, iso, subdivisions, device, edges):
+        """dg_isosurface_create on the field handle h, then its outputs: (V, T, edge ids or None) as numpy arrays or, with device=True, as
+        tensors on the field's device filled on torch's current stream"""
         s = C.c_void_p()
         self.last_isosurface_ms = np.zeros(5)
-        capi.check(capi.lib.dg_isosurface_create(h, float(iso), int(subdivisions), C.byref(s), capi.ptr(self.last_isosurface_ms, capi.F64P)))
+        capi.check(capi.lib.dg_isosurface_create(h, iso, subdivisions, C.byref(s), capi.ptr(self.last_isosurface_ms, capi.F64P)))
         try:
             nv, nt = C.c_uint64(), C.c_uint64()
             capi.check(capi.lib.dg_isosurface_sizes(s, C.byref(nv), C.byref(nt)))
@@ -903,7 +959,11 @@ class CubicLagrangeDiscreteGrid:
             if not device:
                 V = np.empty((nv, 3)); T = np.empty((nt, 3), np.uint32)
                 capi.check(capi.lib.dg_isosurface_copy(s, capi.ptr(V, capi.F64P), capi.ptr(T, capi.U32P)))
-                return V, T
+                E = None
+                if edges:
+                    E = np.empty(nv, np.uint64)
+                    capi.check(capi.lib.dg_isosurface_copy_edges(s, capi.ptr(E, capi.U64P)))
+                return V, T, E
             import torch
             if nv >= 2 ** 31:
                 raise ValueError(f"isosurface: {nv} vertices do not fit the int32 indices of the device route; use device=False")
@@ -914,11 +974,55 @@ class CubicLagrangeDiscreteGrid:
             T = torch.empty((nt, 3), dtype=torch.int32, device=dev)
             st = _device.stream(V)
             capi.check(capi.lib.dg_isosurface_copy_device(s, V.data_ptr(), T.data_ptr(), st))
+            E = None
+            if edges:
+                E = torch.empty(nv, dtype=torch.int64, device=dev)
+                capi.check(capi.lib.dg_isosurface_copy_edges_device(s, E.data_ptr(), st))
             if not capi.EMULATED:
                 torch.cuda.current_stream(dev).synchronize()          # the copies read the handle, released below
-            return V, T
+            return V, T, E
         finally:
             capi.lib.dg_isosurface_destroy(s)
+
+    def _isosurface_trainable(self, field_id, iso, subdivisions, c, edges):
+        """isosurface(..., coefficients=c): dg_field_set_nodes_device on torch's current stream, then K6 (the route of interpolate(coefficients=))"""
+        import torch
+        tf = self._trainable_field(field_id)        # the closures below keep it (not the grid) alive for the backward
+        h, n_nodes = tf.handle, tf.n_nodes
+        if not isinstance(c, torch.Tensor) or c.dtype != torch.float64:
+            raise TypeError(f"isosurface: coefficients must be a float64 tensor (got {type(c).__name__ if not isinstance(c, torch.Tensor) else c.dtype})")
+        if tuple(c.shape) != (n_nodes,):
+            raise ValueError(f"isosurface: coefficients must have shape ({n_nodes},), got {tuple(c.shape)}")
+        if not capi.EMULATED and (not c.is_cuda or c.device.index != tf.device):
+            raise ValueError(f"isosurface: coefficients are on {c.device} but the field lives on cuda:{tf.device}")
+        c = c.contiguous()
+
+        token = object()                   # this call's pack: the backward repacks c unless the field still holds it
+
+        def hold(cc, again):
+            if again and tf.holds is token:
+                return
+            capi.check(capi.lib.dg_field_set_nodes_device(h, cc.data_ptr(), n_nodes, _device.stream(cc)))
+            tf.holds = token
+
+        def run(cc):
+            hold(cc, False)
+            if not capi.EMULATED:
+                torch.cuda.current_stream(cc.device).synchronize()   # dg_isosurface_create runs on the legacy default stream
+            return self._isosurface(h, iso, subdivisions, True, True)
+
+        def vjp(cc, E, grad_V):
+            hold(cc, True)
+            gV = grad_V.to(torch.float64).contiguous()
+            out = torch.empty(n_nodes, dtype=torch.float64, device=cc.device)
+            capi.check(capi.lib.dg_isosurface_vjp_device(h, iso, subdivisions, len(E), E.data_ptr(), gV.data_ptr(), out.data_ptr(),
+                                                         _device.stream(cc)))
+            return out
+        if torch.is_grad_enabled() and c.requires_grad:
+            V, T, E = _isosurface_function().apply(c, run, vjp)
+        else:
+            V, T, E = run(c)
+        return (V, T, E) if edges else (V, T)
 
     def raycast(self, field_id, origins, directions, iso=0.0, t_min=0.0, t_max=math.inf, coefficients=None):
         """The first crossing of {phi = iso} along rays x(t) = origin + t * direction, t in [t_min, t_max] clipped to the domain, on the

@@ -405,6 +405,29 @@ DG_API int dg_isosurface_sizes(const dg_isosurface* s, uint64_t* n_vertices, uin
 DG_API int dg_isosurface_copy(const dg_isosurface* s, double* vertices, uint32_t* triangles);
 DG_API int dg_isosurface_copy_device(const dg_isosurface* s, double* d_vertices, uint32_t* d_triangles, void* stream);
 DG_API int dg_isosurface_destroy(dg_isosurface* s);
+/* dg_isosurface_copy_edges[_device]: edge_ids[n_vertices], the lattice edge 7 * lin(p) + d of every vertex (lin and d as in the contract),
+ *   ascending because the vertices are ordered by it; what dg_isosurface_vjp takes.  The rules of dg_isosurface_copy[_device]: NULL only
+ *   when there are no vertices, the _device form asynchronous on `stream`. */
+DG_API int dg_isosurface_copy_edges(const dg_isosurface* s, uint64_t* edge_ids);
+DG_API int dg_isosurface_copy_edges_device(const dg_isosurface* s, uint64_t* d_edge_ids, void* stream);
+
+/* ---- differentiable level sets (K13, k13_isosurface_grad.cu; beyond the reference) ---------------------------------------------------
+ * dg_isosurface_vjp[_device]: for n vertices of dg_isosurface_create(field, iso, subdivisions), given by their edge ids (or any edges of
+ * that lattice), and the upstream gradient grad_vertices[n x 3] of their positions, grad_nodes[n_nodes] = the gradient with respect to the
+ * field's node values.  The field must be made by dg_field_create_trainable and hold the forward's node values.  Each vertex moves along its
+ * edge with t = (iso - f_p) / (f_q - f_p); a vertex whose lattice values are DBL_MAX or not finite, or whose difference is 0 or not finite,
+ * gets 0.  grad_nodes is always overwritten (zeros for n = 0); it is summed as K11 sums interpolate's VJP, over the 2n edge endpoints, so its
+ * bits depend only on the field's topology and values, iso, subdivisions, the edge ids and grad_vertices (the contract is in
+ * k13_isosurface_grad.cu and DESIGN.md section 3).  First order only; not differentiable in iso.  The edge ids are checked on the device
+ * first (one synchronise).  Device scratch of about 150 B per vertex is taken and released in stream order.  The _device form is queued on
+ * `stream`; the host form uploads every input in one piece and returns when grad_nodes is written.
+ *   DG_ERR_INVALID, before anything is written: NULL field; NULL edge_ids or grad_vertices with n > 0; NULL grad_nodes on a field with nodes;
+ *   a field not made by dg_field_create_trainable or on another device; iso not finite; subdivisions outside 1..16; a lattice of 2^31 points
+ *   or more; n >= 2^31; an edge id that is not an edge of the lattice (lin(p) >= points, or p + delta_d outside it). */
+DG_API int dg_isosurface_vjp(const dg_field* field, double iso, uint32_t subdivisions, uint64_t n, const uint64_t* edge_ids,
+                             const double* grad_vertices, double* grad_nodes);
+DG_API int dg_isosurface_vjp_device(const dg_field* field, double iso, uint32_t subdivisions, uint64_t n, const uint64_t* d_edge_ids,
+                                    const double* d_grad_vertices, double* d_grad_nodes, void* stream);
 
 /* ---- ray casts: the first crossing of {phi = iso} along rays and segments (not in the reference) -----------------------------------------
  * For each ray i (origin origins[3 i..], direction directions[3 i..]) and t in [t_min, t_max] clipped to the domain: the first crossing of
